@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — env-steps/sec of the batched Overcooked step engine on N B200s (BASELINE.json metric).
+"""bench.py — env-steps/sec of the batched Overcooked step engine on N H100s (BASELINE.json metric).
 
 One bench "step" = one pass of the hot path over one batch of synthetic input = one full 400-transition horizon of
 the workload's environments.  The headline workload is BASELINE.json configs[1] (cramped_room, 65 536 environments
@@ -18,6 +18,8 @@ the final counters.
   roofline_k1    the per-transition kernel K1 (400 launches from one CUDA graph), SURVEY 8(d)'s 160 B accounting
   configs        short timed legs of the other BASELINE configs (3, 4, the 2^20-env target, 5), each with its own
                  roofline and a CPU replay of 256 sampled environments (`spot_check`)
+  --dump-outputs DIR   after the timed steps, what the last timed step computed, as DIR/<name>.npy (a fixed, seeded
+                 sample of the environments; float32, or float64 where an int32 value needs more than 24 bits)
   cpu_baseline   the C restatement of the reference's transition (oracle/, kind "port") on the usable host cores, and
                  `reference_python`: the reference's OWN Python OvercookedEnv.step loop timed on the same cores in the
                  same run (oracle/_ref copy, oracle/ref_python_bench.py)
@@ -78,7 +80,7 @@ def load_tensor_peak():
             d = json.load(f)
         if "bf16_tflops" in d:
             return float(d["bf16_tflops"]), "measured (MEASURED_PEAKS.json bf16_tflops, burst)"
-    return 1590.0, "fallback (B200_PROFILING.md 1.59 PFLOP/s)"
+    return 989.0, "data sheet (H100 SXM, 700 W: 989 TFLOP/s dense bf16), not measured"
 
 
 def load_peaks():
@@ -86,17 +88,7 @@ def load_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def load_ncu_summary():
-    """Per-kernel figures read off the committed `ncu --set full` captures (profiles/): warp instructions per
-    warp-transition and DRAM bytes per launch, keyed by workload.  Absent keys stay null in the bench line."""
-    p = os.path.join(ROOT, "profiles", "ncu_summary.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            return json.load(f)
-    return {}
+    return 3350.0, "data sheet (H100 SXM: 3.35 TB/s HBM3), not measured"
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -197,7 +189,7 @@ def bind_rank_to_numa_share(local, world):
 
 
 class ClockSampler(object):
-    """nvidia-smi clock / throttle sampling DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle sampling DURING the timed region."""
 
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown," \
         "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -359,29 +351,37 @@ def run_reference(args, rank, world):
 # ---------------------------------------------------------------------------------------------------------------
 # engine legs
 # ---------------------------------------------------------------------------------------------------------------
-def fused_roofline(S, T, n_envs, launch_s, peak, peak_src, clocks, ncu):
+DUMP_ENVS = 2048  # environments sampled per rank for --dump-outputs: 40 MB for the headline workload
+
+
+def dump_outputs(directory, n_envs, dev, rank, per_env=None, per_step=None):
+    """Write DIR/<name>.npy for every array of `per_env` ([N, ...]) and `per_step` ([T, N, ...]), restricted to the same seeded
+    sample of DUMP_ENVS environments in every run.  Integer values go out as float64 (event masks use 29 bits), the rest as
+    float32; rank r > 0 writes <name>.rank<r>.npy."""
+    import torch
+
+    ids = torch.from_numpy(np.sort(np.random.RandomState(20261015).choice(n_envs, size=min(DUMP_ENVS, n_envs), replace=False))).to(dev)
+    os.makedirs(directory, exist_ok=True)
+    arrays = [(name, a, 0) for name, a in (per_env or {}).items()] + [(name, a, 1) for name, a in (per_step or {}).items()]
+    for name, a, env_axis in arrays:
+        x = a.index_select(env_axis, ids).cpu().numpy()
+        x = x.astype(np.float64 if x.dtype in (np.int32, np.int64) else np.float32)
+        np.save(os.path.join(directory, name + (".rank%d" % rank if rank else "") + ".npy"), x)
+    np.save(os.path.join(directory, "env_ids" + (".rank%d" % rank if rank else "") + ".npy"), ids.cpu().numpy().astype(np.float64))
+
+
+def fused_roofline(S, T, n_envs, launch_s, peak, peak_src):
     """Roofline object of one K5 launch (T transitions of n_envs environments)."""
     bytes_per = 32.0 + 2.0 * 4.0 * S / T
     achieved = n_envs * T * bytes_per / launch_s / 1e9
     r = {
-        "bound": "hbm", "governing": "instruction issue / latency (see issue_bound): the fused kernel streams 32 B per env-step and keeps the record on chip",
+        "bound": "hbm", "governing": "instruction issue / latency: the fused kernel streams 32 B per env-step and keeps the record on chip",
         "kernel": "ovc::rollout_kernel<S=%d> K5: T=%d transitions fused in one launch" % (S, T),
         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
         "algorithmic_bytes_per_env_step": bytes_per, "env_steps_per_launch": n_envs * T, "avg_launch_us": launch_s * 1e6,
-        "traffic": None,
         "note": "algorithmic bytes = 8 B actions in + 24 B outputs per env-step + the record once in and out per launch (2*4*S/T); "
                 "launch duration = CUDA-event time of the timed region / launches",
     }
-    if ncu:
-        if ncu.get("dram_bytes_per_launch") is not None:
-            r["traffic"], r["traffic_source"] = ncu["dram_bytes_per_launch"], ncu.get("source")
-        wi = ncu.get("warp_inst_per_warp_transition")
-        if wi and clocks and clocks.get("sm_mhz"):
-            issued = n_envs * T / 32.0 * wi / launch_s
-            peak_issue = 148 * 4 * clocks["sm_mhz"] * 1e6
-            r["issue_bound"] = {"warp_instructions_per_warp_transition": wi, "source": ncu.get("source"),
-                                "achieved_warp_inst_per_s": issued, "peak_warp_inst_per_s": peak_issue, "frac": issued / peak_issue,
-                                "peak_is": "148 SMs x 4 schedulers x SM clock under load"}
     return r
 
 
@@ -408,9 +408,10 @@ def spot_check_rollout(env, actions, out, n_samples=256, seed=1234):
     return ("ok" if not bad else "MISMATCH in " + ",".join(bad)), len(ids)
 
 
-def engine_leg(name, dev, rank, world, seed, steps, warmup, peak, peak_src, ncu_all, clocks=None, envs=0, io=0, pdl=True, sampler=None):
+def engine_leg(name, dev, rank, world, seed, steps, warmup, peak, peak_src, clocks=None, envs=0, io=0, pdl=True, sampler=None, dump=None):
     """One workload: device-resident action trace, `steps` launches of K5, CUDA events, max over ranks; then the
-    sampled CPU replay.  Returns (dict for the bench line, env, actions, out) — the caller may reuse the buffers."""
+    sampled CPU replay.  Returns (dict for the bench line, env, actions, out) — the caller may reuse the buffers.
+    dump: a directory that receives the last timed launch's outputs (dump_outputs)."""
     import torch
 
     from overcooked_ai_b200 import dist as D
@@ -440,6 +441,9 @@ def engine_leg(name, dev, rank, world, seed, steps, warmup, peak, peak_src, ncu_
     torch.cuda.synchronize(dev)
     D.barrier()
     ms = e0.elapsed_time(e1)
+    if dump is not None:
+        dump_outputs(dump, n_envs, dev, rank, per_env={"state": env.state},
+                     per_step={"sparse": out[0], "shaped": out[1], "done": out[2], "events": out[3]})
     if sampler is not None:
         # the timed region lasts a few milliseconds, less than one nvidia-smi sampling period: keep the SAME launches going
         # (untimed) for ~0.4 s so that the clock / throttle record really is taken under this load
@@ -459,14 +463,14 @@ def engine_leg(name, dev, rank, world, seed, steps, warmup, peak, peak_src, ncu_
     leg = {
         "workload": workload_string(name, n_envs), "what": what, "value": tot_steps / (max_ms * 1e-3), "unit": "env-steps/s",
         "steps": steps, "ms_per_step": max_ms / steps, "state_words": S, "gpu_launches": steps,
-        "roofline": fused_roofline(S, T, n_envs, max_ms * 1e-3 / steps, peak, peak_src, clocks, ncu_all.get(name)),
+        "roofline": fused_roofline(S, T, n_envs, max_ms * 1e-3 / steps, peak, peak_src),
         "spot_check": spot if ok_all == world else "MISMATCH on some rank", "spot_check_envs_per_rank": n_spot,
         "sparse_reward_sum": tot_reward,
     }
     return leg, env, actions, out, clocks
 
 
-def policy_leg(dev, rank, world, seed, steps, warmup, envs=0):
+def policy_leg(dev, rank, world, seed, steps, warmup, envs=0, dump=None):
     """BASELINE config 5: step + lossless_state_encoding feeding a random-init torch CNN policy (one CUDA graph per
     transition).  Spot check: an eager stretch whose sampled actions are recorded and replayed on the CPU oracle."""
     import torch
@@ -499,6 +503,9 @@ def policy_leg(dev, rank, world, seed, steps, warmup, envs=0):
         return e0.elapsed_time(e1)
 
     ms = timed(sp.run, steps, warmup)
+    if dump is not None:
+        dump_outputs(dump, n_envs, dev, rank, per_env={"state": env.state, "actions": sp.actions, "values": sp.values,
+                                                       "ret_sparse": sp.ret_sparse, "ret_mixed": sp.ret_mixed})
     ms_env = timed(sp.env_only, 2, 1) / 2
     tot_steps, max_ms, tot_reward = D.reduce_counters(float(n_envs) * T * steps, ms, float(sp.ret_sparse.sum().item()), device=dev)
     _, max_ms_env, _ = D.reduce_counters(0, ms_env, 0, device=dev)
@@ -551,10 +558,9 @@ def policy_leg(dev, rank, world, seed, steps, warmup, envs=0):
         flops = rows * 2.0 * (512 * 512 + 512 * 160)
         peak_tf, peak_src = load_tensor_peak()
         kernels = {"k7_encode_linear_us": k7, "k9_wide_layers_us": k9, "k8_policy_tail_us": k8,
-                   "roofline_k9": {"bound": "tensor", "kernel": "ovc::wide_layers_kernel (tcgen05.mma, accumulators in TMEM): 512 -> 512 -> 160 for %d rows" % rows,
+                   "roofline_k9": {"bound": "tensor", "kernel": "ovc::wide_layers_kernel (wgmma, accumulators in registers): 512 -> 512 -> 160 for %d rows" % rows,
                                    "achieved": flops / (k9 * 1e-6) / 1e12, "peak": peak_tf, "unit": "TFLOP/s", "frac": flops / (k9 * 1e-6) / 1e12 / peak_tf,
                                    "peak_source": peak_src, "flops_per_launch": flops, "avg_launch_us": k9,
-                                   "traffic": (load_ncu_summary().get("config5_k9") or {}).get("dram_bytes_per_launch"),
                                    "note": "timed alone, back to back (burst peak); achieved = 2 * rows * (512*512 + 512*160) / duration"}}
     return {
         "workload": "config5: %s, %d envs/GPU, self-play: %s -> policy (RllibPPOModel-shaped CNN, random init, shared; "
@@ -562,7 +568,7 @@ def policy_leg(dev, rank, world, seed, steps, warmup, envs=0):
                     "-> returns (ovc_accumulate_returns), whole transition in one CUDA graph" % ("+".join(layouts), n_envs,
                     "K7 (lossless encoding + first layer + leaky ReLU from the packed records, observation never materialised)"
                     if sp.fused_first_layer else "K2 lossless encode bf16",
-                    "K9, one tcgen05 / TMEM kernel" if sp.fused_wide else "library GEMMs",
+                    "K9, one wgmma kernel" if sp.fused_wide else "library GEMMs",
                     "K8 (the dense layers of 64, the heads and the Gumbel-max action draw in one kernel)" if sp.fused_tail else "Gumbel-max sampling"),
         "what": what, "value": tot_steps / (max_ms * 1e-3), "unit": "env-steps/s", "steps": steps, "ms_per_step": max_ms / steps,
         "dtype": "int32 env / bf16 activations / bf16 policy",
@@ -590,6 +596,8 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the short legs of the other BASELINE configs")
     ap.add_argument("--no-pdl", action="store_true", help="disable programmatic dependent launch between K1 launches")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs (a seeded sample of the environments) "
+                                                          "as DIR/<name>.npy, to compare two builds output for output")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
@@ -619,10 +627,9 @@ def main():
     D.init("nccl")
     seed = D.broadcast_seed(20260922, device=dev)
     peak, peak_src = load_peaks()
-    ncu_all = load_ncu_summary()
 
     if args.workload == "config5":
-        leg = policy_leg(dev, rank, world, seed, args.steps, args.warmup, args.envs)
+        leg = policy_leg(dev, rank, world, seed, args.steps, args.warmup, args.envs, dump=args.dump_outputs)
         if rank == 0:
             emit({"metric": METRIC, "value": leg["value"], "unit": "env-steps/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                   "ms_per_step": leg["ms_per_step"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -632,8 +639,8 @@ def main():
 
     # ---- headline: the fused rollout kernel on the chosen workload; clocks sampled over exactly this region ----
     sampler = ClockSampler(local) if rank == 0 else None
-    head, env, actions, out, clocks = engine_leg(args.workload, dev, rank, world, seed, args.steps, args.warmup, peak, peak_src, ncu_all,
-                                                 envs=args.envs, io=args.io, pdl=not args.no_pdl, sampler=sampler)
+    head, env, actions, out, clocks = engine_leg(args.workload, dev, rank, world, seed, args.steps, args.warmup, peak, peak_src,
+                                                 envs=args.envs, io=args.io, pdl=not args.no_pdl, sampler=sampler, dump=args.dump_outputs)
     layouts, _, horizon, _ = WORKLOADS[args.workload]
     n_envs, T, S = env.n_envs, horizon, env.state_words
 
@@ -781,7 +788,7 @@ def main():
         del out_t, out, actions, env
         torch.cuda.empty_cache()
         for name in ("config3", "config4", "target2e20"):
-            configs[name] = guarded(lambda: engine_leg(name, dev, rank, world, seed, 3, 3, peak, peak_src, ncu_all, clocks=clocks)[0])
+            configs[name] = guarded(lambda: engine_leg(name, dev, rank, world, seed, 3, 3, peak, peak_src, clocks=clocks)[0])
             torch.cuda.empty_cache()
         configs["config5"] = guarded(policy_leg, dev, rank, world, seed, 2, 1)
 
@@ -795,7 +802,6 @@ def main():
         "achieved": n_envs * k1_bytes / k1_launch_s / 1e9, "peak": peak, "unit": "GB/s", "frac": n_envs * k1_bytes / k1_launch_s / 1e9 / peak,
         "peak_source": peak_src, "algorithmic_bytes_per_env_step": k1_bytes, "env_steps_per_launch": n_envs, "avg_launch_us": k1_launch_s * 1e6,
         "env_steps_per_s_per_gpu": n_envs / k1_launch_s,
-        "traffic": (ncu_all.get(args.workload + "_k1") or {}).get("dram_bytes_per_launch"),
         "note": "SURVEY 8(d): record read + written, 8 B actions, 24 B outputs per env-step; at this batch size the state (%.1f MB) and the "
                 "outputs are L2 resident, so DRAM traffic is below the algorithmic bytes" % (n_envs * S * 4 / 1e6),
     }
@@ -806,8 +812,9 @@ def main():
         "config": {
             "workload": head["workload"], "state_words": S, "mode": "rollout", "io": args.io,
             "parallelism": "env-index sharding x%d, no data-path collective" % world,
-            "l2": "per bench step the action trace + outputs (%.0f MB) stream through HBM and exceed the 126 MB L2; the %.1f MB state tensor "
-                  "is the carried value (on chip for the whole launch)" % (n_envs * T * 32 / 1e6, n_envs * S * 4 / 1e6),
+            "l2": "per bench step the action trace + outputs (%.0f MB) stream through HBM and exceed the %.0f MB L2; the %.1f MB state tensor "
+                  "is the carried value (on chip for the whole launch)" % (n_envs * T * 32 / 1e6, torch.cuda.get_device_properties(dev).L2_cache_size / 1e6,
+                                                                          n_envs * S * 4 / 1e6),
         },
         "clocks": clocks, "e2e": e2e, "gpu_launches": head["gpu_launches"], "roofline": head["roofline"], "roofline_k1": roofline_k1,
         "spot_check": head["spot_check"], "episode_sparse_reward_sum": head["sparse_reward_sum"],

@@ -1,5 +1,5 @@
 /*
- * ovc_b200.h — C ABI of the B200-native batched Overcooked MDP step engine.
+ * ovc_b200.h — C ABI of the H100-native (sm_90a) batched Overcooked MDP step engine.
  *
  * The reference (HumanCompatibleAI/overcooked_ai) is pure Python and has no FFI layer; the
  * boundary this library replaces is the Python call surface
@@ -453,11 +453,11 @@ int ovc_policy_tail(const void *x, int64_t n_rows, int k0, float in_slope, const
 
 /*
  * ovc_wide_layers (K9): the two wide layers of the rollout policy between ovc_encode_linear and ovc_policy_tail
- * (reference model: ppo_rllib.py:54-62, the two 3x3 convolutions, each folded into one matrix) as one tcgen05 kernel:
+ * (reference model: ppo_rllib.py:54-62, the two 3x3 convolutions, each folded into one matrix) as one wgmma kernel:
  *   a1 = leaky_relu(a0 . w1^T + b1, slope);   z2 = a1 . w2^T + b2
  *   a0 bfloat16 [m][k0], w1 bfloat16 [n1][k0], w2 bfloat16 [n2][n1], biases float32, z2 bfloat16 [m][n2] (pre-activation);
  *   built for k0 = 512, n1 = 512, n2 = 160 (OVC_E_UNSUPPORTED otherwise); operands 16-byte aligned, rows contiguous.
- * The activation tile a1 stays on chip (TMEM -> registers -> shared memory as the second layer's A operand); float32
+ * The activation tile a1 stays on chip (in registers, as the second layer's A operand); float32
  * accumulation, a1 rounded to bfloat16 as a materialised activation would be.
  */
 int ovc_wide_layers(const void *a0, int64_t m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2,

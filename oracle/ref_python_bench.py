@@ -4,8 +4,8 @@ the unmodified OvercookedEnv.step loop (reference overcooked_env.py:244-274, res
 joint actions, horizon 400 — (1) one process pinned to one core, (2) one process per usable core, all pinned,
 started together behind a barrier; optionally (3) the same with lossless_state_encoding_mdp after every step.
 
-TEST / MEASUREMENT INFRASTRUCTURE: imports the reference through oracle/refboot.py (/root/reference in the build
-container, the oracle/_ref copy on the GPU box).  Runs in its own process (bench.py spawns it: no CUDA context is ever
+TEST / MEASUREMENT INFRASTRUCTURE: imports the reference through oracle/refboot.py (OVC_REFERENCE, or
+the oracle/_ref copy).  Runs in its own process (bench.py spawns it: no CUDA context is ever
 forked).  Prints ONE JSON line.
 
     python oracle/ref_python_bench.py [--layout cramped_room] [--seconds 4] [--encode]
@@ -92,6 +92,8 @@ def main():
     args = ap.parse_args()
     from oracle import refboot
 
+    if not refboot.available():  # the workers would die in boot() and leave run() waiting for their results
+        sys.exit("reference tree not found at %s" % refboot.REFERENCE_ROOT)
     cpus = usable_cpus()
     one, _ = run(cpus[:1], args.layout, args.seconds, False)
     allc, per = run(cpus, args.layout, args.seconds, False)

@@ -1,5 +1,5 @@
-"""Import the UNMODIFIED reference implementation: /root/reference in the build container, or the file-by-file copy
-under oracle/_ref/ (oracle/make_ref.py; git-ignored, shipped to the GPU box) where that tree does not exist.
+"""Import the UNMODIFIED reference implementation: the checkout named by OVC_REFERENCE, else the file-by-file copy
+under oracle/_ref/ (oracle/make_ref.py; git-ignored).  Without either, the ``reference``-marked tests skip.
 
 TEST / MEASUREMENT INFRASTRUCTURE.  Used by tools/make_golden.py to generate the fixtures under tests/golden/,
 by the ``reference``-marked tests that compare against the live reference, and by oracle/ref_python_bench.py
@@ -18,13 +18,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def _find_root():
-    """/root/reference in the build container; on the GPU box the file-by-file copy oracle/make_ref.py shipped."""
-    env = os.environ.get("OVC_REFERENCE")
-    if env:
-        return env
-    if os.path.isdir(os.path.join("/root/reference", "src", "overcooked_ai_py")):
-        return "/root/reference"
-    return os.path.join(_HERE, "_ref")
+    """OVC_REFERENCE (a checkout of the reference repository), else the copy oracle/make_ref.py made."""
+    return os.environ.get("OVC_REFERENCE") or os.path.join(_HERE, "_ref")
 
 
 REFERENCE_ROOT = _find_root()

@@ -1,4 +1,4 @@
-"""Build csrc/libovc_b200.so for sm_100a with nvcc (in-tree, so the .so travels to the GPU box).
+"""Build csrc/libovc_b200.so for the H100 (sm_90a) with nvcc, in-tree next to the sources.
 
     python -m overcooked_ai_b200.build [--force]
 """
@@ -13,7 +13,7 @@ DEPS = ["ovc_b200.cu", "ovc_step.cuh", "ovc_obs.cuh", "ovc_encfc.cuh", "ovc_tail
 OUT = os.path.join(CSRC, "libovc_b200.so")
 
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

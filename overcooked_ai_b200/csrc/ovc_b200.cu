@@ -1,4 +1,4 @@
-// ovc_b200.cu — sm_100a kernels + C ABI (include/ovc_b200.h) of the batched Overcooked engine.
+// ovc_b200.cu — sm_90a (H100) kernels + C ABI (include/ovc_b200.h) of the batched Overcooked engine.
 //
 // K1  step_kernel<S, IO>     one joint transition of a tile of TILE environments per CTA.
 //     IO = 1  the tile [TILE][S] int32 is brought into shared memory by ONE 2-D tensor-map TMA load
@@ -11,7 +11,7 @@
 // K4  reset_kernel           masked copy of the per-layout start record.
 // The observation kernels (K2 lossless encode, K3 featurize) live in ovc_obs.cuh, K7 (first policy layer on the
 // encoding, evaluated from the record) and the draw / return kernels in ovc_encfc.cuh, K8 (dense tail of the policy +
-// the draw, one kernel) in ovc_tail.cuh, K9 (the policy's two wide layers as one tcgen05 / TMEM kernel) in ovc_wide.cuh.
+// the draw, one kernel) in ovc_tail.cuh, K9 (the policy's two wide layers as one wgmma kernel) in ovc_wide.cuh.
 //
 // The environment path is integer, branchy and HBM-bound (no contraction anywhere): no tensor cores there.  The policy-in-
 // the-loop kernels K8 / K9 (config 5) are the contractions and use them.
@@ -436,15 +436,15 @@ static int launch_rollout(const StepArgs &a, cudaStream_t st) {
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     // Programmatic dependent launch is for the microsecond-long per-transition kernel.  Here it only lets the next launch's
-    // CTAs sit on the SMs beside a kernel that runs for hundreds of microseconds: measured 0.46 ms instead of 0.36 ms per
-    // launch with back-to-back launches of 1-warp CTAs (profiles/r2_k5_experiments.md), nothing with larger CTAs.  Not used.
+    // CTAs sit on the SMs beside a kernel that runs for hundreds of microseconds: slower with back-to-back launches of
+    // 1-warp CTAs, nothing gained with larger CTAs.  Not used.
     cfg.numAttrs = 0;
     cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tmap, a);
     if (e != cudaSuccess) return cuda_fail(e, "rollout kernel launch");
     return OVC_OK;
 }
 
-// environments per CTA of the rollout kernel (measured, profiles/r2_k5_experiments.md): 2 warps per CTA; a many-layout
+// environments per CTA of the rollout kernel: 2 warps per CTA; a many-layout
 // table set (4.5 KB of shared memory per layout and CTA) wants the largest tile so that enough CTAs fit an SM.  One warp
 // per CTA is as fast at 65 536 environments and slower above.  OVC_K5_TILE overrides (tuning hook).
 static int rollout_tile(int S, long long n_envs, int n_layouts) {

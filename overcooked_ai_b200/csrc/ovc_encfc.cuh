@@ -11,7 +11,7 @@
 // four entries per object in the game (shared by both views).  So a view's row of the product is
 //     bias_l + [urgent] u + sum over ~8 entries of value_k * Wt[feature_k][:]
 // i.e. ~8 row gathers of a table instead of W*H*26 = 520 multiply-adds per output: 40-60x fewer operations than the
-// dense contraction, which is why this runs on the CUDA cores out of shared memory and not on tcgen05.
+// dense contraction, which is why this runs on the CUDA cores out of shared memory and not on wgmma.
 //
 // One CTA per SM keeps a column slice Wt[:, slice] of the 19 dynamic planes in shared memory (380 rows x 256 columns
 // of bf16 = 190 KB on a 5x4 grid); a warp owns one environment at a time: lane l decodes object slot l, the entries go

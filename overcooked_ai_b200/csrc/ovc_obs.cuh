@@ -175,9 +175,9 @@ static int encode_lossless_impl(const ovc_layout_t *layouts, const int32_t *stat
     a.inv_items = (unsigned)((0x100000000ull + (unsigned)(W * H + 2 + (S - 4)) - 1) / (unsigned)(W * H + 2 + (S - 4)));
     a.inv_h = (unsigned)((0x100000000ull + (unsigned)H - 1) / (unsigned)H);
     const int obs_bytes = a.obs_elems * esize;
-    // Tile buffer size.  Measured on B200 (tools/kbench.py, 262 144 envs, fp32): 16 KB 85 %, 24 KB 105 %,
-    // 32 KB 104 %, 48 KB 82 %, 64 KB 79 %, 96 KB 61 % of the measured HBM copy peak — small tiles keep
-    // ~8 CTAs per SM in flight so fill, scatter and bulk store of different tiles overlap.
+    // Tile buffer size: small tiles keep ~8 CTAs per SM (228 KB of shared memory on an H100) in flight so that fill,
+    // scatter and bulk store of different tiles overlap; larger tiles leave the SM waiting on fewer, longer stores.
+    // OVC_ENC_BUF_KB overrides it for a sweep (tools/kbench.py).
     static int buf_kb = 0;
     if (buf_kb == 0) {
         const char *env = getenv("OVC_ENC_BUF_KB");  // tuning knob for experiments

@@ -8,13 +8,12 @@
 //     -> Gumbel-max draw of the action (the ovc_sample_actions definition) -> actions int32, values float32
 //
 // As library calls this is 4 GEMMs with N <= 64, 4 activation passes, 2 copies and the draw: ~12 launches that are
-// each latency bound (12 us per 65 536 x 64 GEMM, 6 us per activation pass; profiles/r2_selfplay_stages_*.json)
-// around 2.5 GFLOP of arithmetic.  Here a warp owns 16 rows at a time and never leaves its registers: the first
+// each latency bound around 2.5 GFLOP of arithmetic.  Here a warp owns 16 rows at a time and never leaves its registers: the first
 // layer's A fragments are 16-byte global loads, every later layer's A fragments ARE the previous layer's accumulator
 // fragments (the m16n8 C layout of two adjacent n-tiles is the m16k16 A layout), weights sit in shared memory in the
 // order the B fragments are read (one 8- or 16-byte LDS per fragment pair, conflict free).  Tensor-core work is
-// mma.sync m16n8k16 bf16 -> fp32: at K, N <= 160 x 64 per layer there is no tile a tcgen05 pipeline (128-row tiles
-// staged through shared memory and TMEM) could amortise its hand-offs over — the chain of four tiny layers is
+// mma.sync m16n8k16 bf16 -> fp32: at K, N <= 160 x 64 per layer there is no tile a wgmma pipeline (64-row warpgroup
+// tiles with operands staged through shared memory) could amortise its hand-offs over — the chain of four tiny layers is
 // dependency bound, and registers are the shortest path between them.
 #pragma once
 #include <cuda_bf16.h>

@@ -1,43 +1,42 @@
 // ovc_wide.cuh — K9 wide_layers_kernel (included by ovc_b200.cu after ovc_tail.cuh): the two wide layers of the rollout
 // policy between K7 and K8 (reference model: human_aware_rl/ppo/ppo_rllib.py:54-62, the two 3x3 convolutions, each folded
-// into one matrix by the host) as ONE tcgen05 kernel:
+// into one matrix by the host) as ONE Hopper wgmma kernel:
 //
 //     a1 = leaky_relu(a0 . W1^T + b1)        a0 [M][512] bf16 (K7's output), W1 [512][512] bf16
 //     z2 = a1 . W2^T + b2                    W2 [160][512] bf16, z2 [M][160] bf16 (K8's input: its leaky ReLU is applied there)
 //
-// The 128 x 512 activation tile a1 never reaches HBM: layer 1 accumulates in TMEM (all 512 columns: two N = 256
-// tcgen05.mma per k-step), the epilogue warps read it back (tcgen05.ld), add the bias, apply the leaky ReLU, round to
-// bf16 and write it to shared memory in the K-major 128-byte-swizzle layout a UMMA descriptor reads — the A operand of
-// layer 2, whose accumulator re-uses TMEM columns 0..159.  As library calls the same work is two GEMMs and an activation
-// pass with a1 written once and read twice (3 x 67 MB per 65 536 rows).
+// The 128 x 512 activation tile a1 never reaches HBM or even shared memory.  Layer 1 is computed 128 columns at a time
+// (a 64 x 128 fp32 accumulator per warpgroup, in registers); the epilogue adds the bias, applies the leaky ReLU and rounds
+// to bf16 straight into the register fragment layout wgmma takes for its A operand, and layer 2 then accumulates those
+// 128 columns' contribution into its own 64 x 160 register accumulator (A from registers, W2 from shared memory).  As
+// library calls the same work is two GEMMs and an activation pass with a1 written once and read twice (3 x 67 MB per
+// 65 536 rows).
 //
-// Persistent: one CTA per SM walks 128-row tiles; 10 warps: warp 0 = TMA producer (one lane), warp 1 = TMEM allocation + MMA issue (one lane),
-// warps 2-9 = epilogue (TMEM lane quadrant = warp & 3, two warps per quadrant share the columns).  Operand tiles arrive by
-// TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) through mbarrier rings.  Layer 1 is computed one N-half at a time
-// (columns 0-255, then 256-511: 8 k-chunks of {a0 128 x 64, W1 256 x 64} = 48 KB each through three stages), so that the
-// epilogue of the first half — TMEM -> registers -> the first four k-chunks of the a1 tile — runs UNDER the second half's
-// MMAs; layer 2's first four k-steps then run under the second half's epilogue.  Shared memory: a1 chunks 0-3 (64 KB) own
-// their space, the three stages (144 KB) follow; once layer 1 is done a1 chunks 4-7 and W2's two-slot ring (160 x 64,
-// 20 KB per chunk) overlay the stages.  Every mbarrier wait is bounded (~10 s; a protocol error traps instead of hanging the GPU).
+// Persistent: one CTA per SM walks 128-row tiles; three warpgroups: warps 0-7 = two consumer warpgroups (rows 0-63 and
+// 64-127 of the tile), warpgroup 2 = TMA producer (one lane).  setmaxnreg moves registers from the producer (40 per thread)
+// to the consumers (232): each SM sub-partition then holds one producer and two consumer warps within its 16 K registers.
+// Operand tiles arrive by TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) through two mbarrier rings: {a0 128 x 64, W1 128 x 64} = 32 KB per stage, four stages, for layer 1, and W2's 160 x 128
+// columns of one chunk = 40 KB per stage, two stages, for layer 2 (208 KB of shared memory in all).  Every mbarrier wait
+// is bounded (~10 s; a protocol error traps instead of hanging the GPU).
 #pragma once
 #include <cuda_bf16.h>
 
 namespace ovc {
 
 constexpr int WL_BM = 128, WL_BK = 64, WL_K0 = 512, WL_N1 = 512, WL_N2 = 160;
-constexpr int WL_KC = WL_K0 / WL_BK;        // k-chunks of layer 1
-constexpr int WL_KC2 = WL_N1 / WL_BK;       // k-chunks of layer 2
-constexpr int WL_THREADS = 320;
-constexpr int WL_STAGES = 3;
+constexpr int WL_NC = 128;                  // layer-1 columns per chunk (one wgmma N)
+constexpr int WL_KC = WL_K0 / WL_BK;        // k-chunks of layer 1 per column chunk
+constexpr int WL_CHUNKS = WL_N1 / WL_NC;    // column chunks of layer 1 = k-chunks of layer 2
+constexpr int WL_THREADS = 384;             // 2 consumer warpgroups + the producer warpgroup
+constexpr int WL_STAGES = 4;
 constexpr uint32_t WL_A_BYTES = WL_BM * WL_BK * 2;            // 16 KB
-constexpr uint32_t WL_B1_BYTES = 256 * WL_BK * 2;             // 32 KB: one N-half of a W1 k-chunk
-constexpr uint32_t WL_STAGE = WL_A_BYTES + WL_B1_BYTES;       // 48 KB
-constexpr uint32_t WL_A1_BYTES = WL_KC2 * WL_A_BYTES;         // 128 KB: the activation tile as layer 2's A operand
-constexpr uint32_t WL_B2_BYTES = WL_N2 * WL_BK * 2;           // 20 KB
-constexpr uint32_t WL_STAGE0 = WL_A1_BYTES / 2;               // stages start behind a1 chunks 0-3
-constexpr uint32_t WL_TILE_BYTES = WL_STAGE0 + WL_STAGES * WL_STAGE;  // 208 KB >= a1 tile + W2 ring (168 KB)
-static_assert(WL_TILE_BYTES >= WL_A1_BYTES + 2 * WL_B2_BYTES, "a1 chunks 4-7 and the W2 ring overlay the stages");
-constexpr uint32_t WL_SMEM = 1024 + WL_TILE_BYTES + (WL_N1 + WL_N2) * 4 + 192;  // tile + biases + 17 mbarriers / the TMEM slot
+constexpr uint32_t WL_B1_BYTES = WL_NC * WL_BK * 2;           // 16 KB
+constexpr uint32_t WL_STAGE = WL_A_BYTES + WL_B1_BYTES;       // 32 KB
+constexpr uint32_t WL_B2_BOX = WL_N2 * WL_BK * 2;             // 20 KB: 64 columns of W2
+constexpr uint32_t WL_B2_STAGE = (WL_NC / WL_BK) * WL_B2_BOX; // 40 KB: W2's columns of one chunk
+constexpr uint32_t WL_TILE_BYTES = WL_STAGES * WL_STAGE + 2 * WL_B2_STAGE;  // 208 KB
+constexpr uint32_t WL_SMEM = 1024 + WL_TILE_BYTES + (WL_N1 + WL_N2) * 4 + 128;  // tiles + biases + 12 mbarriers
+static_assert(WL_SMEM <= 227 * 1024, "one CTA per SM within the opt-in shared memory of sm_90");
 
 struct WideArgs {
     const float *b1, *b2;
@@ -64,54 +63,81 @@ __device__ __forceinline__ void mbar_wait_bounded(uint64_t *bar, uint32_t parity
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst)), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
+template <int N>
+__device__ __forceinline__ void regs_dealloc() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
-// D[tmem] (+)= A[smem desc] . B[smem desc]^T, bf16 x bf16 -> fp32, issued by one thread for the CTA
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all tcgen05.mma issued so far by this thread -> one arrival on `bar` when they have completed
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 consecutive fp32 columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t v[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+template <int N>
+__device__ __forceinline__ void regs_alloc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 
-// UMMA shared-memory descriptor of a K-major bf16 tile stored as rows of 128 bytes (64 elements) with the 128-byte swizzle
+// wgmma shared-memory descriptor of a K-major bf16 tile stored as rows of 128 bytes (64 elements) with the 128-byte swizzle
 // (what TMA's CU_TENSOR_MAP_SWIZZLE_128B writes): start address >> 4, leading byte offset (unused for swizzled K-major) 1,
-// stride byte offset 1024 (8 rows), descriptor version 1 (sm_100), layout type 2 = SWIZZLE_128B.  Tile bases are 1024-byte
-// aligned (base offset 0); a k-step of 16 elements advances the start address by 32 bytes inside the swizzle atom.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-           ((uint64_t)2 << 61);
+// stride byte offset 1024 (8 rows), layout type 1 = SWIZZLE_128B at bit 62.  Tile bases are 1024-byte aligned (base
+// offset 0); a k-step of 16 elements advances the start address by 32 bytes inside the swizzle atom.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-// instruction descriptor, kind::f16: D fp32 (bits 4-5 = 1), A / B bf16 (bits 7-9, 10-12 = 1), both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int m, int n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+
+// d[64] (+)= A[smem desc] . B[smem desc]^T: m64n128k16, bf16 x bf16 -> fp32, both operands K-major
+__device__ __forceinline__ void wgmma_m64n128_ss(float d[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+// d[80] (+)= A[registers] . B[smem desc]^T: m64n160k16, A in the register fragment layout of m64nNk16 (that of mma.sync
+// m16n8k16 per warp, warp w of the warpgroup holding rows 16w..16w+15), B K-major
+__device__ __forceinline__ void wgmma_m64n160_rs(float d[80], const uint32_t a[4], uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %85, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n160k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
+        "{%80, %81, %82, %83}, %84, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+__device__ __forceinline__ uint32_t leaky_bf16x2(float x0, float x1, float slope) {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(fmaxf(x0, x0 * slope), fmaxf(x1, x1 * slope));
+    return *reinterpret_cast<const uint32_t *>(&h);
 }
 
 __global__ void __launch_bounds__(WL_THREADS, 1)
@@ -119,151 +145,116 @@ wide_layers_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_cons
                    const __grid_constant__ CUtensorMap map_w2, const WideArgs p) {
     extern __shared__ char wl_raw[];
     char *tile = reinterpret_cast<char *>((reinterpret_cast<uintptr_t>(wl_raw) + 1023) & ~(uintptr_t)1023);
+    char *w2_tile = tile + WL_STAGES * WL_STAGE;
     float *bias1 = reinterpret_cast<float *>(tile + WL_TILE_BYTES);
     float *bias2 = bias1 + WL_N1;
     uint64_t *bars = reinterpret_cast<uint64_t *>(bias2 + WL_N2);
-    uint64_t *full = bars, *empty = bars + 3, *w2_full = bars + 6, *w2_empty = bars + 8;
-    uint64_t *d1_full = bars + 10 /* [2]: per N-half */, *a1_ready = bars + 12 /* [2] */, *d2_full = bars + 14, *d2_drained = bars + 15;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 16);
+    uint64_t *full = bars, *empty = bars + WL_STAGES, *w2_full = bars + 2 * WL_STAGES, *w2_empty = w2_full + 2;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < WL_STAGES; i++) mbar_init(full + i, 1), mbar_init(empty + i, 1);
-        for (int i = 0; i < 2; i++) mbar_init(w2_full + i, 1), mbar_init(w2_empty + i, 1), mbar_init(d1_full + i, 1), mbar_init(a1_ready + i, 256);
-        mbar_init(d2_full, 1), mbar_init(d2_drained, 256);
+        // a stage is free again when all 8 consumer warps have seen their wgmma reading it complete
+        for (int i = 0; i < WL_STAGES; i++) mbar_init(full + i, 1), mbar_init(empty + i, 8);
+        for (int i = 0; i < 2; i++) mbar_init(w2_full + i, 1), mbar_init(w2_empty + i, 8);
         prefetch_tmap(&map_a0), prefetch_tmap(&map_w1), prefetch_tmap(&map_w2);
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
     for (int i = threadIdx.x; i < WL_N1; i += WL_THREADS) bias1[i] = p.b1[i];
     for (int i = threadIdx.x; i < WL_N2; i += WL_THREADS) bias2[i] = p.b2[i];
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *reinterpret_cast<volatile uint32_t *>(tmem_slot);
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp >= 8) {
+        regs_dealloc<40>();
+        if (warp == 8 && lane == 0) {
             // ---- TMA producer: tiles blockIdx.x, + gridDim.x, ...; the rings' use counters run on across tiles ----
             int it1 = 0, it2 = 0;
-            for (int tile_i = blockIdx.x, ti = 0; tile_i < p.n_tiles; tile_i += gridDim.x, ti++) {
+            for (int tile_i = blockIdx.x; tile_i < p.n_tiles; tile_i += gridDim.x) {
                 const int m0 = tile_i * WL_BM;
-                if (ti) mbar_wait_bounded(d2_full, (ti - 1) & 1);  // the previous tile's layer 2 no longer reads what overlays the stages
-                for (int i = 0; i < 2 * WL_KC; i++, it1++) {  // N-half h = i / 8, k-chunk c = i % 8
-                    const int h = i / WL_KC, c = i % WL_KC, s = it1 % WL_STAGES, u = it1 / WL_STAGES;
-                    mbar_wait_bounded(empty + s, (u & 1) ^ 1);
-                    char *st = tile + WL_STAGE0 + s * WL_STAGE;
-                    mbar_expect_tx(full + s, WL_STAGE);
-                    tma_load_2d(st, &map_a0, c * WL_BK, m0, full + s);
-                    tma_load_2d(st + WL_A_BYTES, &map_w1, c * WL_BK, 256 * h, full + s);
-                }
-                mbar_wait_bounded(d1_full + 1, ti & 1);  // layer 1 has finished reading the stages: W2's ring may overlay them
-                for (int c = 0; c < WL_KC2; c++, it2++) {
+                for (int n = 0; n < WL_CHUNKS; n++) {
+                    for (int c = 0; c < WL_KC; c++, it1++) {
+                        const int s = it1 % WL_STAGES, u = it1 / WL_STAGES;
+                        mbar_wait_bounded(empty + s, (u & 1) ^ 1);
+                        char *st = tile + s * WL_STAGE;
+                        mbar_expect_tx(full + s, WL_STAGE);
+                        tma_load_2d(st, &map_a0, c * WL_BK, m0, full + s);  // rows past M: zero fill, still counted
+                        tma_load_2d(st + WL_A_BYTES, &map_w1, c * WL_BK, n * WL_NC, full + s);
+                    }
                     const int s = it2 & 1, u = it2 >> 1;
+                    it2++;
                     mbar_wait_bounded(w2_empty + s, (u & 1) ^ 1);
-                    mbar_expect_tx(w2_full + s, WL_B2_BYTES);
-                    tma_load_2d(tile + WL_A1_BYTES + s * WL_B2_BYTES, &map_w2, c * WL_BK, 0, w2_full + s);
+                    mbar_expect_tx(w2_full + s, WL_B2_STAGE);
+                    for (int h = 0; h < WL_NC / WL_BK; h++)
+                        tma_load_2d(w2_tile + s * WL_B2_STAGE + h * WL_B2_BOX, &map_w2, n * WL_NC + h * WL_BK, 0, w2_full + s);
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ---- MMA issue ----
-            constexpr uint32_t ID1 = umma_idesc_bf16(WL_BM, 256), ID2 = umma_idesc_bf16(WL_BM, WL_N2);
-            int it1 = 0, it2 = 0;
-            for (int tile_i = blockIdx.x, ti = 0; tile_i < p.n_tiles; tile_i += gridDim.x, ti++) {
-                if (ti) {  // the previous tile's second epilogue has read its accumulator out of TMEM columns 0..159
-                    mbar_wait_bounded(d2_drained, (ti - 1) & 1);
-                    tc_fence_after();
-                }
-                for (int i = 0; i < 2 * WL_KC; i++, it1++) {
-                    const int h = i / WL_KC, c = i % WL_KC, s = it1 % WL_STAGES, u = it1 / WL_STAGES;
-                    mbar_wait_bounded(full + s, u & 1);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(tile + WL_STAGE0 + s * WL_STAGE);
-                    const uint64_t da = umma_desc_sw128(a_addr), db = umma_desc_sw128(a_addr + WL_A_BYTES);
+        return;
+    }
+
+    // ---- consumer warpgroup g: rows 64 g .. 64 g + 63 of the tile; warp w of the group owns 16 of them ----
+    regs_alloc<232>();
+    const int g = warp >> 2, w = warp & 3;
+    float acc1[64], acc2[80];
+    uint32_t a1[WL_NC / 16][4];  // the activation chunk as layer 2's A fragments, one [4] per k-step of 16
 #pragma unroll
-                    for (int k = 0; k < WL_BK / 16; k++) umma_bf16(tmem + 256 * h, da + 2 * k, db + 2 * k, ID1, (c | k) != 0);
-                    umma_commit(empty + s);
-                    if (c == WL_KC - 1) umma_commit(d1_full + h);  // this half of the accumulator is complete
-                }
-                for (int c = 0; c < WL_KC2; c++, it2++) {
-                    if (c == 0 || c == WL_KC2 / 2) {  // a1 chunks 0-3 come from the first half's epilogue, 4-7 from the second's
-                        mbar_wait_bounded(a1_ready + (c ? 1 : 0), ti & 1);
-                        tc_fence_after();
-                    }
-                    const int s = it2 & 1, u = it2 >> 1;
-                    mbar_wait_bounded(w2_full + s, u & 1);
-                    tc_fence_after();
-                    const uint64_t da = umma_desc_sw128(smem_u32(tile + c * WL_A_BYTES));
-                    const uint64_t db = umma_desc_sw128(smem_u32(tile + WL_A1_BYTES + s * WL_B2_BYTES));
+    for (int i = 0; i < 80; i++) acc2[i] = 0.f;
+    int it1 = 0, it2 = 0;
+    for (int tile_i = blockIdx.x; tile_i < p.n_tiles; tile_i += gridDim.x) {
+        for (int n = 0; n < WL_CHUNKS; n++) {
+            // layer 1, columns n*128 .. n*128+127: 8 k-chunks, one stage each; a stage is released once the wgmma
+            // group after it has been issued and it has itself completed (wait_group 1)
 #pragma unroll
-                    for (int k = 0; k < WL_BK / 16; k++) umma_bf16(tmem, da + 2 * k, db + 2 * k, ID2, (c | k) != 0);
-                    umma_commit(w2_empty + s);
-                }
-                umma_commit(d2_full);
+            for (int i = 0; i < 64; i++) acc1[i] = 0.f;
+            int prev = 0;
+            for (int c = 0; c < WL_KC; c++, it1++) {
+                const int s = it1 % WL_STAGES, u = it1 / WL_STAGES;
+                mbar_wait_bounded(full + s, u & 1);
+                const uint32_t a_addr = smem_u32(tile + s * WL_STAGE) + g * (WL_A_BYTES / 2);
+                const uint64_t da = wgmma_desc_sw128(a_addr), db = wgmma_desc_sw128(smem_u32(tile + s * WL_STAGE + WL_A_BYTES));
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < WL_BK / 16; k++) wgmma_m64n128_ss(acc1, da + 2 * k, db + 2 * k, (c | k) != 0);
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (c && lane == 0) mbar_arrive(empty + prev);
+                prev = s;
             }
-        }
-    } else {
-        // ---- epilogue warps: TMEM lane quadrant q, this thread's row r of the tile; the two warps of a quadrant split the columns ----
-        const int q = warp & 3, g = (warp - 2) >> 2, r = q * 32 + lane;
-        const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16);
-        for (int tile_i = blockIdx.x, ti = 0; tile_i < p.n_tiles; tile_i += gridDim.x, ti++) {
-        const int m0 = tile_i * WL_BM;
-        for (int h = 0; h < 2; h++) {
-            mbar_wait_bounded(d1_full + h, ti & 1);
-            tc_fence_after();
-            for (int jj = 0; jj < 4; jj++) {  // 32 columns at a time: bias, leaky ReLU, bf16, 64 bytes into the swizzled a1 tile
-                const int j = 8 * h + 4 * g + jj;
-                uint32_t v[32];
-                tmem_ld32(lane_addr + 32 * j, v);
-                uint32_t w[16];
+            wgmma_wait<0>();
+            if (lane == 0) mbar_arrive(empty + prev);
+            // epilogue 1: bias, leaky ReLU, bf16.  Accumulator n8-group j holds (row l/4, columns 8j + 2(l%4) + {0,1}) in
+            // [4j], [4j+1] and row l/4 + 8 in [4j+2], [4j+3]; k-step q's A fragment is groups 2q (registers 0, 1) and 2q+1 (2, 3).
+            const float *bn = bias1 + n * WL_NC + 2 * (lane & 3);
 #pragma unroll
-                for (int i = 0; i < 16; i++) {
-                    const float x0 = __uint_as_float(v[2 * i]) + bias1[32 * j + 2 * i], x1 = __uint_as_float(v[2 * i + 1]) + bias1[32 * j + 2 * i + 1];
-                    const __nv_bfloat162 hh = __floats2bfloat162_rn(fmaxf(x0, x0 * p.slope), fmaxf(x1, x1 * p.slope));
-                    w[i] = *reinterpret_cast<const uint32_t *>(&hh);
-                }
-                char *rowp = tile + (j >> 1) * WL_A_BYTES + r * 128;
-#pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    const int unit = ((j & 1) * 4 + i) ^ (r & 7);  // 128-byte swizzle: 16-byte unit index XOR (row mod 8)
-                    *reinterpret_cast<uint4 *>(rowp + unit * 16) = make_uint4(w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]);
-                }
+            for (int j = 0; j < WL_NC / 8; j++) {
+                const float b0 = bn[8 * j], b1 = bn[8 * j + 1];
+                a1[j >> 1][(j & 1) * 2] = leaky_bf16x2(acc1[4 * j] + b0, acc1[4 * j + 1] + b1, p.slope);
+                a1[j >> 1][(j & 1) * 2 + 1] = leaky_bf16x2(acc1[4 * j + 2] + b0, acc1[4 * j + 3] + b1, p.slope);
             }
-            tc_fence_before();
-            fence_async_smem();  // generic-proxy stores above -> visible to the tensor core's (async proxy) reads
-            mbar_arrive(a1_ready + h);
-        }
-        mbar_wait_bounded(d2_full, ti & 1);
-        tc_fence_after();
-        const long long row = (long long)m0 + r;
-        for (int j = g ? 3 : 0; j < (g ? WL_N2 / 32 : 3); j++) {
-            uint32_t v[32];
-            tmem_ld32(lane_addr + 32 * j, v);
-            if (row < p.m) {
-                uint4 *dst = reinterpret_cast<uint4 *>(p.z2 + row * WL_N2 + 32 * j);
+            // layer 2: z2 += a1[:, n*128 .. n*128+127] . W2[:, n*128 .. n*128+127]^T
+            const int s = it2 & 1, u = it2 >> 1;
+            it2++;
+            mbar_wait_bounded(w2_full + s, u & 1);
+            const uint32_t b_addr = smem_u32(w2_tile + s * WL_B2_STAGE);
+            wgmma_fence();
 #pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    uint32_t w[4];
-#pragma unroll
-                    for (int e = 0; e < 4; e++) {
-                        const int c0 = 8 * i + 2 * e;
-                        const __nv_bfloat162 hh = __floats2bfloat162_rn(__uint_as_float(v[c0]) + bias2[32 * j + c0],
-                                                                        __uint_as_float(v[c0 + 1]) + bias2[32 * j + c0 + 1]);
-                        w[e] = *reinterpret_cast<const uint32_t *>(&hh);
-                    }
-                    dst[i] = make_uint4(w[0], w[1], w[2], w[3]);
-                }
-            }
+            for (int q = 0; q < WL_NC / 16; q++)
+                wgmma_m64n160_rs(acc2, a1[q], wgmma_desc_sw128(b_addr + (q >> 2) * WL_B2_BOX) + 2 * (q & 3), (n | q) != 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            if (lane == 0) mbar_arrive(w2_empty + s);
         }
-        tc_fence_before();
-        mbar_arrive(d2_drained);  // TMEM columns 0..159 may be overwritten by the next tile's first layer
+        // epilogue 2: bias, bf16, two rows of 160 columns per quad of lanes
+        const long long row = (long long)tile_i * WL_BM + g * 64 + w * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < WL_N2 / 8; j++) {
+            const int col = 8 * j + 2 * (lane & 3);
+            const float b0 = bias2[col], b1 = bias2[col + 1];
+            if (row < p.m)
+                *reinterpret_cast<__nv_bfloat162 *>(p.z2 + row * WL_N2 + col) = __floats2bfloat162_rn(acc2[4 * j] + b0, acc2[4 * j + 1] + b1);
+            if (row + 8 < p.m)
+                *reinterpret_cast<__nv_bfloat162 *>(p.z2 + (row + 8) * WL_N2 + col) = __floats2bfloat162_rn(acc2[4 * j + 2] + b0, acc2[4 * j + 3] + b1);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, 512);
 }
 
 static int make_tmap_bf16(CUtensorMap *m, const void *base, long long rows, int cols, int box_rows) {
@@ -289,7 +280,7 @@ static int wide_layers_impl(const void *a0, long long m, int k0, const void *w1,
     if (m == 0) return OVC_OK;
     CUtensorMap ma, mw1, mw2;
     int rc = make_tmap_bf16(&ma, a0, m, WL_K0, WL_BM);
-    if (!rc) rc = make_tmap_bf16(&mw1, w1, WL_N1, WL_K0, 256);  // one N-half of a k-chunk per box
+    if (!rc) rc = make_tmap_bf16(&mw1, w1, WL_N1, WL_K0, WL_NC);  // one column chunk of a k-chunk per box
     if (!rc) rc = make_tmap_bf16(&mw2, w2, WL_N2, WL_N1, WL_N2);
     if (rc) return rc;
     cudaError_t e = cudaFuncSetAttribute(wide_layers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WL_SMEM);
@@ -300,7 +291,7 @@ static int wide_layers_impl(const void *a0, long long m, int k0, const void *w1,
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     p.b1 = b1, p.b2 = b2, p.z2 = (__nv_bfloat16 *)z2, p.m = m, p.slope = slope;
     p.n_tiles = (int)((m + WL_BM - 1) / WL_BM);
-    // persistent: one CTA per SM walks tiles blockIdx.x, + gridDim.x, ... (barriers, TMEM and biases are set up once)
+    // persistent: one CTA per SM walks tiles blockIdx.x, + gridDim.x, ... (barriers and biases are set up once)
     wide_layers_kernel<<<(unsigned)(p.n_tiles < n_sm ? p.n_tiles : n_sm), WL_THREADS, WL_SMEM, st>>>(ma, mw1, mw2, p);
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "wide_layers kernel launch");

@@ -19,7 +19,7 @@ ppo_rllib_client.py:85-88: conv 5x5x25 'same', conv 3x3x25 'same', conv 3x3x25 '
 of 64, leaky ReLU, heads 6 + 1), random init, shared by both agents.  ``RllibShapedCNN`` is that model in torch
 (the consumer a user brings: cuDNN / cuBLAS); ``DenseGridPolicy`` is the same function as one matrix per layer, and
 on a 5x4 grid ``SelfPlayRollout`` evaluates it entirely with this library's kernels: K7 (encoding + first layer from
-the packed records), K9 (the two wide layers, tcgen05 / TMEM), K8 (dense tail + heads + action draw).
+the packed records), K9 (the two wide layers, wgmma), K8 (dense tail + heads + action draw).
 """
 import torch
 import torch.nn as nn
@@ -86,8 +86,7 @@ class DenseGridPolicy(nn.Module):
     ``pad_to``: every layer's width is rounded up to a multiple of it with zero weights and zero biases (leaky ReLU of 0
     is 0, the next layer's extra input columns are zero too: the function is unchanged).  Widths of 500 / 150 bf16
     elements give rows that are not 16-byte multiples, which sends the library to its Ampere-era ``align2`` mma.sync
-    kernels (measured: 160 us for the first layer at 65 536 rows, profiles/r2_selfplay_stages_before.json); 512 / 160 reach the sm_100
-    kernels.  The two heads are one matrix (6 logits + 1 value, padded to 8).  ``forward`` / ``forward_from`` / ``trunk`` run
+    kernels; 512 / 160 reach its tensor-core kernels for the GPU.  The two heads are one matrix (6 logits + 1 value, padded to 8).  ``forward`` / ``forward_from`` / ``trunk`` run
     it as library GEMMs; ``first_layer_table`` / ``wide_tables`` / ``tail_tables`` hand the same weights to K7 / K9 / K8."""
 
     def __init__(self, cnn, width, height, pad_to=1):
@@ -187,8 +186,8 @@ def fused_kernel_support(dense_model, width, height):
 
 def sample_categorical(logits, noise):
     """One draw per row from softmax(logits) by the Gumbel-max rule: argmax_i (logit_i - log E_i) with E_i ~ Exp(1) picks i
-    with probability softmax(logits)_i — four small kernels where softmax + ``torch.multinomial`` launch about twenty
-    (profiles/r2_selfplay_stages_before.json).  ``logits`` (float32) is overwritten with the perturbed scores, ``noise`` is scratch of
+    with probability softmax(logits)_i — four small kernels where softmax + ``torch.multinomial`` launch about twenty.
+    ``logits`` (float32) is overwritten with the perturbed scores, ``noise`` is scratch of
     the same shape."""
     logits.sub_(noise.exponential_().log_())
     return torch.argmax(logits, dim=-1)
@@ -216,7 +215,7 @@ class SelfPlayRollout(object):
         ONE kernel (``ovc_policy_tail``, K8) on the last convolution's pre-activation; the library GEMMs are then only the
         two wide layers.
         fused_wide (default: with K7 and K8 when the wide layers are 512 -> 512 -> 160, i.e. on 5x4 grids): those two layers
-        run as ONE tcgen05 kernel (``ovc_wide_layers``, K9: the 512-wide activation stays in TMEM / shared memory) — the
+        run as ONE wgmma kernel (``ovc_wide_layers``, K9: the 512-wide activation stays in registers) — the
         whole policy is then K7 -> K9 -> K8, no library call."""
         assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
         self.env = env

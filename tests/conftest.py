@@ -9,8 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-    config.addinivalue_line("markers", "reference: needs the reference tree at /root/reference (build container only)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
+    config.addinivalue_line("markers", "reference: needs the reference tree (OVC_REFERENCE, or the oracle/_ref copy)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -561,9 +561,9 @@ def test_k8_policy_tail_vs_float_reference(k0, n_hidden, n_rows):
 
 @pytest.mark.parametrize("m", [128, 1000, 1, 4096 + 77, 128 * 449 + 5])
 def test_k9_wide_layers_vs_float_reference(m):
-    """K9 (tcgen05: a1 = leaky_relu(a0 W1^T + b1) kept on chip, z2 = a1 W2^T + b2) against a float32 restatement with the
+    """K9 (wgmma: a1 = leaky_relu(a0 W1^T + b1) kept in registers, z2 = a1 W2^T + b2) against a float32 restatement with the
     activation rounded to bf16 between the layers; partial last tiles; the largest case gives every persistent CTA three or
-    four tiles (barrier phases, TMEM and shared-memory re-use across tiles)."""
+    four tiles (barrier phases, accumulator and shared-memory re-use across tiles)."""
     lib = _native.lib()
     rng = np.random.RandomState(m)
     a0 = _bf16(rng.normal(size=(m, 512)))
@@ -983,7 +983,7 @@ def test_packed_event_codes_cover_every_event_pattern():
 def test_two_ranks_mixed_batch_on_gpus():
     """SURVEY 8(e) on hardware: 2 NCCL ranks (one per GPU), a config-3-shaped mixed batch sharded with
     dist.shard_segments, each rank's shard against the oracle, the reduced counters against the whole batch.  Needs two
-    visible GPUs (the 1-GPU lease skips it)."""
+    visible GPUs (skips on a single GPU)."""
     import os
     import subprocess
     import sys

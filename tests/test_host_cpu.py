@@ -523,7 +523,7 @@ def test_sample_categorical_follows_the_softmax():
 
 
 def test_dense_grid_policy_padding_keeps_the_function():
-    """Width padding (16-byte rows for the library's sm_100 GEMM kernels) adds zero weights only; merged heads."""
+    """Width padding (16-byte rows for the library's tensor-core GEMM kernels) adds zero weights only; merged heads."""
     import torch
 
     from overcooked_ai_b200.selfplay import DenseGridPolicy, RllibShapedCNN

@@ -1,5 +1,5 @@
-"""Live differential tests against the UNMODIFIED reference (build container only; skipped where
-/root/reference is absent, e.g. on the GPU box).  Every bundled 2-player layout, fresh random traces each
+"""Live differential tests against the UNMODIFIED reference (skipped unless OVC_REFERENCE names a checkout of it or
+oracle/_ref holds the copy build() makes from OVC_REFERENCE_SRC).  Every bundled 2-player layout, fresh random traces each
 run of the seed list: the C oracle vs the reference's own get_state_transition / lossless_state_encoding /
 featurize_state / potential_function.  This is what keeps the oracle pinned beyond the stored fixtures."""
 import json

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Quick GPU sanity check of one record-I/O strategy of the step kernel against the CPU oracle.
-Run under `timeout` on the GPU box before the full test-suite:  python tools/gpu_sanity.py --io 1"""
+Run under `timeout` on the GPU before the full test-suite:  python tools/gpu_sanity.py --io 1"""
 import argparse
 import os
 import sys

@@ -3,9 +3,9 @@
 
 The reference stores each layout as a Python dict literal in
 src/overcooked_ai_py/data/layouts/<name>.layout (loader: utils.py:31-33, 223-226).  Layouts are an
-input FORMAT of the hot path (SURVEY.md §2 row 11), and the GPU box has no /root/reference, so
-the grids + recipe parameters are normalised once into one JSON document that travels with the
-package.  Run here (container with /root/reference):  python tools/import_layouts.py
+input FORMAT of the hot path (SURVEY.md §2 row 11), and the package must not depend on a checkout of
+the reference, so the grids + recipe parameters are normalised once into one JSON document that travels
+with the package.  With a checkout of the reference:  OVC_REFERENCE=<checkout> python tools/import_layouts.py
 """
 import ast
 import glob
@@ -13,7 +13,7 @@ import json
 import os
 import sys
 
-REF = os.environ.get("OVC_REFERENCE", "/root/reference")
+REF = os.environ["OVC_REFERENCE"]
 SRC = os.path.join(REF, "src/overcooked_ai_py/data/layouts")
 DST = os.path.join(os.path.dirname(__file__), "..", "overcooked_ai_b200", "data", "layouts.json")
 

@@ -3,7 +3,7 @@
 
 Timing: CUDA events around a CUDA-graph replay of `reps` launches (graph removes the Python launch
 cost; what is left per launch is kernel time + launch gap).  For batch sizes whose working set fits
-the 126 MB L2 the numbers are L2-assisted; the 4M-env rows exceed L2 and are HBM-true.
+the L2 (50 MB on an H100) the numbers are L2-assisted; the 4M-env rows exceed L2 and are HBM-true.
 Prints one JSON line per measurement.  Usage: python tools/kbench.py [--layout cramped_room] [--quick]
 """
 import argparse

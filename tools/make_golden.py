@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Generate tests/golden/*.npz by running the UNMODIFIED reference (build container only).
+"""Generate tests/golden/*.npz by running the UNMODIFIED reference (needs OVC_REFERENCE=<a checkout of it>).
 
 Every array written here comes out of the reference's own Python functions
 (OvercookedGridworld.get_state_transition / lossless_state_encoding / featurize_state, imported
-from /root/reference through oracle/refboot.py); the reference's own golden vectors
+from the checkout through oracle/refboot.py); the reference's own golden vectors
 (src/overcooked_ai_py/data/testing/...) are replayed and asserted on the way, so the fixtures pin
 "reference as run here == reference's published expectations".  States are stored as packed int32
 records (include/ovc_b200.h) produced by overcooked_ai_b200.layout.pack_state from the reference

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Launch one kernel family a few times so ncu can capture it (see profiles/).
+"""Launch one kernel family a few times so a profiler (Nsight Compute) can capture it.
     ncu --set full --clock-control none --import-source on -k regex:<name> -s 2 -c 1 -o out python tools/prof_kernels.py --which k5
 """
 import argparse

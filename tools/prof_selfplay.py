@@ -20,7 +20,7 @@ ap.add_argument("--eager", type=int, default=3, help="eager transitions (what nc
 ap.add_argument("--stages", action="store_true", help="time the stages with CUDA events")
 ap.add_argument("--dense", type=int, default=1)
 ap.add_argument("--sub-batches", type=int, default=1)
-ap.add_argument("--wide", type=int, default=1, help="K9 (the two wide layers as one tcgen05 kernel)")
+ap.add_argument("--wide", type=int, default=1, help="K9 (the two wide layers as one wgmma kernel)")
 ap.add_argument("--tail", type=int, default=1, help="K8 (dense tail + heads + draw in one kernel)")
 ap.add_argument("--glue", type=int, default=1, help="ovc_sample_actions / ovc_accumulate_returns instead of tensor-library ops")
 ap.add_argument("--fused", type=int, default=1, help="K7 (encoding + first layer from the record) instead of K2 + first GEMM")

@@ -1,7 +1,7 @@
-"""The reference's own Python path timed in the BUILD container (SURVEY.md §8d "CPU baseline beside it", items 1-3):
+"""The reference's own Python path timed on this host's cores (SURVEY.md §8d "CPU baseline beside it", items 1-3):
 OvercookedEnv.step and lossless_state_encoding_mdp, one process, then one process per visible core.
-TEST / MEASUREMENT INFRASTRUCTURE: imports the unmodified reference through oracle/refboot.py; the GPU box has no
-/root/reference, which is why bench.py's reference arm times the C port there and this number is recorded here.
+TEST / MEASUREMENT INFRASTRUCTURE: imports the unmodified reference through oracle/refboot.py (OVC_REFERENCE or the
+oracle/_ref copy); bench.py's reference arm times the C port, which needs no reference checkout.
 
     python tools/ref_python_baseline.py [episodes]
 """
