@@ -435,6 +435,33 @@ int ovc_accumulate_returns(const int32_t *sparse, const int32_t *shaped, float f
                            float *ret_mixed, void *stream);
 
 /*
+ * What a PPO sample batch keeps of each transition (RLlib's SampleBatch: action_logp, rewards, dones; then its GAE
+ * postprocessing into advantages and value_targets), produced on the device:
+ *
+ * ovc_sample_actions_logp: ovc_sample_actions, and logp[r] = s[a] - (m + log(sum_i exp(s[i] - m))) with s = scores[r],
+ *   m = max_i s[i] over i < n_actions, a = the drawn action (float32): the log-probability of the draw.
+ * ovc_record_transition: ovc_accumulate_returns with the factor read from DEVICE memory (`factor`: one float32, so a
+ *   captured graph follows a factor changed between replays) and, each nullable,
+ *     rewards[2 e + i] = (float)sparse[e] + factor * (float)shaped[e][i]   float32 [n_envs][2], the product rounded first
+ *     dones[e] = done[e] != 0                                              uint8 [n_envs] from ovc_step's int32 done
+ *   ret_sparse / ret_mixed are accumulated as ovc_accumulate_returns does when given.
+ * ovc_gae: generalized advantage estimation over a window of n_steps transitions of n_rows = 2 n_envs agent rows:
+ *     rewards, values, advantages, value_targets float32 [n_steps][n_rows];  dones uint8 [n_steps][n_rows / 2] (one flag
+ *     per environment, shared by its two rows: done = terminal, the next value counts 0);  last_values float32 [n_rows]
+ *   from t = n_steps - 1 down to 0, with A = 0 after the window, every operation rounded to float32 on its own:
+ *     nt = 1 - dones[t][r / 2];  next_v = t < n_steps - 1 ? values[t + 1][r] : last_values[r]
+ *     delta = (rewards[t][r] + (gamma * next_v) * nt) - values[t][r]
+ *     A = delta + ((gamma * lambda) * nt) * A;   advantages[t][r] = A;   value_targets[t][r] = A + values[t][r]
+ *   Float buffers 8-byte aligned.
+ */
+int ovc_sample_actions_logp(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter,
+                            int32_t *actions, float *logp, void *stream);
+int ovc_record_transition(const int32_t *sparse, const int32_t *shaped, const int32_t *done, const float *factor, int64_t n_envs,
+                          float *rewards, uint8_t *dones, int64_t *ret_sparse, float *ret_mixed, void *stream);
+int ovc_gae(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, int64_t n_steps, int64_t n_rows,
+            float gamma, float lambda, float *advantages, float *value_targets, void *stream);
+
+/*
  * ovc_policy_tail: the narrow end of the rollout policy and the action draw in one kernel (reference model:
  * human_aware_rl/ppo/ppo_rllib.py:64-79 — dense layers of 64 after the convolutions, then the action / value heads):
  *   a = leaky_relu(x, in_slope)                          x bfloat16 [n_rows][k0], k0 a multiple of 32 in 32..256
@@ -450,6 +477,12 @@ int ovc_policy_tail(const void *x, int64_t n_rows, int k0, float in_slope, const
                     const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                     float slope, int n_actions, uint64_t seed, uint64_t *counter, int32_t *actions, float *values,
                     float *scores, void *stream);
+/* ovc_policy_tail_logp: ovc_policy_tail, and logp[r] (nullable) = the log-probability of the drawn action under
+ * softmax(s[r][0..n_actions)), as ovc_sample_actions_logp defines it on the float32 heads s. */
+int ovc_policy_tail_logp(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                         const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                         float slope, int n_actions, uint64_t seed, uint64_t *counter, int32_t *actions, float *values,
+                         float *scores, float *logp, void *stream);
 
 /*
  * ovc_wide_layers (K9): the two wide layers of the rollout policy between ovc_encode_linear and ovc_policy_tail

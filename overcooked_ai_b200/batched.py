@@ -360,18 +360,25 @@ class BatchedOvercookedEnv(object):
         l = self.layouts[layout_index]
         return (l.width, l.height, 26)
 
-    def lossless_state_encoding(self, out=None, dtype=torch.float32, view_swap=None):
+    def lossless_state_encoding(self, out=None, dtype=torch.float32, view_swap=None, states=None):
         """lossless_state_encoding (overcooked_mdp.py:2385-2561) of every environment, both players:
         tensor [N, 2, W, H, 26] (index order [x][y][channel], as the reference) when all layouts share
         one grid shape, else a list of such tensors, one per layout segment.  dtype float32 (what the
         reference's RLlib consumer casts to), bfloat16, uint8 or int32.  ``view_swap`` (int32 CUDA tensor [N]):
-        where non-zero, ``out[env, 0]`` is player 1's view (primary-agent-first order of the gym wrapper)."""
+        where non-zero, ``out[env, 0]`` is player 1's view (primary-agent-first order of the gym wrapper).
+        ``states``: encode these records (int32 CUDA tensor [M, S], e.g. gathered from a ``selfplay.SampleBatch``)
+        instead of ``self.state``; the result is then [M, 2, W, H, 26] and every layout must share one grid shape."""
+        rows = self.n_envs if states is None else states.shape[0]
+        if states is not None:
+            assert states.dtype == torch.int32 and states.is_cuda and states.is_contiguous() and states.dim() == 2 and \
+                states.shape[1] == self.state_words, "states: int32 CUDA records [M, %d]" % self.state_words
         if view_swap is not None:
-            assert view_swap.dtype == torch.int32 and view_swap.is_cuda and view_swap.is_contiguous() and view_swap.numel() == self.n_envs
+            assert view_swap.dtype == torch.int32 and view_swap.is_cuda and view_swap.is_contiguous() and view_swap.numel() == rows
         shapes = {(l.width, l.height) for l in self.layouts}
         if len(shapes) == 1:
-            runs = [(0, self.n_envs, 0)]
+            runs = [(0, rows, 0)]
         else:
+            assert states is None, "states= needs layouts of one grid shape"
             assert not self.random_layout, "random_layout needs layouts of one grid shape (pad them, LayoutGenerator does)"
             runs = self.segments()
         outs = []
@@ -383,7 +390,7 @@ class BatchedOvercookedEnv(object):
             assert o.is_cuda and o.is_contiguous() and o.numel() == (e - b) * 2 * W * H * 26
             assert o.dtype in _TORCH_DT, "lossless_state_encoding writes float32, bfloat16, uint8 or int32, not %s" % o.dtype
             _native.check(self._lib.ovc_encode_lossless(
-                self.tables.data_ptr(), self.n_layouts, self.state.data_ptr() + 4 * self.state_words * b,
+                self.tables.data_ptr(), self.n_layouts, (self.state if states is None else states).data_ptr() + 4 * self.state_words * b,
                 0 if view_swap is None else view_swap.data_ptr() + 4 * b, o.data_ptr(),
                 _TORCH_DT[o.dtype], e - b, self.state_words, W, H, self.horizon if self.horizon > 0 else 2**31 - 1,
                 self._stream()))
@@ -412,17 +419,23 @@ class BatchedOvercookedEnv(object):
             self.horizon if self.horizon > 0 else 2**31 - 1, n_out, float(neg_slope), self._stream()))
         return out
 
-    def sample_actions(self, scores, counter, seed=0, out=None):
+    def sample_actions(self, scores, counter, seed=0, out=None, logp_out=None):
         """Joint actions drawn from the policy's logits (ovc_sample_actions: Gumbel-max on Philox draws, one kernel).
         ``scores`` float32 ``[2N, ld]`` (rows ordered [env][agent], the first 6 columns are the logits), ``counter`` an
-        int64 CUDA tensor of 2 zeros that the kernel advances (one step per call; graph-replay safe).  Returns int32 [N, 2]."""
+        int64 CUDA tensor of 2 zeros that the kernel advances (one step per call; graph-replay safe).  Returns int32 [N, 2].
+        ``logp_out`` (float32 [2N]): also the log-probability of each drawn action (ovc_sample_actions_logp)."""
         assert scores.is_cuda and scores.dtype == torch.float32 and scores.dim() == 2 and scores.stride(1) == 1 and scores.shape[0] == 2 * self.n_envs
         assert counter.is_cuda and counter.dtype == torch.int64 and counter.numel() == 2 and counter.is_contiguous()
         if out is None:
             out = torch.empty((self.n_envs, 2), dtype=torch.int32, device=self.device)
         assert out.is_cuda and out.dtype == torch.int32 and out.is_contiguous() and out.numel() == 2 * self.n_envs
-        _native.check(self._lib.ovc_sample_actions(scores.data_ptr(), scores.stride(0), 6, 2 * self.n_envs, int(seed) & (2**64 - 1),
-                                                   counter.data_ptr(), out.data_ptr(), self._stream()))
+        if logp_out is None:
+            _native.check(self._lib.ovc_sample_actions(scores.data_ptr(), scores.stride(0), 6, 2 * self.n_envs, int(seed) & (2**64 - 1),
+                                                       counter.data_ptr(), out.data_ptr(), self._stream()))
+            return out
+        assert logp_out.is_cuda and logp_out.dtype == torch.float32 and logp_out.is_contiguous() and logp_out.numel() == 2 * self.n_envs
+        _native.check(self._lib.ovc_sample_actions_logp(scores.data_ptr(), scores.stride(0), 6, 2 * self.n_envs, int(seed) & (2**64 - 1),
+                                                        counter.data_ptr(), out.data_ptr(), logp_out.data_ptr(), self._stream()))
         return out
 
     def accumulate_returns(self, ret_sparse, ret_mixed, factor=1.0):
@@ -433,6 +446,35 @@ class BatchedOvercookedEnv(object):
         _native.check(self._lib.ovc_accumulate_returns(self.sparse.data_ptr(), self.shaped.data_ptr(), float(factor), self.n_envs,
                                                        0 if ret_sparse is None else ret_sparse.data_ptr(),
                                                        0 if ret_mixed is None else ret_mixed.data_ptr(), self._stream()))
+
+    def record_transition(self, factor, rewards=None, dones=None, ret_sparse=None, ret_mixed=None):
+        """What a sample batch keeps of the last ``step`` (ovc_record_transition, one kernel): ``rewards`` float32 [N, 2] =
+        sparse + factor * shaped[:, i] per agent (rllib.py:328-329), ``dones`` uint8 [N], and the running returns as
+        ``accumulate_returns`` keeps them; each output optional.  ``factor``: float32 CUDA scalar tensor, read by the
+        kernel (a captured graph follows its current value)."""
+        assert factor.is_cuda and factor.dtype == torch.float32 and factor.numel() == 1
+        for t, dt, n in ((rewards, torch.float32, 2), (dones, torch.uint8, 1), (ret_sparse, torch.int64, 1), (ret_mixed, torch.float32, 1)):
+            assert t is None or (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n * self.n_envs)
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        _native.check(self._lib.ovc_record_transition(self.sparse.data_ptr(), self.shaped.data_ptr(), self.done.data_ptr(), factor.data_ptr(),
+                                                      self.n_envs, ptr(rewards), ptr(dones), ptr(ret_sparse), ptr(ret_mixed), self._stream()))
+
+    def gae(self, rewards, values, dones, last_values, gamma, lam, advantages=None, value_targets=None):
+        """Generalized advantage estimation over a window (ovc_gae; include/ovc_b200.h gives the recurrence): rewards /
+        values float32 [T, 2N] (rows [env][agent]), dones uint8 [T, N] (terminal), last_values float32 [2N].  Returns
+        (advantages, value_targets) float32 [T, 2N]."""
+        T = rewards.shape[0]
+        R = 2 * self.n_envs
+        if advantages is None:
+            advantages = torch.empty((T, R), dtype=torch.float32, device=self.device)
+        if value_targets is None:
+            value_targets = torch.empty((T, R), dtype=torch.float32, device=self.device)
+        for t, dt, n in ((rewards, torch.float32, T * R), (values, torch.float32, T * R), (dones, torch.uint8, T * self.n_envs),
+                         (last_values, torch.float32, R), (advantages, torch.float32, T * R), (value_targets, torch.float32, T * R)):
+            assert t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n, (t.dtype, tuple(t.shape))
+        _native.check(self._lib.ovc_gae(rewards.data_ptr(), values.data_ptr(), dones.data_ptr(), last_values.data_ptr(), T, R,
+                                        float(gamma), float(lam), advantages.data_ptr(), value_targets.data_ptr(), self._stream()))
+        return advantages, value_targets
 
     def feature_lut(self):
         if self._lut is None:

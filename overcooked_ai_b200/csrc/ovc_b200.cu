@@ -674,24 +674,51 @@ int ovc_encode_linear(const void *layouts, int n_layouts, const int32_t *state, 
 
 int ovc_sample_actions(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter,
                        int32_t *actions, void *stream) {
-    return ovc::sample_actions_impl(scores, ld, n_actions, n_rows, seed, (unsigned long long *)counter, actions, (cudaStream_t)stream);
+    return ovc::sample_actions_impl(scores, ld, n_actions, n_rows, seed, (unsigned long long *)counter, actions, nullptr, (cudaStream_t)stream);
+}
+
+int ovc_sample_actions_logp(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter,
+                            int32_t *actions, float *logp, void *stream) {
+    return ovc::sample_actions_impl(scores, ld, n_actions, n_rows, seed, (unsigned long long *)counter, actions, logp, (cudaStream_t)stream);
 }
 
 int ovc_accumulate_returns(const int32_t *sparse, const int32_t *shaped, float factor, int64_t n_envs, int64_t *ret_sparse,
                            float *ret_mixed, void *stream) {
-    return ovc::accumulate_returns_impl(sparse, shaped, factor, n_envs, (long long *)ret_sparse, ret_mixed, (cudaStream_t)stream);
+    return ovc::accumulate_returns_impl(sparse, shaped, factor, n_envs, (long long *)ret_sparse, ret_mixed, nullptr, nullptr, nullptr,
+                                        nullptr, (cudaStream_t)stream);
+}
+
+int ovc_record_transition(const int32_t *sparse, const int32_t *shaped, const int32_t *done, const float *factor, int64_t n_envs,
+                          float *rewards, uint8_t *dones, int64_t *ret_sparse, float *ret_mixed, void *stream) {
+    if (!factor) return ovc::fail(OVC_E_BADARG, "null pointer argument");
+    return ovc::accumulate_returns_impl(sparse, shaped, 0.f, n_envs, (long long *)ret_sparse, ret_mixed, factor, done, rewards, dones,
+                                        (cudaStream_t)stream);
+}
+
+int ovc_gae(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, int64_t n_steps, int64_t n_rows,
+            float gamma, float lambda, float *advantages, float *value_targets, void *stream) {
+    return ovc::gae_impl(rewards, values, dones, last_values, n_steps, n_rows, gamma, lambda, advantages, value_targets,
+                         (cudaStream_t)stream);
+}
+
+int ovc_policy_tail_logp(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                         const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                         float slope, int n_actions, uint64_t seed, uint64_t *counter, int32_t *actions, float *values, float *scores,
+                         float *logp, void *stream) {
+    ovc::PolicyTailArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
+    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
+    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
+    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream);
 }
 
 int ovc_policy_tail(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
                     const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                     float slope, int n_actions, uint64_t seed, uint64_t *counter, int32_t *actions, float *values, float *scores,
                     void *stream) {
-    ovc::PolicyTailArgs a;
-    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
-    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
-    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
-    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores;
-    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream);
+    return ovc_policy_tail_logp(x, n_rows, k0, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                n_actions, seed, counter, actions, values, scores, nullptr, stream);
 }
 
 int ovc_wide_layers(const void *a0, int64_t m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2, int n2,

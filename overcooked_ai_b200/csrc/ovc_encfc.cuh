@@ -329,9 +329,11 @@ namespace ovc {
 // (seed, step, row) alone.  counter[0] = the step; counter[1] = arrival count of the CTAs of the current launch: the
 // last CTA to finish advances the step (every CTA has read it by then), so a captured CUDA graph draws fresh numbers at
 // every replay without any host involvement.
+// LOGP: also logp[row] = scores[row][a] - (m + log(sum_i exp(scores[row][i] - m))), m = max_i scores[row][i], at the drawn a.
+template <bool LOGP>
 __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__restrict__ scores, int ld, int n_actions, long long n_rows,
                                                              unsigned long long seed, unsigned long long *counter,
-                                                             int32_t *__restrict__ actions) {
+                                                             int32_t *__restrict__ actions, float *__restrict__ logp) {
     const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(counter);
     const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (row < n_rows) {
@@ -349,6 +351,13 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__rest
             if (v > best_v) best_v = v, best = i;
         }
         actions[row] = best;
+        if constexpr (LOGP) {
+            float m = s[0];
+            for (int i = 1; i < n_actions; i++) m = fmaxf(m, s[i]);
+            float se = 0.f;
+            for (int i = 0; i < n_actions; i++) se += expf(s[i] - m);
+            logp[row] = s[best] - (m + logf(se));
+        }
     }
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -363,37 +372,106 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__rest
 }
 
 // ret_sparse[e] += sparse[e];  ret_mixed[e] += sparse[e] + factor * (shaped[e][0] + shaped[e][1])   (rllib.py:328-329)
+// ovc_record_transition adds what a sample batch keeps of the transition: rewards[2 e + i] = sparse[e] + f * shaped[e][i]
+// (rounded after the product, as a float32 restatement computes it) and dones[e]; f is read from factor_dev when given, so
+// a captured graph follows a factor the host changes between replays.
 __global__ void __launch_bounds__(256) accumulate_returns_kernel(const int32_t *__restrict__ sparse, const int32_t *__restrict__ shaped,
                                                                  float factor, long long n_envs, long long *__restrict__ ret_sparse,
-                                                                 float *__restrict__ ret_mixed) {
+                                                                 float *__restrict__ ret_mixed, const float *__restrict__ factor_dev,
+                                                                 const int32_t *__restrict__ done, float *__restrict__ rewards,
+                                                                 uint8_t *__restrict__ dones) {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n_envs) return;
+    const float f = factor_dev ? *factor_dev : factor;
     const int sp = sparse[e];
     const int2 sh = reinterpret_cast<const int2 *>(shaped)[e];
     if (ret_sparse) ret_sparse[e] += sp;
-    if (ret_mixed) ret_mixed[e] = ((ret_mixed[e] + (float)sp) + factor * (float)sh.x) + factor * (float)sh.y;
+    if (ret_mixed) ret_mixed[e] = ((ret_mixed[e] + (float)sp) + f * (float)sh.x) + f * (float)sh.y;
+    if (rewards)
+        reinterpret_cast<float2 *>(rewards)[e] = make_float2(__fadd_rn((float)sp, __fmul_rn(f, (float)sh.x)), __fadd_rn((float)sp, __fmul_rn(f, (float)sh.y)));
+    if (dones) dones[e] = done[e] != 0;
 }
 
 static int sample_actions_impl(const float *scores, int ld, int n_actions, long long n_rows, unsigned long long seed,
-                               unsigned long long *counter, int32_t *actions, cudaStream_t st) {
+                               unsigned long long *counter, int32_t *actions, float *logp, cudaStream_t st) {
     if (!scores || !counter || !actions) return fail(OVC_E_BADARG, "null pointer argument");
     if (n_actions < 1 || n_actions > 8 || ld < n_actions) return fail(OVC_E_BADARG, "n_actions must be 1..8 and <= ld", n_actions);
     if (n_rows < 0) return fail(OVC_E_BADARG, "negative row count");
     if (n_rows == 0) return OVC_OK;
-    sample_actions_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions);
+    const unsigned grid = (unsigned)((n_rows + 255) / 256);
+    if (logp) sample_actions_kernel<true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, logp);
+    else sample_actions_kernel<false><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, nullptr);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "sample_actions kernel launch");
     return OVC_OK;
 }
 
 static int accumulate_returns_impl(const int32_t *sparse, const int32_t *shaped, float factor, long long n_envs, long long *ret_sparse,
-                                   float *ret_mixed, cudaStream_t st) {
-    if (!sparse || !shaped) return fail(OVC_E_BADARG, "null pointer argument");
+                                   float *ret_mixed, const float *factor_dev, const int32_t *done, float *rewards, uint8_t *dones,
+                                   cudaStream_t st) {
+    if (!sparse || !shaped || (dones && !done)) return fail(OVC_E_BADARG, "null pointer argument");
     if (n_envs < 0) return fail(OVC_E_BADARG, "negative env count");
     if (n_envs == 0) return OVC_OK;
-    accumulate_returns_kernel<<<(unsigned)((n_envs + 255) / 256), 256, 0, st>>>(sparse, shaped, factor, n_envs, ret_sparse, ret_mixed);
+    accumulate_returns_kernel<<<(unsigned)((n_envs + 255) / 256), 256, 0, st>>>(sparse, shaped, factor, n_envs, ret_sparse, ret_mixed,
+                                                                                  factor_dev, done, rewards, dones);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "accumulate_returns kernel launch");
+    return OVC_OK;
+}
+
+// Generalized advantage estimation over a window of T transitions (the postprocessing of RLlib's PPO sample batches),
+// one thread per environment holding its two agent rows, walking t backwards.  Every operation is rounded on its own
+// (no FMA contraction) in the order ovc_gae documents, so a float32 loop on the host reproduces it bit for bit.  A
+// thread's chain is serial in t, so GAE_UNROLL timesteps of loads are issued before they are consumed: with one thread
+// per environment there are too few threads per SM to cover the memory latency otherwise.
+constexpr int GAE_THREADS = 128;
+constexpr int GAE_UNROLL = 16;
+
+__global__ void __launch_bounds__(GAE_THREADS) gae_kernel(const float2 *__restrict__ rewards, const float2 *__restrict__ values,
+                                                          const uint8_t *__restrict__ dones, const float2 *__restrict__ last_values,
+                                                          long long T, long long n_envs, float gamma, float lambda,
+                                                          float2 *__restrict__ adv, float2 *__restrict__ targets) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_envs) return;
+    const float gl = __fmul_rn(gamma, lambda);
+    float2 a = make_float2(0.f, 0.f), nv = last_values[e];
+    for (long long t0 = T - 1; t0 >= 0; t0 -= GAE_UNROLL) {
+        float2 r[GAE_UNROLL], v[GAE_UNROLL];
+        float nt[GAE_UNROLL];
+#pragma unroll
+        for (int k = 0; k < GAE_UNROLL; k++)
+            if (t0 - k >= 0) {
+                const long long i = (t0 - k) * n_envs + e;
+                r[k] = __ldcs(rewards + i), v[k] = __ldcs(values + i), nt[k] = dones[i] ? 0.f : 1.f;
+            }
+#pragma unroll
+        for (int k = 0; k < GAE_UNROLL; k++)
+            if (t0 - k >= 0) {
+                const long long i = (t0 - k) * n_envs + e;
+                const float dx = __fsub_rn(__fadd_rn(r[k].x, __fmul_rn(__fmul_rn(gamma, nv.x), nt[k])), v[k].x);
+                const float dy = __fsub_rn(__fadd_rn(r[k].y, __fmul_rn(__fmul_rn(gamma, nv.y), nt[k])), v[k].y);
+                a.x = __fadd_rn(dx, __fmul_rn(__fmul_rn(gl, nt[k]), a.x));
+                a.y = __fadd_rn(dy, __fmul_rn(__fmul_rn(gl, nt[k]), a.y));
+                __stcs(adv + i, a);
+                __stcs(targets + i, make_float2(__fadd_rn(a.x, v[k].x), __fadd_rn(a.y, v[k].y)));
+                nv = v[k];
+            }
+    }
+}
+
+static int gae_impl(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, long long T,
+                    long long n_rows, float gamma, float lambda, float *adv, float *targets, cudaStream_t st) {
+    if (!rewards || !values || !dones || !last_values || !adv || !targets) return fail(OVC_E_BADARG, "null pointer argument");
+    if (T < 0 || n_rows < 0 || n_rows % 2) return fail(OVC_E_BADARG, "T must be >= 0 and n_rows even and >= 0");
+    if (((uintptr_t)rewards | (uintptr_t)values | (uintptr_t)last_values | (uintptr_t)adv | (uintptr_t)targets) & 7)
+        return fail(OVC_E_BADARG, "float buffers must be 8-byte aligned");
+    const long long n_envs = n_rows / 2;
+    if (T == 0 || n_envs == 0) return OVC_OK;
+    gae_kernel<<<(unsigned)((n_envs + GAE_THREADS - 1) / GAE_THREADS), GAE_THREADS, 0, st>>>(
+        (const float2 *)rewards, (const float2 *)values, dones, (const float2 *)last_values, T, n_envs, gamma, lambda, (float2 *)adv,
+        (float2 *)targets);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "gae kernel launch");
     return OVC_OK;
 }
 

@@ -41,6 +41,7 @@ struct PolicyTailArgs {
     int32_t *actions;              // [n_rows]
     float *values;                 // [n_rows] or null
     float *scores;                 // [n_rows][8] or null
+    float *logp;                   // [n_rows] or null: log-probability of the drawn action (policy_tail_kernel<KS2, true>)
 };
 
 __device__ __forceinline__ void mma_bf16_16816(float c[4], const unsigned a[4], unsigned b0, unsigned b1) {
@@ -89,7 +90,7 @@ __device__ __forceinline__ void to_fragments(unsigned a[4][4], const float acc[8
     }
 }
 
-template <int KS2>  // K0 = 32 * KS2
+template <int KS2, bool LOGP>  // K0 = 32 * KS2; LOGP: also write p.logp (a separate instantiation, so the plain draw is untouched)
 __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const PolicyTailArgs p) {
     constexpr int K0 = 32 * KS2;
     constexpr int FS = K0 % 64 == 32 ? K0 : K0 + 32;  // row stride of the first layer's weights: 32 mod 64 elements, LDS.128 conflict free
@@ -187,8 +188,22 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const Policy
                 const int ob = __shfl_xor_sync(0xFFFFFFFFu, best, d);
                 if (ov > v0 || (ov == v0 && ob < best)) v0 = ov, best = ob;
             }
+            float lp = 0.f;
+            if constexpr (LOGP) {  // log-softmax at the drawn action over the same four lanes: max, then the sum of exp
+                const bool in0 = 2 * t < p.n_actions, in1 = 2 * t + 1 < p.n_actions;
+                float m = fmaxf(in0 ? s0 : -INFINITY, in1 ? s1 : -INFINITY);
+#pragma unroll
+                for (int d = 1; d <= 2; d <<= 1) m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, d));
+                float se = (in0 ? expf(s0 - m) : 0.f) + (in1 ? expf(s1 - m) : 0.f);
+#pragma unroll
+                for (int d = 1; d <= 2; d <<= 1) se += __shfl_xor_sync(0xFFFFFFFFu, se, d);
+                const int src = (lane & ~3) | (best >> 1);  // the lane holding head `best`
+                const float b0 = __shfl_sync(0xFFFFFFFFu, s0, src), b1 = __shfl_sync(0xFFFFFFFFu, s1, src);
+                lp = ((best & 1) ? b1 : b0) - (m + logf(se));
+            }
             if (row < p.n_rows) {
                 if (t == 0) p.actions[row] = best;
+                if constexpr (LOGP) if (t == 0) p.logp[row] = lp;
                 // the value head is head n_actions: lane n_actions / 2 holds it
                 if (p.values && t == (p.n_actions >> 1)) p.values[row] = (p.n_actions & 1) ? s1 : s0;
             }
@@ -226,8 +241,13 @@ static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st) {
     cudaError_t e = cudaSuccess;
 #define OVC_LAUNCH_PT(KS2)                                                                                              \
     case KS2:                                                                                                           \
-        e = cudaFuncSetAttribute(policy_tail_kernel<KS2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);      \
-        if (e == cudaSuccess) policy_tail_kernel<KS2><<<grid, PT_THREADS, smem, st>>>(a);                               \
+        if (a.logp) {                                                                                                   \
+            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            if (e == cudaSuccess) policy_tail_kernel<KS2, true><<<grid, PT_THREADS, smem, st>>>(a);                    \
+        } else {                                                                                                        \
+            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            if (e == cudaSuccess) policy_tail_kernel<KS2, false><<<grid, PT_THREADS, smem, st>>>(a);                   \
+        }                                                                                                               \
         break;
     switch (k0 / 32) {
         OVC_LAUNCH_PT(1) OVC_LAUNCH_PT(2) OVC_LAUNCH_PT(3) OVC_LAUNCH_PT(4) OVC_LAUNCH_PT(5) OVC_LAUNCH_PT(6) OVC_LAUNCH_PT(7) OVC_LAUNCH_PT(8)

@@ -193,6 +193,40 @@ def sample_categorical(logits, noise):
     return torch.argmax(logits, dim=-1)
 
 
+class SampleBatch(object):
+    """One window of T self-play transitions as a PPO learner consumes it (RLlib's per-agent ``SampleBatch``), on the device.
+    Agent rows are ``2 env + agent``, so ``actions[t].view(N, 2)`` is the joint action ``ovc_step`` took.
+
+    states        int32 [T, N, S]    the records the actions were drawn from (observations are re-encoded on demand)
+    actions       int32 [T, 2N]
+    logp          float32 [T, 2N]    log-probability of each action under the behaviour policy
+    values        float32 [T, 2N]    value head on states[t]
+    rewards       float32 [T, 2N]    sparse + reward_shaping_factor * shaped_i (rllib.py:328-329)
+    dones         uint8 [T, N]       the episode ended with transition t (the environment auto-reset)
+    last_values   float32 [2N]       value head on the state after the window (bootstrap)
+    advantages, value_targets  float32 [T, 2N]   GAE (ovc_gae)
+    logits        float32 [T, 2N, 8] the policy's heads (columns 0..5 the logits), only with ``keep_logits``
+    """
+
+    def __init__(self, env, n_steps, keep_logits=False):
+        N, T, dev = env.n_envs, int(n_steps), env.device
+        z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
+        self.env = env
+        self.states = z((T, N, env.state_words), torch.int32)
+        self.actions = z((T, 2 * N), torch.int32)
+        self.logp, self.values, self.rewards, self.advantages, self.value_targets = (z((T, 2 * N), torch.float32) for _ in range(5))
+        self.dones = z((T, N), torch.uint8)
+        self.last_values = z(2 * N, torch.float32)
+        self.logits = z((T, 2 * N, 8), torch.float32) if keep_logits else None
+
+    def observations(self, env_steps, dtype=torch.float32):
+        """lossless_state_encoding ``[M, 2, W, H, 26]`` of the env-steps ``env_steps`` (CUDA int64 [M], flat indices
+        ``t * N + env``), both agents' views in [env][agent] order: rows ``2 m + i`` of the flattened per-agent tensors
+        (``actions.view(-1, 2)[env_steps]`` etc.) belong to view ``i`` of entry ``m``.  Encoded from the stored records by K2."""
+        recs = self.states.view(-1, self.states.shape[-1]).index_select(0, env_steps)
+        return self.env.lossless_state_encoding(dtype=dtype, states=recs)
+
+
 class SelfPlayRollout(object):
     """Policy-in-the-loop rollout: both agents of every environment act from the same network."""
 
@@ -236,6 +270,7 @@ class SelfPlayRollout(object):
             "K7 feeds the dense bf16 policy (first layer width a multiple of 64, table within shared memory)"
         self.fused_first_layer = bool(fused_first_layer)
         self.factor = float(reward_shaping_factor)
+        self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by collect()'s graph
         N = env.n_envs
         if obs_dtype is None:
             obs_dtype = torch.bfloat16 if autocast_dtype == torch.bfloat16 else torch.float32
@@ -274,18 +309,40 @@ class SelfPlayRollout(object):
         assert (2 * N) % self.sub_batches == 0
         self.graph = None
         self.use_graph = use_graph
+        self._collect_graphs = {}  # (n_steps, keep_logits) -> ((gamma, lam), CUDA graph of the window)
+        self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
+        self._boot_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # the bootstrap's draws leave _draw_counter alone
+        self._boot_actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
 
-    def _policy(self):
-        """(scores float32 [2N, 6] = logits, values written to self.values) for the observations in self.obs."""
+    @property
+    def reward_shaping_factor(self):
+        """The factor of the shaped rewards (rllib.py:328-329).  Setting it takes effect in collect() without a re-capture
+        (its graph reads a device scalar); run() re-captures its graph on its next call."""
+        return self.factor
+
+    @reward_shaping_factor.setter
+    def reward_shaping_factor(self, value):
+        if float(value) != self.factor:
+            self.graph = None
+        self.factor = float(value)
+        self._factor.fill_(self.factor)
+
+    def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None):
+        """(scores float32 [2N, 6] = logits, values written to ``values``) for the observations in self.obs, or None when
+        K8 has also drawn the actions (into ``actions``, with ``logp`` when given).  The outputs default to self.actions,
+        self.values, self._scores8 and self._draw_counter."""
         env = self.env
         rows = 2 * env.n_envs
+        actions = self.actions if actions is None else actions
+        vals = self.values.view(rows) if values is None else values
+        scores8 = self._scores8 if scores8 is None else scores8
+        counter = self._draw_counter if counter is None else counter
         with torch.no_grad():
             if self.dense_model is not None:
                 if self.fused_first_layer:
                     flat, first = env.encoded_linear(self._wt0, self._b0, out=self._act0, neg_slope=0.2), 1  # K7
                 else:
                     flat, first = self.obs.view(rows, self.W * self.H * 26), 0
-                vals = self.values.view(rows)
                 step = rows // self.sub_batches
                 if self.fused_tail:  # K8 draws the actions itself: nothing to return
                     if self.fused_wide:
@@ -296,11 +353,13 @@ class SelfPlayRollout(object):
                         for b in range(0, rows, step):
                             self.dense_model.trunk(flat[b:b + step], first, out=self._z[b:b + step])
                     w1, b1, wh, bh, wo, bo = self._tail
-                    _native.check(_native.lib().ovc_policy_tail(
-                        self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
-                        wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1),
-                        self._draw_counter.data_ptr(), self.actions.data_ptr(), vals.data_ptr(),
-                        self._scores8.data_ptr() if self._scores8 is not None else 0, env._stream()))
+                    args = (self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
+                            wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1),
+                            counter.data_ptr(), actions.data_ptr(), vals.data_ptr(), scores8.data_ptr() if scores8 is not None else 0)
+                    if logp is None:
+                        _native.check(_native.lib().ovc_policy_tail(*args, env._stream()))
+                    else:
+                        _native.check(_native.lib().ovc_policy_tail_logp(*args, logp.data_ptr(), env._stream()))
                     return None
                 for b in range(0, rows, step):
                     logits, value = self.dense_model.forward_from(flat[b:b + step], first)
@@ -311,7 +370,7 @@ class SelfPlayRollout(object):
                     x = self.obs.view(rows, self.W, self.H, 26).permute(0, 3, 1, 2)  # (2N,26,W,H), channels-last strides
                     logits, value = self.model(x)
                 self._scores.copy_(logits)
-                self.values.view(rows).copy_(value)
+                vals.copy_(value)
         return self._scores
 
     def _transition(self):
@@ -351,6 +410,80 @@ class SelfPlayRollout(object):
             else:
                 self._transition()
         return n_steps * self.env.n_envs
+
+    def _collect_window(self, b, n_steps, gamma, lam):
+        """n_steps transitions into slots 0.. of ``b`` (the kernels of run(), outputs in place), then the bootstrap value
+        of the state after them and GAE over the whole batch."""
+        env = self.env
+        for t in range(n_steps):
+            b.states[t].copy_(env.state)
+            if not self.fused_first_layer:
+                env.lossless_state_encoding(out=self.obs)  # K2
+            scores = self._policy(actions=b.actions[t], values=b.values[t], logp=b.logp[t], scores8=None if b.logits is None else b.logits[t])
+            if scores is not None:  # library layers: the separate draw kernel
+                env.sample_actions(scores, self._draw_counter, seed=self.seed, out=b.actions[t], logp_out=b.logp[t])
+                if b.logits is not None:
+                    b.logits[t, :, :scores.shape[1]].copy_(scores)
+            env.step(b.actions[t].view(env.n_envs, 2))  # K1 (auto-reset inside)
+            env.record_transition(self._factor, rewards=b.rewards[t], dones=b.dones[t], ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed)
+        if not self.fused_first_layer:
+            env.lossless_state_encoding(out=self.obs)
+        self._policy(actions=self._boot_actions, values=b.last_values, counter=self._boot_counter)
+        env.gae(b.rewards, b.values, b.dones, b.last_values, gamma, lam, b.advantages, b.value_targets)
+
+    def collect(self, n_steps, gamma, lam, keep_logits=False):
+        """Advance every environment n_steps transitions, as run() does (the same kernels and the same draws from the same
+        seed and counter), and return them as a ``SampleBatch`` with GAE(gamma, lam) advantages.  The batch's tensors are
+        reused: the next collect() with the same n_steps / keep_logits overwrites them.  With use_graph the whole window
+        is one CUDA graph (captured once per n_steps / keep_logits; a new gamma or lam re-captures it); no host
+        synchronisation otherwise."""
+        assert self.native_glue, "collect() runs on the native draw / reward kernels (native_glue=True)"
+        assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
+        key = (int(n_steps), bool(keep_logits))
+        b = self._batches.get(key)
+        if b is None:
+            b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits)
+        if not self.use_graph:
+            self._collect_window(b, n_steps, gamma, lam)
+            return b
+        g = self._collect_graphs.get(key)
+        if g is None or g[0] != (gamma, lam):
+            # warm-up + capture must not advance the environments: snapshot, then restore
+            saved = (self.env.state.clone(), self.ret_sparse.clone(), self.ret_mixed.clone(), self._draw_counter.clone())
+            s = torch.cuda.Stream(self.env.device)
+            s.wait_stream(torch.cuda.current_stream(self.env.device))
+            with torch.cuda.stream(s):
+                self._collect_window(b, 1, gamma, lam)
+            torch.cuda.current_stream(self.env.device).wait_stream(s)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                self._collect_window(b, n_steps, gamma, lam)
+            self.env.state.copy_(saved[0]), self.ret_sparse.copy_(saved[1]), self.ret_mixed.copy_(saved[2]), self._draw_counter.copy_(saved[3])
+            g = self._collect_graphs[key] = ((gamma, lam), graph)
+        g[1].replay()
+        return b
+
+    def sync_weights(self):
+        """Re-fold ``self.model`` (e.g. after a learner's update) into the policy the kernels evaluate, in place: the dense
+        model's parameters and the K7 / K9 / K8 tables keep their storage, so the captured graphs of run() and collect()
+        use the new weights without a re-capture."""
+        if self.dense_model is None:
+            return  # the convolutions read self.model's own parameters
+        with torch.no_grad():
+            new = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(self.env.device)
+            if self.autocast_dtype is not None:
+                new = new.to(self.autocast_dtype)
+            for dst, src in zip(self.dense_model.parameters(), new.parameters()):
+                dst.copy_(src)
+            pairs = []
+            if self.fused_first_layer:
+                pairs += zip((self._wt0, self._b0), self.dense_model.first_layer_table())
+            if self.fused_wide:
+                pairs += zip(self._wide, self.dense_model.wide_tables())
+            if self.fused_tail:
+                pairs += zip(self._tail, self.dense_model.tail_tables())
+            for dst, src in pairs:
+                dst.copy_(src)
 
     def env_only(self, n_steps):
         """The same transitions without the policy: encode + step with the last sampled actions

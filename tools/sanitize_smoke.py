@@ -2,7 +2,8 @@
 """Every kernel family at smoke sizes, for compute-sanitizer (memcheck / racecheck / synccheck / initcheck):
 K1 with each record-I/O strategy (2-D TMA tile, 1-D bulk TMA, direct), K5 (the rollout kernel, int32 and
 host-transfer formats, standard and random-start auto-resets, 16- / 32- / 64-word records, a partial last tile),
-the round-1 fused path, K4 reset (copy + random), K2, K3, K6 and the host-buffer pipeline.  Results are checked
+the round-1 fused path, K4 reset (copy + random), K2, K3, K6, the host-buffer pipeline, the policy kernels K7 / K8 and
+the sample-batch kernels (logp draws, ovc_record_transition, ovc_gae through SelfPlayRollout.collect).  Results are checked
 against the CPU oracle on the way, so a run under the sanitizer is also a parity run.
 
     compute-sanitizer --tool racecheck python tools/sanitize_smoke.py
@@ -127,4 +128,24 @@ sp2 = SelfPlayRollout(env, model=sp.model, use_graph=False, fused_tail=False)
 sp2.run(3)
 torch.cuda.synchronize()
 print("K7, K8, sample / accumulate kernels, self-play transitions ok", flush=True)
+# sample batches: K8 and the draw kernel with logp, ovc_record_transition and ovc_gae, through collect()
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
+from ppo_reference import gae_f32, log_softmax_at  # noqa: E402
+
+for r in (sp, sp2):
+    r.reward_shaping_factor = 0.5
+    ref_state = env.state.cpu().numpy().copy()
+    b = r.collect(12, 0.99, 0.95, keep_logits=True)
+    st, ac, rw, dn = (x.cpu().numpy() for x in (b.states, b.actions, b.rewards, b.dones))
+    for t in range(12):
+        assert np.array_equal(st[t], ref_state)
+        sp_, sh_, d_, _ = cpu.step(env._tab_host, env._starts_host, ref_state, ac[t].reshape(n, 2), horizon=40, flags=1)
+        assert np.array_equal(rw[t].reshape(n, 2), sp_[:, None].astype(np.float32) + np.float32(0.5) * sh_.astype(np.float32))
+        assert np.array_equal(dn[t], (d_ != 0).astype(np.uint8))
+        lp = log_softmax_at(b.logits[t].cpu().numpy(), ac[t], 6)
+        assert (np.abs(b.logp[t].cpu().numpy() - lp) <= 1e-5 * (1 + np.abs(lp))).all()
+    adv, tgt = gae_f32(rw, b.values.cpu().numpy(), dn, b.last_values.cpu().numpy(), 0.99, 0.95)
+    assert np.array_equal(b.advantages.cpu().numpy(), adv) and np.array_equal(b.value_targets.cpu().numpy(), tgt)
+torch.cuda.synchronize()
+print("K8 / draw with logp, record_transition, GAE through collect() ok", flush=True)
 print("sanitize_smoke: all ok")
