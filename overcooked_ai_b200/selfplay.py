@@ -73,15 +73,34 @@ class RllibShapedCNN(nn.Module):
         return self.logits(x), self.value(x).squeeze(-1)
 
 
+def _conv_matrix(conv, c, w, h):
+    """(matrix [n_out, n_in], (c_out, w', h')) of a convolution over a (c, x = w, y = h) image, inputs and outputs flat in
+    [x][y][channel] order.  Each tap's weights are placed by index, with no arithmetic, so the matrix holds the convolution's
+    own weights on any device (a convolution of the identity would be rounded to TF32 by cuDNN's default on the GPU)."""
+    k = conv.weight.detach()
+    co, ci, kx, ky = k.shape
+    px, py = conv.padding
+    assert ci == c and conv.stride == (1, 1) and conv.dilation == (1, 1)
+    wo, ho = w + 2 * px - kx + 1, h + 2 * py - ky + 1
+    m = k.new_zeros((w, h, c, wo, ho, co))
+    for dx in range(kx):
+        for dy in range(ky):
+            # out[xo][yo][o] += k[o, :, dx, dy] . in[xo + dx - px][yo + dy - py][:]   (torch's conv2d is a cross-correlation)
+            xo = torch.arange(max(0, px - dx), min(wo, w + px - dx), device=k.device)
+            yo = torch.arange(max(0, py - dy), min(ho, h + py - dy), device=k.device)
+            m[(xo + dx - px)[:, None], (yo + dy - py)[None, :], :, xo[:, None], yo[None, :], :] = k[:, :, dx, dy].t()
+    return m.reshape(w * h * c, wo * ho * co).t().contiguous(), (co, wo, ho)
+
+
 class DenseGridPolicy(nn.Module):
     """The same network as ``RllibShapedCNN`` with every convolution folded into ONE matrix per layer.
 
     On a 5x4 (or 9x5) grid a 'same' convolution spends most of its taps on padding: conv 5x5x26->25 over 20 cells is
     325 k MACs per observation, while the linear map it IS — 520 inputs -> 500 outputs — is 260 k.  cuDNN also runs
     25/26-channel convolutions far below the tensor-core peak, whereas ``[2N, 520] x [520, 500]`` is a plain library
-    GEMM.  The matrices are built once by pushing the identity through each convolution (exact: same weights, same
-    function, only the summation order differs), in the observation kernel's own element order ``[x][y][channel]``, so
-    K2's output is consumed as ``[2N, W*H*26]`` without any permute.
+    GEMM.  The matrices are built once by placing each convolution's weights at the positions of its taps (exact on any
+    device: the same weights, the same function, only the summation order differs), in the observation kernel's own
+    element order ``[x][y][channel]``, so K2's output is consumed as ``[2N, W*H*26]`` without any permute.
 
     ``pad_to``: every layer's width is rounded up to a multiple of it with zero weights and zero biases (leaky ReLU of 0
     is 0, the next layer's extra input columns are zero too: the function is unchanged).  Widths of 500 / 150 bf16
@@ -97,15 +116,9 @@ class DenseGridPolicy(nn.Module):
             mats = []
             shape = (26, width, height)  # (channels, x, y) as the conv sees it
             for conv in (cnn.conv_initial, cnn.conv_0, cnn.conv_1):
-                c, w, h = shape
-                n_in = c * w * h
-                # basis vector k of the flat [x][y][c] input -> NCHW image with a single one
-                eye = torch.eye(n_in, dtype=conv.weight.dtype, device=conv.weight.device).view(n_in, w, h, c).permute(0, 3, 1, 2)
-                out = F.conv2d(eye, conv.weight, None, padding=conv.padding)  # (n_in, c_out, w', h'), bias added separately
-                co, wo, ho = out.shape[1:]
-                mats.append((out.permute(0, 2, 3, 1).reshape(n_in, wo * ho * co).t().contiguous(),   # [n_out, n_in], [x][y][c] order
-                             conv.bias.view(1, 1, co).expand(wo, ho, co).reshape(-1).clone()))
-                shape = (co, wo, ho)
+                m, shape = _conv_matrix(conv, *shape)
+                co, wo, ho = shape
+                mats.append((m, conv.bias.view(1, 1, co).expand(wo, ho, co).reshape(-1).clone()))
             # the first dense layer consumed conv_1's NCHW flatten (c, x, y): re-order its inputs to [x][y][c]
             co, wo, ho = shape
             first = cnn.dense[0]

@@ -10,6 +10,7 @@ from oracle import cpu
 from overcooked_ai_b200 import _native
 from overcooked_ai_b200 import layout as L
 from overcooked_ai_b200.batched import BatchedOvercookedEnv, EpisodeStats, HostRolloutPipeline
+from policy_reference import check_draw, gumbel_scores
 
 pytestmark = pytest.mark.gpu
 
@@ -427,7 +428,7 @@ def test_selfplay_fused_first_layer_equals_unfused_policy():
     assert np.abs(s8[:, :6] - b).max() < 0.02 and np.abs(s8[:, 6] - _np(plain.values).reshape(-1)).max() < 0.02
     assert np.array_equal(s8[:, 6], _np(tail.values).reshape(-1)) and _np(tail._draw_counter).tolist() == [1, 0]
     assert _np(lib_trunk._draw_counter).tolist() == [1, 0]
-    _check_draw(_np(tail.actions).reshape(-1), s8, 11, 0)
+    check_draw(_np(tail.actions).reshape(-1), s8, 11, 0)
     ref_state = _np(env.state).copy()
     for t in range(20):
         fused.run(1)
@@ -435,18 +436,6 @@ def test_selfplay_fused_first_layer_equals_unfused_policy():
         assert np.array_equal(_np(env.state), ref_state), t
     g = SelfPlayRollout(env, model=fused.model, use_graph=True)
     assert g.run(12) == 12 * n
-
-
-def _philox4x32_10(key, c):
-    """numpy restatement of Philox4x32-10 (Salmon et al.): key uint64, c uint32[n, 4] -> uint32[n, 4]."""
-    c = [c[:, i].astype(np.uint64) for i in range(4)]
-    k0, k1 = np.uint64(key & 0xFFFFFFFF), np.uint64(key >> 32)
-    M = np.uint64(0xFFFFFFFF)
-    for _ in range(10):
-        p0, p1 = np.uint64(0xD2511F53) * c[0], np.uint64(0xCD9E8D57) * c[2]
-        c = [(p1 >> np.uint64(32)) ^ c[1] ^ k0, p1 & M, (p0 >> np.uint64(32)) ^ c[3] ^ k1, p0 & M]
-        k0, k1 = (k0 + np.uint64(0x9E3779B9)) & M, (k1 + np.uint64(0xBB67AE85)) & M
-    return np.stack(c, 1).astype(np.uint32)
 
 
 def test_sample_actions_kernel_matches_its_definition_and_softmax():
@@ -463,10 +452,7 @@ def test_sample_actions_kernel_matches_its_definition_and_softmax():
     for step in range(3):
         a = _np(env.sample_actions(scores, counter, seed=seed)).reshape(-1)
         assert _np(counter).tolist() == [step + 1, 0]
-        ctr = np.stack([rows & np.uint64(0xFFFFFFFF), rows >> np.uint64(32), np.full_like(rows, step), np.zeros_like(rows)], 1).astype(np.uint32)
-        d = np.concatenate([_philox4x32_10(seed, ctr), _philox4x32_10(seed, ctr | np.array([0, 0, 0, 1], np.uint32))], 1)[:, :6]
-        u = ((d >> np.uint32(9)).astype(np.float32) + np.float32(0.5)) * np.float32(2.0 ** -23)
-        v = _np(scores)[:, :6] - np.log(-np.log(u))
+        v = gumbel_scores(_np(scores), seed, step)
         want = v.argmax(1)
         top2 = np.sort(v, 1)[:, -2:]
         clear = top2[:, 1] - top2[:, 0] > 1e-4  # libm and the device logf differ in the last bits: near-ties may flip
@@ -501,19 +487,6 @@ def test_selfplay_other_grids_fall_back_to_library_layers(layout, flags):
         cpu.step(env._tab_host, env._starts_host, ref_state, a, horizon=25, flags=1)
         assert np.array_equal(_np(env.state), ref_state), t
     assert len(np.unique(_np(sp.actions))) > 3
-
-
-def _check_draw(actions, scores, seed, step, n_actions=6):
-    """actions == the ovc_sample_actions definition applied to ``scores`` (numpy restatement; near-ties exempt)."""
-    rows = np.arange(len(scores), dtype=np.uint64)
-    ctr = np.stack([rows & np.uint64(0xFFFFFFFF), rows >> np.uint64(32), np.full_like(rows, step), np.zeros_like(rows)], 1).astype(np.uint32)
-    d = np.concatenate([_philox4x32_10(seed, ctr), _philox4x32_10(seed, ctr | np.array([0, 0, 0, 1], np.uint32))], 1)[:, :n_actions]
-    u = ((d >> np.uint32(9)).astype(np.float32) + np.float32(0.5)) * np.float32(2.0 ** -23)
-    v = scores[:, :n_actions] - np.log(-np.log(u))
-    top2 = np.sort(v, 1)[:, -2:]
-    clear = top2[:, 1] - top2[:, 0] > 1e-4  # libm and the device logf differ in the last bits: near-ties may flip
-    assert clear.mean() > 0.995 and np.array_equal(actions[clear], v.argmax(1)[clear])
-    assert actions.min() >= 0 and actions.max() < n_actions
 
 
 def _bf16(x):
@@ -551,7 +524,7 @@ def test_k8_policy_tail_vs_float_reference(k0, n_hidden, n_rows):
         assert np.abs(got - want).max() < 0.03 * max(1.0, np.abs(want).max()), np.abs(got - want).max()
         assert np.array_equal(_np(values), got[:, 6]) and _np(counter).tolist() == [step + 1, 0]
         if n_rows >= 1000:
-            _check_draw(_np(actions), got, 99, step)
+            check_draw(_np(actions), got, 99, step)
         else:
             assert _np(actions).min() >= 0 and _np(actions).max() <= 5
     rc = lib.ovc_policy_tail(tx.data_ptr(), n_rows, 100, 0.2, tw1.data_ptr(), tb1.data_ptr(), twh.data_ptr(), tbh.data_ptr(), n_hidden,
