@@ -497,6 +497,37 @@ int ovc_wide_layers(const void *a0, int64_t m, int k0, const void *w1, const flo
                     int n2, float slope, void *z2, void *stream);
 
 /*
+ * A behaviour-cloned partner on the device (PPO_BC: human_aware_rl's OvercookedMultiAgent pairs the PPO agent with a fixed
+ * BC agent in a seat drawn at every reset; the BC model, imitation/behavior_cloning_tf2.py, is featurize_state -> Dense 64
+ * ReLU -> Dense 64 ReLU -> logits, its action sampled from the softmax).
+ *
+ * ovc_partner_policy (K10): for every environment e with partner_seat[e] in {0, 1} (int32 [n_envs]; -1 = self-play, nothing
+ *   written), the BC policy on player seat's featurize_state view (as ovc_featurize computes it at num_pots = 2: 96 features,
+ *   never materialised) and a draw from it:
+ *     a = bf16(x)                                          x = the 96 features, exact in bfloat16 while |value| <= 256 (every
+ *                                                          shipped layout; cook times above 256 round)
+ *     a = bf16(relu(a . w_first^T + b_first))              w_first bfloat16 [64][96], biases float32
+ *     a = bf16(relu(a . w_hidden[l]^T + b_hidden[l]))      l < n_hidden (0..8), w_hidden bfloat16 [n_hidden][64][64]
+ *     s = a . w_heads^T + b_heads                          w_heads bfloat16 [8][64]: heads 0..n_actions-1 (<= 7) the logits
+ *     actions[2 e + seat] ~ softmax(s[0..n_actions))       the ovc_sample_actions draw on row r = 2 e + seat with this call's
+ *                                                          own seed and counter (uint64[2], same semantics)
+ *   float32 accumulation (K8's mma.sync chain).  `actions` is the int32 [n_envs][2] joint action ovc_step takes: the
+ *   partner's entry is overwritten, the other one is left alone.  scores (nullable) float32 [n_envs][8] = s of partnered
+ *   environments.  n_features must be 96 and width 64 (OVC_E_UNSUPPORTED otherwise); weights 16-byte aligned.
+ * ovc_assign_partners: partner_seat[e] for every e with done[e] != 0 (ovc_step's int32 done; NULL = every environment):
+ *   Philox4x32-10, key = seed, counter = (e low, e high, step low, step high) -> words w0, w1;
+ *   partner_seat[e] = w0 < thr ? w1 >> 31 : -1,  thr = floor(bc_factor * 2^32), saturated: bc_factor >= 1 always pairs,
+ *   bc_factor <= 0 never.  bc_factor is one float32 in DEVICE memory (a captured graph follows an annealed value); counter
+ *   uint64[2] as ovc_sample_actions' (one step per launch).
+ */
+int ovc_partner_policy(const void *layouts, int n_layouts, const void *lut, const int32_t *state, const int32_t *partner_seat,
+                       int64_t n_envs, int state_words, int n_features, int width, const void *w_first, const float *b_first,
+                       const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads, int n_actions,
+                       uint64_t seed, uint64_t *counter, int32_t *actions, float *scores, void *stream);
+int ovc_assign_partners(const int32_t *done, const float *bc_factor, int64_t n_envs, uint64_t seed, uint64_t *counter, int32_t *partner_seat,
+                        void *stream);
+
+/*
  * featurize_state (:2579-2898) with the default planner parameters (NO_COUNTERS_PARAMS,
  * planners.py:27-34): out float32[n_envs][2][F],
  * F = 2*(num_pots*10+28), lut = ovc_feat_lut_entry_t[n_layouts][256][4].  view_swap as above.

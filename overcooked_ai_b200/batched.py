@@ -476,6 +476,45 @@ class BatchedOvercookedEnv(object):
                                         float(gamma), float(lam), advantages.data_ptr(), value_targets.data_ptr(), self._stream()))
         return advantages, value_targets
 
+    def partner_actions(self, tables, partner_seat, counter, seed=0, n_actions=6, out=None, scores=None):
+        """The behaviour-cloned partner's actions (ovc_partner_policy, K10: featurize_state of the partner's view -> the BC
+        MLP -> the ovc_sample_actions draw, one kernel, the features never materialised).  ``tables``: the six tensors of
+        ``selfplay.BCPolicy.tables()``; ``partner_seat`` int32 [N] (-1: no partner, 0 / 1: the partner's player index);
+        ``counter`` int64 CUDA tensor of 2 zeros that the kernel advances.  Writes ``out[e, seat]`` (int32 [N, 2], e.g. the
+        joint action the PPO policy drew) for partnered environments only, and their heads into ``scores`` (float32 [N, 8])
+        when given.  Returns ``out``."""
+        w1, b1, wh, bh, wo, bo = tables
+        for t, dt in ((w1, torch.bfloat16), (b1, torch.float32), (wh, torch.bfloat16), (bh, torch.float32), (wo, torch.bfloat16), (bo, torch.float32)):
+            assert t.is_cuda and t.dtype == dt and t.is_contiguous(), "partner tables: bf16 weights, float32 biases, contiguous CUDA tensors"
+        assert partner_seat.is_cuda and partner_seat.dtype == torch.int32 and partner_seat.is_contiguous() and partner_seat.numel() == self.n_envs
+        assert counter.is_cuda and counter.dtype == torch.int64 and counter.numel() == 2 and counter.is_contiguous()
+        if out is None:
+            out = torch.zeros((self.n_envs, 2), dtype=torch.int32, device=self.device)
+        assert out.is_cuda and out.dtype == torch.int32 and out.is_contiguous() and out.numel() == 2 * self.n_envs
+        if scores is not None:
+            assert scores.is_cuda and scores.dtype == torch.float32 and scores.is_contiguous() and scores.numel() == 8 * self.n_envs
+        _native.check(self._lib.ovc_partner_policy(
+            self.tables.data_ptr(), self.n_layouts, self.feature_lut().data_ptr(), self.state.data_ptr(), partner_seat.data_ptr(),
+            self.n_envs, self.state_words, w1.shape[1], w1.shape[0], w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
+            wh.shape[0], wo.data_ptr(), bo.data_ptr(), int(n_actions), int(seed) & (2**64 - 1), counter.data_ptr(), out.data_ptr(),
+            0 if scores is None else scores.data_ptr(), self._stream()))
+        return out
+
+    def assign_partners(self, partner_seat, bc_factor, counter, seed=0, done=None):
+        """The per-episode seat draw of PPO_BC (ovc_assign_partners): for every environment whose episode ended with the last
+        ``step`` (``done``: int32 [N], e.g. ``self.done``; None = every environment) ``partner_seat[e]`` becomes 0 or 1 (the
+        partner's player index, equally likely) with probability ``bc_factor``, else -1 (self-play).  ``bc_factor``:
+        float32 CUDA scalar tensor, read by the kernel (a captured graph follows its current value); ``counter`` as
+        ``partner_actions``'."""
+        assert partner_seat.is_cuda and partner_seat.dtype == torch.int32 and partner_seat.is_contiguous() and partner_seat.numel() == self.n_envs
+        assert bc_factor.is_cuda and bc_factor.dtype == torch.float32 and bc_factor.numel() == 1
+        assert counter.is_cuda and counter.dtype == torch.int64 and counter.numel() == 2 and counter.is_contiguous()
+        if done is not None:
+            assert done.is_cuda and done.dtype == torch.int32 and done.is_contiguous() and done.numel() == self.n_envs
+        _native.check(self._lib.ovc_assign_partners(0 if done is None else done.data_ptr(), bc_factor.data_ptr(), self.n_envs,
+                                                    int(seed) & (2**64 - 1), counter.data_ptr(), partner_seat.data_ptr(), self._stream()))
+        return partner_seat
+
     def feature_lut(self):
         if self._lut is None:
             lut = np.stack([l.feature_lut() for l in self.layouts]).view(np.uint8).reshape(self.n_layouts, -1)

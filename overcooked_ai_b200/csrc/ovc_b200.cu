@@ -11,7 +11,8 @@
 // K4  reset_kernel           masked copy of the per-layout start record.
 // The observation kernels (K2 lossless encode, K3 featurize) live in ovc_obs.cuh, K7 (first policy layer on the
 // encoding, evaluated from the record) and the draw / return kernels in ovc_encfc.cuh, K8 (dense tail of the policy +
-// the draw, one kernel) in ovc_tail.cuh, K9 (the policy's two wide layers as one wgmma kernel) in ovc_wide.cuh.
+// the draw, one kernel) in ovc_tail.cuh, K9 (the policy's two wide layers as one wgmma kernel) in ovc_wide.cuh, K10 (the
+// behaviour-cloned partner: featurize_state + its MLP + the draw, one kernel) and the partner seat draw in ovc_partner.cuh.
 //
 // The environment path is integer, branchy and HBM-bound (no contraction anywhere): no tensor cores there.  The policy-in-
 // the-loop kernels K8 / K9 (config 5) are the contractions and use them.
@@ -605,6 +606,7 @@ static int step_impl(const void *layouts, int n_layouts, const int32_t *start_re
 #include "ovc_encfc.cuh"
 #include "ovc_tail.cuh"
 #include "ovc_wide.cuh"
+#include "ovc_partner.cuh"
 #include "ovc_potential.cuh"
 #include "ovc_host.cuh"
 
@@ -724,6 +726,26 @@ int ovc_policy_tail(const void *x, int64_t n_rows, int k0, float in_slope, const
 int ovc_wide_layers(const void *a0, int64_t m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2, int n2,
                     float slope, void *z2, void *stream) {
     return ovc::wide_layers_impl(a0, m, k0, w1, b1, n1, w2, b2, n2, slope, z2, (cudaStream_t)stream);
+}
+
+int ovc_partner_policy(const void *layouts, int n_layouts, const void *lut, const int32_t *state, const int32_t *partner_seat,
+                       int64_t n_envs, int state_words, int n_features, int width, const void *w_first, const float *b_first,
+                       const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads, int n_actions,
+                       uint64_t seed, uint64_t *counter, int32_t *actions, float *scores, void *stream) {
+    int rc = ovc::check_common(layouts, n_layouts, state, n_envs, state_words);
+    if (rc) return rc;
+    ovc::PartnerArgs a;
+    a.f.layouts = (const ovc_layout_t *)layouts, a.f.lut = (const ovc_feat_lut_entry_t *)lut, a.f.state = state, a.f.view_swap = nullptr;
+    a.f.out = nullptr, a.f.n_envs = n_envs, a.f.S = state_words, a.f.num_pots = 2, a.f.B = ovc::PP_B, a.f.F = ovc::PP_F, a.f.E = ovc::FEAT_E;
+    a.partner_seat = partner_seat, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first, a.w_hidden = (const __nv_bfloat16 *)w_hidden;
+    a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads, a.n_hidden = n_hidden, a.n_actions = n_actions;
+    a.seed = seed, a.counter = (unsigned long long *)counter, a.actions = actions, a.scores = scores;
+    return ovc::partner_policy_impl(a, n_features, width, (cudaStream_t)stream);
+}
+
+int ovc_assign_partners(const int32_t *done, const float *bc_factor, int64_t n_envs, uint64_t seed, uint64_t *counter, int32_t *partner_seat,
+                        void *stream) {
+    return ovc::assign_partners_impl(done, bc_factor, n_envs, seed, (unsigned long long *)counter, partner_seat, (cudaStream_t)stream);
 }
 
 int ovc_featurize(const void *layouts, int n_layouts, const void *lut, const int32_t *state,

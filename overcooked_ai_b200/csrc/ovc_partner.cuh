@@ -1,0 +1,167 @@
+// ovc_partner.cuh — the behaviour-cloned partner of PPO_BC (included by ovc_b200.cu after ovc_obs.cuh and ovc_tail.cuh).
+//
+// K10 partner_policy_kernel: the BC agent's action from the packed record, features never materialised
+// (reference: human_aware_rl/imitation/behavior_cloning_tf2.py — featurize_state, Dense 64 ReLU, Dense 64 ReLU, 6 logits,
+// the action sampled from the softmax):
+//   phase 1  K3's feat_block for both players of each environment of a 64-environment tile, into a feature-major int16
+//            tile laid out exactly as K3's (column 2 e + j = player j's view: own block, other block, other - self,
+//            self position); only environments with a partner are built
+//   phase 2  warps own 16 environments each and run K8's layer chain on the partner's view column: A fragments read from
+//            the tile and converted to bf16, ReLU between layers, heads padded to 8, then K8's Gumbel-max draw on row
+//            2 e + seat
+// assign_partners_kernel: the per-episode seat draw of OvercookedMultiAgent._populate_agents.
+#pragma once
+
+namespace ovc {
+
+constexpr int PP_THREADS = 128;          // 4 warps x 16 environments = one K3 tile (FEAT_E = 64 environments, 2 views each)
+constexpr int PP_F = 96;                 // featurize_state width at num_pots = 2
+constexpr int PP_B = 46;                 // one player's block at num_pots = 2
+constexpr int PP_TILE_BYTES = PP_F * FEAT_LD * 2;
+
+struct PartnerArgs {
+    FeatArgs f;                          // layouts, lut, state, n_envs, S, num_pots = 2 (the fields feat_block reads)
+    const int32_t *partner_seat;         // [n_envs]: -1 self-play, 0 / 1 the partner's player index
+    const __nv_bfloat16 *w_first;        // [64][96]
+    const float *b_first;
+    const __nv_bfloat16 *w_hidden;       // [n_hidden][64][64]
+    const float *b_hidden;
+    const __nv_bfloat16 *w_heads;        // [8][64]
+    const float *b_heads;
+    int n_hidden, n_actions;
+    unsigned long long seed;
+    unsigned long long *counter;         // [2]: step, arrival scratch (as ovc_sample_actions)
+    int32_t *actions;                    // [n_envs][2]: only [e][seat] of partnered environments is written
+    float *scores;                       // [n_envs][8] or null
+};
+
+__global__ void __launch_bounds__(PP_THREADS) partner_policy_kernel(const PartnerArgs p) {
+    constexpr int KS2 = PP_F / 32;
+    extern __shared__ __align__(16) char pp_smem[];
+    const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(p.counter);
+    const TailSmem w = tail_weights_to_smem<PP_F, PP_THREADS>(pp_smem, p);
+    short *tile = reinterpret_cast<short *>(pp_smem + tail_smem_bytes(PP_F, p.n_hidden));  // [96][FEAT_LD], feature-major
+
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
+    const long long n_tiles = (p.f.n_envs + FEAT_E - 1) / FEAT_E;
+    for (long long tl = blockIdx.x; tl < n_tiles; tl += gridDim.x) {
+        const long long env0 = tl * FEAT_E;
+        __syncthreads();  // the previous tile's reads are done (first pass: the weights are in place)
+        // ---- phase 1: thread (el, j) builds player j's block, as K3 does ----
+        {
+            const int v = threadIdx.x, el = v >> 1, j = v & 1;
+            const long long e = env0 + el;
+            const int seat = e < p.f.n_envs ? __ldg(p.partner_seat + e) : -1;
+            if (seat >= 0) {
+                const int32_t *__restrict__ rec = p.f.state + e * p.f.S;
+                const int lid = __ldg(rec + 3) & 0xFF;
+                const ovc_layout_t *__restrict__ L = p.f.layouts + lid;
+                const unsigned me = (unsigned)__ldg(rec + 1 + j), ot = (unsigned)__ldg(rec + 2 - j);
+                const ovc_feat_lut_entry_t *le = p.f.lut + (size_t)lid * 1024 + ((me & 0xFF) << 2 | ((me >> 8) & 3));
+                feat_block(p.f, L, le, rec, me, tile + v, tile + (size_t)PP_B * FEAT_LD + (v ^ 1));
+                if (j == seat) {  // :2877-2896 tail of the partner's row: other - self, then self position
+                    short *tl4 = tile + (size_t)2 * PP_B * FEAT_LD + v;
+                    tl4[0 * FEAT_LD] = (short)((int)(ot & 15) - (int)(me & 15));
+                    tl4[1 * FEAT_LD] = (short)((int)((ot >> 4) & 15) - (int)((me >> 4) & 15));
+                    tl4[2 * FEAT_LD] = (short)(me & 15);
+                    tl4[3 * FEAT_LD] = (short)((me >> 4) & 15);
+                }
+            }
+        }
+        __syncthreads();
+        // ---- phase 2: warp w evaluates environments 16 w + g and 16 w + g + 8 of the tile ----
+        const int el0 = 16 * warp + g, el1 = el0 + 8;
+        const long long e0 = env0 + el0, e1 = env0 + el1;
+        const int seat0 = e0 < p.f.n_envs ? __ldg(p.partner_seat + e0) : -1, seat1 = e1 < p.f.n_envs ? __ldg(p.partner_seat + e1) : -1;
+        if (__all_sync(0xFFFFFFFFu, seat0 < 0 && seat1 < 0)) continue;  // no partner among the warp's 16 environments
+        // the partner's view column; an environment without a partner reads a column nobody wrote (finite int16 values,
+        // its results are discarded)
+        const short *c0 = tile + 2 * el0 + (seat0 > 0), *c1 = tile + 2 * el1 + (seat1 > 0);
+        auto pair = [](short lo, short hi) {
+            const __nv_bfloat162 h = __floats2bfloat162_rn((float)lo, (float)hi);  // exact while |value| <= 256
+            return *reinterpret_cast<const unsigned *>(&h);
+        };
+        float acc[8][4];
+        first_layer64<KS2>(acc, w, g, t, [&](int s2, unsigned a_lo[4], unsigned a_hi[4]) {
+            const int k = 32 * s2 + 8 * t;
+            short x0[8], x1[8];
+#pragma unroll
+            for (int i = 0; i < 8; i++) x0[i] = c0[(k + i) * FEAT_LD], x1[i] = c1[(k + i) * FEAT_LD];
+            a_lo[0] = pair(x0[0], x0[1]), a_lo[1] = pair(x1[0], x1[1]), a_lo[2] = pair(x0[2], x0[3]), a_lo[3] = pair(x1[2], x1[3]);
+            a_hi[0] = pair(x0[4], x0[5]), a_hi[1] = pair(x1[4], x1[5]), a_hi[2] = pair(x0[6], x0[7]), a_hi[3] = pair(x1[6], x1[7]);
+        });
+        float out[1][4];
+        tail_layers(out, acc, w, p.n_hidden, 0.f, g, t);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const long long e = h ? e1 : e0;
+            const int seat = h ? seat1 : seat0;
+            float lp;
+            const int best = draw_row<false>(out[0][2 * h], out[0][2 * h + 1], p.seed, step, 2 * e + (seat > 0), p.n_actions, lane, t, lp);
+            if (seat >= 0) {
+                if (t == 0) p.actions[2 * e + seat] = best;
+                if (p.scores) *reinterpret_cast<float2 *>(p.scores + e * PT_NOUT + 2 * t) = make_float2(out[0][2 * h], out[0][2 * h + 1]);
+            }
+        }
+    }
+    advance_step(p.counter, step);
+}
+
+static int partner_policy_impl(const PartnerArgs &a, int n_features, int width, cudaStream_t st) {
+    if (!a.f.lut || !a.partner_seat || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || !a.counter || !a.actions ||
+        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)))
+        return fail(OVC_E_BADARG, "null pointer argument");
+    if (n_features != PP_F) return fail(OVC_E_UNSUPPORTED, "partner_policy: built for featurize_state at num_pots = 2 (96 features)", n_features);
+    if (width != PT_H) return fail(OVC_E_UNSUPPORTED, "partner_policy: built for 64-wide layers", width);
+    if (a.n_actions < 1 || a.n_actions > 7) return fail(OVC_E_UNSUPPORTED, "partner_policy: n_actions must be 1..7", a.n_actions);
+    if (a.n_hidden < 0 || a.n_hidden > 8) return fail(OVC_E_BADARG, "n_hidden must be 0..8", a.n_hidden);
+    if ((((uintptr_t)a.w_first | (uintptr_t)a.w_hidden | (uintptr_t)a.w_heads) & 15) != 0) return fail(OVC_E_BADARG, "weights must be 16-byte aligned");
+    if ((((uintptr_t)a.b_first | (uintptr_t)a.b_hidden | (uintptr_t)a.b_heads | (uintptr_t)a.scores) & 7) != 0)
+        return fail(OVC_E_BADARG, "biases and scores must be 8-byte aligned");
+    if (a.f.n_envs == 0) return OVC_OK;
+    int dev = 0, n_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    const size_t smem = tail_smem_bytes(PP_F, a.n_hidden) + PP_TILE_BYTES;
+    cudaError_t e = cudaFuncSetAttribute(partner_policy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return cuda_fail(e, "partner_policy kernel attribute");
+    int per_sm = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, partner_policy_kernel, PP_THREADS, smem);
+    if (e != cudaSuccess) return cuda_fail(e, "partner_policy occupancy");
+    if (per_sm < 1) per_sm = 1;
+    // persistent CTAs: each copies the weights into shared memory once and then walks its share of the tiles
+    const long long n_tiles = (a.f.n_envs + FEAT_E - 1) / FEAT_E, cap = (long long)per_sm * n_sm;
+    partner_policy_kernel<<<(unsigned)(n_tiles < cap ? n_tiles : cap), PP_THREADS, smem, st>>>(a);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "partner_policy kernel launch");
+    return OVC_OK;
+}
+
+// partner_seat[e] for every environment whose episode just ended (done[e] != 0; all with done == NULL): Philox4x32-10 with
+// key = seed, counter = (e low, e high, step low, step high) -> words w0, w1;  seat = w0 < threshold ? w1 >> 31 : -1, where
+// threshold = bc_factor * 2^32 saturated as the random-start draw saturates it (bc_factor >= 1: always a partner).
+__global__ void __launch_bounds__(256) assign_partners_kernel(const int32_t *__restrict__ done, const float *__restrict__ bc_factor, long long n_envs,
+                                                              unsigned long long seed, unsigned long long *counter, int32_t *__restrict__ partner_seat) {
+    const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(counter);
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < n_envs && (!done || done[e] != 0)) {
+        const float f = *bc_factor;
+        const uint32_t thr = f >= 1.f ? 0xFFFFFFFFu : f > 0.f ? (uint32_t)((double)f * 4294967296.0) : 0u;
+        const Philox4 P = philox4x32_10(seed, (uint32_t)e, (uint32_t)((unsigned long long)e >> 32), (uint32_t)step, (uint32_t)(step >> 32));
+        partner_seat[e] = draw_below(P.v[0], thr) ? (int32_t)(P.v[1] >> 31) : -1;
+    }
+    advance_step(counter, step);
+}
+
+static int assign_partners_impl(const int32_t *done, const float *bc_factor, long long n_envs, unsigned long long seed,
+                                unsigned long long *counter, int32_t *partner_seat, cudaStream_t st) {
+    if (!bc_factor || !counter || !partner_seat) return fail(OVC_E_BADARG, "null pointer argument");
+    if (n_envs < 0) return fail(OVC_E_BADARG, "negative env count");
+    if (n_envs == 0) return OVC_OK;
+    assign_partners_kernel<<<(unsigned)((n_envs + 255) / 256), 256, 0, st>>>(done, bc_factor, n_envs, seed, counter, partner_seat);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "assign_partners kernel launch");
+    return OVC_OK;
+}
+
+}  // namespace ovc

@@ -90,36 +90,142 @@ __device__ __forceinline__ void to_fragments(unsigned a[4][4], const float acc[8
     }
 }
 
-template <int KS2, bool LOGP>  // K0 = 32 * KS2; LOGP: also write p.logp (a separate instantiation, so the plain draw is untouched)
-__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const PolicyTailArgs p) {
-    constexpr int K0 = 32 * KS2;
-    constexpr int FS = K0 % 64 == 32 ? K0 : K0 + 32;  // row stride of the first layer's weights: 32 mod 64 elements, LDS.128 conflict free
-    extern __shared__ __align__(16) char pt_smem[];
-    __nv_bfloat16 *w1 = reinterpret_cast<__nv_bfloat16 *>(pt_smem);            // [64][FS], natural k order
-    __nv_bfloat16 *wh = w1 + PT_H * FS;                                       // [n_hidden][64][PT_HS], permuted k order
-    __nv_bfloat16 *wo = wh + p.n_hidden * PT_H * PT_HS;                       // [8][PT_HS], permuted
-    float *b1 = reinterpret_cast<float *>(wo + PT_NOUT * PT_HS);              // [64]
-    float *bh = b1 + PT_H;                                                    // [n_hidden][64]
-    float *bo = bh + p.n_hidden * PT_H;                                       // [8]
+// Shared-memory copy of a tail's weights (K8, K10), in the orders the fragment loads read.  NT threads per CTA.
+struct TailSmem {
+    __nv_bfloat16 *w1, *wh, *wo;  // [64][FS] natural k order; [n_hidden][64][PT_HS] and [8][PT_HS] permuted k order
+    float *b1, *bh, *bo;          // [64], [n_hidden][64], [8]
+};
 
-    const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(p.counter);
-    // ---- weights into shared memory ----
-    for (int i = threadIdx.x; i < PT_H * (K0 / 8); i += PT_THREADS) {
+// row stride of the first layer's weights: 32 mod 64 elements, LDS.128 conflict free
+__host__ __device__ constexpr int tail_fs(int k0) { return k0 % 64 == 32 ? k0 : k0 + 32; }
+
+__host__ __device__ constexpr size_t tail_smem_bytes(int k0, int n_hidden) {
+    return (size_t)PT_H * tail_fs(k0) * 2 + (size_t)(n_hidden * PT_H + PT_NOUT) * PT_HS * 2 + (size_t)(PT_H + n_hidden * PT_H + PT_NOUT) * 4;
+}
+
+template <int K0, int NT, class Args>
+__device__ __forceinline__ TailSmem tail_weights_to_smem(char *smem, const Args &p) {
+    constexpr int FS = tail_fs(K0);
+    TailSmem w;
+    w.w1 = reinterpret_cast<__nv_bfloat16 *>(smem);
+    w.wh = w.w1 + PT_H * FS;
+    w.wo = w.wh + p.n_hidden * PT_H * PT_HS;
+    w.b1 = reinterpret_cast<float *>(w.wo + PT_NOUT * PT_HS);
+    w.bh = w.b1 + PT_H;
+    w.bo = w.bh + p.n_hidden * PT_H;
+    for (int i = threadIdx.x; i < PT_H * (K0 / 8); i += NT) {
         const int n = i / (K0 / 8), c = i - n * (K0 / 8);
-        *reinterpret_cast<uint4 *>(w1 + n * FS + 8 * c) = __ldg(reinterpret_cast<const uint4 *>(p.w_first + (size_t)n * K0) + c);
+        *reinterpret_cast<uint4 *>(w.w1 + n * FS + 8 * c) = __ldg(reinterpret_cast<const uint4 *>(p.w_first + (size_t)n * K0) + c);
     }
-    for (int i = threadIdx.x; i < (p.n_hidden * PT_H + PT_NOUT) * (PT_H / 8); i += PT_THREADS) {
+    for (int i = threadIdx.x; i < (p.n_hidden * PT_H + PT_NOUT) * (PT_H / 8); i += NT) {
         // 8 consecutive inputs of one row (hidden layers' rows, then the heads' with the same stride): natural k = 16 s + r,
         // r = 8 h + 2 tt + e  ->  permuted position 16 s + 4 tt + 2 h + e: the four input pairs go to four 4-byte slots
         const int n = i >> 3, q = i & 7, s2 = q >> 1, h = q & 1;
         const __nv_bfloat16 *src = n < p.n_hidden * PT_H ? p.w_hidden + (size_t)n * PT_H : p.w_heads + (size_t)(n - p.n_hidden * PT_H) * PT_H;
         const uint4 v = __ldg(reinterpret_cast<const uint4 *>(src) + q);
-        unsigned *dst = reinterpret_cast<unsigned *>(wh + n * PT_HS + 16 * s2 + 2 * h);
+        unsigned *dst = reinterpret_cast<unsigned *>(w.wh + n * PT_HS + 16 * s2 + 2 * h);
         dst[0] = v.x, dst[2] = v.y, dst[4] = v.z, dst[6] = v.w;
     }
-    for (int i = threadIdx.x; i < PT_H; i += PT_THREADS) b1[i] = p.b_first[i];
-    for (int i = threadIdx.x; i < p.n_hidden * PT_H; i += PT_THREADS) bh[i] = p.b_hidden[i];
-    for (int i = threadIdx.x; i < PT_NOUT; i += PT_THREADS) bo[i] = p.b_heads[i];
+    for (int i = threadIdx.x; i < PT_H; i += NT) w.b1[i] = p.b_first[i];
+    for (int i = threadIdx.x; i < p.n_hidden * PT_H; i += NT) w.bh[i] = p.b_hidden[i];
+    for (int i = threadIdx.x; i < PT_NOUT; i += NT) w.bo[i] = p.b_heads[i];
+    return w;
+}
+
+// First layer K0 = 32 KS2 -> 64 of the 16 rows of a warp.  Lane (g, t) holds inputs 32 s2 + 8 t + 0..7 of rows g and g + 8:
+// frag(s2, a_lo, a_hi) gives them as the A fragments of k-steps 2 s2 (a_lo) and 2 s2 + 1 (a_hi) — elements 0-3 of the
+// eight feed a_lo (a0 / a2 for row g, a1 / a3 for row g + 8), 4-7 feed a_hi.  The B fragments use the same assignment,
+// so the weights stay in their natural order.
+template <int KS2, class Frag>
+__device__ __forceinline__ void first_layer64(float acc[8][4], const TailSmem &w, int g, int t, Frag &&frag) {
+    constexpr int FS = tail_fs(32 * KS2);
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        const float2 b = *reinterpret_cast<const float2 *>(w.b1 + 8 * j + 2 * t);
+        acc[j][0] = b.x, acc[j][1] = b.y, acc[j][2] = b.x, acc[j][3] = b.y;
+    }
+#pragma unroll
+    for (int s2 = 0; s2 < KS2; s2++) {
+        unsigned a_lo[4], a_hi[4];
+        frag(s2, a_lo, a_hi);
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            const uint4 b = *reinterpret_cast<const uint4 *>(w.w1 + (8 * j + g) * FS + 32 * s2 + 8 * t);
+            mma_bf16_16816(acc[j], a_lo, b.x, b.y);
+            mma_bf16_16816(acc[j], a_hi, b.z, b.w);
+        }
+    }
+}
+
+// The layers after the first: ReLU-family activation, n_hidden 64 -> 64 layers, then the heads.  out[0][0..1]: heads 2 t,
+// 2 t + 1 of row g; out[0][2..3]: the same of row g + 8.
+__device__ __forceinline__ void tail_layers(float out[1][4], float acc[8][4], const TailSmem &w, int n_hidden, float slope, int g, int t) {
+    unsigned a[4][4];
+    to_fragments(a, acc, slope);
+    for (int l = 0; l < n_hidden; l++) {
+        dense64<8>(acc, a, w.wh + l * PT_H * PT_HS, w.bh + l * PT_H, g, t);
+        to_fragments(a, acc, slope);
+    }
+    dense64<1>(out, a, w.wo, w.bo, g, t);
+}
+
+// The draw of ovc_sample_actions on one row whose heads 2 t, 2 t + 1 (s0, s1) lane t of the row's four lanes holds: they
+// use words 2 t, 2 t + 1 of Philox block t / 2 at counter (row, step).  Every lane returns the drawn action; with LOGP
+// also its log-probability (lp).  All 32 lanes must take part (shuffles).
+template <bool LOGP>
+__device__ __forceinline__ int draw_row(float s0, float s1, unsigned long long seed, unsigned long long step, long long row, int n_actions,
+                                        int lane, int t, float &lp) {
+    const Philox4 P = philox4x32_10(seed, (uint32_t)row, (uint32_t)((unsigned long long)row >> 32), (uint32_t)step,
+                                    ((uint32_t)(step >> 32) << 1) | (uint32_t)(t >> 1));
+    const uint32_t d0 = P.v[(2 * t) & 3], d1 = P.v[(2 * t + 1) & 3];
+    const float u0 = ((float)(d0 >> 9) + 0.5f) * 1.1920928955078125e-7f, u1 = ((float)(d1 >> 9) + 0.5f) * 1.1920928955078125e-7f;
+    float v0 = 2 * t < n_actions ? s0 - logf(-logf(u0)) : -INFINITY;
+    const float v1 = 2 * t + 1 < n_actions ? s1 - logf(-logf(u1)) : -INFINITY;
+    int best = 2 * t;
+    if (v1 > v0) v0 = v1, best = 2 * t + 1;
+#pragma unroll
+    for (int d = 1; d <= 2; d <<= 1) {  // argmax over the four lanes of the row (lowest index wins ties, as a serial scan does)
+        const float ov = __shfl_xor_sync(0xFFFFFFFFu, v0, d);
+        const int ob = __shfl_xor_sync(0xFFFFFFFFu, best, d);
+        if (ov > v0 || (ov == v0 && ob < best)) v0 = ov, best = ob;
+    }
+    if constexpr (LOGP) {  // log-softmax at the drawn action over the same four lanes: max, then the sum of exp
+        const bool in0 = 2 * t < n_actions, in1 = 2 * t + 1 < n_actions;
+        float m = fmaxf(in0 ? s0 : -INFINITY, in1 ? s1 : -INFINITY);
+#pragma unroll
+        for (int d = 1; d <= 2; d <<= 1) m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, d));
+        float se = (in0 ? expf(s0 - m) : 0.f) + (in1 ? expf(s1 - m) : 0.f);
+#pragma unroll
+        for (int d = 1; d <= 2; d <<= 1) se += __shfl_xor_sync(0xFFFFFFFFu, se, d);
+        const int src = (lane & ~3) | (best >> 1);  // the lane holding head `best`
+        const float b0 = __shfl_sync(0xFFFFFFFFu, s0, src), b1 = __shfl_sync(0xFFFFFFFFu, s1, src);
+        lp = ((best & 1) ? b1 : b0) - (m + logf(se));
+    }
+    return best;
+}
+
+// The last CTA of a launch to get here advances the draw step (every CTA has read it by then): counter[1] counts arrivals.
+__device__ __forceinline__ void advance_step(unsigned long long *counter, unsigned long long step) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        const unsigned long long arrived = atomicAdd(counter + 1, 1ull);
+        if (arrived == (unsigned long long)gridDim.x - 1) {
+            counter[1] = 0;
+            counter[0] = step + 1;
+            __threadfence();
+        }
+    }
+}
+
+template <int KS2, bool LOGP>  // K0 = 32 * KS2; LOGP: also write p.logp (a separate instantiation, so the plain draw is untouched)
+__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const PolicyTailArgs p) {
+    constexpr int K0 = 32 * KS2;
+    extern __shared__ __align__(16) char pt_smem[];
+
+    const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(p.counter);
+    // ---- weights into shared memory ----
+    const TailSmem w = tail_weights_to_smem<K0, PT_THREADS>(pt_smem, p);
     __syncthreads();
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
@@ -127,9 +233,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const Policy
     const long long n_tiles = (p.n_rows + 15) / 16;
     for (long long tile = (long long)blockIdx.x * (PT_THREADS / 32) + warp; tile < n_tiles; tile += (long long)gridDim.x * (PT_THREADS / 32)) {
         const long long r0 = tile * 16 + g, r1 = r0 + 8;
-        // ---- first layer: A fragments straight from global memory, 16 bytes (8 inputs) per load.  Lane (g, t) holds inputs
-        //      32 s2 + 8 t + 0..7 of rows g and g + 8: elements 0-3 feed k-step 2 s2 (a0/a2 resp. a1/a3), 4-7 feed k-step 2 s2 + 1;
-        //      the B fragments use the same assignment, so the weights stay in their natural order. ----
+        // ---- first layer: A fragments straight from global memory, 16 bytes (8 inputs) per load ----
         uint4 xa[KS2], xb[KS2];
 #pragma unroll
         for (int s2 = 0; s2 < KS2; s2++) {
@@ -137,70 +241,26 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const Policy
             xb[s2] = r1 < p.n_rows ? __ldg(reinterpret_cast<const uint4 *>(p.x + r1 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
         }
         float acc[8][4];
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-            const float2 b = *reinterpret_cast<const float2 *>(b1 + 8 * j + 2 * t);
-            acc[j][0] = b.x, acc[j][1] = b.y, acc[j][2] = b.x, acc[j][3] = b.y;
-        }
-#pragma unroll
-        for (int s2 = 0; s2 < KS2; s2++) {
-            unsigned a_lo[4], a_hi[4];
+        first_layer64<KS2>(acc, w, g, t, [&](int s2, unsigned a_lo[4], unsigned a_hi[4]) {
             a_lo[0] = lrelu_bf16x2(xa[s2].x, in_slope2), a_lo[1] = lrelu_bf16x2(xb[s2].x, in_slope2);
             a_lo[2] = lrelu_bf16x2(xa[s2].y, in_slope2), a_lo[3] = lrelu_bf16x2(xb[s2].y, in_slope2);
             a_hi[0] = lrelu_bf16x2(xa[s2].z, in_slope2), a_hi[1] = lrelu_bf16x2(xb[s2].z, in_slope2);
             a_hi[2] = lrelu_bf16x2(xa[s2].w, in_slope2), a_hi[3] = lrelu_bf16x2(xb[s2].w, in_slope2);
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const uint4 b = *reinterpret_cast<const uint4 *>(w1 + (8 * j + g) * FS + 32 * s2 + 8 * t);
-                mma_bf16_16816(acc[j], a_lo, b.x, b.y);
-                mma_bf16_16816(acc[j], a_hi, b.z, b.w);
-            }
-        }
+        });
         // ---- hidden layers and heads: fragments in, fragments out ----
-        unsigned a[4][4];
-        to_fragments(a, acc, p.slope);
-        for (int l = 0; l < p.n_hidden; l++) {
-            dense64<8>(acc, a, wh + l * PT_H * PT_HS, bh + l * PT_H, g, t);
-            to_fragments(a, acc, p.slope);
-        }
         float out[1][4];
-        dense64<1>(out, a, wo, bo, g, t);  // lane (g, t): heads 2 t, 2 t + 1 of rows g (out[0][0..1]) and g + 8 (out[0][2..3])
+        tail_layers(out, acc, w, p.n_hidden, p.slope, g, t);
         if (p.scores) {
             if (r0 < p.n_rows) *reinterpret_cast<float2 *>(p.scores + r0 * PT_NOUT + 2 * t) = make_float2(out[0][0], out[0][1]);
             if (r1 < p.n_rows) *reinterpret_cast<float2 *>(p.scores + r1 * PT_NOUT + 2 * t) = make_float2(out[0][2], out[0][3]);
         }
-        // ---- the draw (ovc_sample_actions): heads 2 t, 2 t + 1 use words 2 t, 2 t + 1 of block t / 2 ----
+        // ---- the draw (ovc_sample_actions) ----
 #pragma unroll
         for (int h = 0; h < 2; h++) {
             const long long row = h ? r1 : r0;
             const float s0 = out[0][2 * h], s1 = out[0][2 * h + 1];
-            const Philox4 P = philox4x32_10(p.seed, (uint32_t)row, (uint32_t)((unsigned long long)row >> 32), (uint32_t)step,
-                                            ((uint32_t)(step >> 32) << 1) | (uint32_t)(t >> 1));
-            const uint32_t d0 = P.v[(2 * t) & 3], d1 = P.v[(2 * t + 1) & 3];
-            const float u0 = ((float)(d0 >> 9) + 0.5f) * 1.1920928955078125e-7f, u1 = ((float)(d1 >> 9) + 0.5f) * 1.1920928955078125e-7f;
-            float v0 = 2 * t < p.n_actions ? s0 - logf(-logf(u0)) : -INFINITY;
-            const float v1 = 2 * t + 1 < p.n_actions ? s1 - logf(-logf(u1)) : -INFINITY;
-            int best = 2 * t;
-            if (v1 > v0) v0 = v1, best = 2 * t + 1;
-#pragma unroll
-            for (int d = 1; d <= 2; d <<= 1) {  // argmax over the four lanes of the row (lowest index wins ties, as a serial scan does)
-                const float ov = __shfl_xor_sync(0xFFFFFFFFu, v0, d);
-                const int ob = __shfl_xor_sync(0xFFFFFFFFu, best, d);
-                if (ov > v0 || (ov == v0 && ob < best)) v0 = ov, best = ob;
-            }
             float lp = 0.f;
-            if constexpr (LOGP) {  // log-softmax at the drawn action over the same four lanes: max, then the sum of exp
-                const bool in0 = 2 * t < p.n_actions, in1 = 2 * t + 1 < p.n_actions;
-                float m = fmaxf(in0 ? s0 : -INFINITY, in1 ? s1 : -INFINITY);
-#pragma unroll
-                for (int d = 1; d <= 2; d <<= 1) m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, d));
-                float se = (in0 ? expf(s0 - m) : 0.f) + (in1 ? expf(s1 - m) : 0.f);
-#pragma unroll
-                for (int d = 1; d <= 2; d <<= 1) se += __shfl_xor_sync(0xFFFFFFFFu, se, d);
-                const int src = (lane & ~3) | (best >> 1);  // the lane holding head `best`
-                const float b0 = __shfl_sync(0xFFFFFFFFu, s0, src), b1 = __shfl_sync(0xFFFFFFFFu, s1, src);
-                lp = ((best & 1) ? b1 : b0) - (m + logf(se));
-            }
+            const int best = draw_row<LOGP>(s0, s1, p.seed, step, row, p.n_actions, lane, t, lp);
             if (row < p.n_rows) {
                 if (t == 0) p.actions[row] = best;
                 if constexpr (LOGP) if (t == 0) p.logp[row] = lp;
@@ -209,16 +269,7 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const Policy
             }
         }
     }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        const unsigned long long arrived = atomicAdd(p.counter + 1, 1ull);
-        if (arrived == (unsigned long long)gridDim.x - 1) {
-            p.counter[1] = 0;
-            p.counter[0] = step + 1;
-            __threadfence();
-        }
-    }
+    advance_step(p.counter, step);
 }
 
 static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st) {
@@ -234,8 +285,7 @@ static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st) {
     int dev = 0, n_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    const int fs = k0 % 64 == 32 ? k0 : k0 + 32;
-    const size_t smem = (size_t)PT_H * fs * 2 + (size_t)(a.n_hidden * PT_H + PT_NOUT) * PT_HS * 2 + (size_t)(PT_H + a.n_hidden * PT_H + PT_NOUT) * 4 + 16;
+    const size_t smem = tail_smem_bytes(k0, a.n_hidden) + 16;
     const long long n_tiles = (a.n_rows + 15) / 16, want = (n_tiles + PT_THREADS / 32 - 1) / (PT_THREADS / 32);
     const unsigned grid = (unsigned)(want < n_sm ? want : n_sm);
     cudaError_t e = cudaSuccess;

@@ -197,6 +197,51 @@ def fused_kernel_support(dense_model, width, height):
     return k7, k9, k8
 
 
+class BCPolicy(nn.Module):
+    """The behaviour-cloning partner of PPO_BC (human_aware_rl/imitation/behavior_cloning_tf2.py, the default MLP):
+    featurize_state (96 features at num_pots = 2) -> Dense 64 ReLU (x ``num_hidden_layers``) -> ``num_actions`` logits, the
+    action sampled from the softmax.  ``tables()`` hands it to K10 (``BatchedOvercookedEnv.partner_actions``)."""
+
+    def __init__(self, n_features=96, hidden=64, num_hidden_layers=2, num_actions=6):
+        super().__init__()
+        dims = [n_features] + [hidden] * num_hidden_layers
+        self.dense = nn.ModuleList([nn.Linear(dims[i], dims[i + 1]) for i in range(num_hidden_layers)])
+        self.logits = nn.Linear(dims[-1], num_actions)
+
+    def load_keras_weights(self, dense, logits):
+        """The reference's Keras weights: ``dense`` = [(kernel, bias)] of the hidden layers, ``logits`` = (kernel, bias), Keras
+        kernels ``(in, out)``.  Arrays or tensors."""
+        t = lambda a: torch.as_tensor(a, dtype=torch.float32)
+        with torch.no_grad():
+            for mod, (k, b) in zip(self.dense, dense):
+                mod.weight.copy_(t(k).t()), mod.bias.copy_(t(b))
+            self.logits.weight.copy_(t(logits[0]).t()), self.logits.bias.copy_(t(logits[1]))
+        return self
+
+    def forward(self, features):
+        x = features
+        for d in self.dense:
+            x = F.relu(d(x))
+        return self.logits(x)
+
+    def tables(self):
+        """The network in the form ``ovc_partner_policy`` (K10) takes: (w_first bf16 [64, 96], b_first f32 [64], w_hidden bf16
+        [n_hidden, 64, 64], b_hidden f32 [n_hidden, 64], w_heads bf16 [8, 64], b_heads f32 [8]) with n_hidden = the hidden
+        layers after the first; the heads are the logits padded to 8 rows with zeros (row ``num_actions`` is the value row
+        K8 reads; a BC policy has none)."""
+        d = list(self.dense)
+        assert len(d) >= 1 and all(l.out_features == 64 for l in d) and d[0].in_features == 96 and self.logits.out_features <= 7, \
+            "K10 is built for 96 features, 64-wide layers and at most 7 actions"
+        bf = lambda t: t.detach().to(torch.bfloat16).contiguous()
+        f32 = lambda t: t.detach().float().contiguous()
+        dev = self.logits.weight.device
+        wh = torch.stack([l.weight for l in d[1:]]) if len(d) > 1 else torch.zeros((0, 64, 64), device=dev)
+        bh = torch.stack([l.bias for l in d[1:]]) if len(d) > 1 else torch.zeros((0, 64), device=dev)
+        wo, bo = torch.zeros((8, 64), device=dev), torch.zeros(8, device=dev)
+        wo[:self.logits.out_features], bo[:self.logits.out_features] = self.logits.weight.detach(), self.logits.bias.detach()
+        return bf(d[0].weight), f32(d[0].bias), bf(wh), f32(bh), bf(wo), f32(bo)
+
+
 def sample_categorical(logits, noise):
     """One draw per row from softmax(logits) by the Gumbel-max rule: argmax_i (logit_i - log E_i) with E_i ~ Exp(1) picks i
     with probability softmax(logits)_i — four small kernels where softmax + ``torch.multinomial`` launch about twenty.
@@ -219,9 +264,11 @@ class SampleBatch(object):
     last_values   float32 [2N]       value head on the state after the window (bootstrap)
     advantages, value_targets  float32 [T, 2N]   GAE (ovc_gae)
     logits        float32 [T, 2N, 8] the policy's heads (columns 0..5 the logits), only with ``keep_logits``
+    partner_seat  int8 [T, N]        with a BC partner: its player index at transition t (-1: self-play), else None
+    learner_mask  uint8 [T, 2N]      (property) the rows the learner trains on: all rows but the partner's
     """
 
-    def __init__(self, env, n_steps, keep_logits=False):
+    def __init__(self, env, n_steps, keep_logits=False, partner=False):
         N, T, dev = env.n_envs, int(n_steps), env.device
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
         self.env = env
@@ -231,6 +278,17 @@ class SampleBatch(object):
         self.dones = z((T, N), torch.uint8)
         self.last_values = z(2 * N, torch.float32)
         self.logits = z((T, 2 * N, 8), torch.float32) if keep_logits else None
+        self.partner_seat = z((T, N), torch.int8) if partner else None
+
+    @property
+    def learner_mask(self):
+        """uint8 [T, 2N]: 1 on the rows the PPO agent acted on — both rows of a self-play environment, the non-partner row
+        otherwise.  Computed from ``partner_seat``."""
+        T, N = self.dones.shape
+        if self.partner_seat is None:
+            return torch.ones((T, 2 * N), dtype=torch.uint8, device=self.dones.device)
+        agent = torch.arange(2, dtype=torch.int8, device=self.dones.device)
+        return (self.partner_seat.unsqueeze(-1) != agent).to(torch.uint8).view(T, 2 * N)
 
     def observations(self, env_steps, dtype=torch.float32):
         """lossless_state_encoding ``[M, 2, W, H, 26]`` of the env-steps ``env_steps`` (CUDA int64 [M], flat indices
@@ -240,11 +298,20 @@ class SampleBatch(object):
         return self.env.lossless_state_encoding(dtype=dtype, states=recs)
 
 
+# The BC partner's draws use their own Philox keys: seed ^ PARTNER_DRAW_SALT for K10's action draw, seed ^ PARTNER_SEAT_SALT
+# for the seat draw.  A partner action is then never drawn from the noise the PPO draw (key = seed) used on the same row and
+# step, and the seat draw's counters (env, step) cannot meet the action draws' (row, step, block).
+PARTNER_DRAW_SALT = 0x9E3779B97F4A7C15
+PARTNER_SEAT_SALT = 0xD1B54A32D192ED03
+
+
 class SelfPlayRollout(object):
-    """Policy-in-the-loop rollout: both agents of every environment act from the same network."""
+    """Policy-in-the-loop rollout: both agents of every environment act from the same network, or, with a BC ``partner``,
+    one seat of an environment is the partner's in the episodes the seat draw gives it (PPO_BC)."""
 
     def __init__(self, env, model=None, autocast_dtype=torch.bfloat16, use_graph=True, reward_shaping_factor=1.0,
-                 obs_dtype=None, dense=True, sub_batches=1, fused_first_layer=None, native_glue=True, seed=0, fused_tail=None, fused_wide=None):
+                 obs_dtype=None, dense=True, sub_batches=1, fused_first_layer=None, native_glue=True, seed=0, fused_tail=None, fused_wide=None,
+                 partner=None, bc_factor=0.0):
         """obs_dtype: element type K2 writes (default: bfloat16 when the policy runs in bf16 — the plane values are exact
         in bf16 and the conversion pass disappears — else float32).
         dense: evaluate the network through ``DenseGridPolicy`` (one library GEMM per layer, widths padded to 16-byte rows,
@@ -263,7 +330,12 @@ class SelfPlayRollout(object):
         two wide layers.
         fused_wide (default: with K7 and K8 when the wide layers are 512 -> 512 -> 160, i.e. on 5x4 grids): those two layers
         run as ONE wgmma kernel (``ovc_wide_layers``, K9: the 512-wide activation stays in registers) — the
-        whole policy is then K7 -> K9 -> K8, no library call."""
+        whole policy is then K7 -> K9 -> K8, no library call.
+        partner: a ``BCPolicy`` that plays next to the PPO agent (PPO_BC, human_aware_rl's OvercookedMultiAgent): at every
+        episode start (and for every environment at construction) an environment gets the partner with probability
+        ``bc_factor``, in seat 0 or 1 with equal probability (``env.assign_partners``); per transition K10
+        (``env.partner_actions``) overwrites that seat's action after the PPO policy drew both.  Needs native_glue.
+        bc_factor: see the property."""
         assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
         self.env = env
         l = env.layouts[0]
@@ -326,6 +398,18 @@ class SelfPlayRollout(object):
         self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
         self._boot_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # the bootstrap's draws leave _draw_counter alone
         self._boot_actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
+        self.partner = None
+        self.bc = float(bc_factor)
+        if partner is not None:
+            assert self.native_glue, "the BC partner runs on the native draw / reward kernels (native_glue=True)"
+            self.partner = partner.to(dev).eval()
+            self._partner_tables = self.partner.tables()
+            self._partner_n_actions = self.partner.logits.out_features
+            self._bc_factor = torch.full((1,), self.bc, dtype=torch.float32, device=dev)  # read by the seat draw
+            self.partner_seat = torch.full((N,), -1, dtype=torch.int32, device=dev)
+            self._partner_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of K10's draw
+            self._seat_counter = torch.zeros(2, dtype=torch.int64, device=dev)     # [step, scratch] of the seat draw
+            self._assign_partners(None)
 
     @property
     def reward_shaping_factor(self):
@@ -339,6 +423,38 @@ class SelfPlayRollout(object):
             self.graph = None
         self.factor = float(value)
         self._factor.fill_(self.factor)
+
+    @property
+    def bc_factor(self):
+        """Probability that an episode is played with the BC partner (human_aware_rl's ``bc_factor``, annealed by its
+        ``bc_schedule``).  Setting it takes effect at the next episode starts, in run() and collect() alike, without a
+        re-capture (the seat draw reads a device scalar)."""
+        return self.bc
+
+    @bc_factor.setter
+    def bc_factor(self, value):
+        assert self.partner is not None, "bc_factor needs a partner"
+        self.bc = float(value)
+        self._bc_factor.fill_(self.bc)
+
+    def _assign_partners(self, done):
+        self.env.assign_partners(self.partner_seat, self._bc_factor, self._seat_counter, seed=self.seed ^ PARTNER_SEAT_SALT, done=done)
+
+    def _partner_act(self, actions):
+        """K10: the partner's seat of ``actions`` (int32 [N, 2] or [2N]) from the current state."""
+        self.env.partner_actions(self._partner_tables, self.partner_seat, self._partner_counter, seed=self.seed ^ PARTNER_DRAW_SALT,
+                                 n_actions=self._partner_n_actions, out=actions)
+
+    def _snapshot(self):
+        s = [self.env.state, self.ret_sparse, self.ret_mixed, self._draw_counter]
+        if self.partner is not None:
+            s += [self.partner_seat, self._partner_counter, self._seat_counter]
+        return [t.clone() for t in s], s
+
+    @staticmethod
+    def _restore(snap):
+        for saved, live in zip(*snap):
+            live.copy_(saved)
 
     def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None):
         """(scores float32 [2N, 6] = logits, values written to ``values``) for the observations in self.obs, or None when
@@ -394,8 +510,12 @@ class SelfPlayRollout(object):
         if self.native_glue:
             if not self.fused_tail:
                 env.sample_actions(scores, self._draw_counter, seed=self.seed, out=self.actions)
+            if self.partner is not None:
+                self._partner_act(self.actions)  # K10
             env.step(self.actions)  # K1 (auto-reset inside)
             env.accumulate_returns(self.ret_sparse, self.ret_mixed, self.factor)
+            if self.partner is not None:
+                self._assign_partners(env.done)
             return
         self.actions.copy_(sample_categorical(scores, self._noise).view(env.n_envs, 2))
         sparse, shaped, done, events = env.step(self.actions)  # K1 (auto-reset inside)
@@ -406,7 +526,7 @@ class SelfPlayRollout(object):
         """Advance every environment n_steps transitions; returns the number of env-steps done."""
         if self.use_graph and self.graph is None:
             # warm-up + capture must not advance the environments: snapshot, then restore
-            saved = (self.env.state.clone(), self.ret_sparse.clone(), self.ret_mixed.clone(), self._draw_counter.clone())
+            saved = self._snapshot()
             s = torch.cuda.Stream(self.env.device)
             s.wait_stream(torch.cuda.current_stream(self.env.device))
             with torch.cuda.stream(s):
@@ -416,7 +536,7 @@ class SelfPlayRollout(object):
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph):
                 self._transition()
-            self.env.state.copy_(saved[0]), self.ret_sparse.copy_(saved[1]), self.ret_mixed.copy_(saved[2]), self._draw_counter.copy_(saved[3])
+            self._restore(saved)
         for _ in range(n_steps):
             if self.graph is not None:
                 self.graph.replay()
@@ -437,8 +557,13 @@ class SelfPlayRollout(object):
                 env.sample_actions(scores, self._draw_counter, seed=self.seed, out=b.actions[t], logp_out=b.logp[t])
                 if b.logits is not None:
                     b.logits[t, :, :scores.shape[1]].copy_(scores)
+            if self.partner is not None:
+                b.partner_seat[t].copy_(self.partner_seat)
+                self._partner_act(b.actions[t])  # K10
             env.step(b.actions[t].view(env.n_envs, 2))  # K1 (auto-reset inside)
             env.record_transition(self._factor, rewards=b.rewards[t], dones=b.dones[t], ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed)
+            if self.partner is not None:
+                self._assign_partners(env.done)
         if not self.fused_first_layer:
             env.lossless_state_encoding(out=self.obs)
         self._policy(actions=self._boot_actions, values=b.last_values, counter=self._boot_counter)
@@ -449,20 +574,22 @@ class SelfPlayRollout(object):
         seed and counter), and return them as a ``SampleBatch`` with GAE(gamma, lam) advantages.  The batch's tensors are
         reused: the next collect() with the same n_steps / keep_logits overwrites them.  With use_graph the whole window
         is one CUDA graph (captured once per n_steps / keep_logits; a new gamma or lam re-captures it); no host
-        synchronisation otherwise."""
+        synchronisation otherwise.  With a partner, the batch's ``partner_seat`` / ``learner_mask`` say which rows were the
+        partner's; their actions are the partner's, their logp / values / advantages are the PPO network's and meaningless.
+        A seat changes hands only at a done, where GAE cuts, so a learner row's advantages never read a partner step."""
         assert self.native_glue, "collect() runs on the native draw / reward kernels (native_glue=True)"
         assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
         key = (int(n_steps), bool(keep_logits))
         b = self._batches.get(key)
         if b is None:
-            b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits)
+            b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits, partner=self.partner is not None)
         if not self.use_graph:
             self._collect_window(b, n_steps, gamma, lam)
             return b
         g = self._collect_graphs.get(key)
         if g is None or g[0] != (gamma, lam):
             # warm-up + capture must not advance the environments: snapshot, then restore
-            saved = (self.env.state.clone(), self.ret_sparse.clone(), self.ret_mixed.clone(), self._draw_counter.clone())
+            saved = self._snapshot()
             s = torch.cuda.Stream(self.env.device)
             s.wait_stream(torch.cuda.current_stream(self.env.device))
             with torch.cuda.stream(s):
@@ -471,7 +598,7 @@ class SelfPlayRollout(object):
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 self._collect_window(b, n_steps, gamma, lam)
-            self.env.state.copy_(saved[0]), self.ret_sparse.copy_(saved[1]), self.ret_mixed.copy_(saved[2]), self._draw_counter.copy_(saved[3])
+            self._restore(saved)
             g = self._collect_graphs[key] = ((gamma, lam), graph)
         g[1].replay()
         return b

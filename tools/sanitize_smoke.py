@@ -148,4 +148,25 @@ for r in (sp, sp2):
     assert np.array_equal(b.advantages.cpu().numpy(), adv) and np.array_equal(b.value_targets.cpu().numpy(), tgt)
 torch.cuda.synchronize()
 print("K8 / draw with logp, record_transition, GAE through collect() ok", flush=True)
+# the BC partner: K10 (featurize_state + MLP + draw) and the seat draw, alone and through collect()
+from overcooked_ai_b200.selfplay import BCPolicy  # noqa: E402
+
+bc = BCPolicy().cuda()
+seat = torch.from_numpy(rng.randint(-1, 2, size=n).astype(np.int32)).cuda()
+acts = torch.full((n, 2), 9, dtype=torch.int32, device="cuda")
+scores = torch.zeros((n, 8), dtype=torch.float32, device="cuda")
+env.partner_actions(bc.tables(), seat, torch.zeros(2, dtype=torch.int64, device="cuda"), seed=5, out=acts, scores=scores)
+sh = seat.cpu().numpy()
+a_np = acts.cpu().numpy()
+assert (a_np[sh >= 0, sh[sh >= 0]] < 6).all() and (a_np[sh < 0] == 9).all()
+feat = env.featurize_state(num_pots=2)[torch.arange(n, device="cuda"), seat.clamp(min=0).long()]
+want = bc(feat)
+assert ((scores[seat >= 0, :6] - want[seat >= 0]).abs() <= 0.05 * (1 + want[seat >= 0].abs())).all()  # bf16 operands
+factor = torch.full((1,), 0.5, dtype=torch.float32, device="cuda")
+env.assign_partners(seat, factor, torch.zeros(2, dtype=torch.int64, device="cuda"), seed=6, done=env.done)
+sp3 = SelfPlayRollout(env, model=sp.model, use_graph=False, seed=3, partner=bc, bc_factor=0.5)
+b = sp3.collect(12, 0.99, 0.95)
+assert b.learner_mask.shape == (12, 2 * n) and int(b.learner_mask.sum()) >= 12 * n
+torch.cuda.synchronize()
+print("K10 partner policy, assign_partners, collect() with a partner ok", flush=True)
 print("sanitize_smoke: all ok")
