@@ -74,6 +74,7 @@ class BatchedOvercookedEnv(object):
             self.device = torch.device("cuda", torch.cuda.current_device())
         self.layouts = _as_layouts(layouts, mdp_params)
         self.n_layouts = len(self.layouts)
+        self._longest_cook = max(int(l.cook_time.max()) for l in self.layouts)  # bounds the cook-time-remaining plane
         self.n_envs = int(n_envs)
         self.horizon = int(horizon) if horizon < 2**31 else 0
         self.auto_reset = bool(auto_reset)
@@ -367,7 +368,16 @@ class BatchedOvercookedEnv(object):
         reference's RLlib consumer casts to), bfloat16, uint8 or int32.  ``view_swap`` (int32 CUDA tensor [N]):
         where non-zero, ``out[env, 0]`` is player 1's view (primary-agent-first order of the gym wrapper).
         ``states``: encode these records (int32 CUDA tensor [M, S], e.g. gathered from a ``selfplay.SampleBatch``)
-        instead of ``self.state``; the result is then [M, 2, W, H, 26] and every layout must share one grid shape."""
+        instead of ``self.state``; the result is then [M, 2, W, H, 26] and every layout must share one grid shape.
+        uint8 holds every value reachable play produces when no cook time exceeds 255 (the cook-time-remaining plane is
+        the only one above 3), and is refused (ValueError) for a batch with a longer cook time.  A hand-built over-cooked
+        soup (tick > cook time) has a negative cook time remaining (``MDP:2498-2513``), which uint8 cannot hold: its
+        plane value is stored modulo 256."""
+        out_dtypes = {o.dtype for o in (out if isinstance(out, (list, tuple)) else [out]) if o is not None}
+        if torch.uint8 in out_dtypes or (out is None and dtype == torch.uint8):
+            if self._longest_cook > 255:
+                raise ValueError("lossless_state_encoding: a cook time of %d does not fit uint8 (at most 255); use int32, "
+                                 "float32 or bfloat16" % self._longest_cook)
         rows = self.n_envs if states is None else states.shape[0]
         if states is not None:
             assert states.dtype == torch.int32 and states.is_cuda and states.is_contiguous() and states.dim() == 2 and \

@@ -37,6 +37,7 @@ OBJ_MASK = 0x3FFFFF
 MAX_TICK = 16382
 MAX_POTS = 4
 MAX_SLOTS = 124
+MAX_FREE = 128
 NO_SLOT = 0xFF
 LAYOUT_OLD_DYNAMICS = 1
 SUPPORTED_STATE_WORDS = (16, 32, 64, 128)
@@ -273,6 +274,8 @@ class CompiledLayout(object):
             raise ValueError("layout %r has %d pots (max %d)" % (layout_name, self.n_pots, MAX_POTS))
         if self.n_slots > MAX_SLOTS:
             raise ValueError("layout %r has %d object cells (max %d)" % (layout_name, self.n_slots, MAX_SLOTS))
+        if len(self.terrain_pos_dict[" "]) > MAX_FREE:  # free_pos[128] of the table: random start positions draw from it
+            raise ValueError("layout %r has %d floor cells (max %d)" % (layout_name, len(self.terrain_pos_dict[" "]), MAX_FREE))
         self.state_words = next(s for s in SUPPORTED_STATE_WORDS if s >= 4 + self.n_slots)
 
         # ---- recipe tables ----
@@ -359,8 +362,6 @@ class CompiledLayout(object):
             sp[i] = pos_byte(p)
         rec["slot_pos"] = sp
         free = self.terrain_pos_dict[" "]
-        if len(free) > 128:
-            raise ValueError("layout %r has %d floor cells (max 128)" % (self.layout_name, len(free)))
         rec["n_free"] = len(free)
         fp = np.zeros(128, np.uint8)
         for i, p in enumerate(free):

@@ -42,11 +42,12 @@ def _features(env, states):
 
 
 def _heads(feats, ops):
-    """bf16(features) -> the BC MLP with K8's roundings (ReLU, no input activation); asserts the exactness premise."""
+    """bf16(features) -> the BC MLP with K8's roundings (ReLU, no input activation); asserts the exactness premise.  K10
+    stages the features in bfloat16 (DESIGN §4, K10 "Exactness"): features above 256 (a cook time remaining) are rounded to
+    nearest even there, and so they are here."""
     w1, b1, wh, bh, wo, bo = ops
-    s, certs = P.k8_reference(feats, w1, b1, wh, bh, wo, bo, 1.0, 0.0)
+    s, certs = P.k8_reference(P.bf16(feats), w1, b1, wh, bh, wo, bo, 1.0, 0.0)
     assert all(c.holds() for c in certs), "premise: the operands are not exact in float32"
-    assert (np.abs(feats) <= 256).all(), "premise: the features are exact in bfloat16"
     return s
 
 
@@ -117,6 +118,38 @@ def test_k10_exact_on_random_rollouts(layout, n):
             _k10_check(env, seats, _bc_operands(rng, n_hidden), n_actions, seed=n_actions, step=n_hidden * 7 + n_actions)
     _k10_check(env, np.full(n, -1, np.int32), _bc_operands(rng, 1), 6)
     _k10_check(env, np.ones(n, np.int32), _bc_operands(rng, 1), 6)
+
+
+def test_k10_exact_on_l16_features_above_256():
+    """K10 on a 16x16 layout with 4 pots, of which featurize_state (num_pots = 2) shows the 2 nearest, and cook times up to
+    16382: features above 256 that bfloat16 cannot hold reach the first layer rounded to nearest even."""
+    import limit_layouts as LL
+    from overcooked_ai_b200 import layout as L
+
+    lay = LL.l16()
+    n = 601
+    env = BatchedOvercookedEnv(lay, n, horizon=60, auto_reset=True, random_start_pos=True, rnd_obj_prob_thresh=0.8, seed=5)
+    rng = np.random.RandomState(1)
+    acts = rng.randint(0, 6, size=(40, n, 2)).astype(np.int32)
+    acts[rng.rand(40, n, 2) < 0.4] = 5
+    env.rollout(torch.from_numpy(acts).cuda())
+    st = _np(env.state).copy()
+    hand = np.stack([L.pack_state(lay, s, 0, env.state_words) for s in LL.l16_states(lay).values()])
+    st[::40][:len(hand)] = hand
+    env.state.copy_(torch.from_numpy(st))
+    feats = _features(env, st).reshape(-1, 96)
+    big = np.flatnonzero(np.abs(feats).max(0) > 256)  # the pots' cook time remaining, in both blocks
+    assert len(big) and (P.bf16(feats) != feats).any(), "premise: some features are not exact in bfloat16"
+    for n_hidden in (0, 1, 2):
+        ops = list(_bc_operands(rng, n_hidden))
+        ops[0] = ops[0].copy()
+        ops[0][:, big] *= 2.0 ** -6  # keeps every accumulation exact with inputs up to 16384
+        assert (ops[0][:, big] != 0).any()
+        w1 = ops[0]
+        assert not np.array_equal(feats @ w1.T, P.bf16(feats) @ w1.T), "premise: the rounding reaches the first layer"
+        seats = rng.randint(-1, 2, size=n).astype(np.int32)
+        seats[::40] = rng.randint(0, 2, size=len(seats[::40]))
+        _k10_check(env, seats, tuple(ops), 6, seed=3, step=n_hidden)
 
 
 def test_k10_draw_step_past_2_to_the_32():
