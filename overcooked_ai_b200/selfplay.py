@@ -1,25 +1,21 @@
-"""Self-play rollout collection with a torch policy on top of the batched engine (BASELINE config 5).
+"""Self-play rollout collection with the PPO policy in the loop on top of the batched engine (BASELINE config 5).
 
 The reference collects PPO rollouts with Ray workers that each run one Python env and a TF copy of
 the policy (human_aware_rl/rllib/rllib.py:293-342, ppo/ppo_rllib.py:7-80).  Here one process per GPU
 keeps N environments on the device and runs, per transition,
 
-    lossless_state_encoding (K2, [N,2,W,H,26])  ->  policy CNN (torch)  ->  sampling
-    ->  ovc_step (K1)  ->  reward accumulation
+    K7 (encoding + first layer + leaky ReLU from the packed records)  ->  K9 (the two wide layers)
+    ->  K8 (dense tail + heads + action draw)  ->  ovc_step (K1)  ->  reward accumulation
 
-or, with the dense bf16 policy, K7 in place of K2 + the first layer: encoding, first layer and its leaky ReLU evaluated
-from the packed records (``ovc_encode_linear``), the observation tensor never written
-
-with no host round trip; the whole transition can be captured in one CUDA graph.  The observation
-tensor is consumed zero-copy: ``[N,2,W,H,26]`` viewed as ``(2N, 26, W, H)`` is exactly torch's
-channels-last memory format.
+with no host round trip; the whole transition can be captured in one CUDA graph.  Where a grid or a dtype does not suit
+a fused kernel, its layers run as library GEMMs instead: K2 then writes the observation ``[N,2,W,H,26]`` (consumed
+zero-copy as ``[2N, W*H*26]``), and without K8 the draw is its own kernel (``ovc_sample_actions``).
 
 The policy is shaped like the reference's ``RllibPPOModel`` defaults (ppo_rllib.py:43-79 with
 ppo_rllib_client.py:85-88: conv 5x5x25 'same', conv 3x3x25 'same', conv 3x3x25 'valid', 3 dense layers
 of 64, leaky ReLU, heads 6 + 1), random init, shared by both agents.  ``RllibShapedCNN`` is that model in torch
-(the consumer a user brings: cuDNN / cuBLAS); ``DenseGridPolicy`` is the same function as one matrix per layer, and
-on a 5x4 grid ``SelfPlayRollout`` evaluates it entirely with this library's kernels: K7 (encoding + first layer from
-the packed records), K9 (the two wide layers, wgmma), K8 (dense tail + heads + action draw).
+(the module a user trains and loads weights into); ``DenseGridPolicy`` is the same function as one matrix per layer,
+the network ``SelfPlayRollout`` evaluates: on a 5x4 grid entirely with this library's kernels K7, K9 and K8.
 """
 import torch
 import torch.nn as nn
@@ -242,15 +238,6 @@ class BCPolicy(nn.Module):
         return bf(d[0].weight), f32(d[0].bias), bf(wh), f32(bh), bf(wo), f32(bo)
 
 
-def sample_categorical(logits, noise):
-    """One draw per row from softmax(logits) by the Gumbel-max rule: argmax_i (logit_i - log E_i) with E_i ~ Exp(1) picks i
-    with probability softmax(logits)_i — four small kernels where softmax + ``torch.multinomial`` launch about twenty.
-    ``logits`` (float32) is overwritten with the perturbed scores, ``noise`` is scratch of
-    the same shape."""
-    logits.sub_(noise.exponential_().log_())
-    return torch.argmax(logits, dim=-1)
-
-
 class SampleBatch(object):
     """One window of T self-play transitions as a PPO learner consumes it (RLlib's per-agent ``SampleBatch``), on the device.
     Agent rows are ``2 env + agent``, so ``actions[t].view(N, 2)`` is the joint action ``ovc_step`` took.
@@ -307,61 +294,50 @@ PARTNER_SEAT_SALT = 0xD1B54A32D192ED03
 
 class SelfPlayRollout(object):
     """Policy-in-the-loop rollout: both agents of every environment act from the same network, or, with a BC ``partner``,
-    one seat of an environment is the partner's in the episodes the seat draw gives it (PPO_BC)."""
+    one seat of an environment is the partner's in the episodes the seat draw gives it (PPO_BC).  The network evaluated is
+    ``DenseGridPolicy`` of ``model``: K7 / K9 / K8 where they fit, library GEMMs and the draw kernel elsewhere."""
 
     def __init__(self, env, model=None, autocast_dtype=torch.bfloat16, use_graph=True, reward_shaping_factor=1.0,
-                 obs_dtype=None, dense=True, sub_batches=1, fused_first_layer=None, native_glue=True, seed=0, fused_tail=None, fused_wide=None,
-                 partner=None, bc_factor=0.0):
-        """obs_dtype: element type K2 writes (default: bfloat16 when the policy runs in bf16 — the plane values are exact
-        in bf16 and the conversion pass disappears — else float32).
-        dense: evaluate the network through ``DenseGridPolicy`` (one library GEMM per layer, widths padded to 16-byte rows,
-        weights held in ``autocast_dtype``: what autocast computes, without its per-call weight casts) instead of cuDNN
-        convolutions under autocast.
-        sub_batches: the policy runs over this many row blocks one after the other, so that a block's activations
-        (rows x 512 bf16) are still in L2 when the activation pass and the next layer read them.
-        fused_first_layer (default: on for the dense bf16 policy): the observation is never materialised — kernel K7
+                 fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0):
+        """autocast_dtype: the dtype of the dense model (``DenseGridPolicy``, widths padded to 16-byte rows) and of the
+        observation K2 writes for it: bfloat16 (the plane values are exact in bf16), or None for float32 throughout.
+        fused_first_layer (default: on for the bf16 policy): the observation is never materialised — kernel K7
         (``env.encoded_linear``) evaluates encoding + first layer + leaky ReLU from the packed records, and the library
         GEMMs start at the second layer.
-        native_glue: the joint action is drawn by ``ovc_sample_actions`` (Gumbel-max on Philox draws keyed by ``seed``,
-        one kernel) and the rewards are folded into the returns by ``ovc_accumulate_returns`` (one kernel) instead of five
-        and four tensor-library kernels.
-        fused_tail (default: with native_glue on the dense bf16 policy): the dense layers of 64, the heads and the draw run as
-        ONE kernel (``ovc_policy_tail``, K8) on the last convolution's pre-activation; the library GEMMs are then only the
-        two wide layers.
+        fused_tail (default: on for the bf16 policy): the dense layers of 64, the heads and the draw run as ONE kernel
+        (``ovc_policy_tail``, K8) on the last convolution's pre-activation; the library GEMMs are then only the two wide
+        layers.  Without it the joint action is drawn by ``ovc_sample_actions`` (Gumbel-max on Philox draws keyed by
+        ``seed``, one kernel).
         fused_wide (default: with K7 and K8 when the wide layers are 512 -> 512 -> 160, i.e. on 5x4 grids): those two layers
         run as ONE wgmma kernel (``ovc_wide_layers``, K9: the 512-wide activation stays in registers) — the
         whole policy is then K7 -> K9 -> K8, no library call.
         partner: a ``BCPolicy`` that plays next to the PPO agent (PPO_BC, human_aware_rl's OvercookedMultiAgent): at every
         episode start (and for every environment at construction) an environment gets the partner with probability
         ``bc_factor``, in seat 0 or 1 with equal probability (``env.assign_partners``); per transition K10
-        (``env.partner_actions``) overwrites that seat's action after the PPO policy drew both.  Needs native_glue.
+        (``env.partner_actions``) overwrites that seat's action after the PPO policy drew both.
         bc_factor: see the property."""
         assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
+        assert autocast_dtype in (torch.bfloat16, None), "the dense model runs in bfloat16, or in float32 with None"
         self.env = env
         l = env.layouts[0]
         self.W, self.H = l.width, l.height
         dev = env.device
-        self.model = (model or RllibShapedCNN(self.W, self.H)).to(dev).to(memory_format=torch.channels_last).eval()
+        self.model = (model or RllibShapedCNN(self.W, self.H)).to(dev).eval()
         self.autocast_dtype = autocast_dtype
-        self.dense_model = None
-        if dense:
-            self.dense_model = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(dev).eval()
-            if autocast_dtype is not None:
-                self.dense_model = self.dense_model.to(autocast_dtype)
-        k7_ok, k9_ok, k8_ok = fused_kernel_support(self.dense_model, self.W, self.H) if dense else (False, False, False)
+        self.dense_model = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(dev).eval()
+        if autocast_dtype is not None:
+            self.dense_model = self.dense_model.to(autocast_dtype)
+        bf16 = autocast_dtype == torch.bfloat16
+        k7_ok, k9_ok, k8_ok = fused_kernel_support(self.dense_model, self.W, self.H)
         if fused_first_layer is None:
-            fused_first_layer = dense and autocast_dtype == torch.bfloat16 and k7_ok
-        assert not fused_first_layer or (dense and autocast_dtype == torch.bfloat16 and k7_ok), \
-            "K7 feeds the dense bf16 policy (first layer width a multiple of 64, table within shared memory)"
+            fused_first_layer = bf16 and k7_ok
+        assert not fused_first_layer or (bf16 and k7_ok), \
+            "K7 feeds the bf16 policy (first layer width a multiple of 64, table within shared memory)"
         self.fused_first_layer = bool(fused_first_layer)
         self.factor = float(reward_shaping_factor)
-        self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by collect()'s graph
+        self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by the captured graphs
         N = env.n_envs
-        if obs_dtype is None:
-            obs_dtype = torch.bfloat16 if autocast_dtype == torch.bfloat16 else torch.float32
-        if dense and autocast_dtype is not None:
-            assert obs_dtype == autocast_dtype, "the dense policy consumes K2's rows as they are"
-        self.obs = None if self.fused_first_layer else torch.empty((N, 2, self.W, self.H, 26), dtype=obs_dtype, device=dev)
+        self.obs = None if self.fused_first_layer else torch.empty((N, 2, self.W, self.H, 26), dtype=autocast_dtype or torch.float32, device=dev)
         if self.fused_first_layer:
             self._wt0, self._b0 = self.dense_model.first_layer_table()
             self._act0 = torch.empty((2 * N, self._wt0.shape[1]), dtype=torch.bfloat16, device=dev)
@@ -369,11 +345,11 @@ class SelfPlayRollout(object):
         self.ret_sparse = torch.zeros(N, dtype=torch.int64, device=dev)      # running episode return (sparse)
         self.ret_mixed = torch.zeros(N, dtype=torch.float32, device=dev)    # sparse + factor * shaped (rllib.py:328-329)
         self.values = torch.zeros((N, 2), dtype=torch.float32, device=dev)
-        self.native_glue = bool(native_glue)
+        self.native_glue = True  # the draw and the returns are always native kernels; bench.py's launch count reads this
         if fused_tail is None:
-            fused_tail = self.native_glue and dense and autocast_dtype == torch.bfloat16 and k8_ok
-        assert not fused_tail or (self.native_glue and dense and autocast_dtype == torch.bfloat16 and k8_ok), \
-            "K8 ends the dense bf16 policy (64-wide tail behind an input of a multiple of 32, <= 256)"
+            fused_tail = bf16 and k8_ok
+        assert not fused_tail or (bf16 and k8_ok), \
+            "K8 ends the bf16 policy (64-wide tail behind an input of a multiple of 32, <= 256)"
         self.fused_tail = bool(fused_tail)
         if self.fused_tail:
             self._tail = self.dense_model.tail_tables()
@@ -388,11 +364,8 @@ class SelfPlayRollout(object):
         self.seed = int(seed)
         self._draw_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of ovc_sample_actions
         self._scores8 = None  # set to a float32 [2N, 8] tensor to make K8 also write the heads (tests)
-        self._noise = torch.empty((2 * N, 6), dtype=torch.float32, device=dev)
         self._scores = torch.empty((2 * N, 6), dtype=torch.float32, device=dev)
-        self.sub_batches = int(sub_batches)
-        assert (2 * N) % self.sub_batches == 0
-        self.graph = None
+        self.graph = None          # run()'s CUDA graph of one transition
         self.use_graph = use_graph
         self._collect_graphs = {}  # (n_steps, keep_logits) -> ((gamma, lam), CUDA graph of the window)
         self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
@@ -401,7 +374,6 @@ class SelfPlayRollout(object):
         self.partner = None
         self.bc = float(bc_factor)
         if partner is not None:
-            assert self.native_glue, "the BC partner runs on the native draw / reward kernels (native_glue=True)"
             self.partner = partner.to(dev).eval()
             self._partner_tables = self.partner.tables()
             self._partner_n_actions = self.partner.logits.out_features
@@ -413,14 +385,12 @@ class SelfPlayRollout(object):
 
     @property
     def reward_shaping_factor(self):
-        """The factor of the shaped rewards (rllib.py:328-329).  Setting it takes effect in collect() without a re-capture
-        (its graph reads a device scalar); run() re-captures its graph on its next call."""
+        """The factor of the shaped rewards (rllib.py:328-329).  Setting it takes effect in run() and collect() alike,
+        without a re-capture (their graphs read a device scalar)."""
         return self.factor
 
     @reward_shaping_factor.setter
     def reward_shaping_factor(self, value):
-        if float(value) != self.factor:
-            self.graph = None
         self.factor = float(value)
         self._factor.fill_(self.factor)
 
@@ -445,16 +415,25 @@ class SelfPlayRollout(object):
         self.env.partner_actions(self._partner_tables, self.partner_seat, self._partner_counter, seed=self.seed ^ PARTNER_DRAW_SALT,
                                  n_actions=self._partner_n_actions, out=actions)
 
-    def _snapshot(self):
-        s = [self.env.state, self.ret_sparse, self.ret_mixed, self._draw_counter]
+    def _capture(self, warm_up, body):
+        """A CUDA graph of ``body``, captured after ``warm_up`` (on a side stream).  Warm-up and capture must not advance
+        the environments: the state, the returns and the draw counters are restored after them."""
+        live = [self.env.state, self.ret_sparse, self.ret_mixed, self._draw_counter]
         if self.partner is not None:
-            s += [self.partner_seat, self._partner_counter, self._seat_counter]
-        return [t.clone() for t in s], s
-
-    @staticmethod
-    def _restore(snap):
-        for saved, live in zip(*snap):
-            live.copy_(saved)
+            live += [self.partner_seat, self._partner_counter, self._seat_counter]
+        saved = [t.clone() for t in live]
+        dev = self.env.device
+        s = torch.cuda.Stream(dev)
+        s.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(s):
+            warm_up()
+        torch.cuda.current_stream(dev).wait_stream(s)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            body()
+        for t, v in zip(live, saved):
+            t.copy_(v)
+        return graph
 
     def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None):
         """(scores float32 [2N, 6] = logits, values written to ``values``) for the observations in self.obs, or None when
@@ -467,107 +446,80 @@ class SelfPlayRollout(object):
         scores8 = self._scores8 if scores8 is None else scores8
         counter = self._draw_counter if counter is None else counter
         with torch.no_grad():
-            if self.dense_model is not None:
-                if self.fused_first_layer:
-                    flat, first = env.encoded_linear(self._wt0, self._b0, out=self._act0, neg_slope=0.2), 1  # K7
-                else:
-                    flat, first = self.obs.view(rows, self.W * self.H * 26), 0
-                step = rows // self.sub_batches
-                if self.fused_tail:  # K8 draws the actions itself: nothing to return
-                    if self.fused_wide:
-                        w1, b1, w2, b2 = self._wide
-                        _native.check(_native.lib().ovc_wide_layers(flat.data_ptr(), rows, flat.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
-                                                                    w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, self._z.data_ptr(), env._stream()))
-                    else:
-                        for b in range(0, rows, step):
-                            self.dense_model.trunk(flat[b:b + step], first, out=self._z[b:b + step])
-                    w1, b1, wh, bh, wo, bo = self._tail
-                    args = (self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
-                            wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1),
-                            counter.data_ptr(), actions.data_ptr(), vals.data_ptr(), scores8.data_ptr() if scores8 is not None else 0)
-                    if logp is None:
-                        _native.check(_native.lib().ovc_policy_tail(*args, env._stream()))
-                    else:
-                        _native.check(_native.lib().ovc_policy_tail_logp(*args, logp.data_ptr(), env._stream()))
-                    return None
-                for b in range(0, rows, step):
-                    logits, value = self.dense_model.forward_from(flat[b:b + step], first)
-                    self._scores[b:b + step].copy_(logits)
-                    vals[b:b + step].copy_(value)
+            if self.fused_first_layer:
+                flat, first = env.encoded_linear(self._wt0, self._b0, out=self._act0, neg_slope=0.2), 1  # K7
             else:
-                with torch.autocast("cuda", dtype=self.autocast_dtype, enabled=self.autocast_dtype is not None):
-                    x = self.obs.view(rows, self.W, self.H, 26).permute(0, 3, 1, 2)  # (2N,26,W,H), channels-last strides
-                    logits, value = self.model(x)
+                flat, first = self.obs.view(rows, self.W * self.H * 26), 0
+            if not self.fused_tail:
+                logits, value = self.dense_model.forward_from(flat, first)
                 self._scores.copy_(logits)
                 vals.copy_(value)
-        return self._scores
+                return self._scores
+            if self.fused_wide:
+                w1, b1, w2, b2 = self._wide
+                _native.check(_native.lib().ovc_wide_layers(flat.data_ptr(), rows, flat.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
+                                                            w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, self._z.data_ptr(), env._stream()))
+            else:
+                self.dense_model.trunk(flat, first, out=self._z)
+            w1, b1, wh, bh, wo, bo = self._tail
+            args = (self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
+                    wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1),
+                    counter.data_ptr(), actions.data_ptr(), vals.data_ptr(), scores8.data_ptr() if scores8 is not None else 0)
+            if logp is None:
+                _native.check(_native.lib().ovc_policy_tail(*args, env._stream()))
+            else:
+                _native.check(_native.lib().ovc_policy_tail_logp(*args, logp.data_ptr(), env._stream()))
+        return None  # K8 has drawn the actions itself
 
-    def _transition(self):
+    def _transition(self, b=None, t=0):
+        """One transition: K2 or K7, the policy, the draw, K10 for the partner, K1 (auto-reset inside), the returns, the seat
+        draw.  Without ``b`` (run()) the actions and values go to self.actions / self.values; with a ``SampleBatch`` ``b``
+        (collect()) the transition is recorded in its slot ``t``: state, actions, values, logp, logits, rewards, dones and
+        partner seats."""
         env = self.env
+        if b is None:
+            actions, values, logp, logits, rewards, dones = self.actions, None, None, None, None, None
+        else:
+            b.states[t].copy_(env.state)
+            actions, values, logp, rewards, dones = b.actions[t], b.values[t], b.logp[t], b.rewards[t], b.dones[t]
+            logits = None if b.logits is None else b.logits[t]
         if not self.fused_first_layer:
             env.lossless_state_encoding(out=self.obs)  # K2
-        scores = self._policy()
-        if self.native_glue:
-            if not self.fused_tail:
-                env.sample_actions(scores, self._draw_counter, seed=self.seed, out=self.actions)
-            if self.partner is not None:
-                self._partner_act(self.actions)  # K10
-            env.step(self.actions)  # K1 (auto-reset inside)
-            env.accumulate_returns(self.ret_sparse, self.ret_mixed, self.factor)
-            if self.partner is not None:
-                self._assign_partners(env.done)
-            return
-        self.actions.copy_(sample_categorical(scores, self._noise).view(env.n_envs, 2))
-        sparse, shaped, done, events = env.step(self.actions)  # K1 (auto-reset inside)
-        self.ret_sparse.add_(sparse)
-        self.ret_mixed.add_(sparse).add_(shaped[:, 0], alpha=self.factor).add_(shaped[:, 1], alpha=self.factor)
+        scores = self._policy(actions=actions, values=values, logp=logp, scores8=logits)
+        if scores is not None:  # library layers: the separate draw kernel
+            env.sample_actions(scores, self._draw_counter, seed=self.seed, out=actions, logp_out=logp)
+            if logits is not None:
+                logits[:, :scores.shape[1]].copy_(scores)
+        if self.partner is not None:
+            if b is not None:
+                b.partner_seat[t].copy_(self.partner_seat)
+            self._partner_act(actions)  # K10
+        env.step(actions.view(env.n_envs, 2))  # K1 (auto-reset inside)
+        env.record_transition(self._factor, rewards=rewards, dones=dones, ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed)
+        if self.partner is not None:
+            self._assign_partners(env.done)
 
     def run(self, n_steps):
         """Advance every environment n_steps transitions; returns the number of env-steps done."""
         if self.use_graph and self.graph is None:
-            # warm-up + capture must not advance the environments: snapshot, then restore
-            saved = self._snapshot()
-            s = torch.cuda.Stream(self.env.device)
-            s.wait_stream(torch.cuda.current_stream(self.env.device))
-            with torch.cuda.stream(s):
+            def warm_up():
                 for _ in range(3):
                     self._transition()
-            torch.cuda.current_stream(self.env.device).wait_stream(s)
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self._transition()
-            self._restore(saved)
+            self.graph = self._capture(warm_up, self._transition)
+        step = self._transition if self.graph is None else self.graph.replay
         for _ in range(n_steps):
-            if self.graph is not None:
-                self.graph.replay()
-            else:
-                self._transition()
+            step()
         return n_steps * self.env.n_envs
 
     def _collect_window(self, b, n_steps, gamma, lam):
-        """n_steps transitions into slots 0.. of ``b`` (the kernels of run(), outputs in place), then the bootstrap value
-        of the state after them and GAE over the whole batch."""
-        env = self.env
+        """n_steps transitions into slots 0.. of ``b``, then the bootstrap value of the state after them and GAE over the
+        whole batch."""
         for t in range(n_steps):
-            b.states[t].copy_(env.state)
-            if not self.fused_first_layer:
-                env.lossless_state_encoding(out=self.obs)  # K2
-            scores = self._policy(actions=b.actions[t], values=b.values[t], logp=b.logp[t], scores8=None if b.logits is None else b.logits[t])
-            if scores is not None:  # library layers: the separate draw kernel
-                env.sample_actions(scores, self._draw_counter, seed=self.seed, out=b.actions[t], logp_out=b.logp[t])
-                if b.logits is not None:
-                    b.logits[t, :, :scores.shape[1]].copy_(scores)
-            if self.partner is not None:
-                b.partner_seat[t].copy_(self.partner_seat)
-                self._partner_act(b.actions[t])  # K10
-            env.step(b.actions[t].view(env.n_envs, 2))  # K1 (auto-reset inside)
-            env.record_transition(self._factor, rewards=b.rewards[t], dones=b.dones[t], ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed)
-            if self.partner is not None:
-                self._assign_partners(env.done)
+            self._transition(b, t)
         if not self.fused_first_layer:
-            env.lossless_state_encoding(out=self.obs)
+            self.env.lossless_state_encoding(out=self.obs)
         self._policy(actions=self._boot_actions, values=b.last_values, counter=self._boot_counter)
-        env.gae(b.rewards, b.values, b.dones, b.last_values, gamma, lam, b.advantages, b.value_targets)
+        self.env.gae(b.rewards, b.values, b.dones, b.last_values, gamma, lam, b.advantages, b.value_targets)
 
     def collect(self, n_steps, gamma, lam, keep_logits=False):
         """Advance every environment n_steps transitions, as run() does (the same kernels and the same draws from the same
@@ -577,7 +529,6 @@ class SelfPlayRollout(object):
         synchronisation otherwise.  With a partner, the batch's ``partner_seat`` / ``learner_mask`` say which rows were the
         partner's; their actions are the partner's, their logp / values / advantages are the PPO network's and meaningless.
         A seat changes hands only at a done, where GAE cuts, so a learner row's advantages never read a partner step."""
-        assert self.native_glue, "collect() runs on the native draw / reward kernels (native_glue=True)"
         assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
         key = (int(n_steps), bool(keep_logits))
         b = self._batches.get(key)
@@ -588,18 +539,8 @@ class SelfPlayRollout(object):
             return b
         g = self._collect_graphs.get(key)
         if g is None or g[0] != (gamma, lam):
-            # warm-up + capture must not advance the environments: snapshot, then restore
-            saved = self._snapshot()
-            s = torch.cuda.Stream(self.env.device)
-            s.wait_stream(torch.cuda.current_stream(self.env.device))
-            with torch.cuda.stream(s):
-                self._collect_window(b, 1, gamma, lam)
-            torch.cuda.current_stream(self.env.device).wait_stream(s)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                self._collect_window(b, n_steps, gamma, lam)
-            self._restore(saved)
-            g = self._collect_graphs[key] = ((gamma, lam), graph)
+            g = self._collect_graphs[key] = ((gamma, lam), self._capture(lambda: self._collect_window(b, 1, gamma, lam),
+                                                                         lambda: self._collect_window(b, n_steps, gamma, lam)))
         g[1].replay()
         return b
 
@@ -607,8 +548,6 @@ class SelfPlayRollout(object):
         """Re-fold ``self.model`` (e.g. after a learner's update) into the policy the kernels evaluate, in place: the dense
         model's parameters and the K7 / K9 / K8 tables keep their storage, so the captured graphs of run() and collect()
         use the new weights without a re-capture."""
-        if self.dense_model is None:
-            return  # the convolutions read self.model's own parameters
         with torch.no_grad():
             new = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(self.env.device)
             if self.autocast_dtype is not None:

@@ -173,10 +173,11 @@ def test_collect_is_run_plus_the_sample_batch(layout, flags):
     b = sp.collect(T, gamma, lam, keep_logits=True)
     assert np.array_equal(_np(b.states[0]), s0)
     _oracle_check(envs[0], s0, b, H, f)
-    # run() from the same seed and counter: the same draws, the same end state
+    # run() from the same seed and counter: the same draws, the same end state, the same returns
     sp_run.run(T)
     assert torch.equal(envs[2].state, envs[0].state) and torch.equal(sp_run.actions.view(-1), b.actions[T - 1])
     assert torch.equal(sp_run._draw_counter, sp._draw_counter)
+    assert torch.equal(sp_run.ret_sparse, sp.ret_sparse) and torch.equal(sp_run.ret_mixed, sp.ret_mixed)
     # eager == graph, every tensor of the batch
     be = sp_eager.collect(T, gamma, lam, keep_logits=True)
     for k in ("states", "actions", "logp", "values", "rewards", "dones", "last_values", "advantages", "value_targets", "logits"):
@@ -212,6 +213,7 @@ def test_sync_weights_and_shaping_factor_reach_the_captured_graphs():
     env = BatchedOvercookedEnv(layout, n, horizon=H, auto_reset=True)
     sp = SelfPlayRollout(env, model=model, seed=seed, reward_shaping_factor=1.0)
     sp.run(2)  # run()'s graph, captured with the first weights
+    run_graph = sp.graph
     sp.collect(T, 0.99, 0.95)
     graph = sp._collect_graphs[(T, False)][1]
     with torch.no_grad():
@@ -226,9 +228,20 @@ def test_sync_weights_and_shaping_factor_reach_the_captured_graphs():
     sp.run(1)
     a, v, _ = _fresh_eval(layout, n, H, model, s1, step, seed)
     assert np.array_equal(v, _np(sp.values).reshape(-1)) and np.array_equal(a, _np(sp.actions).reshape(-1))
-    # a new shaping factor reaches collect()'s graph without a re-capture
+    # a new shaping factor reaches collect()'s graph and run()'s without a re-capture
     sp.reward_shaping_factor = 0.25
     s2 = _np(env.state).copy()
     b = sp.collect(T, 0.99, 0.95)
     assert sp._collect_graphs[(T, False)][1] is graph
     _oracle_check(env, s2, b, H, 0.25)
+    shaped_seen = False
+    for _ in range(200):  # until a step with shaped rewards has been checked
+        before = _np(sp.ret_mixed).copy()
+        sp.run(1)
+        sh = _np(env.shaped).astype(np.float32)
+        want = before + _np(env.sparse).astype(np.float32) + np.float32(0.25) * sh[:, 0] + np.float32(0.25) * sh[:, 1]
+        assert np.array_equal(_np(sp.ret_mixed), want)
+        shaped_seen = bool(sh.any())
+        if shaped_seen:
+            break
+    assert sp.graph is run_graph and shaped_seen

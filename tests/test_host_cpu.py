@@ -507,21 +507,6 @@ def test_dense_grid_policy_is_the_same_network_as_the_cnn():
         assert torch.allclose(l1, l2, atol=1e-6) and torch.allclose(v1, v2, atol=1e-6)
 
 
-def test_sample_categorical_follows_the_softmax():
-    """selfplay.sample_categorical (Gumbel-max) draws index i with probability softmax(logits)_i."""
-    import torch
-
-    from overcooked_ai_b200.selfplay import sample_categorical
-
-    torch.manual_seed(1)
-    row = torch.tensor([0.0, 1.0, 2.0, -1.0, 0.5, -30.0])
-    n = 400000
-    a = sample_categorical(row.repeat(n, 1), torch.empty(n, 6))
-    freq = torch.bincount(a, minlength=6).double() / n
-    want = torch.softmax(row.double(), -1)
-    assert freq[5] == 0 and torch.all((freq - want).abs() < 4 * torch.sqrt(want * (1 - want) / n) + 1e-9), (freq, want)
-
-
 def test_dense_grid_policy_padding_keeps_the_function():
     """Width padding (16-byte rows for the library's tensor-core GEMM kernels) adds zero weights only; merged heads."""
     import torch
