@@ -71,14 +71,16 @@ env_steps = 0
 for it in range(args.iters):
     sp.reward_shaping_factor = max(0.0, 1.0 - env_steps / args.shaping_horizon)
     sp.bc_factor = schedule(points, env_steps)
-    ret0 = sp.ret_sparse.clone()
     t0 = time.time()
     batch = sp.collect(T, args.gamma, args.lam)
-    episodes = batch.dones.sum()
-    mean_sparse = float((sp.ret_sparse - ret0).sum()) / max(int(episodes), 1)
-    paired = float((batch.partner_seat >= 0).float().mean())
     torch.cuda.synchronize()
     t_collect = time.time() - t0
+    paired = float((batch.partner_seat >= 0).float().mean())
+    # the episodes that ended in the window, split by whether the BC partner played them
+    fin = batch.episodes.finished()
+    with_bc = fin["partner_seat"] >= 0
+    episodes = fin["env_index"].numel()
+    mean_return = lambda m: float(fin["ep_sparse_r"][m].float().mean()) if bool(m.any()) else float("nan")  # noqa: E731
     env_steps += T * N
     mask = batch.learner_mask.view(-1).float()
     adv = batch.advantages.view(-1)
@@ -109,7 +111,7 @@ for it in range(args.iters):
             opt.step()
     sp.sync_weights()
     torch.cuda.synchronize()
-    print("iter %d  bc_factor %.3f  paired env-steps %.3f  shaping %.3f  episodes %d  mean sparse return %.2f  policy loss %.4f  "
-          "value loss %.3f  entropy %.3f  collect %.2f s  learn %.2f s"
-          % (it, sp.bc_factor, paired, sp.reward_shaping_factor, int(episodes), mean_sparse, policy_loss.item(), value_loss.item(),
-             entropy.item(), t_collect, time.time() - t0), flush=True)
+    print("iter %d  bc_factor %.3f  paired env-steps %.3f  shaping %.3f  episodes %d (with BC %d)  mean sparse return: with BC %.2f, "
+          "self-play %.2f  policy loss %.4f  value loss %.3f  entropy %.3f  collect %.2f s  learn %.2f s"
+          % (it, sp.bc_factor, paired, sp.reward_shaping_factor, episodes, int(with_bc.sum()), mean_return(with_bc),
+             mean_return(~with_bc), policy_loss.item(), value_loss.item(), entropy.item(), t_collect, time.time() - t0), flush=True)

@@ -23,6 +23,7 @@ import torch.nn.functional as F
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 from overcooked_ai_b200.batched import BatchedOvercookedEnv  # noqa: E402
+from overcooked_ai_b200.layout import EVENT_TYPES  # noqa: E402
 from overcooked_ai_b200.selfplay import RllibShapedCNN, SelfPlayRollout  # noqa: E402
 
 ap = argparse.ArgumentParser()
@@ -52,13 +53,17 @@ env_steps = 0
 for it in range(args.iters):
     # the reference's linear annealing of the shaping factor (rllib.py:358-368), read by the captured graph
     sp.reward_shaping_factor = max(0.0, 1.0 - env_steps / args.shaping_horizon)
-    ret0 = sp.ret_sparse.clone()
     t0 = time.time()
     batch = sp.collect(T, args.gamma, args.lam)
-    episodes = batch.dones.sum()
-    mean_sparse = float((sp.ret_sparse - ret0).sum()) / max(int(episodes), 1)  # sparse reward per finished episode
     torch.cuda.synchronize()
     t_collect = time.time() - t0
+    # the episodes that ended in the window (TrainingCallbacks.on_episode_end's metrics, rllib.py:480-483)
+    fin = batch.episodes.finished()
+    episodes = fin["env_index"].numel()
+    mean_sparse = float(fin["ep_sparse_r"].float().mean()) if episodes else float("nan")
+    events = fin["ep_game_stats"].sum(1).float().mean(0) if episodes else torch.full((25,), float("nan"))
+    event_means = "  ".join("%s %.2f" % (k, float(events[EVENT_TYPES.index(k)]))
+                            for k in ("soup_delivery", "useful_onion_pickup", "optimal_onion_potting"))
     env_steps += T * N
     adv = batch.advantages.view(-1)
     adv = (adv - adv.mean()) / (adv.std() + 1e-8)
@@ -87,7 +92,7 @@ for it in range(args.iters):
             opt.step()
     sp.sync_weights()
     torch.cuda.synchronize()
-    print("iter %d  shaping %.3f  episodes %d  mean sparse return %.2f  first-minibatch max|ratio-1| %.4f  "
+    print("iter %d  shaping %.3f  episodes %d  mean sparse return %.2f  per episode: %s  first-minibatch max|ratio-1| %.4f  "
           "policy loss %.4f  value loss %.3f  entropy %.3f  collect %.2f s  learn %.2f s"
-          % (it, sp.reward_shaping_factor, int(episodes), mean_sparse, first_ratio, policy_loss.item(), value_loss.item(),
+          % (it, sp.reward_shaping_factor, episodes, mean_sparse, event_means, first_ratio, policy_loss.item(), value_loss.item(),
              entropy.item(), t_collect, time.time() - t0), flush=True)

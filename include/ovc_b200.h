@@ -462,6 +462,57 @@ int ovc_gae(const float *rewards, const float *values, const uint8_t *dones, con
             float gamma, float lambda, float *advantages, float *value_targets, void *stream);
 
 /*
+ * Finished episodes on the device: the per-episode statistics the reference's env reports at an episode's end
+ * (OvercookedEnv.game_stats and the info dict's "episode" entry, overcooked_env.py:363-401; logged by human_aware_rl's
+ * TrainingCallbacks.on_episode_end, rllib.py:480-483), kept in the same kernel as ovc_record_transition.
+ *
+ * ovc_episode_stats_t: device pointers (the struct itself is passed by HOST pointer).  Running state, one entry per env:
+ *   event_counts int32 [n_envs][2][25], sparse_by_agent / shaped_by_agent int64 [n_envs][2], reward_by_agent float32
+ *   [n_envs][2] (nullable), ep_length int32 [n_envs], layout_id int32 [n_envs] (the running episode's layout; initialise it
+ *   from word 3 of the records).  Records: slot k of env e is entry [k][e] of every rec_* array ([capacity][n_envs][...]);
+ *   count / dropped int32 [n_envs] (zero them to clear the buffer).  capacity >= 0; the rec_* pointers may be NULL when it
+ *   is 0, rec_reward_by_agent when reward_by_agent is.
+ * ovc_record_transition_stats: ovc_record_transition, and per env e, in this order:
+ *     d_i = events[e][i] bit 15 (soup_delivery) ? layouts[layout_id[e]].deliver_value[events[e][i] bits 25-28] : 0
+ *     sparse_by_agent[e][i] += d_i;  shaped_by_agent[e][i] += shaped[e][i];  ep_length[e] += 1
+ *     event_counts[e][i][b] += 1 for every set bit b < 25 of events[e][i]
+ *     reward_by_agent[e][i] = reward_by_agent[e][i] + rewards_i (float32, rewards_i as ovc_record_transition defines them,
+ *       with the factor of this call)
+ *     L = layout_id[e];  layout_id[e] = state[e][3] & 0xFF   (the record after the step: a new episode's layout)
+ *     if done[e]:  k = count[e];  if k < capacity: slot k <- (ep_length, L, partner_seat ? partner_seat[e] : -1, sparse,
+ *                  shaped, event counts, reward), count[e] = k + 1;  else dropped[e] += 1;  then the running state is zeroed.
+ *   One thread per env claims its slots without atomics, so the slot order is deterministic (the event counts, each
+ *   owned by one thread, are updated with atomic adds only so that they do not wait for memory).  state: the records ovc_step left ([n_envs][state_words]), events: its
+ *   int32 [n_envs][2] output; layouts: the table it ran on.
+ */
+typedef struct ovc_episode_stats {
+    const void *layouts;
+    const int32_t *state;
+    const int32_t *events;
+    const int32_t *partner_seat; /* nullable: the partner's seat in the ending episode, -1 = self-play */
+    int32_t *event_counts;
+    int64_t *sparse_by_agent;
+    int64_t *shaped_by_agent;
+    float *reward_by_agent; /* nullable */
+    int32_t *ep_length;
+    int32_t *layout_id;
+    int32_t *count;
+    int32_t *dropped;
+    int32_t *rec_length;
+    int32_t *rec_layout;
+    int32_t *rec_partner_seat;
+    int64_t *rec_sparse_by_agent;
+    int64_t *rec_shaped_by_agent;
+    int32_t *rec_event_counts;
+    float *rec_reward_by_agent;
+    int32_t capacity;
+    int32_t state_words;
+} ovc_episode_stats_t; /* 160 bytes */
+int ovc_record_transition_stats(const int32_t *sparse, const int32_t *shaped, const int32_t *done, const float *factor, int64_t n_envs,
+                                float *rewards, uint8_t *dones, int64_t *ret_sparse, float *ret_mixed, const ovc_episode_stats_t *stats,
+                                void *stream);
+
+/*
  * ovc_policy_tail: the narrow end of the rollout policy and the action draw in one kernel (reference model:
  * human_aware_rl/ppo/ppo_rllib.py:64-79 — dense layers of 64 after the convolutions, then the action / value heads):
  *   a = leaky_relu(x, in_slope)                          x bfloat16 [n_rows][k0], k0 a multiple of 32 in 32..256

@@ -457,17 +457,46 @@ class BatchedOvercookedEnv(object):
                                                        0 if ret_sparse is None else ret_sparse.data_ptr(),
                                                        0 if ret_mixed is None else ret_mixed.data_ptr(), self._stream()))
 
-    def record_transition(self, factor, rewards=None, dones=None, ret_sparse=None, ret_mixed=None):
+    def record_transition(self, factor, rewards=None, dones=None, ret_sparse=None, ret_mixed=None, stats=None, records=None,
+                          partner_seat=None):
         """What a sample batch keeps of the last ``step`` (ovc_record_transition, one kernel): ``rewards`` float32 [N, 2] =
         sparse + factor * shaped[:, i] per agent (rllib.py:328-329), ``dones`` uint8 [N], and the running returns as
         ``accumulate_returns`` keeps them; each output optional.  ``factor``: float32 CUDA scalar tensor, read by the
-        kernel (a captured graph follows its current value)."""
+        kernel (a captured graph follows its current value).
+        ``stats`` (an ``EpisodeStats``) with ``records`` (an ``EpisodeRecords``): in the same kernel
+        (ovc_record_transition_stats), fold the step into the running episode statistics and write every episode that
+        ended with it into ``records``; ``partner_seat`` (int32 [N], nullable): the partner's seat each episode was played
+        with, -1 = self-play."""
+        self._record(self.sparse, self.shaped, self.done, self.events, factor, rewards, dones, ret_sparse, ret_mixed, stats, records,
+                     partner_seat)
+
+    def _record(self, sparse, shaped, done, events, factor, rewards=None, dones=None, ret_sparse=None, ret_mixed=None, stats=None,
+                records=None, partner_seat=None):
         assert factor.is_cuda and factor.dtype == torch.float32 and factor.numel() == 1
         for t, dt, n in ((rewards, torch.float32, 2), (dones, torch.uint8, 1), (ret_sparse, torch.int64, 1), (ret_mixed, torch.float32, 1)):
             assert t is None or (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n * self.n_envs)
         ptr = lambda t: 0 if t is None else t.data_ptr()
-        _native.check(self._lib.ovc_record_transition(self.sparse.data_ptr(), self.shaped.data_ptr(), self.done.data_ptr(), factor.data_ptr(),
-                                                      self.n_envs, ptr(rewards), ptr(dones), ptr(ret_sparse), ptr(ret_mixed), self._stream()))
+        if stats is None:
+            assert records is None and partner_seat is None, "records and partner_seat go with stats"
+            _native.check(self._lib.ovc_record_transition(sparse.data_ptr(), shaped.data_ptr(), done.data_ptr(), factor.data_ptr(),
+                                                          self.n_envs, ptr(rewards), ptr(dones), ptr(ret_sparse), ptr(ret_mixed), self._stream()))
+            return
+        assert stats.env is self and records is not None and records.env is self, "stats and records of this environment"
+        for t, n in ((sparse, 1), (shaped, 2), (done, 1), (events, 2), (partner_seat, 1)):
+            assert t is None or (t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n * self.n_envs)
+        d = _native.EpisodeStatsDesc()
+        d.layouts, d.state, d.events, d.partner_seat = self.tables.data_ptr(), self.state.data_ptr(), events.data_ptr(), ptr(partner_seat)
+        d.event_counts, d.sparse_by_agent = stats.event_counts.data_ptr(), stats.cumulative_sparse_rewards_by_agent.data_ptr()
+        d.shaped_by_agent, d.reward_by_agent = stats.cumulative_shaped_rewards_by_agent.data_ptr(), stats.ep_reward_by_agent.data_ptr()
+        d.ep_length, d.layout_id = stats.ep_length.data_ptr(), stats.layout_id.data_ptr()
+        d.count, d.dropped, d.capacity, d.state_words = records.count.data_ptr(), records.dropped.data_ptr(), records.capacity, self.state_words
+        if records.capacity:
+            d.rec_length, d.rec_layout, d.rec_partner_seat = records.length.data_ptr(), records.layout.data_ptr(), records.partner_seat.data_ptr()
+            d.rec_sparse_by_agent, d.rec_shaped_by_agent = records.sparse_r_by_agent.data_ptr(), records.shaped_r_by_agent.data_ptr()
+            d.rec_event_counts, d.rec_reward_by_agent = records.game_stats.data_ptr(), records.reward_by_agent.data_ptr()
+        _native.check(self._lib.ovc_record_transition_stats(sparse.data_ptr(), shaped.data_ptr(), done.data_ptr(), factor.data_ptr(),
+                                                            self.n_envs, ptr(rewards), ptr(dones), ptr(ret_sparse), ptr(ret_mixed),
+                                                            ctypes.byref(d), self._stream()))
 
     def gae(self, rewards, values, dones, last_values, gamma, lam, advantages=None, value_targets=None):
         """Generalized advantage estimation over a window (ovc_gae; include/ovc_b200.h gives the recurrence): rewards /
@@ -744,6 +773,11 @@ class EpisodeStats(object):
     ``cumulative_sparse_rewards_by_agent[N, 2]``, ``cumulative_shaped_rewards_by_agent[N, 2]`` and ``ep_length[N]``.
     ``update`` returns the finished environments' statistics (a dict of tensors, rows selected by ``done``) and
     clears them for the next episode.
+
+    The running state is kept by the kernel of ``env.record_transition(..., stats=, records=)``
+    (ovc_record_transition_stats), which also sums ``ep_reward_by_agent[N, 2]`` (float32, the per-agent rewards
+    ``sparse + factor * shaped_i`` of that call; ``update`` uses factor 1) and keeps ``layout_id[N]``, the layout each
+    running episode is played on (it changes at resets with random_layout).
     """
 
     def __init__(self, env):
@@ -752,33 +786,78 @@ class EpisodeStats(object):
         self.event_counts = torch.zeros((N, 2, 25), dtype=torch.int32, device=dev)
         self.cumulative_sparse_rewards_by_agent = torch.zeros((N, 2), dtype=torch.int64, device=dev)
         self.cumulative_shaped_rewards_by_agent = torch.zeros((N, 2), dtype=torch.int64, device=dev)
+        self.ep_reward_by_agent = torch.zeros((N, 2), dtype=torch.float32, device=dev)
         self.ep_length = torch.zeros(N, dtype=torch.int32, device=dev)
-        self._bits = torch.arange(25, device=dev, dtype=torch.int32)
-        self._lid = env.layout_ids()  # layouts of the running episodes (they change at resets with random_layout)
+        self.layout_id = env.layout_ids()
+        self._records = None  # update()'s one-slot record buffer
+        self._one = None
+
+    def state_tensors(self):
+        """The running state, every tensor the kernel writes."""
+        return [self.event_counts, self.cumulative_sparse_rewards_by_agent, self.cumulative_shaped_rewards_by_agent, self.ep_reward_by_agent,
+                self.ep_length, self.layout_id]
 
     def update(self, sparse, shaped, done, events):
         """Feed the outputs of one step() (tensors [N], [N,2], [N], [N,2]); call it after EVERY step."""
-        self.cumulative_sparse_rewards_by_agent += self.env.sparse_by_agent(events, self._lid)
-        if self.env.random_layout:
-            self._lid = self.env.layout_ids()
-        self.cumulative_shaped_rewards_by_agent += shaped
-        self.event_counts += (events.unsqueeze(-1) >> self._bits) & 1
-        self.ep_length += 1
+        if self._records is None:
+            self._records = EpisodeRecords(self.env, 1)
+            self._one = torch.ones(1, dtype=torch.float32, device=self.env.device)
+        r = self._records
+        r.clear()
+        self.env._record(sparse, shaped, done, events, self._one, stats=self, records=r)
         d = done != 0
         finished = None
         if bool(d.any()):
             idx = torch.nonzero(d).squeeze(1)
             finished = {
                 "env_index": idx,
-                "ep_game_stats": self.event_counts[idx].clone(),
-                "ep_sparse_r_by_agent": self.cumulative_sparse_rewards_by_agent[idx].clone(),
-                "ep_shaped_r_by_agent": self.cumulative_shaped_rewards_by_agent[idx].clone(),
-                "ep_sparse_r": self.cumulative_sparse_rewards_by_agent[idx].sum(1),
-                "ep_shaped_r": self.cumulative_shaped_rewards_by_agent[idx].sum(1),
-                "ep_length": self.ep_length[idx].clone(),
+                "ep_game_stats": r.game_stats[0, idx],
+                "ep_sparse_r_by_agent": r.sparse_r_by_agent[0, idx],
+                "ep_shaped_r_by_agent": r.shaped_r_by_agent[0, idx],
+                "ep_sparse_r": r.sparse_r_by_agent[0, idx].sum(1),
+                "ep_shaped_r": r.shaped_r_by_agent[0, idx].sum(1),
+                "ep_length": r.length[0, idx],
             }
-            self.event_counts[idx] = 0
-            self.cumulative_sparse_rewards_by_agent[idx] = 0
-            self.cumulative_shaped_rewards_by_agent[idx] = 0
-            self.ep_length[idx] = 0
         return finished
+
+
+class EpisodeRecords(object):
+    """The episodes that finished, kept on the device by ``env.record_transition(..., stats=, records=)``: struct-of-arrays
+    tensors ``[capacity, N, ...]`` where slot ``k`` of environment ``e`` is its ``k``-th episode to end since ``clear()``.
+
+    length int32, layout int32 (the layout id the episode was played on), partner_seat int32 (-1: self-play),
+    sparse_r_by_agent / shaped_r_by_agent int64 [.., 2], game_stats int32 [.., 2, 25] (event counts, the ``len()`` of the
+    reference's game_stats lists), reward_by_agent float32 [.., 2] (the sum of the per-agent rewards of the episode);
+    count int32 [N] (episodes written per environment), dropped int32 [N] (episodes that ended with the buffer full,
+    not written)."""
+
+    def __init__(self, env, capacity):
+        self.env = env
+        self.capacity = int(capacity)
+        assert self.capacity >= 0
+        C, N, dev = self.capacity, env.n_envs, env.device
+        z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
+        self.length, self.layout, self.partner_seat = (z((C, N), torch.int32) for _ in range(3))
+        self.sparse_r_by_agent, self.shaped_r_by_agent = z((C, N, 2), torch.int64), z((C, N, 2), torch.int64)
+        self.game_stats = z((C, N, 2, 25), torch.int32)
+        self.reward_by_agent = z((C, N, 2), torch.float32)
+        self._counters = z((2, N), torch.int32)  # count and dropped: one memset clears both
+        self.count, self.dropped = self._counters[0], self._counters[1]
+
+    def tensors(self):
+        return [self.length, self.layout, self.partner_seat, self.sparse_r_by_agent, self.shaped_r_by_agent, self.game_stats,
+                self.reward_by_agent, self._counters]
+
+    def clear(self):
+        """Forget every record (stream ordered, one memset: capturable in a CUDA graph)."""
+        self._counters.zero_()
+
+    def finished(self):
+        """The records as a dict of tensors in the keys of the reference's episode info (overcooked_env.py:363-401) and of
+        ``EpisodeStats.update``: env_index, ep_game_stats, ep_sparse_r(_by_agent), ep_shaped_r(_by_agent), ep_length, plus
+        ep_reward_by_agent, layout and partner_seat.  Rows are ordered by (slot, env).  Synchronises with the host."""
+        k, e = torch.nonzero(torch.arange(self.capacity, device=self.env.device)[:, None] < self.count[None, :], as_tuple=True)
+        sp, sh = self.sparse_r_by_agent[k, e], self.shaped_r_by_agent[k, e]
+        return {"env_index": e, "ep_game_stats": self.game_stats[k, e], "ep_sparse_r_by_agent": sp, "ep_shaped_r_by_agent": sh,
+                "ep_sparse_r": sp.sum(1), "ep_shaped_r": sh.sum(1), "ep_length": self.length[k, e],
+                "ep_reward_by_agent": self.reward_by_agent[k, e], "layout": self.layout[k, e], "partner_seat": self.partner_seat[k, e]}

@@ -687,14 +687,22 @@ int ovc_sample_actions_logp(const float *scores, int ld, int n_actions, int64_t 
 int ovc_accumulate_returns(const int32_t *sparse, const int32_t *shaped, float factor, int64_t n_envs, int64_t *ret_sparse,
                            float *ret_mixed, void *stream) {
     return ovc::accumulate_returns_impl(sparse, shaped, factor, n_envs, (long long *)ret_sparse, ret_mixed, nullptr, nullptr, nullptr,
-                                        nullptr, (cudaStream_t)stream);
+                                        nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int ovc_record_transition(const int32_t *sparse, const int32_t *shaped, const int32_t *done, const float *factor, int64_t n_envs,
                           float *rewards, uint8_t *dones, int64_t *ret_sparse, float *ret_mixed, void *stream) {
     if (!factor) return ovc::fail(OVC_E_BADARG, "null pointer argument");
     return ovc::accumulate_returns_impl(sparse, shaped, 0.f, n_envs, (long long *)ret_sparse, ret_mixed, factor, done, rewards, dones,
-                                        (cudaStream_t)stream);
+                                        nullptr, (cudaStream_t)stream);
+}
+
+int ovc_record_transition_stats(const int32_t *sparse, const int32_t *shaped, const int32_t *done, const float *factor, int64_t n_envs,
+                                float *rewards, uint8_t *dones, int64_t *ret_sparse, float *ret_mixed, const ovc_episode_stats_t *stats,
+                                void *stream) {
+    if (!factor || !stats) return ovc::fail(OVC_E_BADARG, "null pointer argument");
+    return ovc::accumulate_returns_impl(sparse, shaped, 0.f, n_envs, (long long *)ret_sparse, ret_mixed, factor, done, rewards, dones,
+                                        stats, (cudaStream_t)stream);
 }
 
 int ovc_gae(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, int64_t n_steps, int64_t n_rows,

@@ -375,11 +375,78 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__rest
 // ovc_record_transition adds what a sample batch keeps of the transition: rewards[2 e + i] = sparse[e] + f * shaped[e][i]
 // (rounded after the product, as a float32 restatement computes it) and dones[e]; f is read from factor_dev when given, so
 // a captured graph follows a factor the host changes between replays.
+// STATS (ovc_record_transition_stats): also the episode statistics of ovc_episode_stats_t.  The running sums are loaded
+// together with the events and the layout ids, in one round trip to memory; a sum is only written back when its increment
+// is not zero, and an event count is incremented with a reduction that does not wait for memory (each count belongs to
+// one thread, so the result is the same as a load and a store).  Most transitions fire no event, deliver nothing and earn
+// no reward: they write the episode length only.
+__device__ __forceinline__ void episode_stats_update(const ovc_episode_stats_t &s, long long e, long long n_envs, int2 sh, float r0,
+                                                     float r1, bool done) {
+    longlong2 *spa = reinterpret_cast<longlong2 *>(s.sparse_by_agent) + e;
+    longlong2 *sha = reinterpret_cast<longlong2 *>(s.shaped_by_agent) + e;
+    float2 *rwa = s.reward_by_agent ? reinterpret_cast<float2 *>(s.reward_by_agent) + e : nullptr;
+    const int2 ev = __ldg(reinterpret_cast<const int2 *>(s.events) + e);
+    const int lid = s.layout_id[e];
+    const int new_lid = __ldg(s.state + e * s.state_words + 3) & 0xFF;
+    const int len = s.ep_length[e] + 1;
+    const longlong2 spv = *spa, shv = *sha;
+    const float2 rwv = rwa ? *rwa : make_float2(0.f, 0.f);
+    long long d0 = 0, d1 = 0;
+    if ((ev.x | ev.y) & (1 << OVC_EV_SOUP_DELIVERY)) {
+        const int32_t *dv = static_cast<const ovc_layout_t *>(s.layouts)[lid].deliver_value;
+        if ((ev.x >> OVC_EV_SOUP_DELIVERY) & 1) d0 = dv[(ev.x >> OVC_EV_RECIPE_SHIFT) & 15];
+        if ((ev.y >> OVC_EV_SOUP_DELIVERY) & 1) d1 = dv[(ev.y >> OVC_EV_RECIPE_SHIFT) & 15];
+    }
+    int32_t *cnt = s.event_counts + e * (2 * OVC_NUM_EVENTS);
+#pragma unroll
+    for (int i = 0; i < 2; i++)
+        for (unsigned m = (unsigned)(i ? ev.y : ev.x) & ((1u << OVC_NUM_EVENTS) - 1u); m; m &= m - 1)
+            atomicAdd(cnt + i * OVC_NUM_EVENTS + __ffs(m) - 1, 1);
+    // x + 0 == x: the reward sum never holds -0 (it starts at +0 and no reward is -0), so a zero reward may skip the add
+    const float2 rw = make_float2(__fadd_rn(rwv.x, r0), __fadd_rn(rwv.y, r1));
+    if (!done) {
+        if (d0 | d1) *spa = make_longlong2(spv.x + d0, spv.y + d1);
+        if (sh.x | sh.y) *sha = make_longlong2(shv.x + sh.x, shv.y + sh.y);
+        if (rwa && (r0 != 0.f || r1 != 0.f)) *rwa = rw;
+        s.ep_length[e] = len;
+        if (new_lid != lid) s.layout_id[e] = new_lid;
+        return;
+    }
+    // the episode ended: into slot count[e] of the records (or counted as dropped), then a fresh running state.  The event
+    // counts are read and cleared with atomics, the same kind of access as their increments above.
+    const int k = s.count[e];
+    const bool keep = k < s.capacity;
+    const long long slot = (long long)k * n_envs + e;
+    int32_t *dst = keep ? s.rec_event_counts + slot * (2 * OVC_NUM_EVENTS) : nullptr;
+#pragma unroll 10
+    for (int j = 0; j < 2 * OVC_NUM_EVENTS; j++) {
+        const int v = atomicExch(cnt + j, 0);
+        if (keep) dst[j] = v;
+    }
+    if (keep) {
+        s.rec_length[slot] = len;
+        s.rec_layout[slot] = lid;
+        s.rec_partner_seat[slot] = s.partner_seat ? __ldg(s.partner_seat + e) : -1;
+        reinterpret_cast<longlong2 *>(s.rec_sparse_by_agent)[slot] = make_longlong2(spv.x + d0, spv.y + d1);
+        reinterpret_cast<longlong2 *>(s.rec_shaped_by_agent)[slot] = make_longlong2(shv.x + sh.x, shv.y + sh.y);
+        if (rwa) reinterpret_cast<float2 *>(s.rec_reward_by_agent)[slot] = rw;
+        s.count[e] = k + 1;
+    } else {
+        s.dropped[e] += 1;
+    }
+    *spa = make_longlong2(0, 0);
+    *sha = make_longlong2(0, 0);
+    if (rwa) *rwa = make_float2(0.f, 0.f);
+    s.ep_length[e] = 0;
+    s.layout_id[e] = new_lid;
+}
+
+template <bool STATS>
 __global__ void __launch_bounds__(256) accumulate_returns_kernel(const int32_t *__restrict__ sparse, const int32_t *__restrict__ shaped,
                                                                  float factor, long long n_envs, long long *__restrict__ ret_sparse,
                                                                  float *__restrict__ ret_mixed, const float *__restrict__ factor_dev,
                                                                  const int32_t *__restrict__ done, float *__restrict__ rewards,
-                                                                 uint8_t *__restrict__ dones) {
+                                                                 uint8_t *__restrict__ dones, const ovc_episode_stats_t stats) {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n_envs) return;
     const float f = factor_dev ? *factor_dev : factor;
@@ -390,6 +457,9 @@ __global__ void __launch_bounds__(256) accumulate_returns_kernel(const int32_t *
     if (rewards)
         reinterpret_cast<float2 *>(rewards)[e] = make_float2(__fadd_rn((float)sp, __fmul_rn(f, (float)sh.x)), __fadd_rn((float)sp, __fmul_rn(f, (float)sh.y)));
     if (dones) dones[e] = done[e] != 0;
+    if constexpr (STATS)
+        episode_stats_update(stats, e, n_envs, sh, __fadd_rn((float)sp, __fmul_rn(f, (float)sh.x)), __fadd_rn((float)sp, __fmul_rn(f, (float)sh.y)),
+                             done[e] != 0);
 }
 
 static int sample_actions_impl(const float *scores, int ld, int n_actions, long long n_rows, unsigned long long seed,
@@ -408,12 +478,33 @@ static int sample_actions_impl(const float *scores, int ld, int n_actions, long 
 
 static int accumulate_returns_impl(const int32_t *sparse, const int32_t *shaped, float factor, long long n_envs, long long *ret_sparse,
                                    float *ret_mixed, const float *factor_dev, const int32_t *done, float *rewards, uint8_t *dones,
-                                   cudaStream_t st) {
+                                   const ovc_episode_stats_t *stats, cudaStream_t st) {
     if (!sparse || !shaped || (dones && !done)) return fail(OVC_E_BADARG, "null pointer argument");
     if (n_envs < 0) return fail(OVC_E_BADARG, "negative env count");
+    if (stats) {
+        const ovc_episode_stats_t &s = *stats;
+        if (!done || !s.layouts || !s.state || !s.events || !s.event_counts || !s.sparse_by_agent || !s.shaped_by_agent || !s.ep_length ||
+            !s.layout_id || !s.count || !s.dropped)
+            return fail(OVC_E_BADARG, "null pointer argument (episode statistics)");
+        if (s.capacity < 0) return fail(OVC_E_BADARG, "negative record capacity", s.capacity);
+        if (s.capacity > 0 && (!s.rec_length || !s.rec_layout || !s.rec_partner_seat || !s.rec_sparse_by_agent || !s.rec_shaped_by_agent ||
+                               !s.rec_event_counts || (s.reward_by_agent && !s.rec_reward_by_agent)))
+            return fail(OVC_E_BADARG, "null pointer argument (episode records)");
+        if (s.state_words < 4) return fail(OVC_E_BADARG, "state_words too small", s.state_words);
+        if (((uintptr_t)s.event_counts | (uintptr_t)s.rec_event_counts | (uintptr_t)s.events | (uintptr_t)s.reward_by_agent |
+             (uintptr_t)s.rec_reward_by_agent) & 7)
+            return fail(OVC_E_BADARG, "event and reward buffers must be 8-byte aligned");
+        if (((uintptr_t)s.sparse_by_agent | (uintptr_t)s.shaped_by_agent | (uintptr_t)s.rec_sparse_by_agent | (uintptr_t)s.rec_shaped_by_agent) & 15)
+            return fail(OVC_E_BADARG, "int64 sums must be 16-byte aligned");
+    }
     if (n_envs == 0) return OVC_OK;
-    accumulate_returns_kernel<<<(unsigned)((n_envs + 255) / 256), 256, 0, st>>>(sparse, shaped, factor, n_envs, ret_sparse, ret_mixed,
-                                                                                  factor_dev, done, rewards, dones);
+    const unsigned grid = (unsigned)((n_envs + 255) / 256);
+    if (stats)
+        accumulate_returns_kernel<true><<<grid, 256, 0, st>>>(sparse, shaped, factor, n_envs, ret_sparse, ret_mixed, factor_dev, done,
+                                                              rewards, dones, *stats);
+    else
+        accumulate_returns_kernel<false><<<grid, 256, 0, st>>>(sparse, shaped, factor, n_envs, ret_sparse, ret_mixed, factor_dev, done,
+                                                               rewards, dones, ovc_episode_stats_t{});
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "accumulate_returns kernel launch");
     return OVC_OK;

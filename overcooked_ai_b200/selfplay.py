@@ -22,6 +22,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _native
+from .batched import EpisodeRecords, EpisodeStats
 
 
 class RllibShapedCNN(nn.Module):
@@ -253,6 +254,8 @@ class SampleBatch(object):
     logits        float32 [T, 2N, 8] the policy's heads (columns 0..5 the logits), only with ``keep_logits``
     partner_seat  int8 [T, N]        with a BC partner: its player index at transition t (-1: self-play), else None
     learner_mask  uint8 [T, 2N]      (property) the rows the learner trains on: all rows but the partner's
+    episodes      EpisodeRecords     the episodes that ended in the window (``episodes.finished()``), capacity
+                                     ceil(T / horizon): an environment cannot end more episodes in T transitions
     """
 
     def __init__(self, env, n_steps, keep_logits=False, partner=False):
@@ -266,6 +269,7 @@ class SampleBatch(object):
         self.last_values = z(2 * N, torch.float32)
         self.logits = z((T, 2 * N, 8), torch.float32) if keep_logits else None
         self.partner_seat = z((T, N), torch.int8) if partner else None
+        self.episodes = EpisodeRecords(env, -(-T // env.horizon) if env.horizon > 0 else 0)
 
     @property
     def learner_mask(self):
@@ -298,7 +302,7 @@ class SelfPlayRollout(object):
     ``DenseGridPolicy`` of ``model``: K7 / K9 / K8 where they fit, library GEMMs and the draw kernel elsewhere."""
 
     def __init__(self, env, model=None, autocast_dtype=torch.bfloat16, use_graph=True, reward_shaping_factor=1.0,
-                 fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0):
+                 fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0, episode_capacity=1):
         """autocast_dtype: the dtype of the dense model (``DenseGridPolicy``, widths padded to 16-byte rows) and of the
         observation K2 writes for it: bfloat16 (the plane values are exact in bf16), or None for float32 throughout.
         fused_first_layer (default: on for the bf16 policy): the observation is never materialised — kernel K7
@@ -315,7 +319,11 @@ class SelfPlayRollout(object):
         episode start (and for every environment at construction) an environment gets the partner with probability
         ``bc_factor``, in seat 0 or 1 with equal probability (``env.assign_partners``); per transition K10
         (``env.partner_actions``) overwrites that seat's action after the PPO policy drew both.
-        bc_factor: see the property."""
+        bc_factor: see the property.
+        episode_capacity: episodes per environment that ``self.episodes`` holds (an ``EpisodeRecords``): every episode that
+        ends in run() is written there, up to this many per environment since ``self.episodes.clear()`` (the rest are
+        counted in ``episodes.dropped``).  ``self.stats`` (an ``EpisodeStats``) is the running state of the episodes in
+        progress, shared by run() and collect(): an episode may span windows and both calls."""
         assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
         assert autocast_dtype in (torch.bfloat16, None), "the dense model runs in bfloat16, or in float32 with None"
         self.env = env
@@ -345,6 +353,8 @@ class SelfPlayRollout(object):
         self.ret_sparse = torch.zeros(N, dtype=torch.int64, device=dev)      # running episode return (sparse)
         self.ret_mixed = torch.zeros(N, dtype=torch.float32, device=dev)    # sparse + factor * shaped (rllib.py:328-329)
         self.values = torch.zeros((N, 2), dtype=torch.float32, device=dev)
+        self.stats = EpisodeStats(env)
+        self.episodes = EpisodeRecords(env, episode_capacity)
         self.native_glue = True  # the draw and the returns are always native kernels; bench.py's launch count reads this
         if fused_tail is None:
             fused_tail = bf16 and k8_ok
@@ -417,8 +427,9 @@ class SelfPlayRollout(object):
 
     def _capture(self, warm_up, body):
         """A CUDA graph of ``body``, captured after ``warm_up`` (on a side stream).  Warm-up and capture must not advance
-        the environments: the state, the returns and the draw counters are restored after them."""
-        live = [self.env.state, self.ret_sparse, self.ret_mixed, self._draw_counter]
+        the environments: the state, the returns, the episode statistics and records and the draw counters are restored after
+        them."""
+        live = [self.env.state, self.ret_sparse, self.ret_mixed, self._draw_counter] + self.stats.state_tensors() + self.episodes.tensors()
         if self.partner is not None:
             live += [self.partner_seat, self._partner_counter, self._seat_counter]
         saved = [t.clone() for t in live]
@@ -472,10 +483,10 @@ class SelfPlayRollout(object):
         return None  # K8 has drawn the actions itself
 
     def _transition(self, b=None, t=0):
-        """One transition: K2 or K7, the policy, the draw, K10 for the partner, K1 (auto-reset inside), the returns, the seat
-        draw.  Without ``b`` (run()) the actions and values go to self.actions / self.values; with a ``SampleBatch`` ``b``
-        (collect()) the transition is recorded in its slot ``t``: state, actions, values, logp, logits, rewards, dones and
-        partner seats."""
+        """One transition: K2 or K7, the policy, the draw, K10 for the partner, K1 (auto-reset inside), the returns and the
+        episode statistics, the seat draw.  Without ``b`` (run()) the actions and values go to self.actions / self.values and
+        finished episodes to self.episodes; with a ``SampleBatch`` ``b`` (collect()) the transition is recorded in its slot
+        ``t``: state, actions, values, logp, logits, rewards, dones and partner seats, and finished episodes in b.episodes."""
         env = self.env
         if b is None:
             actions, values, logp, logits, rewards, dones = self.actions, None, None, None, None, None
@@ -495,7 +506,10 @@ class SelfPlayRollout(object):
                 b.partner_seat[t].copy_(self.partner_seat)
             self._partner_act(actions)  # K10
         env.step(actions.view(env.n_envs, 2))  # K1 (auto-reset inside)
-        env.record_transition(self._factor, rewards=rewards, dones=dones, ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed)
+        # the seat draw below runs after this kernel, so partner_seat is still the ending episode's
+        env.record_transition(self._factor, rewards=rewards, dones=dones, ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed,
+                              stats=self.stats, records=self.episodes if b is None else b.episodes,
+                              partner_seat=None if self.partner is None else self.partner_seat)
         if self.partner is not None:
             self._assign_partners(env.done)
 
@@ -514,6 +528,7 @@ class SelfPlayRollout(object):
     def _collect_window(self, b, n_steps, gamma, lam):
         """n_steps transitions into slots 0.. of ``b``, then the bootstrap value of the state after them and GAE over the
         whole batch."""
+        b.episodes.clear()
         for t in range(n_steps):
             self._transition(b, t)
         if not self.fused_first_layer:

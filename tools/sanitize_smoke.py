@@ -3,7 +3,8 @@
 K1 with each record-I/O strategy (2-D TMA tile, 1-D bulk TMA, direct), K5 (the rollout kernel, int32 and
 host-transfer formats, standard and random-start auto-resets, 16- / 32- / 64-word records, a partial last tile),
 the round-1 fused path, K4 reset (copy + random), K2, K3, K6, the host-buffer pipeline, the policy kernels K7 / K8 and
-the sample-batch kernels (logp draws, ovc_record_transition, ovc_gae through SelfPlayRollout.collect).  Results are checked
+the sample-batch kernels (logp draws, ovc_record_transition, ovc_gae through SelfPlayRollout.collect), K10 and the seat draw,
+and the episode statistics of ovc_record_transition_stats.  Results are checked
 against the CPU oracle on the way, so a run under the sanitizer is also a parity run.
 
     compute-sanitizer --tool racecheck python tools/sanitize_smoke.py
@@ -169,4 +170,25 @@ b = sp3.collect(12, 0.99, 0.95)
 assert b.learner_mask.shape == (12, 2 * n) and int(b.learner_mask.sum()) >= 12 * n
 torch.cuda.synchronize()
 print("K10 partner policy, assign_partners, collect() with a partner ok", flush=True)
+# the episode statistics (ovc_record_transition_stats): horizon 5 over 15 transitions into 2 slots (the third episode is
+# dropped), random starts so that episodes deliver, against the numpy restatement
+from episode_reference import EpisodeReference, rewards_f32  # noqa: E402
+from overcooked_ai_b200.batched import EpisodeRecords, EpisodeStats  # noqa: E402
+
+env6 = BatchedOvercookedEnv(["cramped_room", "coordination_ring"], n, horizon=5, auto_reset=True, rnd_obj_prob_thresh=0.6, seed=2)
+rs6 = cpu.random_start(2, 0.6)
+ref_state = env6.state.cpu().numpy().copy()
+stats, recs = EpisodeStats(env6), EpisodeRecords(env6, 2)
+ref = EpisodeReference(np.stack([l.deliver_value for l in env6.layouts]), ref_state[:, 3] & 0xFF, 2)
+for a in acts_for(15, n):
+    env6.step(torch.from_numpy(a).cuda())
+    env6.record_transition(factor, stats=stats, records=recs, partner_seat=seat)
+    sp_, sh_, d_, ev_ = cpu.step(env6._tab_host, env6._starts_host, ref_state, a, horizon=5, flags=1, rs=rs6)
+    ref.step(sh_, d_, ev_, ref_state[:, 3] & 0xFF, rewards_f32(sp_, sh_, 0.5), seat.cpu().numpy())
+fin = recs.finished()
+for k, want in ref.finished().items():
+    assert np.array_equal(fin[k].cpu().numpy(), want), k
+assert (recs.dropped.cpu().numpy() == ref.dropped).all() and (ref.dropped == 1).all()
+torch.cuda.synchronize()
+print("episode statistics (record_transition with stats) ok", flush=True)
 print("sanitize_smoke: all ok")
