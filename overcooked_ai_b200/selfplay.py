@@ -181,14 +181,20 @@ class DenseGridPolicy(nn.Module):
         return hv[:, :self.n_actions], hv[:, self.n_actions]
 
 
-def fused_kernel_support(dense_model, width, height):
-    """(K7, K9, K8) usable for this network on this grid: K7 needs the first layer's width to be a multiple of 64 and its
-    narrowest column slice (64 columns of the 19 dynamic planes) to fit shared memory; K9 is built for 512 -> 512 -> 160 (5x4
-    grids); K8 for a tail of 64-wide layers behind an input of a multiple of 32 (<= 256) and at most 7 actions.  Whatever is
-    not supported runs as library GEMMs / the separate draw kernel."""
+K7_MAX_LAYOUTS = 8  # EL_MAX_LAYOUTS of ovc_encode_linear: its prologue folds the terrain sums of at most 8 layouts per call
+
+
+def fused_kernel_support(dense_model, width, height, n_layouts=1):
+    """(K7, K9, K8) usable for this network on this grid with ``n_layouts`` layouts in the batch: K7 needs the first layer's
+    width to be a multiple of 64, its narrowest column slice (64 columns of the 19 dynamic planes) to fit shared memory, and
+    at most ``K7_MAX_LAYOUTS`` (8) layouts; K9 is built for 512 -> 512 -> 160 (5x4 grids); K8 for a tail of 64-wide layers
+    behind an input of a multiple of 32 (<= 256) and at most 7 actions.  Whatever is not supported runs as library GEMMs /
+    the separate draw kernel.  ``SelfPlayRollout`` uses K9 only behind K7, so a pool of more than 8 5x4 layouts runs K2, the
+    wide layers as library GEMMs, then K8."""
     l0, l1, l2 = dense_model.conv_as_linear
     d = list(dense_model.dense)
-    k7 = l0.out_features % 64 == 0 and width * height * 19 * 64 * 2 + 4096 <= 227 * 1024
+    k7 = (l0.out_features % 64 == 0 and width * height * 19 * 64 * 2 + 4096 <= 227 * 1024
+          and n_layouts <= K7_MAX_LAYOUTS)
     k9 = (l1.in_features, l1.out_features, l2.out_features) == (512, 512, 160)
     k8 = all(l.out_features == 64 for l in d) and d[0].in_features % 32 == 0 and d[0].in_features <= 256 and dense_model.n_actions <= 7
     return k7, k9, k8
@@ -299,15 +305,17 @@ PARTNER_SEAT_SALT = 0xD1B54A32D192ED03
 class SelfPlayRollout(object):
     """Policy-in-the-loop rollout: both agents of every environment act from the same network, or, with a BC ``partner``,
     one seat of an environment is the partner's in the episodes the seat draw gives it (PPO_BC).  The network evaluated is
-    ``DenseGridPolicy`` of ``model``: K7 / K9 / K8 where they fit, library GEMMs and the draw kernel elsewhere."""
+    ``DenseGridPolicy`` of ``model``: K7 / K9 / K8 where they fit (``fused_kernel_support``; K7, and K9 behind it, only with
+    at most 8 layouts in ``env``), library GEMMs and the draw kernel elsewhere."""
 
     def __init__(self, env, model=None, autocast_dtype=torch.bfloat16, use_graph=True, reward_shaping_factor=1.0,
                  fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0, episode_capacity=1):
         """autocast_dtype: the dtype of the dense model (``DenseGridPolicy``, widths padded to 16-byte rows) and of the
         observation K2 writes for it: bfloat16 (the plane values are exact in bf16), or None for float32 throughout.
-        fused_first_layer (default: on for the bf16 policy): the observation is never materialised — kernel K7
-        (``env.encoded_linear``) evaluates encoding + first layer + leaky ReLU from the packed records, and the library
-        GEMMs start at the second layer.
+        fused_first_layer (default: on for the bf16 policy where ``fused_kernel_support`` allows K7): the observation is
+        never materialised — kernel K7 (``env.encoded_linear``) evaluates encoding + first layer + leaky ReLU from the
+        packed records, and the library GEMMs start at the second layer.  K7 takes at most 8 layouts per call: on a larger
+        layout pool the default is off (K2 writes the observation) and an explicit True is refused here.
         fused_tail (default: on for the bf16 policy): the dense layers of 64, the heads and the draw run as ONE kernel
         (``ovc_policy_tail``, K8) on the last convolution's pre-activation; the library GEMMs are then only the two wide
         layers.  Without it the joint action is drawn by ``ovc_sample_actions`` (Gumbel-max on Philox draws keyed by
@@ -336,11 +344,12 @@ class SelfPlayRollout(object):
         if autocast_dtype is not None:
             self.dense_model = self.dense_model.to(autocast_dtype)
         bf16 = autocast_dtype == torch.bfloat16
-        k7_ok, k9_ok, k8_ok = fused_kernel_support(self.dense_model, self.W, self.H)
+        k7_ok, k9_ok, k8_ok = fused_kernel_support(self.dense_model, self.W, self.H, env.n_layouts)
         if fused_first_layer is None:
             fused_first_layer = bf16 and k7_ok
         assert not fused_first_layer or (bf16 and k7_ok), \
-            "K7 feeds the bf16 policy (first layer width a multiple of 64, table within shared memory)"
+            "K7 feeds the bf16 policy (first layer width a multiple of 64, table within shared memory, at most %d layouts; " \
+            "this environment has %d)" % (K7_MAX_LAYOUTS, env.n_layouts)
         self.fused_first_layer = bool(fused_first_layer)
         self.factor = float(reward_shaping_factor)
         self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by the captured graphs

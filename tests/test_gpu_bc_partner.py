@@ -103,11 +103,38 @@ def test_k10_exact_on_fixture_states(path):
     _k10_check(env, seats, _bc_operands(rng, 1), 6)
 
 
-@pytest.mark.parametrize("layout,n", [("long_cook_time", 777), ("counter_circuit", 1027), ("cramped_room", 2 * 333 + 1)])
+POOL_5X4 = ["cramped_room", "cramped_room_tomato", "simple_o_t", "simple_tomato", "bonus_order_test", "mdp_test", "m_shaped_s",
+            "simple_o", "cramped_room_o_3orders"]  # the 9 bundled two-player 5x4 layouts
+K10_POOLS = {  # batches whose 64-environment tiles hold several layouts: (layouts, environment arguments for n envs)
+    "interleaved": (["cramped_room", "mdp_test", "bonus_order_test", "m_shaped_s"], lambda n: {"env_layout": np.arange(n) % 4}),
+    "pool_5x4_random_layout": (POOL_5X4, lambda n: {"random_layout": True, "horizon": 8}),  # 3 redraws in the 25 steps
+    "mixed_shapes": (["cramped_room", "counter_circuit", "long_cook_time", "asymmetric_advantages_tomato"], lambda n: {}),
+}
+
+
+def _k10_pool_premises(env, seats):
+    """Every layout occurs, some 64-environment tile holds more than one, and for some partnered environment layout 0's
+    feature LUT gives other features than its own: a K10 that read the wrong layout's tables would fail."""
+    st = _np(env.state)
+    lid = st[:, 3] & 0xFF
+    assert set(lid.tolist()) == set(range(env.n_layouts)), "premise: every layout occurs"
+    assert any(len(np.unique(lid[i:i + 64])) > 1 for i in range(0, len(lid), 64)), "premise: a tile holds several layouts"
+    lut = _np(env.feature_lut())
+    on = np.flatnonzero(seats >= 0)
+    right = cpu.featurize(env._tab_host, lut, st, num_pots=2)[on, seats[on]]
+    wrong = cpu.featurize(env._tab_host, lut[np.zeros(env.n_layouts, np.int64)], st, num_pots=2)[on, seats[on]]
+    assert (right != wrong).any(), "premise: layout 0's LUT featurizes no partnered environment differently"
+
+
+@pytest.mark.parametrize("layout,n", [("long_cook_time", 777), ("counter_circuit", 1027), ("cramped_room", 2 * 333 + 1),
+                                      ("interleaved", 779), ("pool_5x4_random_layout", 1001), ("mixed_shapes", 901)])
 def test_k10_exact_on_random_rollouts(layout, n):
     """Random start states then random play; seats -1 / 0 / 1 mixed in each launch; n_hidden 0, 1, 2 and 1..7 actions;
-    n is not a multiple of the 64-environment tile."""
-    env = BatchedOvercookedEnv(layout, n, horizon=60, auto_reset=True, random_start_pos=True, rnd_obj_prob_thresh=0.6, seed=n)
+    n is not a multiple of the 64-environment tile.  Several layouts per batch (``K10_POOLS``): env_layout interleaving
+    four 5x4 layouts, the nine 5x4 layouts redrawn at every reset (random_layout), and four grid shapes in segments."""
+    layouts, kw = K10_POOLS[layout] if layout in K10_POOLS else (layout, lambda n: {})
+    kw = dict({"horizon": 60}, **kw(n))
+    env = BatchedOvercookedEnv(layouts, n, auto_reset=True, random_start_pos=True, rnd_obj_prob_thresh=0.6, seed=n, **kw)
     rng = np.random.RandomState(n)
     acts = rng.randint(0, 6, size=(25, n, 2)).astype(np.int32)
     acts[rng.rand(25, n, 2) < 0.4] = 5
@@ -118,6 +145,8 @@ def test_k10_exact_on_random_rollouts(layout, n):
             _k10_check(env, seats, _bc_operands(rng, n_hidden), n_actions, seed=n_actions, step=n_hidden * 7 + n_actions)
     _k10_check(env, np.full(n, -1, np.int32), _bc_operands(rng, 1), 6)
     _k10_check(env, np.ones(n, np.int32), _bc_operands(rng, 1), 6)
+    if layout in K10_POOLS:
+        _k10_pool_premises(env, np.ones(n, np.int32))
 
 
 def test_k10_exact_on_l16_features_above_256():

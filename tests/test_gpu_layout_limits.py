@@ -258,12 +258,25 @@ def test_k7_shape_boundary_follows_its_shared_memory():
     net = SimpleNamespace(conv_as_linear=[lin(1, 128), lin(128, 64), lin(64, 64)], dense=[lin(64, 64)], n_actions=6)
     for (W, H), ok in (((13, 7), True), ((7, 13), True), ((12, 8), False), ((16, 6), False)):
         assert fused_kernel_support(net, W, H)[0] == ok, (W, H)
-    # fused_kernel_support has its own bound (independent of the layout count); it agrees with the kernel's for 1 and for 8
-    # layouts on every grid shape up to 16x16 because no such grid has 92-95 cells
+    # fused_kernel_support's shared-memory bound does not depend on the layout count; it agrees with the kernel's for 1 and
+    # for 8 layouts on every grid shape up to 16x16 because no such grid has 92-95 cells
     for W in range(1, 17):
         for H in range(1, 17):
             fit1, fit8 = _k7_smem(W * H, 1) <= cap, _k7_smem(W * H, 8) <= cap
-            assert fused_kernel_support(net, W, H)[0] == fit1 == fit8, (W, H)
+            assert fused_kernel_support(net, W, H)[0] == fused_kernel_support(net, W, H, 8)[0] == fit1 == fit8, (W, H)
+    # the layout count has its own bound: ovc_encode_linear takes 1 and 8 layouts of a 5x4 grid and refuses 9
+    pool = ["cramped_room", "cramped_room_tomato", "simple_o_t", "simple_tomato", "bonus_order_test", "mdp_test",
+            "m_shaped_s", "simple_o", "cramped_room_o_3orders"]
+    wt, bias = torch.zeros((520, 128), dtype=torch.bfloat16, device="cuda"), torch.zeros(128, device="cuda")
+    for k in (1, 8, 9):
+        env = BatchedOvercookedEnv(pool[:k], 2 * k + 1, horizon=40)
+        try:
+            env.encoded_linear(wt, bias)
+            accepted = True
+        except RuntimeError as e:
+            assert "more than 8 layouts per call" in str(e)
+            accepted = False
+        assert fused_kernel_support(net, 5, 4, k)[0] == accepted == (k <= 8), k
 
 
 def _k7_states(layouts, n):

@@ -609,3 +609,20 @@ def test_fused_kernel_support_by_grid():
     for (W, H), want in (((5, 4), (True, True, True)), ((5, 5), (True, False, False)), ((9, 5), (False, False, False))):
         d = DenseGridPolicy(RllibShapedCNN(W, H), W, H, pad_to=16)
         assert fused_kernel_support(d, W, H) == want, (W, H, fused_kernel_support(d, W, H))
+
+
+def test_fused_kernel_support_bounds_the_layout_count():
+    """K7 takes at most 8 layouts per call (EL_MAX_LAYOUTS): above that fused_kernel_support turns K7 off on every grid it
+    would otherwise allow, and leaves K9 and K8 as they are."""
+    from types import SimpleNamespace
+
+    from overcooked_ai_b200.selfplay import K7_MAX_LAYOUTS, fused_kernel_support
+
+    lin = lambda i, o: SimpleNamespace(in_features=i, out_features=o)
+    net = SimpleNamespace(conv_as_linear=[lin(520, 512), lin(512, 512), lin(512, 160)], dense=[lin(160, 64)] * 3, n_actions=6)
+    assert K7_MAX_LAYOUTS == 8
+    assert fused_kernel_support(net, 5, 4) == (True, True, True)
+    for n_layouts, k7 in ((1, True), (2, True), (8, True), (9, False), (12, False), (255, False)):
+        assert fused_kernel_support(net, 5, 4, n_layouts) == (k7, True, True), n_layouts
+        assert fused_kernel_support(net, 13, 7, n_layouts)[0] == k7, n_layouts  # the largest grids K7's table fits
+        assert not fused_kernel_support(net, 12, 8, n_layouts)[0], n_layouts     # refused by shared memory alone

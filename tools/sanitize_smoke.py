@@ -168,8 +168,24 @@ env.assign_partners(seat, factor, torch.zeros(2, dtype=torch.int64, device="cuda
 sp3 = SelfPlayRollout(env, model=sp.model, use_graph=False, seed=3, partner=bc, bc_factor=0.5)
 b = sp3.collect(12, 0.99, 0.95)
 assert b.learner_mask.shape == (12, 2 * n) and int(b.learner_mask.sum()) >= 12 * n
+# three 5x4 layouts interleaved env by env: K10, K7 and the statistics index their per-layout tables with ids 0..2 in one tile
+envp = BatchedOvercookedEnv(["cramped_room", "mdp_test", "bonus_order_test"], n, horizon=6, auto_reset=True,
+                            env_layout=np.arange(n) % 3, rnd_obj_prob_thresh=0.6, seed=4)
+envp.rollout(torch.from_numpy(acts_for(9, n)).cuda())
+st = envp.state.cpu().numpy().copy()
+scores.fill_(float("nan"))
+envp.partner_actions(bc.tables(), seat, torch.zeros(2, dtype=torch.int64, device="cuda"), seed=5, scores=scores)
+feat = envp.featurize_state(num_pots=2)
+assert np.array_equal(feat.cpu().numpy().astype(np.float64), cpu.featurize(envp._tab_host, envp.feature_lut().cpu().numpy(), st, 2))
+want = bc(feat[torch.arange(n, device="cuda"), seat.clamp(min=0).long()])
+assert ((scores[seat >= 0, :6] - want[seat >= 0]).abs() <= 0.05 * (1 + want[seat >= 0].abs())).all()  # bf16 operands
+sp4 = SelfPlayRollout(envp, model=sp.model, use_graph=False, seed=3, partner=bc, bc_factor=0.5)
+assert sp4.fused_first_layer and sp4.fused_wide and sp4.fused_tail
+b = sp4.collect(1, 0.99, 0.95)
+cpu.step(envp._tab_host, envp._starts_host, st, b.actions[0].cpu().numpy().reshape(n, 2), horizon=6, flags=1, rs=cpu.random_start(4, 0.6))
+assert np.array_equal(envp.state.cpu().numpy(), st)
 torch.cuda.synchronize()
-print("K10 partner policy, assign_partners, collect() with a partner ok", flush=True)
+print("K10 partner policy, assign_partners, collect() with a partner, on one layout and on three interleaved ok", flush=True)
 # the episode statistics (ovc_record_transition_stats): horizon 5 over 15 transitions into 2 slots (the third episode is
 # dropped), random starts so that episodes deliver, against the numpy restatement
 from episode_reference import EpisodeReference, rewards_f32  # noqa: E402
