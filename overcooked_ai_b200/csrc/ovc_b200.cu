@@ -87,6 +87,8 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, int c0, int
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"((uint64_t)map) : "memory");
 }
+// brings the line holding p into L2 (no register written, nothing to wait on)
+__device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void bulk_load_1d(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                      smem_u32(dst)),
@@ -213,17 +215,25 @@ __device__ __forceinline__ void write_outputs(const StepArgs &a, long long idx, 
     reinterpret_cast<int2 *>(a.events)[idx] = make_int2((int)o.ev0, (int)o.ev1);
 }
 
-template <bool WIDE>
-__device__ __forceinline__ int2 load_action(const StepArgs &a, long long idx) {
+// address of joint-action element idx: int32 pairs (8 B), OVC_F_ACT_U8 (2 B) or OVC_F_ACT_PACKED (1 B)
+template <bool WIDE, typename I>
+__device__ __forceinline__ const void *action_addr(const StepArgs &a, I idx) {
+    if (!WIDE && (a.flags & OVC_F_ACT_PACKED)) return reinterpret_cast<const unsigned char *>(a.actions) + idx;
+    if (!WIDE && (a.flags & OVC_F_ACT_U8)) return reinterpret_cast<const uchar2 *>(a.actions) + idx;
+    return reinterpret_cast<const int2 *>(a.actions) + idx;
+}
+
+template <bool WIDE, typename I>
+__device__ __forceinline__ int2 load_action(const StepArgs &a, I idx) {
     if (!WIDE && (a.flags & OVC_F_ACT_PACKED)) {
-        const unsigned u = reinterpret_cast<const unsigned char *>(a.actions)[idx];
+        const unsigned u = *static_cast<const unsigned char *>(action_addr<WIDE>(a, idx));
         return make_int2((int)(u & 15u), (int)(u >> 4));
     }
     if (!WIDE && (a.flags & OVC_F_ACT_U8)) {
-        const uchar2 u = reinterpret_cast<const uchar2 *>(a.actions)[idx];
+        const uchar2 u = *static_cast<const uchar2 *>(action_addr<WIDE>(a, idx));
         return make_int2(u.x, u.y);
     }
-    return reinterpret_cast<const int2 *>(a.actions)[idx];
+    return *static_cast<const int2 *>(action_addr<WIDE>(a, idx));
 }
 
 // Shared-memory plan of one CTA (dynamic, 1024-byte aligned so the TMA swizzle pattern lines up with
@@ -429,9 +439,29 @@ static int launch_rollout(const StepArgs &a, cudaStream_t st) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return cuda_fail(e, "rollout kernel shared-memory attribute");
     }
+    const long long grid = (a.n_envs + TILE - 1) / TILE;
+    StepArgs ka = a;
+    ka.flags &= ~F_K5_NO_PREFETCH;
+#if OVC_K5_PREFETCH > 1
+    // The action prefetch pays in a middle range of warps per SM.  With many warps the others hide the action load; with
+    // very few, a transition's own chain outlasts the (then short) DRAM latency, so the load is not on the path either, and
+    // in both cases the prefetch only adds instructions.  The last wave of a grid larger than one wave runs with few
+    // warps while the rest of the SM is idle, so there the prefetch stays on.  cramped_room, TILE = 64, on an H100 (132 SMs):
+    // 16 384 envs (3.9 warps per SM) 4 % slower with it, 32 768 (7.8) about even, 65 536 (15.5) 13 % faster, 131 072
+    // (31, one wave) 3 % slower; asymmetric_advantages at 131 072 envs (two waves) 17 % faster.
+    {
+        int dev = 0, n_sm = 0, per_sm = 0;
+        cudaError_t e = cudaGetDevice(&dev);
+        if (e == cudaSuccess) e = cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+        if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, TILE, smem);
+        if (e != cudaSuccess) return cuda_fail(e, "rollout kernel occupancy");
+        const long long warps = grid * (TILE / 32);
+        if (grid <= (long long)per_sm * n_sm && (warps >= 24LL * n_sm || warps < 12LL * n_sm)) ka.flags |= F_K5_NO_PREFETCH;
+    }
+#endif
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof cfg);
-    cfg.gridDim = dim3((unsigned)((a.n_envs + TILE - 1) / TILE)), cfg.blockDim = dim3(TILE), cfg.dynamicSmemBytes = smem, cfg.stream = st;
+    cfg.gridDim = dim3((unsigned)grid), cfg.blockDim = dim3(TILE), cfg.dynamicSmemBytes = smem, cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
@@ -440,7 +470,7 @@ static int launch_rollout(const StepArgs &a, cudaStream_t st) {
     // CTAs sit on the SMs beside a kernel that runs for hundreds of microseconds: slower with back-to-back launches of
     // 1-warp CTAs, nothing gained with larger CTAs.  Not used.
     cfg.numAttrs = 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tmap, a);
+    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tmap, ka);
     if (e != cudaSuccess) return cuda_fail(e, "rollout kernel launch");
     return OVC_OK;
 }

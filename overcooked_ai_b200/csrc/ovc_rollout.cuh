@@ -25,6 +25,16 @@
 // replay every fixture through both).  Included by ovc_b200.cu after the PTX helpers and StepArgs.
 #pragma once
 
+// Action rows prefetched into L2 ahead of the transition loop.  The demand load of a transition's joint action is
+// issued one transition ahead; on its own it is a DRAM read, and each transition starts by waiting for it.  With
+// OVC_K5_PREFETCH = D >= 2 every thread also prefetches its own action D rows ahead (prefetch.global.L2: no register,
+// no scoreboard), so the demand load hits L2.  0 (or 1): no prefetch, the kernel of the plain distance-1 load.  The
+// host turns the prefetch off for a launch whose grid is resident in one wave at fewer than 12 or at least 24 warps per
+// SM (launch_rollout).
+#ifndef OVC_K5_PREFETCH
+#define OVC_K5_PREFETCH 4
+#endif
+
 namespace ovc {
 
 struct Derived {
@@ -259,6 +269,9 @@ __device__ __forceinline__ unsigned interact_v2(const R &r, uint32_t L, uint32_t
 // (3 % of a transition when they sat in every instantiation), the sparse event stream carries the warp votes.
 constexpr int FMT_WIDE = 0, FMT_HOST = 1, FMT_STREAM = 2;
 
+// A flags bit the host sets per launch (launch_rollout; the ABI's flags leave bits 12-15 free): skip the action prefetch.
+constexpr int F_K5_NO_PREFETCH = 1 << 12;
+
 // Output / action addressing of one thread: ONE 32-bit element index per stream (outputs, actions), advanced by n_envs
 // per transition; every array address is then a single IMAD.WIDE of that index onto the array's base pointer.  (The
 // host keeps n_steps * n_envs below 2^32 per launch by cutting longer rollouts into several launches.)
@@ -284,18 +297,10 @@ struct RollIO {
             vals = reinterpret_cast<unsigned short *>(a.sparse) + (size_t)mi * cap;
         }
     }
-    __device__ __forceinline__ int2 load_action() const {
-        if (!WIDE && (a.flags & OVC_F_ACT_PACKED)) {
-            const unsigned u = reinterpret_cast<const unsigned char *>(a.actions)[ai];
-            return make_int2((int)(u & 15u), (int)(u >> 4));
-        }
-        if (!WIDE && (a.flags & OVC_F_ACT_U8)) {
-            const uchar2 u = reinterpret_cast<const uchar2 *>(a.actions)[ai];
-            return make_int2(u.x, u.y);
-        }
-        return reinterpret_cast<const int2 *>(a.actions)[ai];
-    }
+    __device__ __forceinline__ int2 load_action() const { return ovc::load_action<WIDE>(a, ai); }
     __device__ __forceinline__ void next_action() { ai += n; }
+    // L2 prefetch of the action `rows` rows after the one loaded last (the caller keeps that row below n_steps)
+    __device__ __forceinline__ void prefetch_action(unsigned rows) const { prefetch_l2(action_addr<WIDE>(a, ai + rows * n)); }
     // Writes this transition's outputs and advances to the next transition.  FMT_STREAM: called at ONE program point by
     // every live thread of the warp, once per transition (it votes across the warp).
     __device__ __forceinline__ void write(const RollOut &o, int done_v, bool stepped, uint32_t mask) {
@@ -393,6 +398,12 @@ rollout_kernel(const __grid_constant__ CUtensorMap tmap, const StepArgs a) {
     if (tid == 0) tma_load_2d(tile, &tmap, 0, (int)(env0 * C::ROWS_PER_ENV), bar);  // rows past the end: zero fill, still counted
     int2 act = make_int2(OVC_A_STAY, OVC_A_STAY);
     if (live) act = load_action<WIDE>(a, env);
+#if OVC_K5_PREFETCH > 1
+    // rows 1 .. D-1; the transition loop prefetches row s + D in transition s
+    const bool prefetch = !(a.flags & F_K5_NO_PREFETCH);
+    if (live && prefetch)
+        for (int k = 1; k < OVC_K5_PREFETCH && k < T; k++) prefetch_l2(action_addr<WIDE>(a, (unsigned)env + (unsigned)k * (unsigned)a.n_envs));
+#endif
     __syncthreads();  // barrier initialised + zero fill complete
     mbar_wait(bar, 0);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -529,6 +540,9 @@ rollout_kernel(const __grid_constant__ CUtensorMap tmap, const StepArgs a) {
             int2 nxt = act;
             io.next_action();
             if (s + 1 < T) nxt = io.load_action();  // prefetch
+#if OVC_K5_PREFETCH > 1
+            if (prefetch && s + OVC_K5_PREFETCH < T) io.prefetch_action(OVC_K5_PREFETCH - 1);  // row s + D into L2
+#endif
             const int a0 = act.x, a1 = act.y;
             act = nxt;
             RollOut o{0, 0, 0, 0u, 0u};
