@@ -296,7 +296,8 @@ int ovc_step(const void *layouts, int n_layouts, const int32_t *start_records, i
  * T consecutive transitions in ONE launch (the record stays on chip between transitions).
  * actions int32[T][n_envs][2]; sparse/done int32[T][n_envs]; shaped/events int32[T][n_envs][2] — or the narrower
  * element types the OVC_F_ACT_* / OVC_F_OUT_* flags select (pointers are then reinterpreted; outputs a format does
- * not produce may be NULL).  Semantically identical to T calls of ovc_step with the same flags.
+ * not produce may be NULL).  Every array must be aligned to its element type (OVC_E_BADARG otherwise).  Semantically
+ * identical to T calls of ovc_step with the same flags.
  */
 int ovc_rollout(const void *layouts, int n_layouts, const int32_t *start_records, int32_t *state,
                 const int32_t *actions, int32_t *sparse, int32_t *shaped, int32_t *done,

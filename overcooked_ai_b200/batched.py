@@ -183,20 +183,15 @@ class BatchedOvercookedEnv(object):
         non-zero words compacted in (transition, lane) order, at most ``cap`` per group (the masks count the rest).
         actions: int32 / uint8 [T, N, 2] or one-byte joint actions uint8 [T, N].  Returns (masks, values, dense or None);
         expand with ``expand_stream``."""
-        assert actions.dtype in (torch.int32, torch.uint8) and actions.is_cuda and actions.is_contiguous() and actions.dim() in (2, 3)
+        act_flag = self._action_flag(actions)
         T = actions.shape[0]
-        assert actions.shape[1] == self.n_envs and 1 <= cap <= _native.STREAM_CAP_MAX
+        assert 1 <= cap <= _native.STREAM_CAP_MAX
         if out is None:
             out = self.alloc_stream_out(T, cap, dense_backup=dense_backup)
         masks, values, dense = out
         assert masks.dtype == torch.int32 and tuple(masks.shape) == (T, self.n_groups()) and masks.is_cuda and masks.is_contiguous()
         assert values.dtype == torch.int16 and values.numel() == self.n_groups() * cap and values.is_cuda and values.is_contiguous()
-        flags = self._flags() | _native.F_OUT_STREAM | (int(cap) << _native.F_STREAM_CAP_SHIFT)
-        if actions.dim() == 2:
-            assert actions.dtype == torch.uint8
-            flags |= _native.F_ACT_PACKED
-        elif actions.dtype == torch.uint8:
-            flags |= _native.F_ACT_U8
+        flags = self._flags() | act_flag | _native.F_OUT_STREAM | (int(cap) << _native.F_STREAM_CAP_SHIFT)
         if flags >= 2**31:  # the C int carries the capacity in its upper half
             flags -= 2**32
         _native.check(self._lib.ovc_rollout(
@@ -215,29 +210,28 @@ class BatchedOvercookedEnv(object):
         assert G == self.n_groups() and values.shape[1] == G
         chunk = T if chunk is None else int(chunk)
         assert values.shape[0] == -(-T // chunk)
-        N, cap = self.n_envs, values.shape[2]
-        tbl = self.code_reward_table()
-        lay = self.env_layout_host
-        if self.random_layout:
-            assert (tbl == tbl[:1]).all(), "random_layout with different reward tables: the codes alone do not name the layout"
-            lay = None
-        if out is None:
-            out = {}
-            if sparse:
-                out["sparse"] = torch.empty((T, N), dtype=torch.int16)
-            if shaped:
-                out["shaped"] = torch.empty((T, N, 2), dtype=torch.int8)
-            if done:
-                out["done"] = torch.empty((T, N), dtype=torch.uint8)
-            if events:
-                out["events"] = torch.empty((T, N, 2), dtype=torch.int32)
-        ptr = lambda k: out[k].data_ptr() if k in out else 0
-        tbl = np.ascontiguousarray(tbl, dtype=np.int32)
+        out, tbl, lay, ptrs = self._dense_host_out(T, out, sparse, shaped, done, events)
         over = ctypes.c_int64(0)
         _native.check(self._lib.ovc_expand_stream_host(
-            masks.data_ptr(), values.data_ptr(), T, chunk, cap, N, 0 if lay is None else lay.ctypes.data, tbl.ctypes.data,
-            self.n_layouts, ptr("sparse"), ptr("shaped"), ptr("done"), ptr("events"), int(n_threads), ctypes.byref(over)))
+            masks.data_ptr(), values.data_ptr(), T, chunk, values.shape[2], self.n_envs, lay, tbl.ctypes.data, self.n_layouts, *ptrs,
+            int(n_threads), ctypes.byref(over)))
         return out, int(over.value)
+
+    def _dense_host_out(self, T, out, sparse, shaped, done, events):
+        """What the host expanders take besides the words: the dense arrays (``out``, or new ones for the requested keys), the
+        reward table, the layout ids (a pointer; 0 = one table for all) and the four output pointers (0 = not requested)."""
+        tbl = np.ascontiguousarray(self.code_reward_table(), dtype=np.int32)
+        lay = self.env_layout_host.ctypes.data
+        if self.random_layout:
+            assert (tbl == tbl[:1]).all(), "random_layout with different reward tables: the codes alone do not name the layout"
+            lay = 0
+        if out is None:
+            N = self.n_envs
+            want = (("sparse", sparse, (T, N), torch.int16), ("shaped", shaped, (T, N, 2), torch.int8),
+                    ("done", done, (T, N), torch.uint8), ("events", events, (T, N, 2), torch.int32))
+            out = {k: torch.empty(shape, dtype=dt) for k, on, shape, dt in want if on}
+        ptrs = [out[k].data_ptr() if k in out else 0 for k in ("sparse", "shaped", "done", "events")]
+        return out, tbl, lay, ptrs
 
     def alloc_rollout_out(self, T, narrow=False, pin=False, packed=False, codes=False):
         """Output tensors for rollout(): (sparse[T,N], shaped[T,N,2], done[T,N], events[T,N,2]); int32, or with
@@ -254,9 +248,18 @@ class BatchedOvercookedEnv(object):
             return (mk((T, N), torch.int16), mk((T, N, 2), torch.int8), None, mk((T, N), torch.int16))
         dts = (torch.int16, torch.int8, torch.uint8, torch.int32) if narrow else (torch.int32,) * 4
         shapes = ((T, N), (T, N, 2), (T, N), (T, N, 2))
-        if pin:
-            return tuple(torch.empty(sh, dtype=dt, pin_memory=True) for sh, dt in zip(shapes, dts))
-        return tuple(torch.empty(sh, dtype=dt, device=self.device) for sh, dt in zip(shapes, dts))
+        return tuple(mk(sh, dt) for sh, dt in zip(shapes, dts))
+
+    def _action_flag(self, actions):
+        """Checks an action trace (int32 / uint8 CUDA [T, N, 2], or one-byte joint actions uint8 [T, N]) and returns its
+        OVC_F_ACT_* flag."""
+        assert actions.dtype in (torch.int32, torch.uint8) and actions.is_cuda and actions.is_contiguous() and actions.dim() in (2, 3)
+        assert actions.shape[1] == self.n_envs
+        if actions.dim() == 2:
+            assert actions.dtype == torch.uint8, "one-byte joint actions are uint8 [T, N]"
+            return _native.F_ACT_PACKED
+        assert actions.shape[2] == 2
+        return _native.F_ACT_U8 if actions.dtype == torch.uint8 else 0
 
     def rollout(self, actions, out=None):
         """T transitions in one launch (state stays on chip between them).
@@ -267,20 +270,11 @@ class BatchedOvercookedEnv(object):
                  sets of alloc_rollout_out(narrow= / packed= / codes=).
         Equivalent to T calls of step() with the same actions.
         """
-        assert actions.dtype in (torch.int32, torch.uint8) and actions.is_cuda and actions.is_contiguous() and actions.dim() in (2, 3)
+        flags = self._flags() | self._action_flag(actions)
         T = actions.shape[0]
-        assert actions.shape[1] == self.n_envs
         if out is None:
             out = self.alloc_rollout_out(T)
         sparse, shaped, done, events = out
-        flags = self._flags()
-        if actions.dim() == 2:
-            assert actions.dtype == torch.uint8, "one-byte joint actions are uint8 [T, N]"
-            flags |= _native.F_ACT_PACKED
-        else:
-            assert actions.shape[2] == 2
-            if actions.dtype == torch.uint8:
-                flags |= _native.F_ACT_U8
         if sparse is None:  # codes: 2 bytes per env-step
             assert shaped is None and done is None and events.dtype == torch.int16 and events.dim() == 2
             assert tuple(events.shape) == (T, self.n_envs) and events.is_cuda and events.is_contiguous()
@@ -319,26 +313,8 @@ class BatchedOvercookedEnv(object):
         assert evcode.dtype == torch.int16 and not evcode.is_cuda and evcode.is_contiguous() and evcode.dim() == 2
         T, N = evcode.shape
         assert N == self.n_envs
-        tbl = self.code_reward_table()
-        lay = self.env_layout_host
-        if self.random_layout:
-            assert (tbl == tbl[:1]).all(), "random_layout with different reward tables: the codes alone do not name the layout"
-            lay = None
-        if out is None:
-            out = {}
-            if sparse:
-                out["sparse"] = torch.empty((T, N), dtype=torch.int16)
-            if shaped:
-                out["shaped"] = torch.empty((T, N, 2), dtype=torch.int8)
-            if done:
-                out["done"] = torch.empty((T, N), dtype=torch.uint8)
-            if events:
-                out["events"] = torch.empty((T, N, 2), dtype=torch.int32)
-        ptr = lambda k: out[k].data_ptr() if k in out else 0
-        tbl = np.ascontiguousarray(tbl, dtype=np.int32)
-        _native.check(self._lib.ovc_expand_codes_host(
-            evcode.data_ptr(), T, N, 0 if lay is None else lay.ctypes.data, tbl.ctypes.data, self.n_layouts,
-            ptr("sparse"), ptr("shaped"), ptr("done"), ptr("events"), int(n_threads)))
+        out, tbl, lay, ptrs = self._dense_host_out(T, out, sparse, shaped, done, events)
+        _native.check(self._lib.ovc_expand_codes_host(evcode.data_ptr(), T, N, lay, tbl.ctypes.data, self.n_layouts, *ptrs, int(n_threads)))
         return out
 
     # ---------------------------------------------------------------------------------------------
@@ -651,8 +627,8 @@ class HostRolloutPipeline(object):
         codes=True: one byte of joint action in (wire.pack_actions, actions_host uint8 [T,N]), one int16 word of
         event codes + done + reward-grant bits out — 1 + 2 bytes per env-step, lossless (env.expand_codes).
         host_buffers: number of pinned output sets, used round robin by successive run() calls (2 lets a consumer
-        read pass i while pass i+1 is in flight, see run(wait=False))."""
-        """stream=True: the result as a sparse event stream (OVC_F_OUT_STREAM): per transition one lane mask per 32
+        read pass i while pass i+1 is in flight, see run(wait=False)).
+        stream=True: the result as a sparse event stream (OVC_F_OUT_STREAM): per transition one lane mask per 32
         environments + the non-zero code words, ``stream_fill`` x 32 x chunk value slots per group and chunk (0.125 + 2 x
         stream_fill bytes per env-step device->host instead of 2); run() returns (masks, values) host tensors and
         ``expand(result)`` rebuilds dense arrays, falling back to the dense code words kept on the device for any chunk

@@ -161,13 +161,14 @@ struct StepArgs {
     ovc_random_start_t rs;
 };
 
+// A delivered recipe's row n_onion*4 + n_tomato (rows 1,2,3,4,5,6,8,9,12) <-> its rank 0..8; event code 23 + rank
+__host__ __device__ __forceinline__ unsigned delivery_rank(unsigned row) { return (unsigned)((0x0008007605432100ull >> (row * 4)) & 15u); }
+__host__ __device__ __forceinline__ unsigned delivery_row(unsigned rank) { return (unsigned)((0xC98654321ull >> (rank * 4)) & 15u); }
+
 // 25-bit event mask (+ delivered recipe in bits 25-28) of ONE agent -> 5-bit code (see OVC_F_OUT_PACKED)
 __device__ __forceinline__ unsigned event_code(unsigned ev) {
     if ((ev & 0x1FFFFFFu) == 0) return 0;
-    if (ev & (1u << OVC_EV_SOUP_DELIVERY)) {
-        const unsigned row = (ev >> OVC_EV_RECIPE_SHIFT) & 15u;  // rows 1,2,3,4,5,6,8,9,12 -> ranks 0..8
-        return 23u + (unsigned)((0x0008007605432100ull >> (row * 4)) & 15u);
-    }
+    if (ev & (1u << OVC_EV_SOUP_DELIVERY)) return 23u + delivery_rank((ev >> OVC_EV_RECIPE_SHIFT) & 15u);
     if (ev & ((1u << OVC_EV_POTTING_ONION) | (1u << OVC_EV_POTTING_TOMATO))) {
         const unsigned tom = (ev >> OVC_EV_POTTING_TOMATO) & 1u;
         const unsigned viable = (ev >> (OVC_EV_VIABLE_ONION_POTTING + tom)) & 1u, optimal = (ev >> (OVC_EV_OPTIMAL_ONION_POTTING + tom)) & 1u;
@@ -184,23 +185,26 @@ __device__ __forceinline__ unsigned event_code(unsigned ev) {
     return 12u + ((ev >> OVC_EV_USEFUL_DISH_DROP) & 1u);  // dish_drop
 }
 
+// The 2-byte code word of one env-step (OVC_F_OUT_PACKED; OVC_F_OUT_CODES and OVC_F_OUT_STREAM add the grant bits).
+// The rollout kernel's RollIO::write spells the same expression out (see there).
+__device__ __forceinline__ unsigned code_word(unsigned c0, unsigned c1, unsigned done, bool stepped, bool grant0, bool grant1) {
+    return c0 | (c1 << 5) | (done << 10) | (stepped ? 1u << 11 : 0u) | (grant0 ? 1u << 12 : 0u) | (grant1 ? 1u << 13 : 0u);
+}
+
 // WIDE: the kernel instantiation for int32 actions and int32 outputs (the device-resident formats) — it carries
 // none of the format tests below, which cost 3 % of a fused-rollout transition when they sat in every instantiation.
 template <bool WIDE>
 __device__ __forceinline__ void write_outputs(const StepArgs &a, long long idx, const StepOut &o) {
     if (!WIDE && (a.flags & OVC_F_OUT_CODES)) {  // 2 bytes per env-step: rewards are functions of the codes + two grant bits
-        reinterpret_cast<unsigned short *>(a.events)[idx] =
-            (unsigned short)(event_code(o.ev0) | (event_code(o.ev1) << 5) | ((unsigned)o.done << 10) |
-                             ((o.ev0 & OVC_EVF_STEPPED_DONE) ? 1u << 11 : 0u) | (o.shaped0 != 0 ? 1u << 12 : 0u) |
-                             (o.shaped1 != 0 ? 1u << 13 : 0u));
+        reinterpret_cast<unsigned short *>(a.events)[idx] = (unsigned short)code_word(
+            event_code(o.ev0), event_code(o.ev1), (unsigned)o.done, o.ev0 & OVC_EVF_STEPPED_DONE, o.shaped0 != 0, o.shaped1 != 0);
         return;
     }
     if (!WIDE && (a.flags & OVC_F_OUT_PACKED)) {  // 6 bytes per env-step for host transfer
         reinterpret_cast<short *>(a.sparse)[idx] = (short)o.sparse;
         reinterpret_cast<char2 *>(a.shaped)[idx] = make_char2((signed char)o.shaped0, (signed char)o.shaped1);
-        reinterpret_cast<unsigned short *>(a.events)[idx] =
-            (unsigned short)(event_code(o.ev0) | (event_code(o.ev1) << 5) | ((unsigned)o.done << 10) |
-                             ((o.ev0 & OVC_EVF_STEPPED_DONE) ? 1u << 11 : 0u));
+        reinterpret_cast<unsigned short *>(a.events)[idx] = (unsigned short)code_word(
+            event_code(o.ev0), event_code(o.ev1), (unsigned)o.done, o.ev0 & OVC_EVF_STEPPED_DONE, false, false);
         return;
     }
     if (!WIDE && (a.flags & OVC_F_OUT_NARROW)) {  // uniform branch: int16 / int8x2 / uint8 for host transfer
@@ -402,6 +406,31 @@ static int make_tmap(CUtensorMap *m, int32_t *state, long long n_envs, int box_r
     return OVC_OK;
 }
 
+// The arrays of the transfer format that flags select (OVC_F_ACT_* / OVC_F_OUT_*): bytes per element of each, which is
+// also the alignment the kernels access it with; 0 = the format does not use the array.  An element is one env-step,
+// except with OVC_F_OUT_STREAM, whose sparse / events arrays hold value slots / lane masks sized by the group count.
+struct OutFmt {
+    int act, sparse, shaped, done, events;
+    bool stream;
+    // every array the format uses must be given, except the stream's dense backup of the code words in `done`
+    bool missing(const void *act_p, const void *sparse_p, const void *shaped_p, const void *done_p, const void *events_p) const {
+        return !act_p || !events_p || (sparse && !sparse_p) || (shaped && !shaped_p) || (done && !stream && !done_p);
+    }
+    bool wide() const { return act == 8 && sparse == 4; }  // int32 actions and int32 outputs: the device-resident formats
+};
+
+static OutFmt formats_of(int flags) {
+    OutFmt f;
+    f.act = (flags & OVC_F_ACT_PACKED) ? 1 : (flags & OVC_F_ACT_U8) ? 2 : 8;
+    f.stream = flags & OVC_F_OUT_STREAM;
+    if (f.stream) f.sparse = 2, f.shaped = 0, f.done = 2, f.events = 4;
+    else if (flags & OVC_F_OUT_CODES) f.sparse = 0, f.shaped = 0, f.done = 0, f.events = 2;
+    else if (flags & OVC_F_OUT_PACKED) f.sparse = 2, f.shaped = 2, f.done = 0, f.events = 2;
+    else if (flags & OVC_F_OUT_NARROW) f.sparse = 2, f.shaped = 2, f.done = 1, f.events = 8;
+    else f.sparse = 4, f.shaped = 8, f.done = 4, f.events = 8;
+    return f;
+}
+
 template <int S, int IO>
 static cudaError_t launch_one(const CUtensorMap &tmap, const StepArgs &a, unsigned grid, size_t smem, cudaStream_t st) {
     using C = Cfg<S>;
@@ -413,7 +442,7 @@ static cudaError_t launch_one(const CUtensorMap &tmap, const StepArgs &a, unsign
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = (a.flags & OVC_F_PDL) ? 1 : 0;
-    const bool wide = !(a.flags & (OVC_F_ACT_U8 | OVC_F_ACT_PACKED | OVC_F_OUT_NARROW | OVC_F_OUT_PACKED | OVC_F_OUT_CODES));
+    const bool wide = formats_of(a.flags).wide();
     if (a.has_rs)
         return wide ? cudaLaunchKernelEx(&cfg, step_kernel<S, IO, true, true>, tmap, a)
                     : cudaLaunchKernelEx(&cfg, step_kernel<S, IO, true, false>, tmap, a);
@@ -430,8 +459,8 @@ static int launch_rollout(const StepArgs &a, cudaStream_t st) {
     int rc = make_tmap<S>(&tmap, a.state, a.n_envs, C::BOX_ROWS);
     if (rc) return rc;
     const size_t smem = C::smem_bytes(a.n_layouts);
-    const bool wide = !(a.flags & (OVC_F_ACT_U8 | OVC_F_ACT_PACKED | OVC_F_OUT_NARROW | OVC_F_OUT_PACKED | OVC_F_OUT_CODES | OVC_F_OUT_STREAM));
-    const bool stream = a.flags & OVC_F_OUT_STREAM;
+    const OutFmt f = formats_of(a.flags);
+    const bool wide = f.wide(), stream = f.stream;
     void (*kern)(const CUtensorMap, const StepArgs) =
         a.has_rs ? (wide ? rollout_kernel<S, TILE, true, FMT_WIDE> : stream ? rollout_kernel<S, TILE, true, FMT_STREAM> : rollout_kernel<S, TILE, true, FMT_HOST>)
                  : (wide ? rollout_kernel<S, TILE, false, FMT_WIDE> : stream ? rollout_kernel<S, TILE, false, FMT_STREAM> : rollout_kernel<S, TILE, false, FMT_HOST>);
@@ -529,22 +558,16 @@ static int launch_rollout_any(const StepArgs &a0, cudaStream_t st) {
     }
     if (a0.n_steps <= max_steps) return launch_rollout_tiled<S>(a0, st);
     if (max_steps < 1 || (a0.flags & OVC_F_OUT_STREAM)) return fail(OVC_E_UNSUPPORTED, "rollout too large for one launch (n_steps * n_envs must stay below 2^32)");
-    // bytes per env-step of each array in this transfer format (the table of ovc_host.cuh: formats_of)
-    const int f = a0.flags;
-    const int b_act = (f & OVC_F_ACT_PACKED) ? 1 : (f & OVC_F_ACT_U8) ? 2 : 8;
-    int b_sparse = 4, b_shaped = 8, b_done = 4, b_events = 8;
-    if (f & OVC_F_OUT_CODES) b_sparse = 0, b_shaped = 0, b_done = 0, b_events = 2;
-    else if (f & OVC_F_OUT_PACKED) b_sparse = 2, b_shaped = 2, b_done = 0, b_events = 2;
-    else if (f & OVC_F_OUT_NARROW) b_sparse = 2, b_shaped = 2, b_done = 1, b_events = 8;
+    const OutFmt f = formats_of(a0.flags);
     for (long long t0 = 0; t0 < a0.n_steps; t0 += max_steps) {
         StepArgs a = a0;
         const long long off = t0 * a0.n_envs;
         a.n_steps = (int)(a0.n_steps - t0 < max_steps ? a0.n_steps - t0 : max_steps);
-        a.actions = reinterpret_cast<const int32_t *>(reinterpret_cast<const char *>(a0.actions) + off * b_act);
-        if (a0.sparse) a.sparse = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(a0.sparse) + off * b_sparse);
-        if (a0.shaped) a.shaped = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(a0.shaped) + off * b_shaped);
-        if (a0.done) a.done = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(a0.done) + off * b_done);
-        a.events = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(a0.events) + off * b_events);
+        a.actions = reinterpret_cast<const int32_t *>(reinterpret_cast<const char *>(a0.actions) + off * f.act);
+        if (a0.sparse) a.sparse = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(a0.sparse) + off * f.sparse);
+        if (a0.shaped) a.shaped = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(a0.shaped) + off * f.shaped);
+        if (a0.done) a.done = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(a0.done) + off * f.done);
+        a.events = reinterpret_cast<int32_t *>(reinterpret_cast<char *>(a0.events) + off * f.events);
         const int rc = launch_rollout_tiled<S>(a, st);
         if (rc) return rc;
     }
@@ -590,34 +613,26 @@ static int step_impl(const void *layouts, int n_layouts, const int32_t *start_re
                      void *stream) {
     int rc = check_common(layouts, n_layouts, state, n_envs, S);
     if (rc) return rc;
-    const bool codes = flags & OVC_F_OUT_CODES;
-    const bool is_stream = flags & OVC_F_OUT_STREAM;
-    if (is_stream && (flags & (OVC_F_OUT_CODES | OVC_F_OUT_PACKED | OVC_F_OUT_NARROW)))
+    const OutFmt f = formats_of(flags);
+    if (f.stream && (flags & (OVC_F_OUT_CODES | OVC_F_OUT_PACKED | OVC_F_OUT_NARROW)))
         return fail(OVC_E_BADARG, "OVC_F_OUT_STREAM excludes the other output formats");
-    if (!actions || !events || !start_records || (!codes && !sparse) || (!codes && !is_stream && !shaped) ||
-        (!done && !(flags & (OVC_F_OUT_PACKED | OVC_F_OUT_CODES | OVC_F_OUT_STREAM))))
-        return fail(OVC_E_BADARG, "null pointer argument");
-    if (codes) sparse = nullptr, shaped = nullptr, done = nullptr;
-    if (is_stream) {
-        shaped = nullptr;
-        if ((((unsigned)flags >> OVC_F_STREAM_CAP_SHIFT) & 0xFFFFu) == 0) return fail(OVC_E_BADARG, "OVC_F_OUT_STREAM needs a capacity in flags bits 16-31");
-        if (((uintptr_t)events & 3) || ((uintptr_t)sparse & 1) || ((uintptr_t)done & 1)) return fail(OVC_E_BADARG, "stream buffers are misaligned");
-    }
-    const bool small_out = flags & (OVC_F_OUT_NARROW | OVC_F_OUT_PACKED | OVC_F_OUT_CODES | OVC_F_OUT_STREAM);
-    const bool small_ev = flags & (OVC_F_OUT_PACKED | OVC_F_OUT_CODES | OVC_F_OUT_STREAM);
-    const bool small_act = flags & (OVC_F_ACT_U8 | OVC_F_ACT_PACKED);
-    if (((small_act ? 0 : (uintptr_t)actions) | (small_out ? 0 : (uintptr_t)shaped) | (small_ev ? 0 : (uintptr_t)events)) & 7)
-        return fail(OVC_E_BADARG, "actions / shaped / events must be 8-byte aligned");
-    if ((((flags & OVC_F_ACT_U8) ? (uintptr_t)actions : 0) | (small_out ? ((uintptr_t)shaped | (uintptr_t)sparse) : 0) |
-         (small_ev ? (uintptr_t)events : 0)) & 1)
-        return fail(OVC_E_BADARG, "narrow actions / shaped / sparse must be 2-byte aligned");
+    if (!start_records || f.missing(actions, sparse, shaped, done, events)) return fail(OVC_E_BADARG, "null pointer argument");
+    if (!f.sparse) sparse = nullptr;
+    if (!f.shaped) shaped = nullptr;
+    if (!f.done) done = nullptr;
+    if (f.stream && (((unsigned)flags >> OVC_F_STREAM_CAP_SHIFT) & 0xFFFFu) == 0)
+        return fail(OVC_E_BADARG, "OVC_F_OUT_STREAM needs a capacity in flags bits 16-31");
+    auto misaligned = [](const void *p, int bytes) { return bytes > 1 && (uintptr_t)p % (uintptr_t)bytes != 0; };
+    if (misaligned(actions, f.act) || misaligned(sparse, f.sparse) || misaligned(shaped, f.shaped) || misaligned(done, f.done) ||
+        misaligned(events, f.events))
+        return fail(OVC_E_BADARG, "actions / sparse / shaped / done / events must be aligned to their element size");
     if (n_steps < 1) return fail(OVC_E_BADARG, "n_steps must be >= 1");
     if (n_envs == 0) return OVC_OK;
     int io = (flags & OVC_F_IO_MASK) >> OVC_F_IO_SHIFT;
     if (io == 0) io = 1;
     if (io < 1 || io > 3) return fail(OVC_E_BADARG, "unknown record I/O strategy", (long long)(io));
     if (io == 1 && (n_envs * (S / (S == 16 ? 16 : 32))) > 0x7FFFFFFFLL) io = 2;  // tensor coordinates are int32
-    if (is_stream && (io != 1 || n_layouts > MAX_SMEM_LAYOUTS || n_steps > ROLLOUT_MAX_STEPS))
+    if (f.stream && (io != 1 || n_layouts > MAX_SMEM_LAYOUTS || n_steps > ROLLOUT_MAX_STEPS))
         return fail(OVC_E_UNSUPPORTED, "OVC_F_OUT_STREAM needs the rollout kernel: default record I/O, at most 8 layouts");
     StepArgs a{(const ovc_layout_t *)layouts, start_records, state, actions, sparse, shaped, done, events,
                n_envs, n_layouts, n_steps, horizon, flags, rs != nullptr, rs ? *rs : ovc_random_start_t{0, 0, 0}};

@@ -20,52 +20,29 @@
 
 namespace ovc {
 
-// code -> int32 event mask incl. the delivered-recipe bits (the inverse of event_code() in ovc_b200.cu)
-static void build_code_masks(int32_t mask[32]) {
-    for (int i = 0; i < 32; i++) mask[i] = 0;
-    const int pick[3] = {OVC_EV_ONION_PICKUP, OVC_EV_TOMATO_PICKUP, OVC_EV_DISH_PICKUP};
-    const int drop[3] = {OVC_EV_ONION_DROP, OVC_EV_TOMATO_DROP, OVC_EV_DISH_DROP};
-    for (int k = 0; k < 3; k++)
-        for (int useful = 0; useful < 2; useful++) {  // useful_<obj>_<verb> is the bit after <obj>_<verb>
-            mask[1 + 2 * k + useful] = (1 << pick[k]) | (useful << (pick[k] + 1));
-            mask[8 + 2 * k + useful] = (1 << drop[k]) | (useful << (drop[k] + 1));
-        }
-    mask[7] = 1 << OVC_EV_SOUP_PICKUP;
-    mask[14] = 1 << OVC_EV_SOUP_DROP;
-    for (int tom = 0; tom < 2; tom++) {
-        const int base = 1 << (tom ? OVC_EV_POTTING_TOMATO : OVC_EV_POTTING_ONION);
-        const int opt = 1 << (OVC_EV_OPTIMAL_ONION_POTTING + tom), via = 1 << (OVC_EV_VIABLE_ONION_POTTING + tom);
-        const int cat = 1 << (OVC_EV_CATASTROPHIC_ONION_POTTING + tom), usl = 1 << (OVC_EV_USELESS_ONION_POTTING + tom);
-        mask[15 + 4 * tom + 0] = base | opt | via;
-        mask[15 + 4 * tom + 1] = base | via;
-        mask[15 + 4 * tom + 2] = base | cat;
-        mask[15 + 4 * tom + 3] = base | opt | usl;
+// One OVC_F_OUT_CODES word -> element i of each requested dense array; tb: the reward table of the word's layout
+static inline void expand_word(unsigned w, size_t i, const int32_t *tb, const int32_t *mask, int16_t *sparse, int8_t *shaped,
+                               uint8_t *done, int32_t *events) {
+    const unsigned c0 = w & 31u, c1 = (w >> 5) & 31u;
+    if (sparse) sparse[i] = (int16_t)(tb[c0] + tb[c1]);
+    if (shaped) {
+        shaped[2 * i] = (int8_t)((w >> 12) & 1u ? tb[32 + c0] : 0);
+        shaped[2 * i + 1] = (int8_t)((w >> 13) & 1u ? tb[32 + c1] : 0);
     }
-    int rank = 0;
-    for (int row = 1; row < 16; row++)
-        if ((row >> 2) + (row & 3) <= 3) mask[23 + rank++] = (1 << OVC_EV_SOUP_DELIVERY) | (row << OVC_EV_RECIPE_SHIFT);
+    if (done) done[i] = (uint8_t)((w >> 10) & 1u);
+    if (events) {
+        const bool stepped = (w >> 11) & 1u;  // a finished env was stepped: nothing happened, only the flag is set
+        events[2 * i] = stepped ? (int32_t)OVC_EVF_STEPPED_DONE : mask[c0];
+        events[2 * i + 1] = stepped ? (int32_t)OVC_EVF_STEPPED_DONE : mask[c1];
+    }
 }
 
 static void expand_range(const uint16_t *codes, int64_t lo, int64_t hi, int64_t n_envs, const int32_t *env_layout,
                          const int32_t *reward_tbl, int16_t *sparse, int8_t *shaped, uint8_t *done, int32_t *events,
                          const int32_t *mask) {
     int64_t e = n_envs > 0 ? lo % n_envs : 0;  // env index of word i, carried instead of a 64-bit modulo per word
-    for (int64_t i = lo; i < hi; i++, e = e + 1 == n_envs ? 0 : e + 1) {
-        const unsigned w = codes[i];
-        const unsigned c0 = w & 31u, c1 = (w >> 5) & 31u;
-        const int32_t *tb = reward_tbl + (env_layout ? (size_t)env_layout[e] * 64 : 0);
-        if (sparse) sparse[i] = (int16_t)(tb[c0] + tb[c1]);
-        if (shaped) {
-            shaped[2 * i] = (int8_t)((w >> 12) & 1u ? tb[32 + c0] : 0);
-            shaped[2 * i + 1] = (int8_t)((w >> 13) & 1u ? tb[32 + c1] : 0);
-        }
-        if (done) done[i] = (uint8_t)((w >> 10) & 1u);
-        if (events) {
-            const bool stepped = (w >> 11) & 1u;  // a finished env was stepped: nothing happened, only the flag is set
-            events[2 * i] = stepped ? (int32_t)OVC_EVF_STEPPED_DONE : mask[c0];
-            events[2 * i + 1] = stepped ? (int32_t)OVC_EVF_STEPPED_DONE : mask[c1];
-        }
-    }
+    for (int64_t i = lo; i < hi; i++, e = e + 1 == n_envs ? 0 : e + 1)
+        expand_word(codes[i], (size_t)i, reward_tbl + (env_layout ? (size_t)env_layout[e] * 64 : 0), mask, sparse, shaped, done, events);
 }
 
 // A small persistent worker pool: spawning a hundred threads per call costs more than expanding 26 M words.
@@ -157,8 +134,8 @@ static int expand_codes_host(const uint16_t *codes, int64_t n_steps, int64_t n_e
     if (env_layout)
         for (int64_t e = 0; e < n_envs; e++)
             if (env_layout[e] < 0 || env_layout[e] >= n_layouts) return fail(OVC_E_BADARG, "layout id out of range", (long long)e);
-    int32_t mask[32];
-    build_code_masks(mask);
+    int32_t mask[32];  // code -> int32 event mask incl. the delivered-recipe bits
+    for (int c = 0; c < 32; c++) mask[c] = (int32_t)code_mask_of(c);
     const int64_t n = n_steps * n_envs;
     if (n_threads <= 0) n_threads = default_host_threads();
     if (n_threads > 256) n_threads = 256;
@@ -230,6 +207,10 @@ static void expand_stream_range(const uint32_t *masks, const uint16_t *values, i
     alignas(64) int8_t b_shaped[SEG_GROUPS * 64];
     alignas(64) uint8_t b_done[SEG_GROUPS * 32];
     alignas(64) int32_t b_events[SEG_GROUPS * 64];
+    int16_t *const r_sparse = sparse ? b_sparse : nullptr;  // the row buffers of the requested arrays
+    int8_t *const r_shaped = shaped ? b_shaped : nullptr;
+    uint8_t *const r_done = done ? b_done : nullptr;
+    int32_t *const r_events = events ? b_events : nullptr;
     int64_t over = 0;
     for (int64_t s0 = g0; s0 < g1; s0 += SEG_GROUPS) {
         const int64_t s1 = s0 + SEG_GROUPS < g1 ? s0 + SEG_GROUPS : g1;
@@ -256,22 +237,9 @@ static void expand_stream_range(const uint32_t *masks, const uint16_t *values, i
                     m &= m - 1;
                     const uint32_t kk = k++;
                     if (kk >= (uint64_t)cap) continue;  // dropped by the kernel: counted at the chunk boundary
-                    const unsigned w = vals[kk];
                     const int64_t e = g * 32 + l;
-                    const size_t i = (size_t)(e - e0);
-                    const unsigned c0 = w & 31u, c1 = (w >> 5) & 31u;
-                    const int32_t *tb = reward_tbl + (env_layout ? (size_t)env_layout[e] * 64 : 0);
-                    if (sparse) b_sparse[i] = (int16_t)(tb[c0] + tb[c1]);
-                    if (shaped) {
-                        b_shaped[2 * i] = (int8_t)((w >> 12) & 1u ? tb[32 + c0] : 0);
-                        b_shaped[2 * i + 1] = (int8_t)((w >> 13) & 1u ? tb[32 + c1] : 0);
-                    }
-                    if (done) b_done[i] = (uint8_t)((w >> 10) & 1u);
-                    if (events) {
-                        const bool stepped = (w >> 11) & 1u;
-                        b_events[2 * i] = stepped ? (int32_t)OVC_EVF_STEPPED_DONE : mask[c0];
-                        b_events[2 * i + 1] = stepped ? (int32_t)OVC_EVF_STEPPED_DONE : mask[c1];
-                    }
+                    expand_word(vals[kk], (size_t)(e - e0), reward_tbl + (env_layout ? (size_t)env_layout[e] * 64 : 0), mask, r_sparse,
+                                r_shaped, r_done, r_events);
                 }
             }
             const size_t row = (size_t)t * (size_t)n_envs + (size_t)e0;
@@ -297,7 +265,7 @@ static int expand_stream_host(const uint32_t *masks, const uint16_t *values, int
         for (int64_t e = 0; e < n_envs; e++)
             if (env_layout[e] < 0 || env_layout[e] >= n_layouts) return fail(OVC_E_BADARG, "layout id out of range", (long long)e);
     int32_t mask[32];
-    build_code_masks(mask);
+    for (int c = 0; c < 32; c++) mask[c] = (int32_t)code_mask_of(c);
     const int64_t G = (n_envs + 31) / 32;
     int64_t over = 0;
     if (n_threads <= 0) n_threads = default_host_threads();
@@ -319,23 +287,6 @@ static int expand_stream_host(const uint32_t *masks, const uint16_t *values, int
 // ------------------------------------------------------------------------------------------------
 // host-buffer rollout pipeline (ovc_pipeline_*): H2D / rollout kernel / D2H on three streams
 // ------------------------------------------------------------------------------------------------
-struct OutFmt {
-    int act, sparse, shaped, done, events;  // bytes per env-step of each array (0 = not produced)
-    bool stream;                            // OVC_F_OUT_STREAM: sizes come from the group count and the capacity instead
-};
-
-static OutFmt formats_of(int flags) {
-    OutFmt f;
-    f.act = (flags & OVC_F_ACT_PACKED) ? 1 : (flags & OVC_F_ACT_U8) ? 2 : 8;
-    f.stream = flags & OVC_F_OUT_STREAM;
-    if (f.stream) f.sparse = 0, f.shaped = 0, f.done = 0, f.events = 0;
-    else if (flags & OVC_F_OUT_CODES) f.sparse = 0, f.shaped = 0, f.done = 0, f.events = 2;
-    else if (flags & OVC_F_OUT_PACKED) f.sparse = 2, f.shaped = 2, f.done = 0, f.events = 2;
-    else if (flags & OVC_F_OUT_NARROW) f.sparse = 2, f.shaped = 2, f.done = 1, f.events = 8;
-    else f.sparse = 4, f.shaped = 8, f.done = 4, f.events = 8;
-    return f;
-}
-
 }  // namespace ovc
 
 struct ovc_pipeline {
@@ -365,8 +316,7 @@ static int pipeline_create(const ovc_pipeline_desc_t *desc, ovc_pipeline_t **out
     if (rc) return rc;
     const OutFmt f = formats_of(desc->flags);
     for (int b = 0; b < 2; b++)
-        if (!desc->d_actions[b] || !desc->d_events[b] || ((f.sparse || f.stream) && !desc->d_sparse[b]) || (f.shaped && !desc->d_shaped[b]) ||
-            (f.done && !desc->d_done[b]))
+        if (f.missing(desc->d_actions[b], desc->d_sparse[b], desc->d_shaped[b], desc->d_done[b], desc->d_events[b]))
             return fail(OVC_E_BADARG, "missing device staging buffer");
     if (f.stream && (desc->stream_cap < 1 || desc->stream_cap > OVC_F_STREAM_CAP_MAX))
         return fail(OVC_E_BADARG, "stream_cap must be 1..65535", (long long)desc->stream_cap);
@@ -403,8 +353,7 @@ static int pipeline_join(ovc_pipeline_t *p, cudaStream_t caller) {
 static int pipeline_run(ovc_pipeline_t *p, const void *h_actions, void *h_sparse, void *h_shaped, void *h_done, void *h_events,
                         int n_steps, cudaStream_t caller, int join, int64_t *ticket) {
     const OutFmt &f = p->fmt;
-    if (!h_actions || !h_events || ((f.sparse || f.stream) && !h_sparse) || (f.shaped && !h_shaped) || (f.done && !h_done))
-        return fail(OVC_E_BADARG, "null host buffer");
+    if (f.missing(h_actions, h_sparse, h_shaped, h_done, h_events)) return fail(OVC_E_BADARG, "null host buffer");
     if (n_steps < 1) return fail(OVC_E_BADARG, "n_steps must be >= 1");
     const ovc_pipeline_desc_t &d = p->d;
     const size_t N = (size_t)d.n_envs, G = (N + 31) / 32;
@@ -440,15 +389,16 @@ static int pipeline_run(ovc_pipeline_t *p, const void *h_actions, void *h_sparse
         p->comp_rec[b] = true;
         // stage 3: results to the host
         OVC_CK(cudaStreamWaitEvent(p->s_d2h, p->ev_comp[b], 0), "pipeline wait");
-        if (f.sparse) OVC_CK(cudaMemcpyAsync((char *)h_sparse + off * f.sparse, d.d_sparse[b], cnt * f.sparse, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
-        if (f.shaped) OVC_CK(cudaMemcpyAsync((char *)h_shaped + off * f.shaped, d.d_shaped[b], cnt * f.shaped, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
-        if (f.done) OVC_CK(cudaMemcpyAsync((char *)h_done + off * f.done, d.d_done[b], cnt * f.done, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
-        if (f.stream) {
-            const size_t c = (size_t)(t0 / d.chunk), vbytes = G * (size_t)d.stream_cap * 2;
-            OVC_CK(cudaMemcpyAsync((char *)h_events + (size_t)t0 * G * 4, d.d_events[b], (size_t)tc * G * 4, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
+        if (f.stream) {  // the lane masks and the value slots; the dense backup stays on the device
+            const size_t c = (size_t)(t0 / d.chunk), vbytes = G * (size_t)d.stream_cap * f.sparse;
+            OVC_CK(cudaMemcpyAsync((char *)h_events + (size_t)t0 * G * f.events, d.d_events[b], (size_t)tc * G * f.events, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
             OVC_CK(cudaMemcpyAsync((char *)h_sparse + c * vbytes, d.d_sparse[b], vbytes, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
-        } else
+        } else {
+            if (f.sparse) OVC_CK(cudaMemcpyAsync((char *)h_sparse + off * f.sparse, d.d_sparse[b], cnt * f.sparse, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
+            if (f.shaped) OVC_CK(cudaMemcpyAsync((char *)h_shaped + off * f.shaped, d.d_shaped[b], cnt * f.shaped, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
+            if (f.done) OVC_CK(cudaMemcpyAsync((char *)h_done + off * f.done, d.d_done[b], cnt * f.done, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
             OVC_CK(cudaMemcpyAsync((char *)h_events + off * f.events, d.d_events[b], cnt * f.events, cudaMemcpyDeviceToHost, p->s_d2h), "pipeline D2H copy");
+        }
         OVC_CK(cudaEventRecord(p->ev_d2h[b], p->s_d2h), "pipeline record");
         p->d2h_rec[b] = true;
     }

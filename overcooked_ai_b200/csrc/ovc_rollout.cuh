@@ -96,8 +96,9 @@ __device__ __forceinline__ int recipe_row5(unsigned k5) {  // (count, kinds) fie
     return ((n - nt) << 2) | nt;
 }
 
-// 5-bit event code -> 25-bit event mask (+ delivered recipe in bits 25-28); inverse of event_code()
-__device__ __forceinline__ unsigned code_mask_of(int c) {
+// 5-bit event code -> 25-bit event mask (+ delivered recipe in bits 25-28); inverse of event_code().  The host
+// expanders (ovc_host.cuh) fill their table from it too.
+__host__ __device__ __forceinline__ unsigned code_mask_of(int c) {
     if (c == 0) return 0u;
     if (c <= 6) {
         const int b = (0x0A0005 >> (((c - 1) >> 1) * 8)) & 0xFF;  // onion / tomato / dish _pickup
@@ -116,8 +117,7 @@ __device__ __forceinline__ unsigned code_mask_of(int c) {
         const unsigned cat = 1u << (OVC_EV_CATASTROPHIC_ONION_POTTING + tom), usl = 1u << (OVC_EV_USELESS_ONION_POTTING + tom);
         return base | (cls == 0 ? (opt | via) : cls == 1 ? via : cls == 2 ? cat : (opt | usl));
     }
-    const unsigned row = (unsigned)((0xC98654321ull >> ((c - 23) * 4)) & 15u);  // rank -> n_onion*4 + n_tomato
-    return (1u << OVC_EV_SOUP_DELIVERY) | (row << OVC_EV_RECIPE_SHIFT);
+    return (1u << OVC_EV_SOUP_DELIVERY) | (delivery_row((unsigned)(c - 23)) << OVC_EV_RECIPE_SHIFT);
 }
 
 // Shared-memory record of one thread.  The TMA swizzle XORs the 16-byte-chunk index with address bits 7.. ; for
@@ -310,6 +310,8 @@ struct RollIO {
             // What a rollout produces is mostly zeros.  Per warp (32 consecutive environments) and transition: ONE
             // 32-bit lane mask of the non-zero code words (__ballot_sync), and the non-zero words compacted behind the
             // group's earlier ones (rank among the voters = popcount of the lower lanes).
+            // The code word of code_word() (ovc_b200.cu), spelled out here and below: built through that function the
+            // stream and host-format kernels compile to different code, and the stream kernel ran 3 % slower (H100).
             const unsigned w = o.c0 | (o.c1 << 5) | ((unsigned)done_v << 10) | (stepped ? 1u << 11 : 0u) |
                                (o.sh0 != 0 ? 1u << 12 : 0u) | (o.sh1 != 0 ? 1u << 13 : 0u);
             const unsigned m = __ballot_sync(live_mask, w != 0);
@@ -417,7 +419,7 @@ rollout_kernel(const __grid_constant__ CUtensorMap tmap, const StepArgs a) {
             const int n = k5 & 3, row = recipe_row5(k5);
             D->cook5[k5] = L->cook_time[row];
             D->deliver5[k5] = L->deliver_value[row];
-            D->dcode5[k5] = (uint8_t)(23u + (unsigned)((0x0008007605432100ull >> (row * 4)) & 15u));
+            D->dcode5[k5] = (uint8_t)(23u + delivery_rank((unsigned)row));
             const int old_val = L->best_value[n ? row : 0];
 #pragma unroll
             for (int tom = 0; tom < 2; tom++) {  // log_object_potting :2121-2140 + is_potting_* :2256-2308

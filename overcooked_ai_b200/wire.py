@@ -93,6 +93,9 @@ def replay_table(layout, state_dicts, joint_actions, rewards=None):
     return rec, act, rew
 
 
+_DELIVERY_ROWS = [r for r in range(1, 16) if (r >> 2) + (r & 3) <= 3]  # n_onion*4 + n_tomato: 1,2,3,4,5,6,8,9,12 (code 23 + rank)
+
+
 def _event_code_table():
     """32 event codes (include/ovc_b200.h, OVC_F_OUT_PACKED) -> int32 event mask incl. the delivered-recipe bits."""
     E = {n: i for i, n in enumerate(L.EVENT_TYPES)}
@@ -107,8 +110,7 @@ def _event_code_table():
         combos = (("optimal", "viable"), ("viable",), ("catastrophic",), ("optimal", "useless"))
         for c, names in enumerate(combos):
             t[15 + 4 * k + c] = base | sum(1 << E["%s_%s_potting" % (nm, obj)] for nm in names)
-    rows = [r for r in range(1, 16) if (r >> 2) + (r & 3) <= 3]  # 1,2,3,4,5,6,8,9,12
-    for rank, row in enumerate(rows):
+    for rank, row in enumerate(_DELIVERY_ROWS):
         t[23 + rank] = (1 << E["soup_delivery"]) | (row << L.EV_RECIPE_SHIFT)
     return t.astype(np.int32)
 
@@ -127,9 +129,8 @@ def code_reward_table(layouts):
     """int32 [n_layouts, 2, 32]: [l][0][code] = delivery reward of the code's recipe on layout l, [l][1][code] = the
     shaped reward an agent gets WITH that code when its grant bit is set (include/ovc_b200.h, OVC_F_OUT_CODES)."""
     t = np.zeros((len(layouts), 2, 32), np.int32)
-    rows = [r for r in range(1, 16) if (r >> 2) + (r & 3) <= 3]
     for i, l in enumerate(layouts):
-        for rank, row in enumerate(rows):
+        for rank, row in enumerate(_DELIVERY_ROWS):
             t[i, 0, 23 + rank] = int(l.deliver_value[row])
         t[i, 1, 15:23] = int(l.reward_shaping_params["PLACEMENT_IN_POT_REW"])
         t[i, 1, 6] = int(l.reward_shaping_params["DISH_PICKUP_REWARD"])

@@ -873,7 +873,8 @@ def test_more_than_eight_layouts_uses_global_tables():
     assert env.n_layouts == 12 and env.state_words == 32
     rng = np.random.RandomState(12)
     acts = _random_actions(rng, 100, n, 0.4)
-    ref_state = _np(env.state).copy()
+    s0 = _np(env.state).copy()
+    ref_state = s0.copy()
     want = cpu.rollout(env._tab_host, env._starts_host, ref_state, acts, horizon=40, flags=1, n_threads=4)
     d = torch.from_numpy(acts).cuda()
     for t in range(30):
@@ -883,6 +884,16 @@ def test_more_than_eight_layouts_uses_global_tables():
     got = env.rollout(d[30:].contiguous())
     for g, w in zip(got, want):
         assert np.array_equal(_np(g), w[30:])
+    assert np.array_equal(_np(env.state), ref_state)
+    # OVC_F_OUT_CODES through the step kernel's multi-transition loop (the rollout kernel takes at most 8 layouts)
+    from overcooked_ai_b200 import wire
+
+    env.state.copy_(torch.from_numpy(s0))
+    words = env.alloc_rollout_out(100, codes=True)[3]
+    env.rollout(torch.from_numpy(wire.pack_actions(acts)).cuda(), out=(None, None, None, words))
+    dense = env.expand_codes(words.cpu(), events=True)
+    for k, w in zip(("sparse", "shaped", "done", "events"), want):
+        assert np.array_equal(dense[k].numpy(), w), k
     assert np.array_equal(_np(env.state), ref_state)
     f = _np(env.featurize_state(2))
     assert np.array_equal(f.astype(np.float64), cpu.featurize(env._tab_host, lut_bytes(env.layouts), ref_state, 2))
@@ -944,6 +955,12 @@ def test_packed_event_codes_cover_every_event_pattern():
         ev, dn = wire.decode_event_codes(_np(out[3]))
         assert np.array_equal(ev, _np(full[3])) and np.array_equal(_np(out[0]), _np(full[0])) and np.array_equal(_np(out[1]), _np(full[1]))
         seen |= set(np.unique(_np(out[3]).astype(np.int32) & 31).tolist()) | set(np.unique((_np(out[3]).astype(np.int32) >> 5) & 31).tolist())
+        env.state.copy_(torch.from_numpy(s0))  # OVC_F_OUT_CODES from the step kernel (T = 1), one-byte actions
+        words = env.alloc_rollout_out(1, codes=True)[3]
+        env.rollout(torch.from_numpy(wire.pack_actions(a)[None]).cuda(), out=(None, None, None, words))
+        dense = env.expand_codes(words.cpu(), events=True)
+        for k, f in zip(("sparse", "shaped", "done", "events"), full):
+            assert np.array_equal(dense[k].numpy(), _np(f)), (path, k)
     assert len(seen) >= 24, sorted(seen)
     env = BatchedOvercookedEnv("cramped_room", 64, horizon=3, auto_reset=False)
     acts = torch.zeros((5, 64, 2), dtype=torch.uint8, device="cuda")
@@ -1006,6 +1023,11 @@ env.reset()
 out = env.alloc_rollout_out(T, packed=True)                           # uint8 actions, packed outputs
 env.rollout(torch.from_numpy(acts.astype(np.uint8)).cuda(), out=out)
 assert np.array_equal(out[0].cpu().numpy(), want[0]) and np.array_equal(out[1].cpu().numpy(), want[1])
+env.reset()
+out = env.alloc_rollout_out(T, narrow=True)                           # uint8 actions, narrow outputs
+env.rollout(torch.from_numpy(acts.astype(np.uint8)).cuda(), out=out)
+for g, w in zip(out, want):
+    assert np.array_equal(g.cpu().numpy(), w)
 print("CUT_OK")
 """
     out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600,

@@ -439,6 +439,35 @@ def test_pipeline_descriptor_layout_matches_the_c_struct():
     lib.ovc_pipeline_destroy(None)
 
 
+@pytest.mark.parametrize("fmt", ["int32", "narrow", "packed", "codes", "stream"])
+def test_rollout_refuses_arrays_that_break_their_alignment(fmt):
+    """ovc_rollout and ovc_step refuse an action or output array that is not aligned to the element size its transfer
+    format stores it with (OVC_E_BADARG), and accept the same call with aligned arrays.  Every call has n_envs = 0 and is
+    refused or accepted before anything is launched: no GPU is needed and no kernel runs."""
+    lib = _native.lib()
+    buf = (ctypes.c_char * 4096)()
+    base = ctypes.addressof(buf) + (-ctypes.addressof(buf)) % 64  # 64-byte aligned; nothing is dereferenced
+    stream = _native.F_OUT_STREAM | (8 << _native.F_STREAM_CAP_SHIFT)
+    # output flag, and the alignment of sparse / shaped / done / events (0: the format does not use the array)
+    out_flag, out_align = {"int32": (0, (4, 8, 4, 8)), "narrow": (_native.F_OUT_NARROW, (2, 2, 1, 8)),
+                           "packed": (_native.F_OUT_PACKED, (2, 2, 0, 2)), "codes": (_native.F_OUT_CODES, (0, 0, 0, 2)),
+                           "stream": (stream, (2, 0, 2, 4))}[fmt]
+    for act_flag, act_align in ((0, 8), (_native.F_ACT_U8, 2), (_native.F_ACT_PACKED, 1)):
+        flags = out_flag | act_flag
+        calls = [lambda p: lib.ovc_rollout(base, 1, base, base, *p, 0, 3, 16, 400, flags, None, None)]
+        if fmt != "stream":
+            calls.append(lambda p: lib.ovc_step(base, 1, base, base, *p, 0, 16, 400, flags, None, None))
+        for call in calls:
+            ptrs = [base + 512 * k for k in range(5)]  # actions, sparse, shaped, done, events
+            assert call(ptrs) == 0, lib.ovc_last_error().decode()
+            for k, align in enumerate((act_align,) + out_align):
+                if align > 1:
+                    bad = list(ptrs)
+                    bad[k] += align // 2
+                    rc = call(bad)
+                    assert rc == -1 and "aligned" in lib.ovc_last_error().decode(), (fmt, act_flag, k, rc)
+
+
 def test_recipe_config_validity_rules():
     """Recipe.configure's rules (overcooked_mdp.py:236-300) as restated in layout._check_recipe_config; the verdicts
     below are the reference's (tests/test_oracle_live_reference.py checks them live where the reference is present)."""
