@@ -535,6 +535,31 @@ int ovc_policy_tail_logp(const void *x, int64_t n_rows, int k0, float in_slope, 
                          const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                          float slope, int n_actions, uint64_t seed, uint64_t *counter, int32_t *actions, float *values,
                          float *scores, float *logp, void *stream);
+/* ovc_policy_hidden: ovc_policy_tail's layers up to the last 64-wide one, without the heads and the draw:
+ * hidden bfloat16 [n_rows][64] = that layer's activation a (rounded to bfloat16 as above).  The input of the LSTM policy
+ * (ovc_lstm_head).  Arguments as ovc_policy_tail's; hidden 4-byte aligned. */
+int ovc_policy_hidden(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                      const void *w_hidden, const float *b_hidden, int n_hidden, float slope, void *hidden, void *stream);
+
+/*
+ * ovc_lstm_head (K11): the recurrent end of the reference's LSTM PPO model (ppo_rllib.py:89-238, RllibLSTMPPOModel:
+ * tf.keras.layers.LSTM(256) on the dense layers' output, the logits / value heads on its output) and the action draw:
+ *   x bfloat16 [n_rows][64]; h_in bfloat16 [n_rows][256], c_in float32 [n_rows][256], both taken as zero for rows 2 e, 2 e + 1
+ *     where reset[e] != 0 (reset int32 [ceil(n_rows / 2)], nullable: no reset)
+ *   gates = [x | h_in] . w^T + b        w bfloat16 [1024][320] = [W_ih | W_hh], b float32 [1024] = b_ih + b_hh, gate rows
+ *                                       permuted: row 64 j + 8 (4 half + gate) + n is gate (i, f, g, o) of hidden unit
+ *                                       16 j + 8 half + n
+ *   c_out = sigmoid(f) * c_in + sigmoid(i) * tanh(g);   h_out = bfloat16(sigmoid(o) * tanh(c_out))
+ *   s = h_out . w_heads^T + b_heads     w_heads bfloat16 [8][256]: heads 0..n_actions-1 the logits, head n_actions the value
+ *   actions / values / logp / scores as ovc_policy_tail_logp's (same seed / counter semantics; values, logp, scores nullable)
+ *   snap_h bfloat16 / snap_c float32 [n_rows][256] (nullable): the state the row used, after the reset rule.
+ * h_out / c_out may alias h_in / c_in (in-place update).  float32 accumulation (mma.sync m16n8k16), accurate expf / tanhf.
+ * x, h_in, w, w_heads, snap_h 16-byte aligned; c_in, c_out, snap_c, b, b_heads, scores 8-byte aligned.
+ */
+int ovc_lstm_head(const void *x, const void *h_in, const float *c_in, const int32_t *reset, int64_t n_rows, const void *w,
+                  const float *b, const void *w_heads, const float *b_heads, int n_actions, uint64_t seed, uint64_t *counter,
+                  void *h_out, float *c_out, void *snap_h, float *snap_c, int32_t *actions, float *values, float *logp,
+                  float *scores, void *stream);
 
 /*
  * ovc_wide_layers (K9): the two wide layers of the rollout policy between ovc_encode_linear and ovc_policy_tail

@@ -84,6 +84,8 @@ def lib():
     L.ovc_accumulate_returns.argtypes = [vp, vp, ctypes.c_float, i64, vp, vp, vp]
     L.ovc_policy_tail.argtypes = [vp, i64, i32, ctypes.c_float, vp, vp, vp, vp, i32, vp, vp, ctypes.c_float, i32, ctypes.c_uint64, vp, vp, vp, vp, vp]
     L.ovc_policy_tail_logp.argtypes = L.ovc_policy_tail.argtypes[:-1] + [vp, vp]
+    L.ovc_policy_hidden.argtypes = [vp, i64, i32, ctypes.c_float, vp, vp, vp, vp, i32, ctypes.c_float, vp, vp]
+    L.ovc_lstm_head.argtypes = [vp, vp, vp, vp, i64, vp, vp, vp, vp, i32, ctypes.c_uint64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.ovc_sample_actions_logp.argtypes = [vp, i32, i32, i64, ctypes.c_uint64, vp, vp, vp, vp]
     L.ovc_record_transition.argtypes = [vp, vp, vp, vp, i64, vp, vp, vp, vp, vp]
     L.ovc_record_transition_stats.argtypes = [vp, vp, vp, vp, i64, vp, vp, vp, vp, ctypes.POINTER(EpisodeStatsDesc), vp]
@@ -103,7 +105,7 @@ def lib():
     L.ovc_pipeline_destroy.argtypes = [vp]
     L.ovc_pipeline_destroy.restype = None
     for f in (L.ovc_step, L.ovc_rollout, L.ovc_reset, L.ovc_encode_lossless, L.ovc_encode_linear, L.ovc_sample_actions, L.ovc_accumulate_returns, L.ovc_policy_tail, L.ovc_wide_layers, L.ovc_featurize, L.ovc_potential,
-              L.ovc_policy_tail_logp, L.ovc_sample_actions_logp, L.ovc_record_transition, L.ovc_record_transition_stats, L.ovc_gae, L.ovc_partner_policy, L.ovc_assign_partners, L.ovc_expand_codes_host, L.ovc_expand_stream_host, L.ovc_pipeline_create, L.ovc_pipeline_run, L.ovc_pipeline_wait, L.ovc_pipeline_join):
+              L.ovc_policy_tail_logp, L.ovc_policy_hidden, L.ovc_lstm_head, L.ovc_sample_actions_logp, L.ovc_record_transition, L.ovc_record_transition_stats, L.ovc_gae, L.ovc_partner_policy, L.ovc_assign_partners, L.ovc_expand_codes_host, L.ovc_expand_stream_host, L.ovc_pipeline_create, L.ovc_pipeline_run, L.ovc_pipeline_wait, L.ovc_pipeline_join):
         f.restype = i32
     if L.ovc_abi_version() != ABI_VERSION:
         raise NativeLibraryError("ABI version mismatch: library %d, binding %d" % (L.ovc_abi_version(), ABI_VERSION))
@@ -116,7 +118,7 @@ EXPORTED_SYMBOLS = (
     "ovc_step", "ovc_rollout", "ovc_reset", "ovc_encode_lossless", "ovc_encode_linear", "ovc_sample_actions", "ovc_accumulate_returns", "ovc_policy_tail", "ovc_wide_layers", "ovc_featurize", "ovc_potential",
     "ovc_potential_table_size", "ovc_expand_codes_host", "ovc_expand_stream_host",
     "ovc_policy_tail_logp", "ovc_sample_actions_logp", "ovc_record_transition", "ovc_record_transition_stats", "ovc_gae",
-    "ovc_partner_policy", "ovc_assign_partners",
+    "ovc_partner_policy", "ovc_assign_partners", "ovc_policy_hidden", "ovc_lstm_head",
     "ovc_pipeline_create", "ovc_pipeline_run", "ovc_pipeline_wait", "ovc_pipeline_join", "ovc_pipeline_destroy",
 )
 

@@ -652,6 +652,7 @@ static int step_impl(const void *layouts, int n_layouts, const int32_t *start_re
 #include "ovc_tail.cuh"
 #include "ovc_wide.cuh"
 #include "ovc_partner.cuh"
+#include "ovc_lstm.cuh"
 #include "ovc_potential.cuh"
 #include "ovc_host.cuh"
 
@@ -766,6 +767,30 @@ int ovc_policy_tail_logp(const void *x, int64_t n_rows, int k0, float in_slope, 
     a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
     a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
     return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream);
+}
+
+int ovc_policy_hidden(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                      const void *w_hidden, const float *b_hidden, int n_hidden, float slope, void *hidden, void *stream) {
+    ovc::PolicyTailArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
+    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden;
+    a.w_heads = (const __nv_bfloat16 *)w_first, a.b_heads = b_first;  // staged, never read (see policy_tail_impl)
+    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = 1, a.in_slope = in_slope, a.slope = slope, a.seed = 0;
+    a.counter = nullptr, a.actions = nullptr, a.values = nullptr, a.hidden = (__nv_bfloat16 *)hidden, a.logp = nullptr;
+    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, true);
+}
+
+int ovc_lstm_head(const void *x, const void *h_in, const float *c_in, const int32_t *reset, int64_t n_rows, const void *w,
+                  const float *b, const void *w_heads, const float *b_heads, int n_actions, uint64_t seed, uint64_t *counter,
+                  void *h_out, float *c_out, void *snap_h, float *snap_c, int32_t *actions, float *values, float *logp,
+                  float *scores, void *stream) {
+    ovc::LstmHeadArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.h_in = (const __nv_bfloat16 *)h_in, a.c_in = c_in, a.reset = reset, a.n_rows = n_rows;
+    a.w = (const __nv_bfloat16 *)w, a.b = b, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
+    a.n_actions = n_actions, a.seed = seed, a.counter = (unsigned long long *)counter;
+    a.h_out = (__nv_bfloat16 *)h_out, a.c_out = c_out, a.snap_h = (__nv_bfloat16 *)snap_h, a.snap_c = snap_c;
+    a.actions = actions, a.values = values, a.logp = logp, a.scores = scores;
+    return ovc::lstm_head_impl(a, (cudaStream_t)stream);
 }
 
 int ovc_policy_tail(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,

@@ -40,8 +40,11 @@ struct PolicyTailArgs {
     unsigned long long *counter;   // [2]: step, arrival scratch (as ovc_sample_actions)
     int32_t *actions;              // [n_rows]
     float *values;                 // [n_rows] or null
-    float *scores;                 // [n_rows][8] or null
-    float *logp;                   // [n_rows] or null: log-probability of the drawn action (policy_tail_kernel<KS2, true>)
+    union {                        // (a union: the parameter block, and so the code, of the drawing kernels stays as it was)
+        float *scores;             // [n_rows][8] or null
+        __nv_bfloat16 *hidden;     // [n_rows][64]: the last 64-wide activation (policy_tail_kernel<KS2, false, true>)
+    };
+    float *logp;                   // [n_rows] or null: log-probability of the drawn action (policy_tail_kernel<KS2, true, false>)
 };
 
 __device__ __forceinline__ void mma_bf16_16816(float c[4], const unsigned a[4], unsigned b0, unsigned b1) {
@@ -158,15 +161,25 @@ __device__ __forceinline__ void first_layer64(float acc[8][4], const TailSmem &w
 }
 
 // The layers after the first: ReLU-family activation, n_hidden 64 -> 64 layers, then the heads.  out[0][0..1]: heads 2 t,
-// 2 t + 1 of row g; out[0][2..3]: the same of row g + 8.
-__device__ __forceinline__ void tail_layers(float out[1][4], float acc[8][4], const TailSmem &w, int n_hidden, float slope, int g, int t) {
+// 2 t + 1 of row g; out[0][2..3]: the same of row g + 8.  Without ``out`` (HEADS false) it stops before the heads and
+// leaves the last layer's activations bf16(act(z)) in ``a`` as A fragments.
+template <bool HEADS = true>
+__device__ __forceinline__ void tail_layers(float out[1][4], float acc[8][4], const TailSmem &w, int n_hidden, float slope, int g, int t,
+                                            unsigned (*a_out)[4] = nullptr) {
     unsigned a[4][4];
     to_fragments(a, acc, slope);
     for (int l = 0; l < n_hidden; l++) {
         dense64<8>(acc, a, w.wh + l * PT_H * PT_HS, w.bh + l * PT_H, g, t);
         to_fragments(a, acc, slope);
     }
-    dense64<1>(out, a, w.wo, w.bo, g, t);
+    if constexpr (HEADS) {
+        dense64<1>(out, a, w.wo, w.bo, g, t);
+    } else {
+#pragma unroll
+        for (int s = 0; s < 4; s++)
+#pragma unroll
+            for (int i = 0; i < 4; i++) a_out[s][i] = a[s][i];
+    }
 }
 
 // The draw of ovc_sample_actions on one row whose heads 2 t, 2 t + 1 (s0, s1) lane t of the row's four lanes holds: they
@@ -218,12 +231,15 @@ __device__ __forceinline__ void advance_step(unsigned long long *counter, unsign
     }
 }
 
-template <int KS2, bool LOGP>  // K0 = 32 * KS2; LOGP: also write p.logp (a separate instantiation, so the plain draw is untouched)
+// K0 = 32 * KS2; LOGP: also write p.logp (a separate instantiation, so the plain draw is untouched); HIDDEN: stop after the
+// last 64-wide layer and write its activations to p.hidden instead of the heads and the draw (the LSTM policy's input;
+// the counter is neither read nor advanced)
+template <int KS2, bool LOGP, bool HIDDEN>
 __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const PolicyTailArgs p) {
     constexpr int K0 = 32 * KS2;
     extern __shared__ __align__(16) char pt_smem[];
 
-    const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(p.counter);
+    const unsigned long long step = HIDDEN ? 0ull : *reinterpret_cast<volatile unsigned long long *>(p.counter);
     // ---- weights into shared memory ----
     const TailSmem w = tail_weights_to_smem<K0, PT_THREADS>(pt_smem, p);
     __syncthreads();
@@ -247,6 +263,18 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const Policy
             a_hi[0] = lrelu_bf16x2(xa[s2].z, in_slope2), a_hi[1] = lrelu_bf16x2(xb[s2].z, in_slope2);
             a_hi[2] = lrelu_bf16x2(xa[s2].w, in_slope2), a_hi[3] = lrelu_bf16x2(xb[s2].w, in_slope2);
         });
+        if constexpr (HIDDEN) {  // the A fragments of the last layer's activations, written as [row][64]
+            unsigned a[4][4];
+            tail_layers<false>(nullptr, acc, w, p.n_hidden, p.slope, g, t, a);
+#pragma unroll
+            for (int s = 0; s < 4; s++) {
+                unsigned *h0 = reinterpret_cast<unsigned *>(p.hidden + r0 * PT_H + 16 * s + 2 * t);
+                unsigned *h1 = reinterpret_cast<unsigned *>(p.hidden + r1 * PT_H + 16 * s + 2 * t);
+                if (r0 < p.n_rows) h0[0] = a[s][0], h0[4] = a[s][2];
+                if (r1 < p.n_rows) h1[0] = a[s][1], h1[4] = a[s][3];
+            }
+            continue;
+        }
         // ---- hidden layers and heads: fragments in, fragments out ----
         float out[1][4];
         tail_layers(out, acc, w, p.n_hidden, p.slope, g, t);
@@ -269,13 +297,17 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const Policy
             }
         }
     }
-    advance_step(p.counter, step);
+    if constexpr (!HIDDEN) advance_step(p.counter, step);
 }
 
-static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st) {
-    if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || !a.counter || !a.actions || (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)))
+// hid: the HIDDEN instantiation into a.hidden (no heads, no draw; a.w_heads / a.b_heads are staged but never read, so the
+// entry point passes the first layer's tables, which are at least as large, in their place)
+static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bool hid = false) {
+    if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || (hid ? !a.hidden : (!a.counter || !a.actions)) ||
+        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)))
         return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)a.x | (uintptr_t)a.w_first) & 15) != 0) return fail(OVC_E_BADARG, "x and w_first must be 16-byte aligned");
+    if (hid && ((uintptr_t)a.hidden & 3) != 0) return fail(OVC_E_BADARG, "hidden must be 4-byte aligned");
     if (k0 < 32 || k0 > 256 || k0 % 32) return fail(OVC_E_BADARG, "k0 must be a multiple of 32 in 32..256", k0);
     if (a.n_hidden < 0 || a.n_hidden > 8) return fail(OVC_E_BADARG, "n_hidden must be 0..8", a.n_hidden);
     if (a.n_actions < 1 || a.n_actions > 7) return fail(OVC_E_BADARG, "n_actions must be 1..7 (head n_actions is the value)", a.n_actions);
@@ -291,12 +323,15 @@ static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st) {
     cudaError_t e = cudaSuccess;
 #define OVC_LAUNCH_PT(KS2)                                                                                              \
     case KS2:                                                                                                           \
-        if (a.logp) {                                                                                                   \
-            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (e == cudaSuccess) policy_tail_kernel<KS2, true><<<grid, PT_THREADS, smem, st>>>(a);                    \
+        if (hid) {                                                                                                      \
+            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            if (e == cudaSuccess) policy_tail_kernel<KS2, false, true><<<grid, PT_THREADS, smem, st>>>(a);             \
+        } else if (a.logp) {                                                                                            \
+            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            if (e == cudaSuccess) policy_tail_kernel<KS2, true, false><<<grid, PT_THREADS, smem, st>>>(a);             \
         } else {                                                                                                        \
-            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (e == cudaSuccess) policy_tail_kernel<KS2, false><<<grid, PT_THREADS, smem, st>>>(a);                   \
+            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            if (e == cudaSuccess) policy_tail_kernel<KS2, false, false><<<grid, PT_THREADS, smem, st>>>(a);            \
         }                                                                                                               \
         break;
     switch (k0 / 32) {

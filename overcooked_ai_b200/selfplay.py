@@ -17,6 +17,8 @@ of 64, leaky ReLU, heads 6 + 1), random init, shared by both agents.  ``RllibSha
 (the module a user trains and loads weights into); ``DenseGridPolicy`` is the same function as one matrix per layer,
 the network ``SelfPlayRollout`` evaluates: on a 5x4 grid entirely with this library's kernels K7, K9 and K8.
 """
+import copy
+
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -60,14 +62,88 @@ class RllibShapedCNN(nn.Module):
             self.value.weight.copy_(t(value[0]).t()), self.value.bias.copy_(t(value[1]))
         return self
 
-    def forward(self, obs_nchw):
+    dense_slope = 0.3  # RllibPPOModel's LeakyReLU() layers (Keras' default alpha)
+
+    def trunk(self, obs_nchw):
+        """The convolutions and the dense layers: the last dense layer's activation [B, hidden]."""
         x = F.leaky_relu(self.conv_initial(obs_nchw), 0.2)
         x = F.leaky_relu(self.conv_0(x), 0.2)
         x = F.leaky_relu(self.conv_1(x), 0.2)
         x = x.flatten(1)
         for d in self.dense:
-            x = F.leaky_relu(d(x), 0.3)
+            x = F.leaky_relu(d(x), self.dense_slope)
+        return x
+
+    def forward(self, obs_nchw):
+        x = self.trunk(obs_nchw)
         return self.logits(x), self.value(x).squeeze(-1)
+
+
+class RllibLSTMShapedCNN(RllibShapedCNN):
+    """The reference's ``RllibLSTMPPOModel`` (ppo_rllib.py:89-238, ``use_lstm``): ``RllibShapedCNN``'s convolutions and dense
+    layers, then an LSTM of ``cell_size`` (256, ``CELL_SIZE``) and the logits / value heads on its output.  The gates follow
+    ``tf.keras.layers.LSTM``'s defaults (order i, f, c, o; sigmoid recurrent activation, tanh activation, one bias), which is
+    torch's ``LSTMCell`` with Keras' bias in ``bias_ih`` and ``bias_hh`` zero.
+
+    dense_slope: the negative slope of the dense layers' leaky ReLU.  The default 0.2 is ``tf.nn.leaky_relu``'s alpha, the
+    activation the reference's LSTM model is recalled to give its ``TimeDistributed(Dense)`` layers (the CNN model's
+    ``LeakyReLU()`` layers use 0.3); this is not pinned against the reference's source, so set it when loading weights
+    from a model whose slope is known."""
+
+    def __init__(self, width, height, in_planes=26, num_filters=25, hidden=64, num_hidden_layers=3, num_actions=6,
+                 cell_size=256, dense_slope=0.2):
+        super().__init__(width, height, in_planes, num_filters, hidden, num_hidden_layers, num_actions)
+        self.dense_slope = float(dense_slope)
+        self.lstm = nn.LSTMCell(hidden, cell_size)
+        with torch.no_grad():
+            self.lstm.bias_hh.zero_()
+        self.logits = nn.Linear(cell_size, num_actions)
+        self.value = nn.Linear(cell_size, 1)
+
+    def load_keras_weights(self, conv, dense, lstm, logits, value):
+        """As ``RllibShapedCNN.load_keras_weights``, and ``lstm`` = (kernel [in, 4 cell], recurrent_kernel [cell, 4 cell],
+        bias [4 cell]) of the Keras LSTM layer, gate order i, f, c, o.  ``logits`` / ``value`` read the LSTM's output."""
+        super().load_keras_weights(conv, dense, logits, value)
+        t = lambda a: torch.as_tensor(a, dtype=torch.float32)
+        k, rk, b = lstm
+        with torch.no_grad():
+            self.lstm.weight_ih.copy_(t(k).t()), self.lstm.weight_hh.copy_(t(rk).t())
+            self.lstm.bias_ih.copy_(t(b)), self.lstm.bias_hh.zero_()
+        return self
+
+    def initial_state(self, batch):
+        """(h, c) of zeros [batch, cell]: RLlib's ``get_initial_state``."""
+        z = self.lstm.weight_hh.new_zeros((batch, self.lstm.hidden_size))
+        return z, z.clone()
+
+    def forward(self, obs_nchw, state):
+        """One step: (logits, value, (h, c)) from observations [B, 26, W, H] and the state (h, c) [B, cell]."""
+        h, c = self.lstm(self.trunk(obs_nchw), state)
+        return self.logits(h), self.value(h).squeeze(-1), (h, c)
+
+    def forward_sequence(self, obs, h0, c0, reset=None):
+        """obs [L, B, 26, W, H] from the state (h0, c0) [B, cell]; the state is zeroed before step t wherever reset[t]
+        ([L, B], nullable).  Returns logits [L, B, n_actions], values [L, B] and the final (h, c)."""
+        L, B = obs.shape[:2]
+        x = self.trunk(obs.flatten(0, 1)).view(L, B, -1)
+        h, c, out = h0, c0, []
+        for t in range(L):
+            if reset is not None:
+                keep = (reset[t] == 0).unsqueeze(-1)
+                h, c = torch.where(keep, h, torch.zeros_like(h)), torch.where(keep, c, torch.zeros_like(c))
+            h, c = self.lstm(x[t], (h, c))
+            out.append(h)
+        y = torch.stack(out)
+        return self.logits(y), self.value(y).squeeze(-1), (h, c)
+
+
+def lstm_gate_permutation(cell):
+    """The order in which ``ovc_lstm_head`` (K11) takes the 4 cell gate rows of an LSTM (torch's / Keras' blocks i, f, g, o
+    of ``cell`` rows): row 64 j + 8 (4 half + gate) + n is gate ``gate`` of hidden unit 16 j + 8 half + n, so that one lane
+    of the kernel holds all four gates of its units."""
+    p = torch.arange(4 * cell)
+    j, q, n = p // 64, (p % 64) // 8, p % 8
+    return (q % 4) * cell + 16 * j + 8 * (q // 4) + n
 
 
 def _conv_matrix(conv, c, w, h):
@@ -123,8 +199,13 @@ class DenseGridPolicy(nn.Module):
             mats += [(d.weight, d.bias) for d in cnn.dense[1:]]
             mats.append((torch.cat([cnn.logits.weight, cnn.value.weight]), torch.cat([cnn.logits.bias, cnn.value.bias])))
             self.n_actions = cnn.logits.out_features
+            self.dense_slope = cnn.dense_slope
+            # RllibLSTMShapedCNN: the LSTM between the dense layers and the heads, kept as it is (lstm_tables folds it for K11)
+            self.lstm = copy.deepcopy(cnn.lstm) if hasattr(cnn, "lstm") else None
             layers, n_in = [], mats[0][0].shape[1]  # the input width is K2's row: never padded
-            for m, bias in mats:
+            for i, (m, bias) in enumerate(mats):
+                if i == len(mats) - 1 and self.lstm is not None:
+                    n_in = self.lstm.hidden_size  # the heads read the LSTM's output
                 lin = nn.Linear(n_in, up(m.shape[0]))
                 lin.weight.zero_(), lin.bias.zero_()
                 lin.weight[:m.shape[0], :m.shape[1]].copy_(m), lin.bias[:m.shape[0]].copy_(bias)
@@ -144,16 +225,36 @@ class DenseGridPolicy(nn.Module):
         lin = self.conv_as_linear[0]
         return lin.weight.detach().t().contiguous().to(torch.bfloat16), lin.bias.detach().float().contiguous()
 
-    def tail_tables(self):
-        """The dense tail in the form ``ovc_policy_tail`` (K8) takes: (w_first bf16 [64, k0], b_first f32 [64], w_hidden bf16
-        [n_hidden, 64, 64], b_hidden f32 [n_hidden, 64], w_heads bf16 [8, 64], b_heads f32 [8]).  Its input is the LAST
+    def hidden_tables(self):
+        """The dense layers in the form ``ovc_policy_tail`` (K8) and ``ovc_policy_hidden`` take: (w_first bf16 [64, k0],
+        b_first f32 [64], w_hidden bf16 [n_hidden, 64, 64], b_hidden f32 [n_hidden, 64]).  Their input is the LAST
         convolution's pre-activation (``trunk``)."""
         d = list(self.dense)
-        assert all(l.out_features == 64 for l in d) and d[0].in_features % 32 == 0 and d[0].in_features <= 256 and self.n_actions <= 7
+        assert all(l.out_features == 64 for l in d) and d[0].in_features % 32 == 0 and d[0].in_features <= 256
         bf = lambda t: t.detach().to(torch.bfloat16).contiguous()
         f32 = lambda t: t.detach().float().contiguous()
-        return (bf(d[0].weight), f32(d[0].bias), bf(torch.stack([l.weight for l in d[1:]])), f32(torch.stack([l.bias for l in d[1:]])),
-                bf(self.heads.weight[:8]), f32(self.heads.bias[:8]))
+        return bf(d[0].weight), f32(d[0].bias), bf(torch.stack([l.weight for l in d[1:]])), f32(torch.stack([l.bias for l in d[1:]]))
+
+    def tail_tables(self):
+        """The dense tail in the form ``ovc_policy_tail`` (K8) takes: ``hidden_tables()`` and (w_heads bf16 [8, 64], b_heads
+        f32 [8])."""
+        assert self.lstm is None and self.n_actions <= 7
+        return self.hidden_tables() + (self.heads.weight[:8].detach().to(torch.bfloat16).contiguous(),
+                                       self.heads.bias[:8].detach().float().contiguous())
+
+    def lstm_tables(self):
+        """The LSTM and the heads in the form ``ovc_lstm_head`` (K11) takes: (w bf16 [4 cell, in + cell] = [W_ih | W_hh], b f32
+        [4 cell] = b_ih + b_hh (one float32 sum), both with the gate rows in ``lstm_gate_permutation`` order; w_heads bf16
+        [8, cell], b_heads f32 [8]).  Read from the parameters as they are: fold before casting this module to bfloat16
+        (``SelfPlayRollout`` does), or the biases are rounded to bfloat16 first."""
+        l = self.lstm
+        assert l is not None and (l.input_size, l.hidden_size) == (64, 256) and self.n_actions <= 7, \
+            "K11 is built for an LSTM of 256 on 64 inputs and at most 7 actions"
+        perm = lstm_gate_permutation(l.hidden_size).to(l.weight_ih.device)
+        w = torch.cat([l.weight_ih, l.weight_hh], 1).detach()[perm]
+        b = (l.bias_ih.detach().float() + l.bias_hh.detach().float())[perm]
+        return (w.to(torch.bfloat16).contiguous(), b.contiguous(), self.heads.weight[:8].detach().to(torch.bfloat16).contiguous(),
+                self.heads.bias[:8].detach().float().contiguous())
 
     def wide_tables(self):
         """The two wide layers in the form ``ovc_wide_layers`` (K9) takes: (w1 bf16 [n1, k0], b1 f32, w2 bf16 [n2, n1], b2 f32)."""
@@ -170,14 +271,19 @@ class DenseGridPolicy(nn.Module):
         last = convs[-1]
         return torch.addmm(last.bias, x, last.weight.t(), out=out)
 
-    def forward_from(self, x, first):
-        """The layers from index ``first`` on (0: the whole network from the observation; 1: from the first layer's
-        activations, e.g. K7's output)."""
+    def hidden_from(self, x, first):
+        """The layers from index ``first`` up to the last dense layer's activation (what ``ovc_policy_hidden`` writes)."""
         for lin in self.conv_as_linear[first:]:
             x = F.leaky_relu(lin(x), 0.2, inplace=True)
         for d in self.dense:
-            x = F.leaky_relu(d(x), 0.3, inplace=True)
-        hv = self.heads(x)
+            x = F.leaky_relu(d(x), self.dense_slope, inplace=True)
+        return x
+
+    def forward_from(self, x, first):
+        """The layers from index ``first`` on (0: the whole network from the observation; 1: from the first layer's
+        activations, e.g. K7's output).  Not for the LSTM policy (its heads read the LSTM)."""
+        assert self.lstm is None
+        hv = self.heads(self.hidden_from(x, first))
         return hv[:, :self.n_actions], hv[:, self.n_actions]
 
 
@@ -262,9 +368,20 @@ class SampleBatch(object):
     learner_mask  uint8 [T, 2N]      (property) the rows the learner trains on: all rows but the partner's
     episodes      EpisodeRecords     the episodes that ended in the window (``episodes.finished()``), capacity
                                      ceil(T / horizon): an environment cannot end more episodes in T transitions
+
+    With the LSTM policy (``RllibLSTMShapedCNN``) the window is cut into chunks of ``seq_len`` = L transitions (RLlib's
+    ``max_seq_len``), and the batch holds the recurrent state each chunk starts from:
+
+    seq_len       int                L (None without the LSTM policy)
+    state_h       bfloat16 [ceil(T/L), 2N, 256]   the LSTM state h / c the policy used at t = k L (zero where an episode
+    state_c       float32 [ceil(T/L), 2N, 256]    started there)
+
+    A learner replays chunk k from (state_h[k], state_c[k]) and zeroes the state before step t > k L wherever
+    dones[t - 1] (the environment auto-reset: a new episode starts at t), as ``RllibLSTMShapedCNN.forward_sequence`` does
+    with ``reset[t] = dones[t - 1]`` (``reset[k L]`` = 0: the stored state already follows the rule).
     """
 
-    def __init__(self, env, n_steps, keep_logits=False, partner=False):
+    def __init__(self, env, n_steps, keep_logits=False, partner=False, seq_len=None):
         N, T, dev = env.n_envs, int(n_steps), env.device
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
         self.env = env
@@ -276,6 +393,9 @@ class SampleBatch(object):
         self.logits = z((T, 2 * N, 8), torch.float32) if keep_logits else None
         self.partner_seat = z((T, N), torch.int8) if partner else None
         self.episodes = EpisodeRecords(env, -(-T // env.horizon) if env.horizon > 0 else 0)
+        self.seq_len = seq_len
+        self.state_h = z((-(-T // seq_len), 2 * N, 256), torch.bfloat16) if seq_len else None
+        self.state_c = z((-(-T // seq_len), 2 * N, 256), torch.float32) if seq_len else None
 
     @property
     def learner_mask(self):
@@ -309,7 +429,8 @@ class SelfPlayRollout(object):
     at most 8 layouts in ``env``), library GEMMs and the draw kernel elsewhere."""
 
     def __init__(self, env, model=None, autocast_dtype=torch.bfloat16, use_graph=True, reward_shaping_factor=1.0,
-                 fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0, episode_capacity=1):
+                 fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0, episode_capacity=1,
+                 max_seq_len=20):
         """autocast_dtype: the dtype of the dense model (``DenseGridPolicy``, widths padded to 16-byte rows) and of the
         observation K2 writes for it: bfloat16 (the plane values are exact in bf16), or None for float32 throughout.
         fused_first_layer (default: on for the bf16 policy where ``fused_kernel_support`` allows K7): the observation is
@@ -331,7 +452,15 @@ class SelfPlayRollout(object):
         episode_capacity: episodes per environment that ``self.episodes`` holds (an ``EpisodeRecords``): every episode that
         ends in run() is written there, up to this many per environment since ``self.episodes.clear()`` (the rest are
         counted in ``episodes.dropped``).  ``self.stats`` (an ``EpisodeStats``) is the running state of the episodes in
-        progress, shared by run() and collect(): an episode may span windows and both calls."""
+        progress, shared by run() and collect(): an episode may span windows and both calls.
+        model: an ``RllibShapedCNN`` (default, random init) or an ``RllibLSTMShapedCNN`` (``use_lstm``).  The LSTM policy runs
+        the same trunk, then the dense layers (K8's hidden output, ``ovc_policy_hidden``, where K8 fits, else library GEMMs),
+        then K11 (``ovc_lstm_head``: the LSTM cell, the heads and the draw) on the live state ``self.h`` (bf16 [2N, 256]) /
+        ``self.c`` (float32 [2N, 256]), zeroed at every auto-reset (K11 is passed the previous transition's ``env.done``); after
+        an ``env.reset()`` outside run() / collect(), call ``reset_state()``.  It needs the bf16 policy.  The LSTM's tables
+        are folded from the float32 model (the gate bias is one float32 sum of its two biases).
+        max_seq_len: RLlib's model-config key for the LSTM policy: collect() records the state every ``max_seq_len``
+        transitions (``SampleBatch.state_h`` / ``state_c``)."""
         assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
         assert autocast_dtype in (torch.bfloat16, None), "the dense model runs in bfloat16, or in float32 with None"
         self.env = env
@@ -339,8 +468,13 @@ class SelfPlayRollout(object):
         self.W, self.H = l.width, l.height
         dev = env.device
         self.model = (model or RllibShapedCNN(self.W, self.H)).to(dev).eval()
+        self.lstm = isinstance(self.model, RllibLSTMShapedCNN)
+        assert not self.lstm or autocast_dtype == torch.bfloat16, \
+            "the LSTM policy runs as ovc_lstm_head (K11), which takes bfloat16 operands: autocast_dtype=None is not supported"
         self.autocast_dtype = autocast_dtype
         self.dense_model = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(dev).eval()
+        if self.lstm:  # folded before the cast: K11's gate bias is the float32 sum of the model's float32 biases
+            self._lstm_tables = self.dense_model.lstm_tables()
         if autocast_dtype is not None:
             self.dense_model = self.dense_model.to(autocast_dtype)
         bf16 = autocast_dtype == torch.bfloat16
@@ -371,8 +505,16 @@ class SelfPlayRollout(object):
             "K8 ends the bf16 policy (64-wide tail behind an input of a multiple of 32, <= 256)"
         self.fused_tail = bool(fused_tail)
         if self.fused_tail:
-            self._tail = self.dense_model.tail_tables()
+            self._tail = self.dense_model.hidden_tables() if self.lstm else self.dense_model.tail_tables()
             self._z = torch.empty((2 * N, self._tail[0].shape[1]), dtype=torch.bfloat16, device=dev)  # last convolution, pre-activation
+        if self.lstm:
+            self.max_seq_len = int(max_seq_len)
+            assert self.max_seq_len >= 1
+            cell =self.model.lstm.hidden_size
+            self._x = torch.empty((2 * N, self.model.lstm.input_size), dtype=torch.bfloat16, device=dev)  # the LSTM's input
+            self.h = torch.zeros((2 * N, cell), dtype=torch.bfloat16, device=dev)  # the live state, zero at every episode start
+            self.c = torch.zeros((2 * N, cell), dtype=torch.float32, device=dev)
+            self._h_boot, self._c_boot = torch.empty_like(self.h), torch.empty_like(self.c)  # the bootstrap's (discarded) state
         if fused_wide is None:
             fused_wide = self.fused_tail and self.fused_first_layer and k9_ok
         assert not fused_wide or (self.fused_tail and self.fused_first_layer and k9_ok), \
@@ -439,6 +581,8 @@ class SelfPlayRollout(object):
         the environments: the state, the returns, the episode statistics and records and the draw counters are restored after
         them."""
         live = [self.env.state, self.ret_sparse, self.ret_mixed, self._draw_counter] + self.stats.state_tensors() + self.episodes.tensors()
+        if self.lstm:
+            live += [self.h, self.c, self.env.done]  # env.done: the next transition's LSTM reset
         if self.partner is not None:
             live += [self.partner_seat, self._partner_counter, self._seat_counter]
         saved = [t.clone() for t in live]
@@ -455,10 +599,11 @@ class SelfPlayRollout(object):
             t.copy_(v)
         return graph
 
-    def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None):
+    def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None, state_out=None, snap=None):
         """(scores float32 [2N, 6] = logits, values written to ``values``) for the observations in self.obs, or None when
-        K8 has also drawn the actions (into ``actions``, with ``logp`` when given).  The outputs default to self.actions,
-        self.values, self._scores8 and self._draw_counter."""
+        K8 or K11 has also drawn the actions (into ``actions``, with ``logp`` when given).  The outputs default to
+        self.actions, self.values, self._scores8 and self._draw_counter.  LSTM policy: K11 reads the live state and writes
+        the new one to ``state_out`` (h, c) (default: in place), the state it used to ``snap`` (h, c) when given."""
         env = self.env
         rows = 2 * env.n_envs
         actions = self.actions if actions is None else actions
@@ -470,6 +615,10 @@ class SelfPlayRollout(object):
                 flat, first = env.encoded_linear(self._wt0, self._b0, out=self._act0, neg_slope=0.2), 1  # K7
             else:
                 flat, first = self.obs.view(rows, self.W * self.H * 26), 0
+            lstm_head = lambda: self._lstm_head(actions, vals, logp, scores8, counter, state_out or (self.h, self.c), snap)
+            if self.lstm and not self.fused_tail:
+                self._x.copy_(self.dense_model.hidden_from(flat, first))
+                return lstm_head()
             if not self.fused_tail:
                 logits, value = self.dense_model.forward_from(flat, first)
                 self._scores.copy_(logits)
@@ -481,6 +630,12 @@ class SelfPlayRollout(object):
                                                             w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, self._z.data_ptr(), env._stream()))
             else:
                 self.dense_model.trunk(flat, first, out=self._z)
+            if self.lstm:
+                w1, b1, wh, bh = self._tail
+                _native.check(_native.lib().ovc_policy_hidden(self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(),
+                                                              wh.data_ptr(), bh.data_ptr(), wh.shape[0], self.dense_model.dense_slope,
+                                                              self._x.data_ptr(), env._stream()))
+                return lstm_head()
             w1, b1, wh, bh, wo, bo = self._tail
             args = (self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
                     wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1),
@@ -490,6 +645,18 @@ class SelfPlayRollout(object):
             else:
                 _native.check(_native.lib().ovc_policy_tail_logp(*args, logp.data_ptr(), env._stream()))
         return None  # K8 has drawn the actions itself
+
+    def _lstm_head(self, actions, values, logp, scores8, counter, state_out, snap):
+        """K11 on self._x and the live state, reset where the previous transition ended an episode (env.done)."""
+        w, b, wo, bo = self._lstm_tables
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        snap_h, snap_c = snap or (None, None)
+        _native.check(_native.lib().ovc_lstm_head(
+            self._x.data_ptr(), self.h.data_ptr(), self.c.data_ptr(), self.env.done.data_ptr(), self._x.shape[0], w.data_ptr(),
+            b.data_ptr(), wo.data_ptr(), bo.data_ptr(), self.dense_model.n_actions, self.seed & (2**64 - 1), counter.data_ptr(),
+            state_out[0].data_ptr(), state_out[1].data_ptr(), ptr(snap_h), ptr(snap_c), actions.data_ptr(), ptr(values), ptr(logp),
+            ptr(scores8), self.env._stream()))
+        return None  # K11 has drawn the actions
 
     def _transition(self, b=None, t=0):
         """One transition: K2 or K7, the policy, the draw, K10 for the partner, K1 (auto-reset inside), the returns and the
@@ -505,7 +672,10 @@ class SelfPlayRollout(object):
             logits = None if b.logits is None else b.logits[t]
         if not self.fused_first_layer:
             env.lossless_state_encoding(out=self.obs)  # K2
-        scores = self._policy(actions=actions, values=values, logp=logp, scores8=logits)
+        snap = None
+        if self.lstm and b is not None and t % b.seq_len == 0:
+            snap = (b.state_h[t // b.seq_len], b.state_c[t // b.seq_len])
+        scores = self._policy(actions=actions, values=values, logp=logp, scores8=logits, snap=snap)
         if scores is not None:  # library layers: the separate draw kernel
             env.sample_actions(scores, self._draw_counter, seed=self.seed, out=actions, logp_out=logp)
             if logits is not None:
@@ -542,7 +712,9 @@ class SelfPlayRollout(object):
             self._transition(b, t)
         if not self.fused_first_layer:
             self.env.lossless_state_encoding(out=self.obs)
-        self._policy(actions=self._boot_actions, values=b.last_values, counter=self._boot_counter)
+        # the LSTM's bootstrap step writes its state to scratch: the next window continues from the live state
+        self._policy(actions=self._boot_actions, values=b.last_values, counter=self._boot_counter,
+                     state_out=(self._h_boot, self._c_boot) if self.lstm else None)
         self.env.gae(b.rewards, b.values, b.dones, b.last_values, gamma, lam, b.advantages, b.value_targets)
 
     def collect(self, n_steps, gamma, lam, keep_logits=False):
@@ -557,7 +729,8 @@ class SelfPlayRollout(object):
         key = (int(n_steps), bool(keep_logits))
         b = self._batches.get(key)
         if b is None:
-            b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits, partner=self.partner is not None)
+            b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits, partner=self.partner is not None,
+                                                 seq_len=self.max_seq_len if self.lstm else None)
         if not self.use_graph:
             self._collect_window(b, n_steps, gamma, lam)
             return b
@@ -574,19 +747,25 @@ class SelfPlayRollout(object):
         use the new weights without a re-capture."""
         with torch.no_grad():
             new = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(self.env.device)
+            pairs = list(zip(self._lstm_tables, new.lstm_tables())) if self.lstm else []  # from the float32 fold, as in __init__
             if self.autocast_dtype is not None:
                 new = new.to(self.autocast_dtype)
             for dst, src in zip(self.dense_model.parameters(), new.parameters()):
                 dst.copy_(src)
-            pairs = []
             if self.fused_first_layer:
                 pairs += zip((self._wt0, self._b0), self.dense_model.first_layer_table())
             if self.fused_wide:
                 pairs += zip(self._wide, self.dense_model.wide_tables())
             if self.fused_tail:
-                pairs += zip(self._tail, self.dense_model.tail_tables())
+                pairs += zip(self._tail, self.dense_model.hidden_tables() if self.lstm else self.dense_model.tail_tables())
             for dst, src in pairs:
                 dst.copy_(src)
+
+    def reset_state(self):
+        """Zero the LSTM policy's live state.  run() and collect() zero it at every auto-reset (through ``env.done``); call
+        this after resetting the environments directly (``env.reset()``), so that the new episodes start from zero state."""
+        assert self.lstm, "only the LSTM policy has a recurrent state"
+        self.h.zero_(), self.c.zero_()
 
     def env_only(self, n_steps):
         """The same transitions without the policy: encode + step with the last sampled actions

@@ -4,7 +4,7 @@ K1 with each record-I/O strategy (2-D TMA tile, 1-D bulk TMA, direct), K5 (the r
 host-transfer formats, standard and random-start auto-resets, 16- / 32- / 64-word records, a partial last tile),
 the round-1 fused path, K4 reset (copy + random), K2, K3, K6, the host-buffer pipeline, the policy kernels K7 / K8 and
 the sample-batch kernels (logp draws, ovc_record_transition, ovc_gae through SelfPlayRollout.collect), K10 and the seat draw,
-and the episode statistics of ovc_record_transition_stats.  Results are checked
+the episode statistics of ovc_record_transition_stats, and the LSTM policy (K8's hidden output, K11).  Results are checked
 against the CPU oracle on the way, so a run under the sanitizer is also a parity run.
 
     compute-sanitizer --tool racecheck python tools/sanitize_smoke.py
@@ -207,4 +207,19 @@ for k, want in ref.finished().items():
 assert (recs.dropped.cpu().numpy() == ref.dropped).all() and (ref.dropped == 1).all()
 torch.cuda.synchronize()
 print("episode statistics (record_transition with stats) ok", flush=True)
+# the LSTM policy: K8's hidden output and K11 (ovc_lstm_head) through collect() on a 5x4 grid (K7 -> K9 -> K8 hidden -> K11)
+# and on a 9x5 grid (library layers -> K11), episodes ending inside the window
+from overcooked_ai_b200.selfplay import RllibLSTMShapedCNN  # noqa: E402
+
+for name in ("cramped_room", "asymmetric_advantages"):
+    env7 = BatchedOvercookedEnv(name, 37, horizon=3, auto_reset=True)
+    l7 = env7.layouts[0]
+    sp7 = SelfPlayRollout(env7, model=RllibLSTMShapedCNN(l7.width, l7.height), use_graph=False, seed=4, max_seq_len=2)
+    st = env7.state.cpu().numpy().copy()
+    b = sp7.collect(5, 0.99, 0.95, keep_logits=True)
+    for t in range(5):
+        cpu.step(env7._tab_host, env7._starts_host, st, b.actions[t].cpu().numpy().reshape(-1, 2), horizon=3, flags=1)
+    assert np.array_equal(env7.state.cpu().numpy(), st) and b.dones.any()
+torch.cuda.synchronize()
+print("LSTM policy (K8 hidden output, K11) through collect() ok", flush=True)
 print("sanitize_smoke: all ok")
