@@ -418,6 +418,18 @@ int ovc_encode_linear(const void *layouts, int n_layouts, const int32_t *state, 
                       int height, int horizon, int n_out, float neg_slope, void *stream);
 
 /*
+ * One view per environment (an agent pair: each agent's network sees its own seat only).  Common to every *_view entry
+ * point: environment e's agent sits at player p(e) = seat ^ (swap[e] != 0), seat 0 or 1 (OVC_E_BADARG otherwise), swap
+ * int32 [n] or NULL (no swap), 4-byte aligned; compact row r is environment r and its joint row is g(r) = 2 r + p(r).
+ *
+ * ovc_encode_linear_view: ovc_encode_linear for player p(e)'s view only, out bfloat16 [n_envs][n_out]; row e is bit for
+ *   bit row g(e) of ovc_encode_linear (without view_swap) on the same operands.  Same limits as ovc_encode_linear.
+ */
+int ovc_encode_linear_view(const void *layouts, int n_layouts, const int32_t *state, const int32_t *swap, int seat,
+                           const void *wt, const float *bias, void *out, int64_t n_envs, int state_words, int width,
+                           int height, int horizon, int n_out, float neg_slope, void *stream);
+
+/*
  * The two ends of a policy-in-the-loop transition around ovc_step (the reference's rollout worker samples the joint
  * action from the policy's action distribution and mixes the rewards, human_aware_rl/rllib/rllib.py:302-342):
  *
@@ -434,6 +446,12 @@ int ovc_sample_actions(const float *scores, int ld, int n_actions, int64_t n_row
                        int32_t *actions, void *stream);
 int ovc_accumulate_returns(const int32_t *sparse, const int32_t *shaped, float factor, int64_t n_envs, int64_t *ret_sparse,
                            float *ret_mixed, void *stream);
+/* ovc_sample_actions_view: the ovc_sample_actions draw for one agent per environment (the *_view row map, see
+ * ovc_encode_linear_view): scores row r, Philox counter row g(r), written to actions[g(r)] of the int32 [n_rows][2] joint
+ * action (the other seat's entry untouched); logp[r] (nullable) as ovc_sample_actions_logp.  scores, actions, logp 4-byte
+ * aligned. */
+int ovc_sample_actions_view(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter,
+                            const int32_t *swap, int seat, int32_t *actions, float *logp, void *stream);
 
 /*
  * What a PPO sample batch keeps of each transition (RLlib's SampleBatch: action_logp, rewards, dones; then its GAE
@@ -540,6 +558,14 @@ int ovc_policy_tail_logp(const void *x, int64_t n_rows, int k0, float in_slope, 
  * (ovc_lstm_head).  Arguments as ovc_policy_tail's; hidden 4-byte aligned. */
 int ovc_policy_hidden(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
                       const void *w_hidden, const float *b_hidden, int n_hidden, float slope, void *hidden, void *stream);
+/* ovc_policy_tail_view: ovc_policy_tail_logp on one agent's rows (the *_view row map, see ovc_encode_linear_view): x row r
+ * is environment r's agent; the draw uses the joint row g(r) with this call's seed and counter and writes actions[g(r)]
+ * of the int32 [n_rows][2] joint action (the other seat's entry untouched); values[r], logp[r], scores[r] (each
+ * nullable) as ovc_policy_tail_logp.  actions, values, logp 4-byte aligned, scores 8-byte aligned. */
+int ovc_policy_tail_view(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                         const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                         float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *swap, int seat, int32_t *actions,
+                         float *values, float *scores, float *logp, void *stream);
 
 /*
  * ovc_lstm_head (K11): the recurrent end of the reference's LSTM PPO model (ppo_rllib.py:89-238, RllibLSTMPPOModel:
@@ -560,6 +586,15 @@ int ovc_lstm_head(const void *x, const void *h_in, const float *c_in, const int3
                   const float *b, const void *w_heads, const float *b_heads, int n_actions, uint64_t seed, uint64_t *counter,
                   void *h_out, float *c_out, void *snap_h, float *snap_c, int32_t *actions, float *values, float *logp,
                   float *scores, void *stream);
+/* ovc_lstm_head_view: ovc_lstm_head on one agent's rows (the *_view row map, see ovc_encode_linear_view): the state
+ * h_in / c_in / h_out / c_out / snap_* is [n_rows][256], one row per environment for this agent; row r is zeroed where
+ * reset[r] != 0 (reset int32 [n_rows], nullable, 4-byte aligned); the draw uses the joint row g(r) and writes
+ * actions[g(r)] of the int32 [n_rows][2] joint action (the other seat's entry untouched); values / logp / scores row r.
+ * actions, values, logp 4-byte aligned, the rest as ovc_lstm_head. */
+int ovc_lstm_head_view(const void *x, const void *h_in, const float *c_in, const int32_t *reset, int64_t n_rows, const void *w,
+                       const float *b, const void *w_heads, const float *b_heads, int n_actions, uint64_t seed, uint64_t *counter,
+                       const int32_t *swap, int seat, void *h_out, float *c_out, void *snap_h, float *snap_c, int32_t *actions,
+                       float *values, float *logp, float *scores, void *stream);
 
 /*
  * ovc_wide_layers (K9): the two wide layers of the rollout policy between ovc_encode_linear and ovc_policy_tail

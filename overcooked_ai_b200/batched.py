@@ -405,6 +405,45 @@ class BatchedOvercookedEnv(object):
             self.horizon if self.horizon > 0 else 2**31 - 1, n_out, float(neg_slope), self._stream()))
         return out
 
+    def encoded_linear_view(self, wt, bias, seat, swap=None, out=None, neg_slope=0.2):
+        """``encoded_linear`` for one view per environment (ovc_encode_linear_view): ``out[e]`` (bfloat16 ``[N, n_out]``) is
+        the view of player ``seat ^ (swap[e] != 0)``, bit for bit the row ``encoded_linear`` writes for that view.  ``swap``:
+        int32 CUDA tensor [N] or None."""
+        assert len({(l.width, l.height) for l in self.layouts}) == 1, "one grid shape per call (group envs by layout)"
+        W, H = self.layouts[0].width, self.layouts[0].height
+        assert wt.is_cuda and wt.dtype == torch.bfloat16 and wt.is_contiguous() and wt.shape[0] == W * H * 26, wt.shape
+        n_out = wt.shape[1]
+        assert bias.is_cuda and bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == n_out
+        if swap is not None:
+            assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == self.n_envs
+        if out is None:
+            out = torch.empty((self.n_envs, n_out), dtype=torch.bfloat16, device=self.device)
+        assert out.is_cuda and out.dtype == torch.bfloat16 and out.is_contiguous() and out.numel() == self.n_envs * n_out
+        _native.check(self._lib.ovc_encode_linear_view(
+            self.tables.data_ptr(), self.n_layouts, self.state.data_ptr(), 0 if swap is None else swap.data_ptr(), int(seat),
+            wt.data_ptr(), bias.data_ptr(), out.data_ptr(), self.n_envs, self.state_words, W, H,
+            self.horizon if self.horizon > 0 else 2**31 - 1, n_out, float(neg_slope), self._stream()))
+        return out
+
+    def sample_actions_view(self, scores, counter, seat, swap=None, seed=0, out=None, logp_out=None):
+        """``sample_actions`` for one agent per environment (ovc_sample_actions_view): ``scores`` float32 ``[N, ld]`` (row e:
+        the agent at player ``p = seat ^ (swap[e] != 0)``) is drawn with the Philox counter of joint row ``2 e + p`` into
+        ``out[e, p]`` (int32 [N, 2]; the other seat is left alone).  ``logp_out`` float32 [N] optional.  Returns ``out``."""
+        assert scores.is_cuda and scores.dtype == torch.float32 and scores.dim() == 2 and scores.stride(1) == 1 and scores.shape[0] == self.n_envs
+        assert counter.is_cuda and counter.dtype == torch.int64 and counter.numel() == 2 and counter.is_contiguous()
+        if swap is not None:
+            assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == self.n_envs
+        if out is None:
+            out = torch.zeros((self.n_envs, 2), dtype=torch.int32, device=self.device)
+        assert out.is_cuda and out.dtype == torch.int32 and out.is_contiguous() and out.numel() == 2 * self.n_envs
+        if logp_out is not None:
+            assert logp_out.is_cuda and logp_out.dtype == torch.float32 and logp_out.is_contiguous() and logp_out.numel() == self.n_envs
+        _native.check(self._lib.ovc_sample_actions_view(
+            scores.data_ptr(), scores.stride(0), 6, self.n_envs, int(seed) & (2**64 - 1), counter.data_ptr(),
+            0 if swap is None else swap.data_ptr(), int(seat), out.data_ptr(), 0 if logp_out is None else logp_out.data_ptr(),
+            self._stream()))
+        return out
+
     def sample_actions(self, scores, counter, seed=0, out=None, logp_out=None):
         """Joint actions drawn from the policy's logits (ovc_sample_actions: Gumbel-max on Philox draws, one kernel).
         ``scores`` float32 ``[2N, ld]`` (rows ordered [env][agent], the first 6 columns are the logits), ``counter`` an

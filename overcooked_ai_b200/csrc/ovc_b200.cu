@@ -720,6 +720,23 @@ int ovc_encode_linear(const void *layouts, int n_layouts, const int32_t *state, 
                                    state_words, width, height, horizon, n_out, neg_slope, (cudaStream_t)stream);
 }
 
+int ovc_encode_linear_view(const void *layouts, int n_layouts, const int32_t *state, const int32_t *swap, int seat, const void *wt,
+                           const float *bias, void *out, int64_t n_envs, int state_words, int width, int height, int horizon,
+                           int n_out, float neg_slope, void *stream) {
+    int rc = ovc::check_common(layouts, n_layouts, state, n_envs, state_words);
+    if (rc) return rc;
+    if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
+    return ovc::encode_linear_impl((const ovc_layout_t *)layouts, n_layouts, state, swap, wt, bias, out, n_envs, state_words, width,
+                                   height, horizon, n_out, neg_slope, (cudaStream_t)stream, seat);
+}
+
+int ovc_sample_actions_view(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter,
+                            const int32_t *swap, int seat, int32_t *actions, float *logp, void *stream) {
+    if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
+    return ovc::sample_actions_impl(scores, ld, n_actions, n_rows, seed, (unsigned long long *)counter, actions, logp, (cudaStream_t)stream,
+                                    swap, seat);
+}
+
 int ovc_sample_actions(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter,
                        int32_t *actions, void *stream) {
     return ovc::sample_actions_impl(scores, ld, n_actions, n_rows, seed, (unsigned long long *)counter, actions, nullptr, (cudaStream_t)stream);
@@ -769,6 +786,19 @@ int ovc_policy_tail_logp(const void *x, int64_t n_rows, int k0, float in_slope, 
     return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream);
 }
 
+int ovc_policy_tail_view(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                         const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                         float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *swap, int seat, int32_t *actions,
+                         float *values, float *scores, float *logp, void *stream) {
+    ovc::PolicyTailArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
+    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
+    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
+    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
+    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, swap, seat);
+}
+
 int ovc_policy_hidden(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
                       const void *w_hidden, const float *b_hidden, int n_hidden, float slope, void *hidden, void *stream) {
     ovc::PolicyTailArgs a;
@@ -791,6 +821,20 @@ int ovc_lstm_head(const void *x, const void *h_in, const float *c_in, const int3
     a.h_out = (__nv_bfloat16 *)h_out, a.c_out = c_out, a.snap_h = (__nv_bfloat16 *)snap_h, a.snap_c = snap_c;
     a.actions = actions, a.values = values, a.logp = logp, a.scores = scores;
     return ovc::lstm_head_impl(a, (cudaStream_t)stream);
+}
+
+int ovc_lstm_head_view(const void *x, const void *h_in, const float *c_in, const int32_t *reset, int64_t n_rows, const void *w,
+                       const float *b, const void *w_heads, const float *b_heads, int n_actions, uint64_t seed, uint64_t *counter,
+                       const int32_t *swap, int seat, void *h_out, float *c_out, void *snap_h, float *snap_c, int32_t *actions,
+                       float *values, float *logp, float *scores, void *stream) {
+    ovc::LstmHeadArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.h_in = (const __nv_bfloat16 *)h_in, a.c_in = c_in, a.reset = reset, a.n_rows = n_rows;
+    a.w = (const __nv_bfloat16 *)w, a.b = b, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
+    a.n_actions = n_actions, a.seed = seed, a.counter = (unsigned long long *)counter;
+    a.h_out = (__nv_bfloat16 *)h_out, a.c_out = c_out, a.snap_h = (__nv_bfloat16 *)snap_h, a.snap_c = snap_c;
+    a.actions = actions, a.values = values, a.logp = logp, a.scores = scores, a.swap = swap, a.seat = seat;
+    if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
+    return ovc::lstm_head_impl(a, (cudaStream_t)stream, true);
 }
 
 int ovc_policy_tail(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,

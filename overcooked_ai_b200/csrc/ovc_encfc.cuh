@@ -38,6 +38,7 @@ struct EncLinArgs {
     long long n_envs;
     int n_layouts, S, W, H, horizon, n_out, n_workers;
     float neg_slope;
+    int seat;                  // one view (encode_linear_kernel<CPL, true>): the agent's seat, view_swap its per-env swap
 };
 
 __device__ __forceinline__ int el_dyn_plane(int plane) { return plane < 10 ? plane : plane - 6; }
@@ -104,7 +105,10 @@ __device__ __forceinline__ void el_gather(float acc[CPL], const __nv_bfloat16 *t
     }
 }
 
-template <int CPL>
+// VIEW: one view per environment, player p(e) = seat ^ (view_swap[e] != 0), written to out[e] ([n_envs][n_out]); the
+// object part and that view's gathers run in the same order as in the two-view kernel, so the row is bit-identical to
+// row 2 e + p(e) of it.
+template <int CPL, bool VIEW>
 __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncLinArgs a) {
     constexpr int CS = 32 * CPL;  // columns per CTA
     extern __shared__ __align__(16) char el_smem[];
@@ -234,8 +238,7 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncL
         // the two views: own cell / orientation in planes 0, 2..5, the partner's in planes 1, 6..9 (:2468-2479)
         const int ori0 = (p0 >> 8) & 3, ori1 = (p1 >> 8) & 3;
         const int swap = a.view_swap ? (__ldg(a.view_swap + env) != 0) : 0;
-#pragma unroll
-        for (int p = 0; p < 2; p++) {  // p = the player whose view this is
+        auto view = [&](int p, long long row) {  // p = the player whose view this is
             float acc[CPL];
 #pragma unroll
             for (int i = 0; i < CPL; i++) acc[i] = common[i];
@@ -252,11 +255,16 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncL
                 const __nv_bfloat162 h = __floats2bfloat162_rn(fmaxf(x0, x0 * a.neg_slope), fmaxf(x1, x1 * a.neg_slope));
                 packed[i] = *reinterpret_cast<const unsigned *>(&h);
             }
-            const long long row = 2 * env + (swap ? 1 - p : p);
             __nv_bfloat16 *dst = a.out + row * a.n_out + col0 + lane * CPL;
             if constexpr (CPL == 8) *reinterpret_cast<uint4 *>(dst) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
             else if constexpr (CPL == 4) *reinterpret_cast<uint2 *>(dst) = make_uint2(packed[0], packed[1]);
             else *reinterpret_cast<unsigned *>(dst) = packed[0];
+        };
+        if constexpr (VIEW) {
+            view(a.seat ^ swap, env);
+        } else {
+#pragma unroll
+            for (int p = 0; p < 2; p++) view(p, 2 * env + (swap ? 1 - p : p));
         }
     }
 }
@@ -266,11 +274,13 @@ static size_t encode_linear_smem(int cpl, int n_rows, int n_layouts) {
     return (size_t)n_rows * CS * 2 + ((size_t)n_layouts + 1) * CS * 4 + (size_t)n_layouts * (16 * 4 + 2 * 4 + 128 * 2 + 256) + 16;
 }
 
+// seat < 0: both views (ovc_encode_linear); 0 / 1: one view per environment (ovc_encode_linear_view, view_swap = swap)
 static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const int32_t *state, const int32_t *view_swap,
                               const void *wt, const float *bias, void *out, long long n_envs, int S, int W, int H, int horizon,
-                              int n_out, float neg_slope, cudaStream_t st) {
+                              int n_out, float neg_slope, cudaStream_t st, int seat = -1) {
     if (!out || !wt || !bias) return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)out | (uintptr_t)wt) & 15) != 0) return fail(OVC_E_BADARG, "weights and output must be 16-byte aligned");
+    if (seat >= 0 && ((uintptr_t)view_swap & 3) != 0) return fail(OVC_E_BADARG, "swap must be 4-byte aligned");
     if (W < 1 || W > 16 || H < 1 || H > 16) return fail(OVC_E_BADARG, "grid shape out of range");
     if (n_out < 64 || n_out % 64) return fail(OVC_E_BADARG, "n_out must be a positive multiple of 64", n_out);
     if (!(neg_slope >= 0.f && neg_slope <= 1.f)) return fail(OVC_E_BADARG, "negative slope must lie in [0, 1]");
@@ -291,7 +301,7 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
     EncLinArgs a;
     a.layouts = layouts, a.state = state, a.view_swap = view_swap, a.wt = (const __nv_bfloat16 *)wt, a.bias = bias;
     a.out = (__nv_bfloat16 *)out, a.n_envs = n_envs, a.n_layouts = n_layouts, a.S = S, a.W = W, a.H = H, a.horizon = horizon;
-    a.n_out = n_out, a.neg_slope = neg_slope;
+    a.n_out = n_out, a.neg_slope = neg_slope, a.seat = seat;
     const int n_slices = n_out / (32 * cpl);
     const long long want = (n_envs + EL_THREADS / 32 - 1) / (EL_THREADS / 32);
     int workers = n_sm / n_slices;
@@ -300,15 +310,21 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
     a.n_workers = workers;
     const size_t smem = encode_linear_smem(cpl, n_rows, n_layouts);
     cudaError_t e;
-#define OVC_LAUNCH_EL(C)                                                                                           \
-    do {                                                                                                           \
-        e = cudaFuncSetAttribute(encode_linear_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                               \
-        encode_linear_kernel<C><<<(unsigned)(workers * n_slices), EL_THREADS, smem, st>>>(a);                      \
+#define OVC_LAUNCH_EL(C, V)                                                                                           \
+    do {                                                                                                              \
+        e = cudaFuncSetAttribute(encode_linear_kernel<C, V>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+        if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                                  \
+        encode_linear_kernel<C, V><<<(unsigned)(workers * n_slices), EL_THREADS, smem, st>>>(a);                      \
     } while (0)
-    if (cpl == 8) OVC_LAUNCH_EL(8);
-    else if (cpl == 4) OVC_LAUNCH_EL(4);
-    else OVC_LAUNCH_EL(2);
+    if (seat >= 0) {
+        if (cpl == 8) OVC_LAUNCH_EL(8, true);
+        else if (cpl == 4) OVC_LAUNCH_EL(4, true);
+        else OVC_LAUNCH_EL(2, true);
+    } else {
+        if (cpl == 8) OVC_LAUNCH_EL(8, false);
+        else if (cpl == 4) OVC_LAUNCH_EL(4, false);
+        else OVC_LAUNCH_EL(2, false);
+    }
 #undef OVC_LAUNCH_EL
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel launch");
@@ -330,18 +346,22 @@ namespace ovc {
 // last CTA to finish advances the step (every CTA has read it by then), so a captured CUDA graph draws fresh numbers at
 // every replay without any host involvement.
 // LOGP: also logp[row] = scores[row][a] - (m + log(sum_i exp(scores[row][i] - m))), m = max_i scores[row][i], at the drawn a.
-template <bool LOGP>
+// VIEW: row r is one agent's row of environment r, at player p(r) = seat ^ (swap[r] != 0) (swap nullable): the draw uses
+// the joint row g = 2 r + p(r) and writes actions[g]; scores and logp stay indexed by r.
+template <bool LOGP, bool VIEW = false>
 __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__restrict__ scores, int ld, int n_actions, long long n_rows,
                                                              unsigned long long seed, unsigned long long *counter,
-                                                             int32_t *__restrict__ actions, float *__restrict__ logp) {
+                                                             int32_t *__restrict__ actions, float *__restrict__ logp,
+                                                             const int32_t *__restrict__ swap = nullptr, int seat = 0) {
     const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(counter);
     const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (row < n_rows) {
         const float *s = scores + row * ld;
+        const long long g = VIEW ? 2 * row + (seat ^ (swap && swap[row] != 0)) : row;
         const uint32_t c3 = (uint32_t)(step >> 32) << 1;
-        const Philox4 A = philox4x32_10(seed, (uint32_t)row, (uint32_t)((unsigned long long)row >> 32), (uint32_t)step, c3);
+        const Philox4 A = philox4x32_10(seed, (uint32_t)g, (uint32_t)((unsigned long long)g >> 32), (uint32_t)step, c3);
         Philox4 B = A;
-        if (n_actions > 4) B = philox4x32_10(seed, (uint32_t)row, (uint32_t)((unsigned long long)row >> 32), (uint32_t)step, c3 | 1u);
+        if (n_actions > 4) B = philox4x32_10(seed, (uint32_t)g, (uint32_t)((unsigned long long)g >> 32), (uint32_t)step, c3 | 1u);
         int best = 0;
         float best_v = -INFINITY;
         for (int i = 0; i < n_actions; i++) {
@@ -350,7 +370,7 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__rest
             const float v = s[i] - logf(-logf(u));
             if (v > best_v) best_v = v, best = i;
         }
-        actions[row] = best;
+        actions[g] = best;
         if constexpr (LOGP) {
             float m = s[0];
             for (int i = 1; i < n_actions; i++) m = fmaxf(m, s[i]);
@@ -462,15 +482,25 @@ __global__ void __launch_bounds__(256) accumulate_returns_kernel(const int32_t *
                              done[e] != 0);
 }
 
+// seat < 0: rows are joint rows (ovc_sample_actions[_logp]); 0 / 1: one agent's rows (ovc_sample_actions_view)
 static int sample_actions_impl(const float *scores, int ld, int n_actions, long long n_rows, unsigned long long seed,
-                               unsigned long long *counter, int32_t *actions, float *logp, cudaStream_t st) {
+                               unsigned long long *counter, int32_t *actions, float *logp, cudaStream_t st,
+                               const int32_t *swap = nullptr, int seat = -1) {
     if (!scores || !counter || !actions) return fail(OVC_E_BADARG, "null pointer argument");
     if (n_actions < 1 || n_actions > 8 || ld < n_actions) return fail(OVC_E_BADARG, "n_actions must be 1..8 and <= ld", n_actions);
     if (n_rows < 0) return fail(OVC_E_BADARG, "negative row count");
+    if (seat >= 0 && (((uintptr_t)scores | (uintptr_t)actions | (uintptr_t)logp | (uintptr_t)swap) & 3) != 0)
+        return fail(OVC_E_BADARG, "scores, actions, logp and swap must be 4-byte aligned");
     if (n_rows == 0) return OVC_OK;
     const unsigned grid = (unsigned)((n_rows + 255) / 256);
-    if (logp) sample_actions_kernel<true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, logp);
-    else sample_actions_kernel<false><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, nullptr);
+    if (seat >= 0) {
+        if (logp) sample_actions_kernel<true, true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, logp, swap, seat);
+        else sample_actions_kernel<false, true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, nullptr, swap, seat);
+    } else if (logp) {
+        sample_actions_kernel<true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, logp);
+    } else {
+        sample_actions_kernel<false><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, nullptr);
+    }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "sample_actions kernel launch");
     return OVC_OK;

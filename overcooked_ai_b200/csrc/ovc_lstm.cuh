@@ -58,6 +58,8 @@ struct LstmHeadArgs {
     float *snap_c;                 // [n_rows][256] or null
     int32_t *actions;              // [n_rows]
     float *values, *logp, *scores; // [n_rows], [n_rows], [n_rows][8]; each nullable
+    const int32_t *swap;           // one view (lstm_head_kernel<true>): [n_rows] or null, and the seat: row r is environment
+    int seat;                      // r's agent at player seat ^ (swap[r] != 0), reset[r] its reset
 };
 
 __device__ __forceinline__ void lh_load_slice(__nv_bfloat16 *dst, const __nv_bfloat16 *w, int slice) {
@@ -77,6 +79,9 @@ __device__ __forceinline__ unsigned lh_pack(float a, float b) {
     return *reinterpret_cast<const unsigned *>(&h);
 }
 
+// VIEW: one agent's row per environment: row r resets with reset[r], draws on the joint row g = view_row(r) and writes
+// actions[g]; the state, values, logp and scores stay indexed by r.
+template <bool VIEW>
 __global__ void __launch_bounds__(LH_THREADS, 1) lstm_head_kernel(const LstmHeadArgs p) {
     extern __shared__ __align__(16) char lh_smem[];
     __nv_bfloat16 *ring = reinterpret_cast<__nv_bfloat16 *>(lh_smem);  // [2][64][LH_WS]
@@ -100,7 +105,7 @@ __global__ void __launch_bounds__(LH_THREADS, 1) lstm_head_kernel(const LstmHead
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const long long r0 = tile * LH_ROWS + warp * 16 + g, r1 = r0 + 8;
         const bool in0 = r0 < p.n_rows, in1 = r1 < p.n_rows;
-        const bool z0 = !in0 || (p.reset && p.reset[r0 >> 1]), z1 = !in1 || (p.reset && p.reset[r1 >> 1]);
+        const bool z0 = !in0 || (p.reset && p.reset[VIEW ? r0 : r0 >> 1]), z1 = !in1 || (p.reset && p.reset[VIEW ? r1 : r1 >> 1]);
         // ---- A fragments of [x | h_in]: 8 consecutive inputs of rows g, g + 8 per 32-wide block ----
         uint4 xa[LH_KS2], xb[LH_KS2];
 #pragma unroll
@@ -193,9 +198,10 @@ __global__ void __launch_bounds__(LH_THREADS, 1) lstm_head_kernel(const LstmHead
         // ---- the draw (ovc_sample_actions, as K8) ----
         auto draw = [&](long long row, float s0, float s1) {
             float lp = 0.f;
-            const int best = draw_row<true>(s0, s1, p.seed, step, row, p.n_actions, lane, t, lp);
+            const long long g = VIEW ? view_row(p.swap, p.seat, row, p.n_rows) : row;
+            const int best = draw_row<true>(s0, s1, p.seed, step, g, p.n_actions, lane, t, lp);
             if (row < p.n_rows) {
-                if (t == 0) p.actions[row] = best;
+                if (t == 0) p.actions[g] = best;
                 if (p.logp && t == 0) p.logp[row] = lp;
                 if (p.values && t == (p.n_actions >> 1)) p.values[row] = (p.n_actions & 1) ? s1 : s0;
             }
@@ -206,7 +212,8 @@ __global__ void __launch_bounds__(LH_THREADS, 1) lstm_head_kernel(const LstmHead
     advance_step(p.counter, step);
 }
 
-static int lstm_head_impl(const LstmHeadArgs &a, cudaStream_t st) {
+// view: the one-view instantiation (a.swap / a.seat, ovc_lstm_head_view)
+static int lstm_head_impl(const LstmHeadArgs &a, cudaStream_t st, bool view = false) {
     if (!a.x || !a.h_in || !a.c_in || !a.w || !a.b || !a.w_heads || !a.b_heads || !a.counter || !a.h_out || !a.c_out || !a.actions)
         return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)a.x | (uintptr_t)a.h_in | (uintptr_t)a.w | (uintptr_t)a.w_heads | (uintptr_t)a.snap_h) & 15) != 0)
@@ -214,6 +221,8 @@ static int lstm_head_impl(const LstmHeadArgs &a, cudaStream_t st) {
     if ((((uintptr_t)a.c_in | (uintptr_t)a.c_out | (uintptr_t)a.snap_c | (uintptr_t)a.b | (uintptr_t)a.b_heads | (uintptr_t)a.scores) & 7) != 0 ||
         ((uintptr_t)a.h_out & 3) != 0)
         return fail(OVC_E_BADARG, "c_in, c_out, snap_c, b, b_heads and scores must be 8-byte aligned, h_out 4-byte aligned");
+    if (view && (((uintptr_t)a.actions | (uintptr_t)a.values | (uintptr_t)a.logp | (uintptr_t)a.reset | (uintptr_t)a.swap) & 3) != 0)
+        return fail(OVC_E_BADARG, "actions, values, logp, reset and swap must be 4-byte aligned");
     if (a.n_actions < 1 || a.n_actions > 7) return fail(OVC_E_BADARG, "n_actions must be 1..7 (head n_actions is the value)", a.n_actions);
     if (a.n_rows < 0) return fail(OVC_E_BADARG, "negative row count");
     if (a.n_rows == 0) return OVC_OK;
@@ -222,9 +231,11 @@ static int lstm_head_impl(const LstmHeadArgs &a, cudaStream_t st) {
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     const long long n_tiles = (a.n_rows + LH_ROWS - 1) / LH_ROWS;
     const unsigned grid = (unsigned)(n_tiles < n_sm ? n_tiles : n_sm);
-    cudaError_t e = cudaFuncSetAttribute(lstm_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LH_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(view ? lstm_head_kernel<true> : lstm_head_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)LH_SMEM);
     if (e != cudaSuccess) return cuda_fail(e, "lstm_head kernel attribute");
-    lstm_head_kernel<<<grid, LH_THREADS, LH_SMEM, st>>>(a);
+    if (view) lstm_head_kernel<true><<<grid, LH_THREADS, LH_SMEM, st>>>(a);
+    else lstm_head_kernel<false><<<grid, LH_THREADS, LH_SMEM, st>>>(a);
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "lstm_head kernel launch");
     return OVC_OK;

@@ -217,6 +217,12 @@ __device__ __forceinline__ int draw_row(float s0, float s1, unsigned long long s
     return best;
 }
 
+// The joint row 2 r + p(r) of compact row r, whose agent sits at player p(r) = seat ^ (swap[r] != 0) (swap nullable);
+// rows past the end map to 2 r + seat (their draws are discarded)
+__device__ __forceinline__ long long view_row(const int32_t *swap, int seat, long long r, long long n_rows) {
+    return 2 * r + (seat ^ (swap && r < n_rows && __ldg(swap + r) != 0));
+}
+
 // The last CTA of a launch to get here advances the draw step (every CTA has read it by then): counter[1] counts arrivals.
 __device__ __forceinline__ void advance_step(unsigned long long *counter, unsigned long long step) {
     __syncthreads();
@@ -233,9 +239,12 @@ __device__ __forceinline__ void advance_step(unsigned long long *counter, unsign
 
 // K0 = 32 * KS2; LOGP: also write p.logp (a separate instantiation, so the plain draw is untouched); HIDDEN: stop after the
 // last 64-wide layer and write its activations to p.hidden instead of the heads and the draw (the LSTM policy's input;
-// the counter is neither read nor advanced)
-template <int KS2, bool LOGP, bool HIDDEN>
-__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const PolicyTailArgs p) {
+// the counter is neither read nor advanced).  VIEW: row r is one agent's row of environment r (view_row): the draw uses
+// the joint row g and writes p.actions[g]; values, logp and scores stay indexed by r.  The one-view kernel is a kernel of
+// its own (policy_tail_view_kernel, swap and seat as extra parameters): a larger PolicyTailArgs would change the code of
+// every instantiation.
+template <int KS2, bool LOGP, bool HIDDEN, bool VIEW>
+__device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const int32_t *swap, int seat) {
     constexpr int K0 = 32 * KS2;
     extern __shared__ __align__(16) char pt_smem[];
 
@@ -288,9 +297,10 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const Policy
             const long long row = h ? r1 : r0;
             const float s0 = out[0][2 * h], s1 = out[0][2 * h + 1];
             float lp = 0.f;
-            const int best = draw_row<LOGP>(s0, s1, p.seed, step, row, p.n_actions, lane, t, lp);
+            const long long g = VIEW ? view_row(swap, seat, row, p.n_rows) : row;
+            const int best = draw_row<LOGP>(s0, s1, p.seed, step, g, p.n_actions, lane, t, lp);
             if (row < p.n_rows) {
-                if (t == 0) p.actions[row] = best;
+                if (t == 0) p.actions[g] = best;
                 if constexpr (LOGP) if (t == 0) p.logp[row] = lp;
                 // the value head is head n_actions: lane n_actions / 2 holds it
                 if (p.values && t == (p.n_actions >> 1)) p.values[row] = (p.n_actions & 1) ? s1 : s0;
@@ -300,14 +310,30 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const Policy
     if constexpr (!HIDDEN) advance_step(p.counter, step);
 }
 
+template <int KS2, bool LOGP, bool HIDDEN>
+__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const PolicyTailArgs p) {
+    policy_tail_body<KS2, LOGP, HIDDEN, false>(p, nullptr, 0);
+}
+
+template <int KS2, bool LOGP>
+__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_view_kernel(const PolicyTailArgs p, const int32_t *swap, int seat) {
+    policy_tail_body<KS2, LOGP, false, true>(p, swap, seat);
+}
+
 // hid: the HIDDEN instantiation into a.hidden (no heads, no draw; a.w_heads / a.b_heads are staged but never read, so the
-// entry point passes the first layer's tables, which are at least as large, in their place)
-static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bool hid = false) {
+// entry point passes the first layer's tables, which are at least as large, in their place).  seat >= 0: the one-view
+// kernel with swap (ovc_policy_tail_view); -1: the two-view ones.
+static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bool hid = false, const int32_t *swap = nullptr,
+                            int seat = -1) {
+    const bool view = seat >= 0;
     if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || (hid ? !a.hidden : (!a.counter || !a.actions)) ||
         (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)))
         return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)a.x | (uintptr_t)a.w_first) & 15) != 0) return fail(OVC_E_BADARG, "x and w_first must be 16-byte aligned");
     if (hid && ((uintptr_t)a.hidden & 3) != 0) return fail(OVC_E_BADARG, "hidden must be 4-byte aligned");
+    if (view && (((uintptr_t)a.actions | (uintptr_t)a.values | (uintptr_t)a.logp | (uintptr_t)swap) & 3) != 0)
+        return fail(OVC_E_BADARG, "actions, values, logp and swap must be 4-byte aligned");
+    if (view && ((uintptr_t)a.scores & 7) != 0) return fail(OVC_E_BADARG, "scores must be 8-byte aligned");
     if (k0 < 32 || k0 > 256 || k0 % 32) return fail(OVC_E_BADARG, "k0 must be a multiple of 32 in 32..256", k0);
     if (a.n_hidden < 0 || a.n_hidden > 8) return fail(OVC_E_BADARG, "n_hidden must be 0..8", a.n_hidden);
     if (a.n_actions < 1 || a.n_actions > 7) return fail(OVC_E_BADARG, "n_actions must be 1..7 (head n_actions is the value)", a.n_actions);
@@ -321,23 +347,24 @@ static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bo
     const long long n_tiles = (a.n_rows + 15) / 16, want = (n_tiles + PT_THREADS / 32 - 1) / (PT_THREADS / 32);
     const unsigned grid = (unsigned)(want < n_sm ? want : n_sm);
     cudaError_t e = cudaSuccess;
-#define OVC_LAUNCH_PT(KS2)                                                                                              \
-    case KS2:                                                                                                           \
-        if (hid) {                                                                                                      \
-            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (e == cudaSuccess) policy_tail_kernel<KS2, false, true><<<grid, PT_THREADS, smem, st>>>(a);             \
-        } else if (a.logp) {                                                                                            \
-            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (e == cudaSuccess) policy_tail_kernel<KS2, true, false><<<grid, PT_THREADS, smem, st>>>(a);             \
-        } else {                                                                                                        \
-            e = cudaFuncSetAttribute(policy_tail_kernel<KS2, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (e == cudaSuccess) policy_tail_kernel<KS2, false, false><<<grid, PT_THREADS, smem, st>>>(a);            \
-        }                                                                                                               \
+#define OVC_PT_KERNEL(ARGS, ...)                                                                                 \
+    do {                                                                                                         \
+        e = cudaFuncSetAttribute(__VA_ARGS__, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);           \
+        if (e == cudaSuccess) __VA_ARGS__<<<grid, PT_THREADS, smem, st>>> ARGS;                                  \
+    } while (0)
+#define OVC_LAUNCH_PT(KS2)                                                                                       \
+    case KS2:                                                                                                    \
+        if (hid) OVC_PT_KERNEL((a), policy_tail_kernel<KS2, false, true>);                                       \
+        else if (view && a.logp) OVC_PT_KERNEL((a, swap, seat), policy_tail_view_kernel<KS2, true>);             \
+        else if (view) OVC_PT_KERNEL((a, swap, seat), policy_tail_view_kernel<KS2, false>);                      \
+        else if (a.logp) OVC_PT_KERNEL((a), policy_tail_kernel<KS2, true, false>);                               \
+        else OVC_PT_KERNEL((a), policy_tail_kernel<KS2, false, false>);                                          \
         break;
     switch (k0 / 32) {
         OVC_LAUNCH_PT(1) OVC_LAUNCH_PT(2) OVC_LAUNCH_PT(3) OVC_LAUNCH_PT(4) OVC_LAUNCH_PT(5) OVC_LAUNCH_PT(6) OVC_LAUNCH_PT(7) OVC_LAUNCH_PT(8)
     }
 #undef OVC_LAUNCH_PT
+#undef OVC_PT_KERNEL
     if (e != cudaSuccess) return cuda_fail(e, "policy_tail kernel attribute");
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "policy_tail kernel launch");

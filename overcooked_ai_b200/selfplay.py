@@ -422,7 +422,94 @@ PARTNER_DRAW_SALT = 0x9E3779B97F4A7C15
 PARTNER_SEAT_SALT = 0xD1B54A32D192ED03
 
 
-class SelfPlayRollout(object):
+class _FoldedPolicy(object):
+    """A PPO network in the form the policy kernels take: ``model`` (``RllibShapedCNN`` or ``RllibLSTMShapedCNN``), its
+    ``DenseGridPolicy`` and the K7 / K9 / K8 / K11 tables, with the kernels ``fused_kernel_support`` allows on ``env``'s grid.
+    ``SelfPlayRollout`` evaluates it on both views of every environment, an ``AgentPairRollout`` agent on one."""
+
+    def _fold(self, env, model, autocast_dtype, fused_first_layer, fused_tail, fused_wide):
+        """See ``SelfPlayRollout.__init__`` for the arguments; ``self.env`` is ``env``."""
+        assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
+        assert autocast_dtype in (torch.bfloat16, None), "the dense model runs in bfloat16, or in float32 with None"
+        l = env.layouts[0]
+        self.W, self.H = l.width, l.height
+        dev = env.device
+        self.model = (model or RllibShapedCNN(self.W, self.H)).to(dev).eval()
+        self.lstm = isinstance(self.model, RllibLSTMShapedCNN)
+        assert not self.lstm or autocast_dtype == torch.bfloat16, \
+            "the LSTM policy runs as ovc_lstm_head (K11), which takes bfloat16 operands: autocast_dtype=None is not supported"
+        self.autocast_dtype = autocast_dtype
+        self.dense_model = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(dev).eval()
+        if self.lstm:  # folded before the cast: K11's gate bias is the float32 sum of the model's float32 biases
+            self._lstm_tables = self.dense_model.lstm_tables()
+        if autocast_dtype is not None:
+            self.dense_model = self.dense_model.to(autocast_dtype)
+        bf16 = autocast_dtype == torch.bfloat16
+        k7_ok, k9_ok, k8_ok = fused_kernel_support(self.dense_model, self.W, self.H, env.n_layouts)
+        if fused_first_layer is None:
+            fused_first_layer = bf16 and k7_ok
+        assert not fused_first_layer or (bf16 and k7_ok), \
+            "K7 feeds the bf16 policy (first layer width a multiple of 64, table within shared memory, at most %d layouts; " \
+            "this environment has %d)" % (K7_MAX_LAYOUTS, env.n_layouts)
+        self.fused_first_layer = bool(fused_first_layer)
+        if self.fused_first_layer:
+            self._wt0, self._b0 = self.dense_model.first_layer_table()
+        if fused_tail is None:
+            fused_tail = bf16 and k8_ok
+        assert not fused_tail or (bf16 and k8_ok), \
+            "K8 ends the bf16 policy (64-wide tail behind an input of a multiple of 32, <= 256)"
+        self.fused_tail = bool(fused_tail)
+        if self.fused_tail:
+            self._tail = self.dense_model.hidden_tables() if self.lstm else self.dense_model.tail_tables()
+        if fused_wide is None:
+            fused_wide = self.fused_tail and self.fused_first_layer and k9_ok
+        assert not fused_wide or (self.fused_tail and self.fused_first_layer and k9_ok), \
+            "K9 sits between K7 and K8 and is built for 512 -> 512 -> 160"
+        self.fused_wide = bool(fused_wide)
+        if self.fused_wide:
+            self._wide = self.dense_model.wide_tables()
+
+    def sync_weights(self):
+        """Re-fold ``self.model`` (e.g. after a learner's update) into the policy the kernels evaluate, in place: the dense
+        model's parameters and the K7 / K9 / K8 tables keep their storage, so the captured graphs of run() and collect()
+        use the new weights without a re-capture."""
+        with torch.no_grad():
+            new = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(self.env.device)
+            pairs = list(zip(self._lstm_tables, new.lstm_tables())) if self.lstm else []  # from the float32 fold, as in __init__
+            if self.autocast_dtype is not None:
+                new = new.to(self.autocast_dtype)
+            for dst, src in zip(self.dense_model.parameters(), new.parameters()):
+                dst.copy_(src)
+            if self.fused_first_layer:
+                pairs += zip((self._wt0, self._b0), self.dense_model.first_layer_table())
+            if self.fused_wide:
+                pairs += zip(self._wide, self.dense_model.wide_tables())
+            if self.fused_tail:
+                pairs += zip(self._tail, self.dense_model.hidden_tables() if self.lstm else self.dense_model.tail_tables())
+            for dst, src in pairs:
+                dst.copy_(src)
+
+
+
+def _capture_graph(env, live, warm_up, body):
+    """A CUDA graph of ``body``, captured after ``warm_up`` (on a side stream).  The tensors ``live`` (what warm-up and
+    capture advance: the state, returns, statistics, counters...) are restored after them."""
+    saved = [t.clone() for t in live]
+    dev = env.device
+    s = torch.cuda.Stream(dev)
+    s.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(s):
+        warm_up()
+    torch.cuda.current_stream(dev).wait_stream(s)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        body()
+    for t, v in zip(live, saved):
+        t.copy_(v)
+    return graph
+
+
+class SelfPlayRollout(_FoldedPolicy):
     """Policy-in-the-loop rollout: both agents of every environment act from the same network, or, with a BC ``partner``,
     one seat of an environment is the partner's in the episodes the seat draw gives it (PPO_BC).  The network evaluated is
     ``DenseGridPolicy`` of ``model``: K7 / K9 / K8 where they fit (``fused_kernel_support``; K7, and K9 behind it, only with
@@ -461,36 +548,14 @@ class SelfPlayRollout(object):
         are folded from the float32 model (the gate bias is one float32 sum of its two biases).
         max_seq_len: RLlib's model-config key for the LSTM policy: collect() records the state every ``max_seq_len``
         transitions (``SampleBatch.state_h`` / ``state_c``)."""
-        assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
-        assert autocast_dtype in (torch.bfloat16, None), "the dense model runs in bfloat16, or in float32 with None"
         self.env = env
-        l = env.layouts[0]
-        self.W, self.H = l.width, l.height
+        self._fold(env, model, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
         dev = env.device
-        self.model = (model or RllibShapedCNN(self.W, self.H)).to(dev).eval()
-        self.lstm = isinstance(self.model, RllibLSTMShapedCNN)
-        assert not self.lstm or autocast_dtype == torch.bfloat16, \
-            "the LSTM policy runs as ovc_lstm_head (K11), which takes bfloat16 operands: autocast_dtype=None is not supported"
-        self.autocast_dtype = autocast_dtype
-        self.dense_model = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(dev).eval()
-        if self.lstm:  # folded before the cast: K11's gate bias is the float32 sum of the model's float32 biases
-            self._lstm_tables = self.dense_model.lstm_tables()
-        if autocast_dtype is not None:
-            self.dense_model = self.dense_model.to(autocast_dtype)
-        bf16 = autocast_dtype == torch.bfloat16
-        k7_ok, k9_ok, k8_ok = fused_kernel_support(self.dense_model, self.W, self.H, env.n_layouts)
-        if fused_first_layer is None:
-            fused_first_layer = bf16 and k7_ok
-        assert not fused_first_layer or (bf16 and k7_ok), \
-            "K7 feeds the bf16 policy (first layer width a multiple of 64, table within shared memory, at most %d layouts; " \
-            "this environment has %d)" % (K7_MAX_LAYOUTS, env.n_layouts)
-        self.fused_first_layer = bool(fused_first_layer)
         self.factor = float(reward_shaping_factor)
         self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by the captured graphs
         N = env.n_envs
         self.obs = None if self.fused_first_layer else torch.empty((N, 2, self.W, self.H, 26), dtype=autocast_dtype or torch.float32, device=dev)
         if self.fused_first_layer:
-            self._wt0, self._b0 = self.dense_model.first_layer_table()
             self._act0 = torch.empty((2 * N, self._wt0.shape[1]), dtype=torch.bfloat16, device=dev)
         self.actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
         self.ret_sparse = torch.zeros(N, dtype=torch.int64, device=dev)      # running episode return (sparse)
@@ -499,13 +564,7 @@ class SelfPlayRollout(object):
         self.stats = EpisodeStats(env)
         self.episodes = EpisodeRecords(env, episode_capacity)
         self.native_glue = True  # the draw and the returns are always native kernels; bench.py's launch count reads this
-        if fused_tail is None:
-            fused_tail = bf16 and k8_ok
-        assert not fused_tail or (bf16 and k8_ok), \
-            "K8 ends the bf16 policy (64-wide tail behind an input of a multiple of 32, <= 256)"
-        self.fused_tail = bool(fused_tail)
         if self.fused_tail:
-            self._tail = self.dense_model.hidden_tables() if self.lstm else self.dense_model.tail_tables()
             self._z = torch.empty((2 * N, self._tail[0].shape[1]), dtype=torch.bfloat16, device=dev)  # last convolution, pre-activation
         if self.lstm:
             self.max_seq_len = int(max_seq_len)
@@ -515,13 +574,6 @@ class SelfPlayRollout(object):
             self.h = torch.zeros((2 * N, cell), dtype=torch.bfloat16, device=dev)  # the live state, zero at every episode start
             self.c = torch.zeros((2 * N, cell), dtype=torch.float32, device=dev)
             self._h_boot, self._c_boot = torch.empty_like(self.h), torch.empty_like(self.c)  # the bootstrap's (discarded) state
-        if fused_wide is None:
-            fused_wide = self.fused_tail and self.fused_first_layer and k9_ok
-        assert not fused_wide or (self.fused_tail and self.fused_first_layer and k9_ok), \
-            "K9 sits between K7 and K8 and is built for 512 -> 512 -> 160"
-        self.fused_wide = bool(fused_wide)
-        if self.fused_wide:
-            self._wide = self.dense_model.wide_tables()
         self.seed = int(seed)
         self._draw_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of ovc_sample_actions
         self._scores8 = None  # set to a float32 [2N, 8] tensor to make K8 also write the heads (tests)
@@ -585,19 +637,7 @@ class SelfPlayRollout(object):
             live += [self.h, self.c, self.env.done]  # env.done: the next transition's LSTM reset
         if self.partner is not None:
             live += [self.partner_seat, self._partner_counter, self._seat_counter]
-        saved = [t.clone() for t in live]
-        dev = self.env.device
-        s = torch.cuda.Stream(dev)
-        s.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(s):
-            warm_up()
-        torch.cuda.current_stream(dev).wait_stream(s)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            body()
-        for t, v in zip(live, saved):
-            t.copy_(v)
-        return graph
+        return _capture_graph(self.env, live, warm_up, body)
 
     def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None, state_out=None, snap=None):
         """(scores float32 [2N, 6] = logits, values written to ``values``) for the observations in self.obs, or None when
@@ -741,26 +781,6 @@ class SelfPlayRollout(object):
         g[1].replay()
         return b
 
-    def sync_weights(self):
-        """Re-fold ``self.model`` (e.g. after a learner's update) into the policy the kernels evaluate, in place: the dense
-        model's parameters and the K7 / K9 / K8 tables keep their storage, so the captured graphs of run() and collect()
-        use the new weights without a re-capture."""
-        with torch.no_grad():
-            new = DenseGridPolicy(self.model, self.W, self.H, pad_to=16).to(self.env.device)
-            pairs = list(zip(self._lstm_tables, new.lstm_tables())) if self.lstm else []  # from the float32 fold, as in __init__
-            if self.autocast_dtype is not None:
-                new = new.to(self.autocast_dtype)
-            for dst, src in zip(self.dense_model.parameters(), new.parameters()):
-                dst.copy_(src)
-            if self.fused_first_layer:
-                pairs += zip((self._wt0, self._b0), self.dense_model.first_layer_table())
-            if self.fused_wide:
-                pairs += zip(self._wide, self.dense_model.wide_tables())
-            if self.fused_tail:
-                pairs += zip(self._tail, self.dense_model.hidden_tables() if self.lstm else self.dense_model.tail_tables())
-            for dst, src in pairs:
-                dst.copy_(src)
-
     def reset_state(self):
         """Zero the LSTM policy's live state.  run() and collect() zero it at every auto-reset (through ``env.done``); call
         this after resetting the environments directly (``env.reset()``), so that the new episodes start from zero state."""
@@ -777,3 +797,198 @@ class SelfPlayRollout(object):
                 self.env.lossless_state_encoding(out=self.obs)
             self.env.step(self.actions)
         return n_steps * self.env.n_envs
+
+
+class _NetworkAgent(_FoldedPolicy):
+    """One network agent of an ``AgentPairRollout``: its policy on ONE view per environment, the view of player
+    ``p(e) = seat ^ swap[e]``, written to ``actions[e, p(e)]`` of the joint action.  Where K7 fits: K7's one-view form
+    (``encoded_linear_view``) -> K9 on N rows -> K8's one-view draw (``ovc_policy_tail_view``), or K8's hidden output -> K11's
+    one-view form (``ovc_lstm_head_view``) for the LSTM model; elsewhere rows 2 e + p(e) of the observation ``self.obs``
+    (K2's output, which the pair writes once per transition for all its agents: set it before act()), the dense model on N
+    rows (K7 -> library layers where K7 fits but K8 does not) and the one-view draw (``sample_actions_view``, or K11).  Its
+    draws use key ``seed`` and a counter of its own, on the joint row 2 e + p(e): the numbers a self-play rollout with the
+    same seed draws for that row."""
+
+    def __init__(self, env, model, seat, swap, seed, autocast_dtype):
+        self.env = env
+        self._fold(env, model, autocast_dtype, None, None, None)
+        N, dev = env.n_envs, env.device
+        self.seat, self.swap, self.seed = int(seat), swap, int(seed)
+        self._counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of this agent's draws
+        self._scores8 = None  # set to a float32 [N, 8] tensor to make K8 / K11 also write the heads (tests)
+        self.values = torch.zeros(N, dtype=torch.float32, device=dev)
+        self.obs = None  # [N, 2, W, H, 26] without K7, shared with the other agent of the pair
+        if self.fused_first_layer:
+            self._act0 = torch.empty((N, self._wt0.shape[1]), dtype=torch.bfloat16, device=dev)
+        else:
+            self._rows = 2 * torch.arange(N, device=dev) + (self.seat if swap is None else self.seat ^ (swap != 0).long())  # 2 e + p(e)
+            self._flat = torch.empty((N, self.W * self.H * 26), dtype=autocast_dtype or torch.float32, device=dev)
+        if not self.fused_tail and not self.lstm:  # library layers: the logits the draw reads
+            self._scores = torch.empty((N, 6), dtype=torch.float32, device=dev)
+        if self.fused_tail:
+            self._z = torch.empty((N, self._tail[0].shape[1]), dtype=torch.bfloat16, device=dev)
+        if self.lstm:
+            cell = self.model.lstm.hidden_size
+            self._x = torch.empty((N, self.model.lstm.input_size), dtype=torch.bfloat16, device=dev)
+            self.h = torch.zeros((N, cell), dtype=torch.bfloat16, device=dev)  # the live state, zero at every episode start
+            self.c = torch.zeros((N, cell), dtype=torch.float32, device=dev)
+
+    def live(self):
+        """The tensors a transition advances (restored around graph capture)."""
+        return [self._counter] + ([self.h, self.c] if self.lstm else [])
+
+    def act(self, actions):
+        """This agent's entries of ``actions`` (int32 [N, 2]) from the current state (without K7: from ``self.obs``, K2's
+        encoding of it); values into ``self.values``.  The LSTM state is zeroed where the previous transition ended an
+        episode (``env.done``)."""
+        env, N = self.env, self.env.n_envs
+        lib, seed = _native.lib(), self.seed & (2**64 - 1)
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        with torch.no_grad():
+            if self.fused_first_layer:
+                flat, first = env.encoded_linear_view(self._wt0, self._b0, self.seat, self.swap, out=self._act0, neg_slope=0.2), 1  # K7
+            else:
+                flat, first = torch.index_select(self.obs.view(2 * N, -1), 0, self._rows, out=self._flat), 0
+            if self.fused_wide:
+                w1, b1, w2, b2 = self._wide
+                _native.check(lib.ovc_wide_layers(flat.data_ptr(), N, flat.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
+                                                  w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, self._z.data_ptr(), env._stream()))
+            elif self.fused_tail:
+                self.dense_model.trunk(flat, first, out=self._z)
+            if self.lstm:
+                if self.fused_tail:
+                    w1, b1, wh, bh = self._tail
+                    _native.check(lib.ovc_policy_hidden(self._z.data_ptr(), N, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(),
+                                                        wh.data_ptr(), bh.data_ptr(), wh.shape[0], self.dense_model.dense_slope,
+                                                        self._x.data_ptr(), env._stream()))
+                else:
+                    self._x.copy_(self.dense_model.hidden_from(flat, first))
+                w, b, wo, bo = self._lstm_tables
+                _native.check(lib.ovc_lstm_head_view(
+                    self._x.data_ptr(), self.h.data_ptr(), self.c.data_ptr(), env.done.data_ptr(), N, w.data_ptr(), b.data_ptr(),
+                    wo.data_ptr(), bo.data_ptr(), self.dense_model.n_actions, seed, self._counter.data_ptr(), ptr(self.swap), self.seat,
+                    self.h.data_ptr(), self.c.data_ptr(), 0, 0, actions.data_ptr(), self.values.data_ptr(), 0, ptr(self._scores8),
+                    env._stream()))
+            elif self.fused_tail:
+                w1, b1, wh, bh, wo, bo = self._tail
+                _native.check(lib.ovc_policy_tail_view(
+                    self._z.data_ptr(), N, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
+                    wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, seed, self._counter.data_ptr(),
+                    ptr(self.swap), self.seat, actions.data_ptr(), self.values.data_ptr(), ptr(self._scores8), 0, env._stream()))
+            else:
+                logits, value = self.dense_model.forward_from(flat, first)
+                self._scores.copy_(logits)
+                self.values.copy_(value)
+                env.sample_actions_view(self._scores, self._counter, self.seat, self.swap, seed=self.seed, out=actions)
+
+
+class _BCAgent(object):
+    """A ``BCPolicy`` agent of an ``AgentPairRollout``: K10 with ``partner_seat[e] = p(e)`` in every environment, its draws
+    keyed by ``seed ^ PARTNER_DRAW_SALT`` on a counter of its own (the draws of PPO_BC's partner)."""
+
+    def __init__(self, env, policy, seat, swap, seed):
+        self.env, self.policy = env, policy.to(env.device).eval()
+        self.seat, self.seed = int(seat), int(seed)
+        self._tables = self.policy.tables()
+        self._n_actions = self.policy.logits.out_features
+        self.partner_seat = (torch.full((env.n_envs,), self.seat, dtype=torch.int32, device=env.device) if swap is None
+                             else (self.seat ^ (swap != 0).int()).to(torch.int32).contiguous())
+        self._counter = torch.zeros(2, dtype=torch.int64, device=env.device)
+
+    def live(self):
+        return [self._counter]
+
+    def act(self, actions):
+        self.env.partner_actions(self._tables, self.partner_seat, self._counter, seed=self.seed ^ PARTNER_DRAW_SALT,
+                                 n_actions=self._n_actions, out=actions)
+
+    def sync_weights(self):
+        for dst, src in zip(self._tables, self.policy.tables()):
+            dst.copy_(src)
+
+
+class AgentPairRollout(object):
+    """Two different agents in fixed seats, each evaluated on its own seat's view only: the reference's evaluation of an agent
+    pair (rllib.py ``evaluate``: ``AgentEvaluator.evaluate_agent_pair(AgentPair(agent_0_policy, agent_1_policy))``) with N
+    environments on the device.  PPO against a held-out BC human proxy, cross-play of two PPO agents, BC against BC.
+
+    agents: (agent0, agent1), each an ``RllibShapedCNN``, an ``RllibLSTMShapedCNN`` or a ``BCPolicy`` (the same object twice
+    is allowed).  Agent 0 plays player ``swap[e]`` of environment e, agent 1 the other one.  A network agent runs its own
+    policy on N rows (the one-view forms of K7 / K8 / K11 and the draw, with K9 on N rows, where ``fused_kernel_support``
+    allows them; K2, the dense model on the agent's rows and the one-view draw elsewhere); a BC agent is K10.
+    swap: int32 CUDA tensor [N] or None (no swap): both seat orders in one batch; fixed for the rollout's lifetime.
+    seed: the draws' key.  Each agent has its own counter; network agents use ``seed``, BC agents ``seed ^
+    PARTNER_DRAW_SALT`` (K10's key in PPO_BC).  A pair therefore draws what ``SelfPlayRollout`` (both agents one network) or
+    PPO_BC (``SelfPlayRollout(partner=..., bc_factor=1)``) draw on the same rows and steps.
+    autocast_dtype: as ``SelfPlayRollout``'s, for every network agent (an LSTM agent needs bfloat16).
+    episode_capacity: as ``SelfPlayRollout``'s.  Every finished episode's ``partner_seat`` is agent 1's player.
+
+    A transition is K2 (once, when a network agent runs without K7), agent 0's policy, agent 1's policy, K1 (auto-reset
+    inside), then ``record_transition`` with the episode statistics.  ``ret_sparse`` is the running sparse return of every environment."""
+
+    def __init__(self, env, agents, swap=None, seed=0, use_graph=True, episode_capacity=1, autocast_dtype=torch.bfloat16):
+        assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
+        assert len(agents) == 2, "agents: (agent0, agent1)"
+        for a in agents:
+            assert isinstance(a, (RllibShapedCNN, BCPolicy)), "an agent is an RllibShapedCNN, an RllibLSTMShapedCNN or a BCPolicy"
+            assert not isinstance(a, RllibLSTMShapedCNN) or autocast_dtype == torch.bfloat16, \
+                "the LSTM policy runs as ovc_lstm_head (K11), which takes bfloat16 operands: autocast_dtype=None is not supported"
+        N, dev = env.n_envs, env.device
+        if swap is not None:
+            assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == N, "swap: int32 CUDA [N]"
+        self.env, self.swap, self.seed, self.use_graph = env, swap, int(seed), use_graph
+        self.agents = [_BCAgent(env, a, seat, swap, seed) if isinstance(a, BCPolicy) else _NetworkAgent(env, a, seat, swap, seed, autocast_dtype)
+                       for seat, a in enumerate(agents)]
+        # network agents without K7 read K2's observation, written once per transition for both of them
+        library = [a for a in self.agents if isinstance(a, _NetworkAgent) and not a.fused_first_layer]
+        l = env.layouts[0]
+        self.obs = torch.empty((N, 2, l.width, l.height, 26), dtype=autocast_dtype or torch.float32, device=dev) if library else None
+        for a in library:
+            a.obs = self.obs
+        self.actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
+        self.ret_sparse = torch.zeros(N, dtype=torch.int64, device=dev)
+        self._factor = torch.ones(1, dtype=torch.float32, device=dev)  # the episode records' rewards: sparse + shaped
+        self.partner_seat = (torch.ones(N, dtype=torch.int32, device=dev) if swap is None
+                             else (1 ^ (swap != 0).int()).to(torch.int32).contiguous())  # agent 1's player
+        self.stats = EpisodeStats(env)
+        self.episodes = EpisodeRecords(env, episode_capacity)
+        self.graph = None
+
+    def _transition(self):
+        env = self.env
+        if self.obs is not None:
+            env.lossless_state_encoding(out=self.obs)  # K2
+        for a in self.agents:
+            a.act(self.actions)
+        env.step(self.actions)  # K1 (auto-reset inside)
+        env.record_transition(self._factor, ret_sparse=self.ret_sparse, stats=self.stats, records=self.episodes,
+                              partner_seat=self.partner_seat)
+
+    def run(self, n_steps):
+        """Advance every environment n_steps transitions (one CUDA graph per transition with use_graph); returns the number
+        of env-steps done."""
+        if self.use_graph and self.graph is None:
+            live = [self.env.state, self.env.done, self.ret_sparse] + self.stats.state_tensors() + self.episodes.tensors()
+            for a in self.agents:
+                live += a.live()
+
+            def warm_up():
+                for _ in range(3):
+                    self._transition()
+            self.graph = _capture_graph(self.env, live, warm_up, self._transition)
+        step = self._transition if self.graph is None else self.graph.replay
+        for _ in range(n_steps):
+            step()
+        return n_steps * self.env.n_envs
+
+    def sync_weights(self):
+        """Re-fold every agent's network (e.g. a learner's after an update) in place: the captured graph uses the new weights
+        without a re-capture."""
+        for a in self.agents:
+            a.sync_weights()
+
+    def reset_state(self):
+        """Zero the LSTM agents' live state; call it after resetting the environments directly (``env.reset()``)."""
+        for a in self.agents:
+            if getattr(a, "lstm", False):
+                a.h.zero_(), a.c.zero_()

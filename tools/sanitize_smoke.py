@@ -4,7 +4,8 @@ K1 with each record-I/O strategy (2-D TMA tile, 1-D bulk TMA, direct), K5 (the r
 host-transfer formats, standard and random-start auto-resets, 16- / 32- / 64-word records, a partial last tile),
 the round-1 fused path, K4 reset (copy + random), K2, K3, K6, the host-buffer pipeline, the policy kernels K7 / K8 and
 the sample-batch kernels (logp draws, ovc_record_transition, ovc_gae through SelfPlayRollout.collect), K10 and the seat draw,
-the episode statistics of ovc_record_transition_stats, and the LSTM policy (K8's hidden output, K11).  Results are checked
+the episode statistics of ovc_record_transition_stats, the LSTM policy (K8's hidden output, K11), and agent pairs (the
+one-view forms of K7, K8, K11 and the draw).  Results are checked
 against the CPU oracle on the way, so a run under the sanitizer is also a parity run.
 
     compute-sanitizer --tool racecheck python tools/sanitize_smoke.py
@@ -222,4 +223,22 @@ for name in ("cramped_room", "asymmetric_advantages"):
     assert np.array_equal(env7.state.cpu().numpy(), st) and b.dones.any()
 torch.cuda.synchronize()
 print("LSTM policy (K8 hidden output, K11) through collect() ok", flush=True)
+# agent pairs: the one-view forms of K7 -> K9 -> K8, K8 hidden -> K11 and K10 on a 5x4 grid, and the library layers with
+# the one-view draw on a 9x5 grid, mixed seats, episodes ending inside the run; the environments follow the oracle
+from overcooked_ai_b200.selfplay import AgentPairRollout, RllibShapedCNN  # noqa: E402
+
+for name, agents in (("cramped_room", lambda W, H: (RllibShapedCNN(W, H), RllibLSTMShapedCNN(W, H))),
+                     ("cramped_room", lambda W, H: (RllibLSTMShapedCNN(W, H), BCPolicy())),
+                     ("asymmetric_advantages", lambda W, H: (RllibShapedCNN(W, H), RllibLSTMShapedCNN(W, H)))):
+    env8 = BatchedOvercookedEnv(name, 37, horizon=3, auto_reset=True)
+    l8 = env8.layouts[0]
+    swap8 = torch.from_numpy((rng.rand(37) < 0.5).astype(np.int32)).cuda()
+    pair = AgentPairRollout(env8, agents(l8.width, l8.height), swap=swap8, seed=4, use_graph=False)
+    st = env8.state.cpu().numpy().copy()
+    for t in range(5):
+        pair.run(1)
+        cpu.step(env8._tab_host, env8._starts_host, st, pair.actions.cpu().numpy(), horizon=3, flags=1)
+    assert np.array_equal(env8.state.cpu().numpy(), st)
+torch.cuda.synchronize()
+print("agent pairs (one-view K7 / K8 / K11 / draw, K10) ok", flush=True)
 print("sanitize_smoke: all ok")
