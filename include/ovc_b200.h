@@ -595,6 +595,21 @@ int ovc_lstm_head_view(const void *x, const void *h_in, const float *c_in, const
                        const float *b, const void *w_heads, const float *b_heads, int n_actions, uint64_t seed, uint64_t *counter,
                        const int32_t *swap, int seat, void *h_out, float *c_out, void *snap_h, float *snap_c, int32_t *actions,
                        float *values, float *logp, float *scores, void *stream);
+/* ovc_record_transition_view: ovc_record_transition (stats NULL) or ovc_record_transition_stats (stats given) for one
+ * agent per environment (the *_view row map, see ovc_encode_linear_view): rewards float32 [n_envs] (required, 4-byte
+ * aligned) with
+ *     rewards[e] = (float)sparse[e] + factor * (float)shaped[e][p(e)]   the product rounded first
+ *   bit for bit rewards[g(e)] of ovc_record_transition; dones, ret_sparse, ret_mixed and the episode statistics and
+ *   records exactly as those calls write them. */
+int ovc_record_transition_view(const int32_t *sparse, const int32_t *shaped, const int32_t *done, const float *factor, int64_t n_envs,
+                               const int32_t *swap, int seat, float *rewards, uint8_t *dones, int64_t *ret_sparse, float *ret_mixed,
+                               const ovc_episode_stats_t *stats, void *stream);
+/* ovc_gae_view: ovc_gae over n_envs rows, one per environment (an agent pair's learner): rewards, values, advantages,
+ * value_targets float32 [n_steps][n_envs], dones uint8 [n_steps][n_envs], last_values float32 [n_envs]; the recurrence
+ * and rounding order are ovc_gae's, so the result is bit for bit ovc_gae's on those rows of a two-row layout.  Float
+ * buffers 4-byte aligned. */
+int ovc_gae_view(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, int64_t n_steps,
+                 int64_t n_envs, float gamma, float lambda, float *advantages, float *value_targets, void *stream);
 
 /*
  * ovc_wide_layers (K9): the two wide layers of the rollout policy between ovc_encode_linear and ovc_policy_tail

@@ -94,6 +94,8 @@ def lib():
     L.ovc_record_transition.argtypes = [vp, vp, vp, vp, i64, vp, vp, vp, vp, vp]
     L.ovc_record_transition_stats.argtypes = [vp, vp, vp, vp, i64, vp, vp, vp, vp, ctypes.POINTER(EpisodeStatsDesc), vp]
     L.ovc_gae.argtypes = [vp, vp, vp, vp, i64, i64, ctypes.c_float, ctypes.c_float, vp, vp, vp]
+    L.ovc_record_transition_view.argtypes = [vp, vp, vp, vp, i64, vp, i32, vp, vp, vp, vp, ctypes.POINTER(EpisodeStatsDesc), vp]
+    L.ovc_gae_view.argtypes = L.ovc_gae.argtypes
     L.ovc_wide_layers.argtypes = [vp, i64, i32, vp, vp, i32, vp, vp, i32, ctypes.c_float, vp, vp]
     L.ovc_featurize.argtypes = [vp, i32, vp, vp, vp, vp, i64, i32, i32, vp]
     L.ovc_partner_policy.argtypes = [vp, i32, vp, vp, vp, i64, i32, i32, i32, vp, vp, vp, vp, i32, vp, vp, i32, ctypes.c_uint64, vp, vp, vp, vp]
@@ -110,7 +112,7 @@ def lib():
     L.ovc_pipeline_destroy.restype = None
     for f in (L.ovc_step, L.ovc_rollout, L.ovc_reset, L.ovc_encode_lossless, L.ovc_encode_linear, L.ovc_sample_actions, L.ovc_accumulate_returns, L.ovc_policy_tail, L.ovc_wide_layers, L.ovc_featurize, L.ovc_potential,
               L.ovc_policy_tail_logp, L.ovc_policy_hidden, L.ovc_lstm_head,
-              L.ovc_encode_linear_view, L.ovc_sample_actions_view, L.ovc_policy_tail_view, L.ovc_lstm_head_view, L.ovc_sample_actions_logp, L.ovc_record_transition, L.ovc_record_transition_stats, L.ovc_gae, L.ovc_partner_policy, L.ovc_assign_partners, L.ovc_expand_codes_host, L.ovc_expand_stream_host, L.ovc_pipeline_create, L.ovc_pipeline_run, L.ovc_pipeline_wait, L.ovc_pipeline_join):
+              L.ovc_encode_linear_view, L.ovc_sample_actions_view, L.ovc_policy_tail_view, L.ovc_lstm_head_view, L.ovc_sample_actions_logp, L.ovc_record_transition, L.ovc_record_transition_stats, L.ovc_gae, L.ovc_record_transition_view, L.ovc_gae_view, L.ovc_partner_policy, L.ovc_assign_partners, L.ovc_expand_codes_host, L.ovc_expand_stream_host, L.ovc_pipeline_create, L.ovc_pipeline_run, L.ovc_pipeline_wait, L.ovc_pipeline_join):
         f.restype = i32
     if L.ovc_abi_version() != ABI_VERSION:
         raise NativeLibraryError("ABI version mismatch: library %d, binding %d" % (L.ovc_abi_version(), ABI_VERSION))
@@ -125,6 +127,7 @@ EXPORTED_SYMBOLS = (
     "ovc_policy_tail_logp", "ovc_sample_actions_logp", "ovc_record_transition", "ovc_record_transition_stats", "ovc_gae",
     "ovc_partner_policy", "ovc_assign_partners", "ovc_policy_hidden", "ovc_lstm_head",
     "ovc_encode_linear_view", "ovc_sample_actions_view", "ovc_policy_tail_view", "ovc_lstm_head_view",
+    "ovc_record_transition_view", "ovc_gae_view",
     "ovc_pipeline_create", "ovc_pipeline_run", "ovc_pipeline_wait", "ovc_pipeline_join", "ovc_pipeline_destroy",
 )
 

@@ -485,33 +485,50 @@ class BatchedOvercookedEnv(object):
         self._record(self.sparse, self.shaped, self.done, self.events, factor, rewards, dones, ret_sparse, ret_mixed, stats, records,
                      partner_seat)
 
+    def record_transition_view(self, factor, seat, swap, rewards, dones=None, ret_sparse=None, ret_mixed=None, stats=None, records=None,
+                               partner_seat=None):
+        """``record_transition`` for ONE agent per environment (ovc_record_transition_view): ``rewards`` float32 [N] is the
+        reward of the agent at player ``seat ^ (swap[e] != 0)`` (``swap`` int32 CUDA [N] or None), bit for bit the entry
+        ``record_transition`` writes for that player; everything else as ``record_transition``."""
+        if swap is not None:
+            assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == self.n_envs
+        self._record(self.sparse, self.shaped, self.done, self.events, factor, rewards, dones, ret_sparse, ret_mixed, stats, records,
+                     partner_seat, view=(int(seat), swap))
+
     def _record(self, sparse, shaped, done, events, factor, rewards=None, dones=None, ret_sparse=None, ret_mixed=None, stats=None,
-                records=None, partner_seat=None):
+                records=None, partner_seat=None, view=None):
         assert factor.is_cuda and factor.dtype == torch.float32 and factor.numel() == 1
-        for t, dt, n in ((rewards, torch.float32, 2), (dones, torch.uint8, 1), (ret_sparse, torch.int64, 1), (ret_mixed, torch.float32, 1)):
+        for t, dt, n in ((rewards, torch.float32, 1 if view else 2), (dones, torch.uint8, 1), (ret_sparse, torch.int64, 1),
+                         (ret_mixed, torch.float32, 1)):
             assert t is None or (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n * self.n_envs)
         ptr = lambda t: 0 if t is None else t.data_ptr()
+        d = None
         if stats is None:
             assert records is None and partner_seat is None, "records and partner_seat go with stats"
-            _native.check(self._lib.ovc_record_transition(sparse.data_ptr(), shaped.data_ptr(), done.data_ptr(), factor.data_ptr(),
-                                                          self.n_envs, ptr(rewards), ptr(dones), ptr(ret_sparse), ptr(ret_mixed), self._stream()))
-            return
-        assert stats.env is self and records is not None and records.env is self, "stats and records of this environment"
-        for t, n in ((sparse, 1), (shaped, 2), (done, 1), (events, 2), (partner_seat, 1)):
-            assert t is None or (t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n * self.n_envs)
-        d = _native.EpisodeStatsDesc()
-        d.layouts, d.state, d.events, d.partner_seat = self.tables.data_ptr(), self.state.data_ptr(), events.data_ptr(), ptr(partner_seat)
-        d.event_counts, d.sparse_by_agent = stats.event_counts.data_ptr(), stats.cumulative_sparse_rewards_by_agent.data_ptr()
-        d.shaped_by_agent, d.reward_by_agent = stats.cumulative_shaped_rewards_by_agent.data_ptr(), stats.ep_reward_by_agent.data_ptr()
-        d.ep_length, d.layout_id = stats.ep_length.data_ptr(), stats.layout_id.data_ptr()
-        d.count, d.dropped, d.capacity, d.state_words = records.count.data_ptr(), records.dropped.data_ptr(), records.capacity, self.state_words
-        if records.capacity:
-            d.rec_length, d.rec_layout, d.rec_partner_seat = records.length.data_ptr(), records.layout.data_ptr(), records.partner_seat.data_ptr()
-            d.rec_sparse_by_agent, d.rec_shaped_by_agent = records.sparse_r_by_agent.data_ptr(), records.shaped_r_by_agent.data_ptr()
-            d.rec_event_counts, d.rec_reward_by_agent = records.game_stats.data_ptr(), records.reward_by_agent.data_ptr()
-        _native.check(self._lib.ovc_record_transition_stats(sparse.data_ptr(), shaped.data_ptr(), done.data_ptr(), factor.data_ptr(),
-                                                            self.n_envs, ptr(rewards), ptr(dones), ptr(ret_sparse), ptr(ret_mixed),
-                                                            ctypes.byref(d), self._stream()))
+        else:
+            assert stats.env is self and records is not None and records.env is self, "stats and records of this environment"
+            for t, n in ((sparse, 1), (shaped, 2), (done, 1), (events, 2), (partner_seat, 1)):
+                assert t is None or (t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n * self.n_envs)
+            d = _native.EpisodeStatsDesc()
+            d.layouts, d.state, d.events, d.partner_seat = self.tables.data_ptr(), self.state.data_ptr(), events.data_ptr(), ptr(partner_seat)
+            d.event_counts, d.sparse_by_agent = stats.event_counts.data_ptr(), stats.cumulative_sparse_rewards_by_agent.data_ptr()
+            d.shaped_by_agent, d.reward_by_agent = stats.cumulative_shaped_rewards_by_agent.data_ptr(), stats.ep_reward_by_agent.data_ptr()
+            d.ep_length, d.layout_id = stats.ep_length.data_ptr(), stats.layout_id.data_ptr()
+            d.count, d.dropped, d.capacity, d.state_words = records.count.data_ptr(), records.dropped.data_ptr(), records.capacity, self.state_words
+            if records.capacity:
+                d.rec_length, d.rec_layout, d.rec_partner_seat = records.length.data_ptr(), records.layout.data_ptr(), records.partner_seat.data_ptr()
+                d.rec_sparse_by_agent, d.rec_shaped_by_agent = records.sparse_r_by_agent.data_ptr(), records.shaped_r_by_agent.data_ptr()
+                d.rec_event_counts, d.rec_reward_by_agent = records.game_stats.data_ptr(), records.reward_by_agent.data_ptr()
+        args = (sparse.data_ptr(), shaped.data_ptr(), done.data_ptr(), factor.data_ptr(), self.n_envs)
+        outs = (ptr(rewards), ptr(dones), ptr(ret_sparse), ptr(ret_mixed))
+        if view is not None:
+            seat, swap = view
+            _native.check(self._lib.ovc_record_transition_view(*args, ptr(swap), seat, *outs, None if d is None else ctypes.byref(d),
+                                                               self._stream()))
+        elif d is None:
+            _native.check(self._lib.ovc_record_transition(*args, *outs, self._stream()))
+        else:
+            _native.check(self._lib.ovc_record_transition_stats(*args, *outs, ctypes.byref(d), self._stream()))
 
     def gae(self, rewards, values, dones, last_values, gamma, lam, advantages=None, value_targets=None):
         """Generalized advantage estimation over a window (ovc_gae; include/ovc_b200.h gives the recurrence): rewards /
@@ -528,6 +545,17 @@ class BatchedOvercookedEnv(object):
             assert t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n, (t.dtype, tuple(t.shape))
         _native.check(self._lib.ovc_gae(rewards.data_ptr(), values.data_ptr(), dones.data_ptr(), last_values.data_ptr(), T, R,
                                         float(gamma), float(lam), advantages.data_ptr(), value_targets.data_ptr(), self._stream()))
+        return advantages, value_targets
+
+    def gae_view(self, rewards, values, dones, last_values, gamma, lam, advantages, value_targets):
+        """``gae`` over ONE row per environment (ovc_gae_view): rewards / values / advantages / value_targets float32 [T, N],
+        dones uint8 [T, N], last_values float32 [N]; bit for bit ``gae`` on those rows of a two-row layout."""
+        T, N = rewards.shape[0], self.n_envs
+        for t, dt, n in ((rewards, torch.float32, T * N), (values, torch.float32, T * N), (dones, torch.uint8, T * N),
+                         (last_values, torch.float32, N), (advantages, torch.float32, T * N), (value_targets, torch.float32, T * N)):
+            assert t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n, (t.dtype, tuple(t.shape))
+        _native.check(self._lib.ovc_gae_view(rewards.data_ptr(), values.data_ptr(), dones.data_ptr(), last_values.data_ptr(), T, N,
+                                             float(gamma), float(lam), advantages.data_ptr(), value_targets.data_ptr(), self._stream()))
         return advantages, value_targets
 
     def partner_actions(self, tables, partner_seat, counter, seed=0, n_actions=6, out=None, scores=None):

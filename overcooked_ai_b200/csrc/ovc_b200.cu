@@ -774,6 +774,19 @@ int ovc_gae(const float *rewards, const float *values, const uint8_t *dones, con
                          (cudaStream_t)stream);
 }
 
+int ovc_record_transition_view(const int32_t *sparse, const int32_t *shaped, const int32_t *done, const float *factor, int64_t n_envs,
+                               const int32_t *swap, int seat, float *rewards, uint8_t *dones, int64_t *ret_sparse, float *ret_mixed,
+                               const ovc_episode_stats_t *stats, void *stream) {
+    return ovc::record_transition_view_impl(sparse, shaped, done, factor, n_envs, swap, seat, rewards, dones, (long long *)ret_sparse,
+                                            ret_mixed, stats, (cudaStream_t)stream);
+}
+
+int ovc_gae_view(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, int64_t n_steps,
+                 int64_t n_envs, float gamma, float lambda, float *advantages, float *value_targets, void *stream) {
+    return ovc::gae_view_impl(rewards, values, dones, last_values, n_steps, n_envs, gamma, lambda, advantages, value_targets,
+                              (cudaStream_t)stream);
+}
+
 int ovc_policy_tail_logp(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
                          const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                          float slope, int n_actions, uint64_t seed, uint64_t *counter, int32_t *actions, float *values, float *scores,

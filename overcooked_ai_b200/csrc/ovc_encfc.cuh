@@ -506,9 +506,9 @@ static int sample_actions_impl(const float *scores, int ld, int n_actions, long 
     return OVC_OK;
 }
 
-static int accumulate_returns_impl(const int32_t *sparse, const int32_t *shaped, float factor, long long n_envs, long long *ret_sparse,
-                                   float *ret_mixed, const float *factor_dev, const int32_t *done, float *rewards, uint8_t *dones,
-                                   const ovc_episode_stats_t *stats, cudaStream_t st) {
+// The argument checks of ovc_accumulate_returns / ovc_record_transition[_stats] / ovc_record_transition_view.
+static int check_record_args(const int32_t *sparse, const int32_t *shaped, long long n_envs, const int32_t *done, const uint8_t *dones,
+                             const ovc_episode_stats_t *stats) {
     if (!sparse || !shaped || (dones && !done)) return fail(OVC_E_BADARG, "null pointer argument");
     if (n_envs < 0) return fail(OVC_E_BADARG, "negative env count");
     if (stats) {
@@ -527,6 +527,13 @@ static int accumulate_returns_impl(const int32_t *sparse, const int32_t *shaped,
         if (((uintptr_t)s.sparse_by_agent | (uintptr_t)s.shaped_by_agent | (uintptr_t)s.rec_sparse_by_agent | (uintptr_t)s.rec_shaped_by_agent) & 15)
             return fail(OVC_E_BADARG, "int64 sums must be 16-byte aligned");
     }
+    return OVC_OK;
+}
+
+static int accumulate_returns_impl(const int32_t *sparse, const int32_t *shaped, float factor, long long n_envs, long long *ret_sparse,
+                                   float *ret_mixed, const float *factor_dev, const int32_t *done, float *rewards, uint8_t *dones,
+                                   const ovc_episode_stats_t *stats, cudaStream_t st) {
+    if (int rc = check_record_args(sparse, shaped, n_envs, done, dones, stats)) return rc;
     if (n_envs == 0) return OVC_OK;
     const unsigned grid = (unsigned)((n_envs + 255) / 256);
     if (stats)
@@ -537,6 +544,51 @@ static int accumulate_returns_impl(const int32_t *sparse, const int32_t *shaped,
                                                                rewards, dones, ovc_episode_stats_t{});
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "accumulate_returns kernel launch");
+    return OVC_OK;
+}
+
+// ovc_record_transition_view: accumulate_returns_kernel's transition with ONE reward per environment, the agent's at player
+// p(e) = seat ^ (swap[e] != 0): rewards[e] is bit for bit rewards[2 e + p(e)] of ovc_record_transition.  A kernel of its own:
+// an extra parameter in accumulate_returns_kernel would change the code of its existing instantiations.
+template <bool STATS>
+__global__ void __launch_bounds__(256) record_transition_view_kernel(const int32_t *__restrict__ sparse, const int32_t *__restrict__ shaped,
+                                                                     long long n_envs, long long *__restrict__ ret_sparse,
+                                                                     float *__restrict__ ret_mixed, const float *__restrict__ factor_dev,
+                                                                     const int32_t *__restrict__ done, const int32_t *__restrict__ swap,
+                                                                     int seat, float *__restrict__ rewards, uint8_t *__restrict__ dones,
+                                                                     const ovc_episode_stats_t stats) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_envs) return;
+    const float f = *factor_dev;
+    const int sp = sparse[e];
+    const int2 sh = reinterpret_cast<const int2 *>(shaped)[e];
+    if (ret_sparse) ret_sparse[e] += sp;
+    if (ret_mixed) ret_mixed[e] = ((ret_mixed[e] + (float)sp) + f * (float)sh.x) + f * (float)sh.y;
+    const int p = seat ^ (swap && swap[e] != 0);
+    rewards[e] = __fadd_rn((float)sp, __fmul_rn(f, (float)(p ? sh.y : sh.x)));
+    if (dones) dones[e] = done[e] != 0;
+    if constexpr (STATS)
+        episode_stats_update(stats, e, n_envs, sh, __fadd_rn((float)sp, __fmul_rn(f, (float)sh.x)), __fadd_rn((float)sp, __fmul_rn(f, (float)sh.y)),
+                             done[e] != 0);
+}
+
+static int record_transition_view_impl(const int32_t *sparse, const int32_t *shaped, const int32_t *done, const float *factor_dev,
+                                       long long n_envs, const int32_t *swap, int seat, float *rewards, uint8_t *dones,
+                                       long long *ret_sparse, float *ret_mixed, const ovc_episode_stats_t *stats, cudaStream_t st) {
+    if (!factor_dev || !rewards) return fail(OVC_E_BADARG, "null pointer argument");
+    if (int rc = check_record_args(sparse, shaped, n_envs, done, dones, stats)) return rc;
+    if (seat != 0 && seat != 1) return fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
+    if (((uintptr_t)rewards | (uintptr_t)swap) & 3) return fail(OVC_E_BADARG, "rewards and swap must be 4-byte aligned");
+    if (n_envs == 0) return OVC_OK;
+    const unsigned grid = (unsigned)((n_envs + 255) / 256);
+    if (stats)
+        record_transition_view_kernel<true><<<grid, 256, 0, st>>>(sparse, shaped, n_envs, ret_sparse, ret_mixed, factor_dev, done, swap,
+                                                                  seat, rewards, dones, *stats);
+    else
+        record_transition_view_kernel<false><<<grid, 256, 0, st>>>(sparse, shaped, n_envs, ret_sparse, ret_mixed, factor_dev, done, swap,
+                                                                   seat, rewards, dones, ovc_episode_stats_t{});
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "record_transition_view kernel launch");
     return OVC_OK;
 }
 
@@ -593,6 +645,52 @@ static int gae_impl(const float *rewards, const float *values, const uint8_t *do
         (float2 *)targets);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "gae kernel launch");
+    return OVC_OK;
+}
+
+// ovc_gae_view: gae_kernel on ONE row per environment (an agent pair's learner), the same recurrence, rounding order and
+// load unroll; a kernel of its own so that gae_kernel's code stays as it is.  Without a minimum of 4 CTAs per SM ptxas gives it
+// 255 registers (2 CTAs per SM); with it, 64 and no spill, the 16 timesteps' loads still issued before they are consumed.
+__global__ void __launch_bounds__(GAE_THREADS, 4) gae_view_kernel(const float *__restrict__ rewards, const float *__restrict__ values,
+                                                               const uint8_t *__restrict__ dones, const float *__restrict__ last_values,
+                                                               long long T, long long n_envs, float gamma, float lambda,
+                                                               float *__restrict__ adv, float *__restrict__ targets) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_envs) return;
+    const float gl = __fmul_rn(gamma, lambda);
+    float a = 0.f, nv = last_values[e];
+    for (long long t0 = T - 1; t0 >= 0; t0 -= GAE_UNROLL) {
+        float r[GAE_UNROLL], v[GAE_UNROLL], nt[GAE_UNROLL];
+#pragma unroll
+        for (int k = 0; k < GAE_UNROLL; k++)
+            if (t0 - k >= 0) {
+                const long long i = (t0 - k) * n_envs + e;
+                r[k] = __ldcs(rewards + i), v[k] = __ldcs(values + i), nt[k] = dones[i] ? 0.f : 1.f;
+            }
+#pragma unroll
+        for (int k = 0; k < GAE_UNROLL; k++)
+            if (t0 - k >= 0) {
+                const long long i = (t0 - k) * n_envs + e;
+                const float d = __fsub_rn(__fadd_rn(r[k], __fmul_rn(__fmul_rn(gamma, nv), nt[k])), v[k]);
+                a = __fadd_rn(d, __fmul_rn(__fmul_rn(gl, nt[k]), a));
+                __stcs(adv + i, a);
+                __stcs(targets + i, __fadd_rn(a, v[k]));
+                nv = v[k];
+            }
+    }
+}
+
+static int gae_view_impl(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, long long T,
+                         long long n_envs, float gamma, float lambda, float *adv, float *targets, cudaStream_t st) {
+    if (!rewards || !values || !dones || !last_values || !adv || !targets) return fail(OVC_E_BADARG, "null pointer argument");
+    if (T < 0 || n_envs < 0) return fail(OVC_E_BADARG, "T and n_envs must be >= 0");
+    if (((uintptr_t)rewards | (uintptr_t)values | (uintptr_t)last_values | (uintptr_t)adv | (uintptr_t)targets) & 3)
+        return fail(OVC_E_BADARG, "float buffers must be 4-byte aligned");
+    if (T == 0 || n_envs == 0) return OVC_OK;
+    gae_view_kernel<<<(unsigned)((n_envs + GAE_THREADS - 1) / GAE_THREADS), GAE_THREADS, 0, st>>>(rewards, values, dones, last_values, T,
+                                                                                                   n_envs, gamma, lambda, adv, targets);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "gae_view kernel launch");
     return OVC_OK;
 }
 

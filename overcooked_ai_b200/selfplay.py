@@ -365,6 +365,7 @@ class SampleBatch(object):
     advantages, value_targets  float32 [T, 2N]   GAE (ovc_gae)
     logits        float32 [T, 2N, 8] the policy's heads (columns 0..5 the logits), only with ``keep_logits``
     partner_seat  int8 [T, N]        with a BC partner: its player index at transition t (-1: self-play), else None
+                                     (``one_view``: agent 1's player)
     learner_mask  uint8 [T, 2N]      (property) the rows the learner trains on: all rows but the partner's
     episodes      EpisodeRecords     the episodes that ended in the window (``episodes.finished()``), capacity
                                      ceil(T / horizon): an environment cannot end more episodes in T transitions
@@ -379,29 +380,38 @@ class SampleBatch(object):
     A learner replays chunk k from (state_h[k], state_c[k]) and zeroes the state before step t > k L wherever
     dones[t - 1] (the environment auto-reset: a new episode starts at t), as ``RllibLSTMShapedCNN.forward_sequence`` does
     with ``reset[t] = dones[t - 1]`` (``reset[k L]`` = 0: the stored state already follows the rule).
+
+    ``one_view`` (``AgentPairRollout.collect``: a learner next to a different agent): ONE row per environment, the learner's.
+    Every [T, 2N] / [2N] field above is then [T, N] / [N] (row e: the learner of environment e, at player
+    ``1 - partner_seat[t, e]``), ``state_h`` / ``state_c`` are [ceil(T/L), N, 256], ``partner_seat`` is agent 1's player and
+    ``learner_mask`` is all ones.
     """
 
-    def __init__(self, env, n_steps, keep_logits=False, partner=False, seq_len=None):
+    def __init__(self, env, n_steps, keep_logits=False, partner=False, seq_len=None, one_view=False):
         N, T, dev = env.n_envs, int(n_steps), env.device
+        R = N if one_view else 2 * N
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
         self.env = env
+        self.one_view = bool(one_view)
         self.states = z((T, N, env.state_words), torch.int32)
-        self.actions = z((T, 2 * N), torch.int32)
-        self.logp, self.values, self.rewards, self.advantages, self.value_targets = (z((T, 2 * N), torch.float32) for _ in range(5))
+        self.actions = z((T, R), torch.int32)
+        self.logp, self.values, self.rewards, self.advantages, self.value_targets = (z((T, R), torch.float32) for _ in range(5))
         self.dones = z((T, N), torch.uint8)
-        self.last_values = z(2 * N, torch.float32)
-        self.logits = z((T, 2 * N, 8), torch.float32) if keep_logits else None
-        self.partner_seat = z((T, N), torch.int8) if partner else None
+        self.last_values = z(R, torch.float32)
+        self.logits = z((T, R, 8), torch.float32) if keep_logits else None
+        self.partner_seat = z((T, N), torch.int8) if partner or one_view else None
         self.episodes = EpisodeRecords(env, -(-T // env.horizon) if env.horizon > 0 else 0)
         self.seq_len = seq_len
-        self.state_h = z((-(-T // seq_len), 2 * N, 256), torch.bfloat16) if seq_len else None
-        self.state_c = z((-(-T // seq_len), 2 * N, 256), torch.float32) if seq_len else None
+        self.state_h = z((-(-T // seq_len), R, 256), torch.bfloat16) if seq_len else None
+        self.state_c = z((-(-T // seq_len), R, 256), torch.float32) if seq_len else None
 
     @property
     def learner_mask(self):
-        """uint8 [T, 2N]: 1 on the rows the PPO agent acted on — both rows of a self-play environment, the non-partner row
-        otherwise.  Computed from ``partner_seat``."""
+        """uint8 [T, 2N] (``one_view``: [T, N]): 1 on the rows the PPO agent acted on — both rows of a self-play environment,
+        the non-partner row otherwise, every row of a one-view batch.  Computed from ``partner_seat``."""
         T, N = self.dones.shape
+        if self.one_view:
+            return torch.ones((T, N), dtype=torch.uint8, device=self.dones.device)
         if self.partner_seat is None:
             return torch.ones((T, 2 * N), dtype=torch.uint8, device=self.dones.device)
         agent = torch.arange(2, dtype=torch.int8, device=self.dones.device)
@@ -410,9 +420,13 @@ class SampleBatch(object):
     def observations(self, env_steps, dtype=torch.float32):
         """lossless_state_encoding ``[M, 2, W, H, 26]`` of the env-steps ``env_steps`` (CUDA int64 [M], flat indices
         ``t * N + env``), both agents' views in [env][agent] order: rows ``2 m + i`` of the flattened per-agent tensors
-        (``actions.view(-1, 2)[env_steps]`` etc.) belong to view ``i`` of entry ``m``.  Encoded from the stored records by K2."""
+        (``actions.view(-1, 2)[env_steps]`` etc.) belong to view ``i`` of entry ``m``.  Encoded from the stored records by K2.
+        ``one_view``: the learner's view only, ``[M, W, H, 26]`` (row m belongs to ``actions.view(-1)[env_steps[m]]``)."""
         recs = self.states.view(-1, self.states.shape[-1]).index_select(0, env_steps)
-        return self.env.lossless_state_encoding(dtype=dtype, states=recs)
+        if not self.one_view:
+            return self.env.lossless_state_encoding(dtype=dtype, states=recs)
+        learner = (1 - self.partner_seat.view(-1).index_select(0, env_steps)).to(torch.int32).contiguous()  # view_swap: this view first
+        return self.env.lossless_state_encoding(dtype=dtype, states=recs, view_swap=learner)[:, 0]
 
 
 # The BC partner's draws use their own Philox keys: seed ^ PARTNER_DRAW_SALT for K10's action draw, seed ^ PARTNER_SEAT_SALT
@@ -807,21 +821,23 @@ class _NetworkAgent(_FoldedPolicy):
     (K2's output, which the pair writes once per transition for all its agents: set it before act()), the dense model on N
     rows (K7 -> library layers where K7 fits but K8 does not) and the one-view draw (``sample_actions_view``, or K11).  Its
     draws use key ``seed`` and a counter of its own, on the joint row 2 e + p(e): the numbers a self-play rollout with the
-    same seed draws for that row."""
+    same seed draws for that row.  ``live_seats``: ``swap`` (0 / 1 only) changes between transitions; ``follow_seats()``
+    recomputes the joint rows from it."""
 
-    def __init__(self, env, model, seat, swap, seed, autocast_dtype):
+    def __init__(self, env, model, seat, swap, seed, autocast_dtype, live_seats=False):
         self.env = env
         self._fold(env, model, autocast_dtype, None, None, None)
         N, dev = env.n_envs, env.device
-        self.seat, self.swap, self.seed = int(seat), swap, int(seed)
+        self.seat, self.swap, self.seed, self.live_seats = int(seat), swap, int(seed), live_seats
         self._counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of this agent's draws
         self._scores8 = None  # set to a float32 [N, 8] tensor to make K8 / K11 also write the heads (tests)
         self.values = torch.zeros(N, dtype=torch.float32, device=dev)
         self.obs = None  # [N, 2, W, H, 26] without K7, shared with the other agent of the pair
+        self._base = 2 * torch.arange(N, device=dev) + self.seat
+        self._rows = 2 * torch.arange(N, device=dev) + (self.seat if swap is None else self.seat ^ (swap != 0).long())  # 2 e + p(e)
         if self.fused_first_layer:
             self._act0 = torch.empty((N, self._wt0.shape[1]), dtype=torch.bfloat16, device=dev)
         else:
-            self._rows = 2 * torch.arange(N, device=dev) + (self.seat if swap is None else self.seat ^ (swap != 0).long())  # 2 e + p(e)
             self._flat = torch.empty((N, self.W * self.H * 26), dtype=autocast_dtype or torch.float32, device=dev)
         if not self.fused_tail and not self.lstm:  # library layers: the logits the draw reads
             self._scores = torch.empty((N, 6), dtype=torch.float32, device=dev)
@@ -835,15 +851,24 @@ class _NetworkAgent(_FoldedPolicy):
 
     def live(self):
         """The tensors a transition advances (restored around graph capture)."""
-        return [self._counter] + ([self.h, self.c] if self.lstm else [])
+        return [self._counter] + ([self.h, self.c] if self.lstm else []) + ([self._rows] if self.live_seats else [])
 
-    def act(self, actions):
+    def follow_seats(self):
+        """The joint rows 2 e + (seat ^ swap[e]) after the seats changed (swap 0 / 1)."""
+        torch.add(self._base, self.swap, alpha=1 - 2 * self.seat, out=self._rows)
+
+    def act(self, actions, values=None, logp=None, scores8=None, counter=None, state_out=None, snap=None):
         """This agent's entries of ``actions`` (int32 [N, 2]) from the current state (without K7: from ``self.obs``, K2's
-        encoding of it); values into ``self.values``.  The LSTM state is zeroed where the previous transition ended an
-        episode (``env.done``)."""
+        encoding of it); values into ``values`` (default ``self.values``), and, each optional, the log-probability of the
+        draw into ``logp`` and the heads into ``scores8`` (float32 [N, 8]).  ``counter``: the draw's counter (default this
+        agent's).  The LSTM state is zeroed where the previous transition ended an episode (``env.done``); K11 writes the new
+        state to ``state_out`` (h, c) (default: in place) and the state it used to ``snap`` (h, c) when given."""
         env, N = self.env, self.env.n_envs
         lib, seed = _native.lib(), self.seed & (2**64 - 1)
         ptr = lambda t: 0 if t is None else t.data_ptr()
+        values = self.values if values is None else values
+        scores8 = self._scores8 if scores8 is None else scores8
+        counter = self._counter if counter is None else counter
         with torch.no_grad():
             if self.fused_first_layer:
                 flat, first = env.encoded_linear_view(self._wt0, self._b0, self.seat, self.swap, out=self._act0, neg_slope=0.2), 1  # K7
@@ -864,39 +889,51 @@ class _NetworkAgent(_FoldedPolicy):
                 else:
                     self._x.copy_(self.dense_model.hidden_from(flat, first))
                 w, b, wo, bo = self._lstm_tables
+                h_out, c_out = state_out or (self.h, self.c)
+                snap_h, snap_c = snap or (None, None)
                 _native.check(lib.ovc_lstm_head_view(
                     self._x.data_ptr(), self.h.data_ptr(), self.c.data_ptr(), env.done.data_ptr(), N, w.data_ptr(), b.data_ptr(),
-                    wo.data_ptr(), bo.data_ptr(), self.dense_model.n_actions, seed, self._counter.data_ptr(), ptr(self.swap), self.seat,
-                    self.h.data_ptr(), self.c.data_ptr(), 0, 0, actions.data_ptr(), self.values.data_ptr(), 0, ptr(self._scores8),
-                    env._stream()))
+                    wo.data_ptr(), bo.data_ptr(), self.dense_model.n_actions, seed, counter.data_ptr(), ptr(self.swap), self.seat,
+                    h_out.data_ptr(), c_out.data_ptr(), ptr(snap_h), ptr(snap_c), actions.data_ptr(), values.data_ptr(), ptr(logp),
+                    ptr(scores8), env._stream()))
             elif self.fused_tail:
                 w1, b1, wh, bh, wo, bo = self._tail
                 _native.check(lib.ovc_policy_tail_view(
                     self._z.data_ptr(), N, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
-                    wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, seed, self._counter.data_ptr(),
-                    ptr(self.swap), self.seat, actions.data_ptr(), self.values.data_ptr(), ptr(self._scores8), 0, env._stream()))
+                    wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, seed, counter.data_ptr(),
+                    ptr(self.swap), self.seat, actions.data_ptr(), values.data_ptr(), ptr(scores8), ptr(logp), env._stream()))
             else:
                 logits, value = self.dense_model.forward_from(flat, first)
                 self._scores.copy_(logits)
-                self.values.copy_(value)
-                env.sample_actions_view(self._scores, self._counter, self.seat, self.swap, seed=self.seed, out=actions)
+                values.copy_(value)
+                env.sample_actions_view(self._scores, counter, self.seat, self.swap, seed=self.seed, out=actions, logp_out=logp)
+                if scores8 is not None:
+                    scores8[:, :self._scores.shape[1]].copy_(self._scores)
 
 
 class _BCAgent(object):
     """A ``BCPolicy`` agent of an ``AgentPairRollout``: K10 with ``partner_seat[e] = p(e)`` in every environment, its draws
-    keyed by ``seed ^ PARTNER_DRAW_SALT`` on a counter of its own (the draws of PPO_BC's partner)."""
+    keyed by ``seed ^ PARTNER_DRAW_SALT`` on a counter of its own (the draws of PPO_BC's partner).  ``live_seats``: ``swap``
+    (0 / 1 only) changes between transitions; ``follow_seats()`` recomputes ``partner_seat`` from it."""
 
-    def __init__(self, env, policy, seat, swap, seed):
+    def __init__(self, env, policy, seat, swap, seed, live_seats=False):
         self.env, self.policy = env, policy.to(env.device).eval()
-        self.seat, self.seed = int(seat), int(seed)
+        self.seat, self.seed, self.swap, self.live_seats = int(seat), int(seed), swap, live_seats
         self._tables = self.policy.tables()
         self._n_actions = self.policy.logits.out_features
-        self.partner_seat = (torch.full((env.n_envs,), self.seat, dtype=torch.int32, device=env.device) if swap is None
-                             else (self.seat ^ (swap != 0).int()).to(torch.int32).contiguous())
+        if live_seats and self.seat == 0:
+            self.partner_seat = swap  # p(e) = swap[e]: the live seats themselves
+        else:
+            self.partner_seat = (torch.full((env.n_envs,), self.seat, dtype=torch.int32, device=env.device) if swap is None
+                                 else (self.seat ^ (swap != 0).int()).to(torch.int32).contiguous())
         self._counter = torch.zeros(2, dtype=torch.int64, device=env.device)
 
     def live(self):
-        return [self._counter]
+        return [self._counter] + ([self.partner_seat] if self.live_seats and self.seat else [])
+
+    def follow_seats(self):
+        if self.seat:
+            torch.bitwise_xor(self.swap, 1, out=self.partner_seat)
 
     def act(self, actions):
         self.env.partner_actions(self._tables, self.partner_seat, self._counter, seed=self.seed ^ PARTNER_DRAW_SALT,
@@ -908,27 +945,38 @@ class _BCAgent(object):
 
 
 class AgentPairRollout(object):
-    """Two different agents in fixed seats, each evaluated on its own seat's view only: the reference's evaluation of an agent
-    pair (rllib.py ``evaluate``: ``AgentEvaluator.evaluate_agent_pair(AgentPair(agent_0_policy, agent_1_policy))``) with N
-    environments on the device.  PPO against a held-out BC human proxy, cross-play of two PPO agents, BC against BC.
+    """Two different agents, each evaluated on its own seat's view only: the reference's evaluation of an agent pair
+    (rllib.py ``evaluate``: ``AgentEvaluator.evaluate_agent_pair(AgentPair(agent_0_policy, agent_1_policy))``) with N
+    environments on the device — PPO against a held-out BC human proxy, cross-play of two PPO agents, BC against BC — and,
+    with ``collect()``, PPO training of agent 0 next to a fixed agent 1 (a best response, the second stage of fictitious
+    co-play, training against a held-out PPO, LSTM or BC partner).
 
     agents: (agent0, agent1), each an ``RllibShapedCNN``, an ``RllibLSTMShapedCNN`` or a ``BCPolicy`` (the same object twice
     is allowed).  Agent 0 plays player ``swap[e]`` of environment e, agent 1 the other one.  A network agent runs its own
     policy on N rows (the one-view forms of K7 / K8 / K11 and the draw, with K9 on N rows, where ``fused_kernel_support``
     allows them; K2, the dense model on the agent's rows and the one-view draw elsewhere); a BC agent is K10.
     swap: int32 CUDA tensor [N] or None (no swap): both seat orders in one batch; fixed for the rollout's lifetime.
+    random_seats: instead of ``swap``, agent 1's player ``partner_seat[e]`` is drawn at construction and again for every
+    environment whose episode ended (the reference's gym ``Overcooked`` wrapper and ``OvercookedMultiAgent`` redraw the
+    agents' players at every reset): PPO_BC's seat draw (``env.assign_partners``) at a ``bc_factor`` of 1, key ``seed ^
+    PARTNER_SEAT_SALT``, with a counter of its own, so that ``(learner, bc)`` plays exactly the seats of
+    ``SelfPlayRollout(learner, partner=bc, bc_factor=1)``.  Not together with ``swap``.
     seed: the draws' key.  Each agent has its own counter; network agents use ``seed``, BC agents ``seed ^
     PARTNER_DRAW_SALT`` (K10's key in PPO_BC).  A pair therefore draws what ``SelfPlayRollout`` (both agents one network) or
     PPO_BC (``SelfPlayRollout(partner=..., bc_factor=1)``) draw on the same rows and steps.
     autocast_dtype: as ``SelfPlayRollout``'s, for every network agent (an LSTM agent needs bfloat16).
     episode_capacity: as ``SelfPlayRollout``'s.  Every finished episode's ``partner_seat`` is agent 1's player.
+    max_seq_len: as ``SelfPlayRollout``'s, for an LSTM learner's ``collect()``.
 
     A transition is K2 (once, when a network agent runs without K7), agent 0's policy, agent 1's policy, K1 (auto-reset
-    inside), then ``record_transition`` with the episode statistics.  ``ret_sparse`` is the running sparse return of every environment."""
+    inside), ``record_transition`` with the episode statistics (``record_transition_view`` of agent 0's row in collect()),
+    then, with random_seats, the seat draw.  ``ret_sparse`` is the running sparse return of every environment."""
 
-    def __init__(self, env, agents, swap=None, seed=0, use_graph=True, episode_capacity=1, autocast_dtype=torch.bfloat16):
+    def __init__(self, env, agents, swap=None, seed=0, use_graph=True, episode_capacity=1, autocast_dtype=torch.bfloat16,
+                 random_seats=False, max_seq_len=20):
         assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
         assert len(agents) == 2, "agents: (agent0, agent1)"
+        assert not (random_seats and swap is not None), "random_seats draws the seats: pass no swap tensor with it"
         for a in agents:
             assert isinstance(a, (RllibShapedCNN, BCPolicy)), "an agent is an RllibShapedCNN, an RllibLSTMShapedCNN or a BCPolicy"
             assert not isinstance(a, RllibLSTMShapedCNN) or autocast_dtype == torch.bfloat16, \
@@ -937,8 +985,23 @@ class AgentPairRollout(object):
         if swap is not None:
             assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == N, "swap: int32 CUDA [N]"
         self.env, self.swap, self.seed, self.use_graph = env, swap, int(seed), use_graph
-        self.agents = [_BCAgent(env, a, seat, swap, seed) if isinstance(a, BCPolicy) else _NetworkAgent(env, a, seat, swap, seed, autocast_dtype)
-                       for seat, a in enumerate(agents)]
+        self.random_seats = bool(random_seats)
+        self.max_seq_len = int(max_seq_len)
+        assert self.max_seq_len >= 1
+        if self.random_seats:
+            # agent 1's player, drawn for every environment now and at every episode end; agent k then sits at player
+            # (1 - k) ^ partner_seat[e], i.e. it is passed seat 1 - k and swap = partner_seat
+            self.partner_seat = torch.full((N,), -1, dtype=torch.int32, device=dev)
+            self._seat_factor = torch.ones(1, dtype=torch.float32, device=dev)
+            self._seat_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of the seat draw
+            self._assign_seats(None)
+            seats, swap = (1, 0), self.partner_seat
+        else:
+            seats = (0, 1)
+            self.partner_seat = (torch.ones(N, dtype=torch.int32, device=dev) if swap is None
+                                 else (1 ^ (swap != 0).int()).to(torch.int32).contiguous())  # agent 1's player
+        self.agents = [_BCAgent(env, a, seat, swap, seed, self.random_seats) if isinstance(a, BCPolicy)
+                       else _NetworkAgent(env, a, seat, swap, seed, autocast_dtype, self.random_seats) for seat, a in zip(seats, agents)]
         # network agents without K7 read K2's observation, written once per transition for both of them
         library = [a for a in self.agents if isinstance(a, _NetworkAgent) and not a.fused_first_layer]
         l = env.layouts[0]
@@ -947,42 +1010,125 @@ class AgentPairRollout(object):
             a.obs = self.obs
         self.actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
         self.ret_sparse = torch.zeros(N, dtype=torch.int64, device=dev)
-        self._factor = torch.ones(1, dtype=torch.float32, device=dev)  # the episode records' rewards: sparse + shaped
-        self.partner_seat = (torch.ones(N, dtype=torch.int32, device=dev) if swap is None
-                             else (1 ^ (swap != 0).int()).to(torch.int32).contiguous())  # agent 1's player
+        self.factor = 1.0
+        self._factor = torch.ones(1, dtype=torch.float32, device=dev)  # reward_shaping_factor, read by the captured graphs
         self.stats = EpisodeStats(env)
         self.episodes = EpisodeRecords(env, episode_capacity)
         self.graph = None
+        self._collect_graphs = {}  # (n_steps, keep_logits) -> ((gamma, lam), CUDA graph of the window)
+        self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
+        self._boot_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # the bootstrap's draws leave the learner's counter alone
+        self._boot_actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
+        learner = self.agents[0]
+        if getattr(learner, "lstm", False):  # the bootstrap's (discarded) LSTM state
+            self._h_boot, self._c_boot = torch.empty_like(learner.h), torch.empty_like(learner.c)
 
-    def _transition(self):
+    @property
+    def reward_shaping_factor(self):
+        """The factor of the shaped rewards in collect()'s rewards and in the episode records' ``ep_reward_by_agent``
+        (rllib.py:328-329; default 1).  Setting it takes effect without a re-capture (the graphs read a device scalar)."""
+        return self.factor
+
+    @reward_shaping_factor.setter
+    def reward_shaping_factor(self, value):
+        self.factor = float(value)
+        self._factor.fill_(self.factor)
+
+    def _assign_seats(self, done):
+        self.env.assign_partners(self.partner_seat, self._seat_factor, self._seat_counter, seed=self.seed ^ PARTNER_SEAT_SALT, done=done)
+
+    def _transition(self, b=None, t=0):
+        """One transition.  Without ``b`` (run()) finished episodes go to self.episodes; with a one-view ``SampleBatch`` ``b``
+        (collect()) agent 0's row is recorded in its slot ``t``: state, action, value, logp, logits, reward, done, agent 1's
+        player, the LSTM state every seq_len transitions, and finished episodes in b.episodes."""
         env = self.env
+        learner, partner = self.agents
         if self.obs is not None:
             env.lossless_state_encoding(out=self.obs)  # K2
-        for a in self.agents:
-            a.act(self.actions)
+        if b is None:
+            learner.act(self.actions)
+        else:
+            b.states[t].copy_(env.state)
+            snap = None
+            if b.seq_len and t % b.seq_len == 0:
+                snap = (b.state_h[t // b.seq_len], b.state_c[t // b.seq_len])
+            learner.act(self.actions, values=b.values[t], logp=b.logp[t], scores8=None if b.logits is None else b.logits[t], snap=snap)
+            torch.index_select(self.actions.view(-1), 0, learner._rows, out=b.actions[t])
+            b.partner_seat[t].copy_(self.partner_seat)
+        partner.act(self.actions)
         env.step(self.actions)  # K1 (auto-reset inside)
-        env.record_transition(self._factor, ret_sparse=self.ret_sparse, stats=self.stats, records=self.episodes,
-                              partner_seat=self.partner_seat)
+        if b is None:
+            env.record_transition(self._factor, ret_sparse=self.ret_sparse, stats=self.stats, records=self.episodes,
+                                  partner_seat=self.partner_seat)
+        else:
+            env.record_transition_view(self._factor, learner.seat, learner.swap, b.rewards[t], dones=b.dones[t], ret_sparse=self.ret_sparse,
+                                       stats=self.stats, records=b.episodes, partner_seat=self.partner_seat)
+        if self.random_seats:  # after the record: the ending episode's seats went into it
+            self._assign_seats(env.done)
+            for a in self.agents:
+                a.follow_seats()
+
+    def _capture(self, warm_up, body):
+        """A CUDA graph of ``body``; the state, the returns, the statistics, the counters and the seats are restored after
+        warm-up and capture."""
+        live = [self.env.state, self.env.done, self.ret_sparse] + self.stats.state_tensors() + self.episodes.tensors()
+        if self.random_seats:
+            live += [self.partner_seat, self._seat_counter]
+        for a in self.agents:
+            live += a.live()
+        return _capture_graph(self.env, live, warm_up, body)
 
     def run(self, n_steps):
         """Advance every environment n_steps transitions (one CUDA graph per transition with use_graph); returns the number
         of env-steps done."""
         if self.use_graph and self.graph is None:
-            live = [self.env.state, self.env.done, self.ret_sparse] + self.stats.state_tensors() + self.episodes.tensors()
-            for a in self.agents:
-                live += a.live()
-
             def warm_up():
                 for _ in range(3):
                     self._transition()
-            self.graph = _capture_graph(self.env, live, warm_up, self._transition)
+            self.graph = self._capture(warm_up, self._transition)
         step = self._transition if self.graph is None else self.graph.replay
         for _ in range(n_steps):
             step()
         return n_steps * self.env.n_envs
 
+    def _collect_window(self, b, n_steps, gamma, lam):
+        b.episodes.clear()
+        for t in range(n_steps):
+            self._transition(b, t)
+        if self.obs is not None:
+            self.env.lossless_state_encoding(out=self.obs)
+        # the learner's bootstrap value at the seats after the window; its LSTM state goes to scratch
+        self.agents[0].act(self._boot_actions, values=b.last_values, counter=self._boot_counter,
+                           state_out=(self._h_boot, self._c_boot) if self.agents[0].lstm else None)
+        self.env.gae_view(b.rewards, b.values, b.dones, b.last_values, gamma, lam, b.advantages, b.value_targets)
+
+    def collect(self, n_steps, gamma, lam, keep_logits=False):
+        """Advance every environment n_steps transitions, as run() does (the same kernels and draws), and return agent 0's
+        side of them as a one-view ``SampleBatch`` (one row per environment: agent 0's action, logp, value, reward and GAE
+        advantages; ``partner_seat`` is agent 1's player) for a PPO update of agent 0 next to the fixed agent 1.  The batch's
+        tensors are reused by the next collect() with the same n_steps / keep_logits.  With use_graph the whole window is one
+        CUDA graph (captured once per n_steps / keep_logits; a new gamma or lam re-captures it).  After an update, call
+        ``sync_weights()``; a population member is swapped into agent 1 the same way (``load_state_dict`` on its model, then
+        ``sync_weights()``)."""
+        assert isinstance(self.agents[0], _NetworkAgent), "collect() trains agents[0]: an RllibShapedCNN or RllibLSTMShapedCNN, not a BCPolicy"
+        assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
+        key = (int(n_steps), bool(keep_logits))
+        b = self._batches.get(key)
+        if b is None:
+            b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits, seq_len=self.max_seq_len if self.agents[0].lstm else None,
+                                                 one_view=True)
+        if not self.use_graph:
+            self._collect_window(b, n_steps, gamma, lam)
+            return b
+        g = self._collect_graphs.get(key)
+        if g is None or g[0] != (gamma, lam):
+            g = self._collect_graphs[key] = ((gamma, lam), self._capture(lambda: self._collect_window(b, 1, gamma, lam),
+                                                                         lambda: self._collect_window(b, n_steps, gamma, lam)))
+        g[1].replay()
+        return b
+
     def sync_weights(self):
-        """Re-fold every agent's network (e.g. a learner's after an update) in place: the captured graph uses the new weights
+        """Re-fold every agent's network (e.g. a learner's after an update) in place: the captured graphs use the new weights
         without a re-capture."""
         for a in self.agents:
             a.sync_weights()

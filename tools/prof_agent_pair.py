@@ -6,6 +6,10 @@ file under --out:
   AgentPairRollout((PPO_A, PPO_B)) against SelfPlayRollout(PPO_A), alternated in one process, 3 times each;
   per-kernel times, best of 3 over 50 launches: K7 one view (N rows) against two views (2N rows), K9 on N against 2N rows,
   K8 with the one-view draw on N rows against the two-view K8 on 2N rows, K11 one view against two views;
+  collect(T) of a learner next to a fixed partner (AgentPairRollout(..., random_seats=True).collect): (PPO, BC) against
+  SelfPlayRollout(PPO, partner=BC, bc_factor=1).collect, (PPO, frozen PPO) against self-play collect, and (LSTM PPO, BC),
+  alternated in one process, 3 times each;
+  per-kernel times of the learner-row record and GAE kernels against their two-row forms (best of 3 over 50 launches);
   the card's name and power limit, read in the same run.
 
     python tools/prof_agent_pair.py --out DIR
@@ -64,6 +68,39 @@ for k, v in times.items():
     out["run_us_per_transition_" + k] = min(v) * 1e3 / T
 out["pair_ppo_bc_over_ppo_bc"] = min(times["pair_ppo_bc"]) / min(times["ppo_bc_bc_factor_1"])
 out["pair_ppo_a_ppo_b_over_selfplay"] = min(times["pair_ppo_a_ppo_b"]) / min(times["selfplay_ppo_a"])
+
+# collect(T): a learner next to a fixed partner against the same network's PPO_BC / self-play collect
+collects = {"pair_ppo_bc": AgentPairRollout(env(), (ppo_a, bc), seed=1, random_seats=True),
+            "ppo_bc_bc_factor_1": runs["ppo_bc_bc_factor_1"],
+            "pair_ppo_a_frozen_ppo_b": AgentPairRollout(env(), (ppo_a, ppo_b), seed=1, random_seats=True),
+            "selfplay_ppo_a": runs["selfplay_ppo_a"],
+            "pair_lstm_bc": AgentPairRollout(env(), (RllibLSTMShapedCNN(5, 4).cuda(), bc), seed=1, random_seats=True)}
+for r in collects.values():
+    r.collect(T, 0.99, 0.98)  # capture + warm
+torch.cuda.synchronize()
+ctimes = {k: [] for k in collects}
+for _ in range(3):
+    for k, r in collects.items():
+        ctimes[k].append(ms(lambda: r.collect(T, 0.99, 0.98)))
+for k, v in ctimes.items():
+    out["collect_ms_" + k] = v
+out["collect_pair_ppo_bc_over_ppo_bc"] = min(ctimes["pair_ppo_bc"]) / min(ctimes["ppo_bc_bc_factor_1"])
+out["collect_pair_ppo_a_frozen_ppo_b_over_selfplay"] = min(ctimes["pair_ppo_a_frozen_ppo_b"]) / min(ctimes["selfplay_ppo_a"])
+bp, bs = collects["pair_ppo_bc"]._batches[(T, False)], collects["selfplay_ppo_a"]._batches[(T, False)]
+ce = collects["pair_ppo_bc"].env
+one = torch.ones(1, device="cuda")
+ret = torch.zeros(N, dtype=torch.int64, device="cuda")
+record = {"record_transition_view_stats_us": lambda: ce.record_transition_view(one, 1, None, bp.rewards[0], dones=bp.dones[0], ret_sparse=ret,
+                                                                               stats=collects["pair_ppo_bc"].stats, records=bp.episodes),
+          "record_transition_stats_us": lambda: ce.record_transition(one, rewards=bs.rewards[0], dones=bp.dones[0], ret_sparse=ret,
+                                                                     stats=collects["pair_ppo_bc"].stats, records=bp.episodes),
+          "gae_view_us": lambda: ce.gae_view(bp.rewards, bp.values, bp.dones, bp.last_values, 0.99, 0.98, bp.advantages, bp.value_targets),
+          "gae_two_rows_us": lambda: ce.gae(bs.rewards, bs.values, bs.dones, bs.last_values, 0.99, 0.98, bs.advantages, bs.value_targets)}
+for f in record.values():
+    f()
+torch.cuda.synchronize()
+for k, f in record.items():
+    out[k] = min(ms(f, reps=50) for _ in range(3)) * 1e3
 
 # per-kernel: one view (N rows) against two views (2N rows)
 sp, agent = runs["selfplay_ppo_a"], runs["pair_ppo_bc"].agents[0]

@@ -241,4 +241,17 @@ for name, agents in (("cramped_room", lambda W, H: (RllibShapedCNN(W, H), RllibL
     assert np.array_equal(env8.state.cpu().numpy(), st)
 torch.cuda.synchronize()
 print("agent pairs (one-view K7 / K8 / K11 / draw, K10) ok", flush=True)
+# a learner next to a fixed partner: collect() with random seats (the learner-row record kernel with statistics, the seat
+# draw, the learner-row GAE) on a 5x4 grid (CNN and LSTM learners) and on a 9x5 grid (library layers), 37 environments,
+# episodes ending inside the window
+for name, agents in (("cramped_room", lambda W, H: (RllibShapedCNN(W, H), BCPolicy())),
+                     ("cramped_room", lambda W, H: (RllibLSTMShapedCNN(W, H), RllibShapedCNN(W, H))),
+                     ("asymmetric_advantages", lambda W, H: (RllibShapedCNN(W, H), RllibShapedCNN(W, H)))):
+    env9 = BatchedOvercookedEnv(name, 37, horizon=3, auto_reset=True)
+    l9 = env9.layouts[0]
+    pair = AgentPairRollout(env9, agents(l9.width, l9.height), seed=4, use_graph=False, random_seats=True, max_seq_len=2)
+    b = pair.collect(5, 0.99, 0.95, keep_logits=True)
+    assert b.dones.any() and (b.partner_seat >= 0).all()
+torch.cuda.synchronize()
+print("learner-row collect (record_transition_view, gae_view, seat draw) ok", flush=True)
 print("sanitize_smoke: all ok")
