@@ -655,6 +655,58 @@ int ovc_assign_partners(const int32_t *done, const float *bc_factor, int64_t n_e
                         void *stream);
 
 /*
+ * A population of partners (fictitious co-play, training against a set of checkpoints, PPO_BC with several BC human
+ * proxies): each environment plays one of n_members (1..64, OVC_E_BADARG otherwise) members in one seat, drawn per episode,
+ * and each member's kernels run on its own environments only.
+ *
+ * ovc_group_members: a stable counting sort of the environments by member (int32 [n_envs], every value in
+ *   [0, n_members); other values are undefined behaviour): order int32 [n_envs] = the environment indices grouped by member,
+ *   ascending within a group; offsets int32 [n_members + 1] = the group starts (offsets[n_members] = n_envs), so member k's
+ *   environments are order[offsets[k] .. offsets[k + 1]).  One CTA, no host synchronisation.  n_envs < 2^31; n_envs = 0
+ *   writes nothing.  member, order, offsets 4-byte aligned.
+ * ovc_assign_members: for every environment e with done[e] != 0 (ovc_step's int32 done; done = NULL: every environment),
+ *   in this order:
+ *     record  if done != NULL, rec_member != NULL and count[e] < capacity: rec_member[count[e]][e] = member[e]
+ *             (rec_member int32 [capacity][n_envs]: the slot ovc_record_transition_stats writes the ending episode to when it
+ *             runs after this call with the same count, int32 [n_envs]; at a full buffer nothing is written)
+ *     draw    if thresholds != NULL: Philox4x32-10, key = seed, counter = (e low, e high, step low, step high) -> word w0;
+ *             member[e] = #{k < n_members - 1 : w0 >= thresholds[k]}
+ *   thresholds int64 [n_members - 1] in DEVICE memory (a captured graph follows a changed distribution), computed by the
+ *   host as floor(cdf[k] * 2^32) with cdf[k] the float64 cumulative share of members 0..k: a member of weight 0 is never
+ *   drawn.  counter uint64[2] as ovc_sample_actions' (one step per launch), used and advanced only with thresholds.
+ *   done, member, rec_member, count 4-byte aligned, thresholds and counter 8-byte aligned; capacity >= 0.
+ *
+ * The rows map of the *_rows forms below (one member's share of one-view rows): compact row r in [range[0], range[1]) is
+ * environment e = rows[r] (int32, in [0, n_envs)), whose agent sits at player p(e) = seat ^ (swap[e] != 0) (swap nullable,
+ * seat 0 or 1); its joint row is 2 e + p(e).  range points to two int32 in DEVICE memory (e.g. offsets + k of
+ * ovc_group_members, with rows = order), so one captured launch serves any group size; the range is clipped to
+ * [0, n_rows).  rows, range, swap 4-byte aligned.  Each form computes on row r bit for bit what its one-view form computes
+ * on the row of environment rows[r], and leaves every other row and the other seat's action entries untouched.
+ *
+ * ovc_encode_linear_rows: ovc_encode_linear_view on the rows map: out[r] (bfloat16 [n_envs][n_out]) = environment rows[r]'s
+ *   row of ovc_encode_linear_view.  A CTA with no rows in the range exits before it loads its weight slice.
+ * ovc_wide_layers_range: ovc_wide_layers on rows [range[0], range[1]) of a0 / z2 ([m][...], m < 2^31); other rows of z2 untouched.
+ * ovc_policy_tail_rows: ovc_policy_tail_view on the rows map: x, values, scores, logp row r; the draw on the joint row of
+ *   environment rows[r] into actions (int32 [n_rows][2]).  Every CTA advances the counter, also for an empty range.
+ * ovc_sample_actions_rows: ovc_sample_actions_view on the rows map: scores / logp row r, the draw on the joint row of
+ *   environment rows[r].  Every CTA advances the counter, also for an empty range.  counter 8-byte aligned.
+ */
+int ovc_group_members(const int32_t *member, int n_members, int64_t n_envs, int32_t *order, int32_t *offsets, void *stream);
+int ovc_assign_members(const int32_t *done, const int64_t *thresholds, int n_members, int64_t n_envs, uint64_t seed, uint64_t *counter,
+                       int32_t *member, int32_t *rec_member, const int32_t *count, int capacity, void *stream);
+int ovc_encode_linear_rows(const void *layouts, int n_layouts, const int32_t *state, const int32_t *swap, int seat, const int32_t *rows,
+                           const int32_t *range, const void *wt, const float *bias, void *out, int64_t n_envs, int state_words, int width,
+                           int height, int horizon, int n_out, float neg_slope, void *stream);
+int ovc_wide_layers_range(const void *a0, int64_t m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2,
+                          int n2, float slope, const int32_t *range, void *z2, void *stream);
+int ovc_policy_tail_rows(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                         const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                         float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *swap, int seat, const int32_t *rows,
+                         const int32_t *range, int32_t *actions, float *values, float *scores, float *logp, void *stream);
+int ovc_sample_actions_rows(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter, const int32_t *swap,
+                            int seat, const int32_t *rows, const int32_t *range, int32_t *actions, float *logp, void *stream);
+
+/*
  * featurize_state (:2579-2898) with the default planner parameters (NO_COUNTERS_PARAMS,
  * planners.py:27-34): out float32[n_envs][2][F],
  * F = 2*(num_pots*10+28), lut = ovc_feat_lut_entry_t[n_layouts][256][4].  view_swap as above.

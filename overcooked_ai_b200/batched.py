@@ -444,6 +444,76 @@ class BatchedOvercookedEnv(object):
             self._stream()))
         return out
 
+    def encoded_linear_rows(self, wt, bias, seat, swap, rows, rng, out, neg_slope=0.2):
+        """``encoded_linear_view`` on the rows map (ovc_encode_linear_rows): ``out[r]`` (bfloat16 ``[N, n_out]``) for the
+        compact rows ``r`` in ``[rng[0], rng[1])`` only, the row ``encoded_linear_view`` writes for environment ``rows[r]``.
+        ``rows`` int32 CUDA [N] (e.g. ``group_members``' order), ``rng`` two int32 in device memory (e.g. ``offsets[k:k + 2]``)."""
+        assert len({(l.width, l.height) for l in self.layouts}) == 1, "one grid shape per call (group envs by layout)"
+        W, H = self.layouts[0].width, self.layouts[0].height
+        assert wt.is_cuda and wt.dtype == torch.bfloat16 and wt.is_contiguous() and wt.shape[0] == W * H * 26, wt.shape
+        n_out = wt.shape[1]
+        assert bias.is_cuda and bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == n_out
+        for t, n in ((swap, self.n_envs), (rows, self.n_envs), (rng, 2)):
+            assert t is None or (t.dtype == torch.int32 and t.is_cuda and t.is_contiguous() and t.numel() == n)
+        assert out.is_cuda and out.dtype == torch.bfloat16 and out.is_contiguous() and out.numel() == self.n_envs * n_out
+        _native.check(self._lib.ovc_encode_linear_rows(
+            self.tables.data_ptr(), self.n_layouts, self.state.data_ptr(), 0 if swap is None else swap.data_ptr(), int(seat),
+            rows.data_ptr(), rng.data_ptr(), wt.data_ptr(), bias.data_ptr(), out.data_ptr(), self.n_envs, self.state_words, W, H,
+            self.horizon if self.horizon > 0 else 2**31 - 1, n_out, float(neg_slope), self._stream()))
+        return out
+
+    def sample_actions_rows(self, scores, counter, seat, swap, rows, rng, seed=0, out=None, logp_out=None):
+        """``sample_actions_view`` on the rows map (ovc_sample_actions_rows): ``scores`` float32 ``[N, ld]`` row r (for r in
+        ``[rng[0], rng[1])``) is environment ``rows[r]``'s agent, drawn with the Philox counter of its joint row into
+        ``out`` (int32 [N, 2]); ``logp_out[r]`` optional.  The counter advances by one whatever the range holds."""
+        assert scores.is_cuda and scores.dtype == torch.float32 and scores.dim() == 2 and scores.stride(1) == 1 and scores.shape[0] == self.n_envs
+        assert counter.is_cuda and counter.dtype == torch.int64 and counter.numel() == 2 and counter.is_contiguous()
+        for t, n in ((swap, self.n_envs), (rows, self.n_envs), (rng, 2)):
+            assert t is None or (t.dtype == torch.int32 and t.is_cuda and t.is_contiguous() and t.numel() == n)
+        assert out.is_cuda and out.dtype == torch.int32 and out.is_contiguous() and out.numel() == 2 * self.n_envs
+        if logp_out is not None:
+            assert logp_out.is_cuda and logp_out.dtype == torch.float32 and logp_out.is_contiguous() and logp_out.numel() == self.n_envs
+        _native.check(self._lib.ovc_sample_actions_rows(
+            scores.data_ptr(), scores.stride(0), 6, self.n_envs, int(seed) & (2**64 - 1), counter.data_ptr(),
+            0 if swap is None else swap.data_ptr(), int(seat), rows.data_ptr(), rng.data_ptr(), out.data_ptr(),
+            0 if logp_out is None else logp_out.data_ptr(), self._stream()))
+        return out
+
+    def group_members(self, member, n_members, order, offsets):
+        """The environments grouped by population member (ovc_group_members, a stable counting sort on the device):
+        ``member`` int32 [N] with values in [0, n_members); writes ``order`` int32 [N] (environment indices by member,
+        ascending within a member) and ``offsets`` int32 [n_members + 1] (member k's environments are
+        ``order[offsets[k]:offsets[k + 1]]``)."""
+        assert 1 <= n_members <= 64
+        for t, n in ((member, self.n_envs), (order, self.n_envs), (offsets, n_members + 1)):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n
+        _native.check(self._lib.ovc_group_members(member.data_ptr(), int(n_members), self.n_envs, order.data_ptr(), offsets.data_ptr(),
+                                                  self._stream()))
+        return order, offsets
+
+    def assign_members(self, member, n_members, thresholds=None, counter=None, seed=0, done=None, records=None):
+        """The per-episode population draw (ovc_assign_members): for every environment whose episode ended with the last
+        ``step`` (``done`` int32 [N], e.g. ``self.done``; None = every environment), first the ending episode's member into
+        ``records.partner_member`` (an ``EpisodeRecords`` built with ``members=True``, before ``record_transition`` writes
+        the episode to the same slot), then, with ``thresholds`` (int64 CUDA [n_members - 1], ``member_thresholds``), a new
+        member drawn from them.  ``counter`` as ``partner_actions``'."""
+        assert member.is_cuda and member.dtype == torch.int32 and member.is_contiguous() and member.numel() == self.n_envs
+        if thresholds is not None:
+            assert thresholds.is_cuda and thresholds.dtype == torch.int64 and thresholds.is_contiguous() and thresholds.numel() >= n_members - 1
+            assert counter.is_cuda and counter.dtype == torch.int64 and counter.numel() == 2 and counter.is_contiguous()
+        if done is not None:
+            assert done.is_cuda and done.dtype == torch.int32 and done.is_contiguous() and done.numel() == self.n_envs
+        rec = None
+        if records is not None:
+            assert records.env is self and records.partner_member is not None, "records built with members=True"
+            rec = records
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        _native.check(self._lib.ovc_assign_members(
+            ptr(done), ptr(thresholds), int(n_members), self.n_envs, int(seed) & (2**64 - 1), ptr(counter), member.data_ptr(),
+            0 if rec is None or rec.capacity == 0 else rec.partner_member.data_ptr(), 0 if rec is None else rec.count.data_ptr(),
+            0 if rec is None else rec.capacity, self._stream()))
+        return member
+
     def sample_actions(self, scores, counter, seed=0, out=None, logp_out=None):
         """Joint actions drawn from the policy's logits (ovc_sample_actions: Gumbel-max on Philox draws, one kernel).
         ``scores`` float32 ``[2N, ld]`` (rows ordered [env][agent], the first 6 columns are the logits), ``counter`` an
@@ -872,9 +942,10 @@ class EpisodeRecords(object):
     sparse_r_by_agent / shaped_r_by_agent int64 [.., 2], game_stats int32 [.., 2, 25] (event counts, the ``len()`` of the
     reference's game_stats lists), reward_by_agent float32 [.., 2] (the sum of the per-agent rewards of the episode);
     count int32 [N] (episodes written per environment), dropped int32 [N] (episodes that ended with the buffer full,
-    not written)."""
+    not written).  ``members=True`` (a population of partners): also partner_member int32 [capacity, N], the member each
+    episode was played with (written by ``env.assign_members``); None otherwise."""
 
-    def __init__(self, env, capacity):
+    def __init__(self, env, capacity, members=False):
         self.env = env
         self.capacity = int(capacity)
         assert self.capacity >= 0
@@ -886,10 +957,11 @@ class EpisodeRecords(object):
         self.reward_by_agent = z((C, N, 2), torch.float32)
         self._counters = z((2, N), torch.int32)  # count and dropped: one memset clears both
         self.count, self.dropped = self._counters[0], self._counters[1]
+        self.partner_member = z((C, N), torch.int32) if members else None
 
     def tensors(self):
         return [self.length, self.layout, self.partner_seat, self.sparse_r_by_agent, self.shaped_r_by_agent, self.game_stats,
-                self.reward_by_agent, self._counters]
+                self.reward_by_agent, self._counters] + ([] if self.partner_member is None else [self.partner_member])
 
     def clear(self):
         """Forget every record (stream ordered, one memset: capturable in a CUDA graph)."""
@@ -898,9 +970,13 @@ class EpisodeRecords(object):
     def finished(self):
         """The records as a dict of tensors in the keys of the reference's episode info (overcooked_env.py:363-401) and of
         ``EpisodeStats.update``: env_index, ep_game_stats, ep_sparse_r(_by_agent), ep_shaped_r(_by_agent), ep_length, plus
-        ep_reward_by_agent, layout and partner_seat.  Rows are ordered by (slot, env).  Synchronises with the host."""
+        ep_reward_by_agent, layout and partner_seat (and partner_member with ``members=True``).  Rows are ordered by (slot,
+        env).  Synchronises with the host."""
         k, e = torch.nonzero(torch.arange(self.capacity, device=self.env.device)[:, None] < self.count[None, :], as_tuple=True)
         sp, sh = self.sparse_r_by_agent[k, e], self.shaped_r_by_agent[k, e]
-        return {"env_index": e, "ep_game_stats": self.game_stats[k, e], "ep_sparse_r_by_agent": sp, "ep_shaped_r_by_agent": sh,
-                "ep_sparse_r": sp.sum(1), "ep_shaped_r": sh.sum(1), "ep_length": self.length[k, e],
-                "ep_reward_by_agent": self.reward_by_agent[k, e], "layout": self.layout[k, e], "partner_seat": self.partner_seat[k, e]}
+        out = {"env_index": e, "ep_game_stats": self.game_stats[k, e], "ep_sparse_r_by_agent": sp, "ep_shaped_r_by_agent": sh,
+               "ep_sparse_r": sp.sum(1), "ep_shaped_r": sh.sum(1), "ep_length": self.length[k, e],
+               "ep_reward_by_agent": self.reward_by_agent[k, e], "layout": self.layout[k, e], "partner_seat": self.partner_seat[k, e]}
+        if self.partner_member is not None:
+            out["partner_member"] = self.partner_member[k, e]
+        return out

@@ -883,6 +883,53 @@ int ovc_assign_partners(const int32_t *done, const float *bc_factor, int64_t n_e
     return ovc::assign_partners_impl(done, bc_factor, n_envs, seed, (unsigned long long *)counter, partner_seat, (cudaStream_t)stream);
 }
 
+int ovc_group_members(const int32_t *member, int n_members, int64_t n_envs, int32_t *order, int32_t *offsets, void *stream) {
+    return ovc::group_members_impl(member, n_members, n_envs, order, offsets, (cudaStream_t)stream);
+}
+
+int ovc_assign_members(const int32_t *done, const int64_t *thresholds, int n_members, int64_t n_envs, uint64_t seed, uint64_t *counter,
+                       int32_t *member, int32_t *rec_member, const int32_t *count, int capacity, void *stream) {
+    return ovc::assign_members_impl(done, (const long long *)thresholds, n_members, n_envs, seed, (unsigned long long *)counter, member,
+                                    rec_member, count, capacity, (cudaStream_t)stream);
+}
+
+int ovc_encode_linear_rows(const void *layouts, int n_layouts, const int32_t *state, const int32_t *swap, int seat, const int32_t *rows,
+                           const int32_t *range, const void *wt, const float *bias, void *out, int64_t n_envs, int state_words, int width,
+                           int height, int horizon, int n_out, float neg_slope, void *stream) {
+    int rc = ovc::check_common(layouts, n_layouts, state, n_envs, state_words);
+    if (rc) return rc;
+    if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
+    if (!rows || !range) return ovc::fail(OVC_E_BADARG, "null pointer argument");
+    return ovc::encode_linear_impl((const ovc_layout_t *)layouts, n_layouts, state, swap, wt, bias, out, n_envs, state_words, width,
+                                   height, horizon, n_out, neg_slope, (cudaStream_t)stream, seat, rows, range);
+}
+
+int ovc_wide_layers_range(const void *a0, int64_t m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2,
+                          int n2, float slope, const int32_t *range, void *z2, void *stream) {
+    if (!range) return ovc::fail(OVC_E_BADARG, "null pointer argument");
+    return ovc::wide_layers_impl(a0, m, k0, w1, b1, n1, w2, b2, n2, slope, z2, (cudaStream_t)stream, range);
+}
+
+int ovc_policy_tail_rows(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                         const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                         float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *swap, int seat, const int32_t *rows,
+                         const int32_t *range, int32_t *actions, float *values, float *scores, float *logp, void *stream) {
+    ovc::PolicyTailArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
+    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
+    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
+    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
+    if (!rows || !range) return ovc::fail(OVC_E_BADARG, "null pointer argument");
+    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, swap, seat, rows, range);
+}
+
+int ovc_sample_actions_rows(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter, const int32_t *swap,
+                            int seat, const int32_t *rows, const int32_t *range, int32_t *actions, float *logp, void *stream) {
+    return ovc::sample_actions_rows_impl(scores, ld, n_actions, n_rows, seed, (unsigned long long *)counter, swap, seat, rows, range, actions,
+                                         logp, (cudaStream_t)stream);
+}
+
 int ovc_featurize(const void *layouts, int n_layouts, const void *lut, const int32_t *state,
                   const int32_t *view_swap, float *out, int64_t n_envs, int state_words, int num_pots, void *stream) {
     int rc = ovc::check_common(layouts, n_layouts, state, n_envs, state_words);

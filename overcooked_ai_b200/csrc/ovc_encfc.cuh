@@ -39,6 +39,8 @@ struct EncLinArgs {
     int n_layouts, S, W, H, horizon, n_out, n_workers;
     float neg_slope;
     int seat;                  // one view (encode_linear_kernel<CPL, true>): the agent's seat, view_swap its per-env swap
+    const int32_t *rows;       // the rows map (encode_linear_kernel<CPL, true, true>): compact row r is environment rows[r]
+    const int32_t *range;      //   for r in [range[0], range[1]) (device memory)
 };
 
 __device__ __forceinline__ int el_dyn_plane(int plane) { return plane < 10 ? plane : plane - 6; }
@@ -107,8 +109,9 @@ __device__ __forceinline__ void el_gather(float acc[CPL], const __nv_bfloat16 *t
 
 // VIEW: one view per environment, player p(e) = seat ^ (view_swap[e] != 0), written to out[e] ([n_envs][n_out]); the
 // object part and that view's gathers run in the same order as in the two-view kernel, so the row is bit-identical to
-// row 2 e + p(e) of it.
-template <int CPL, bool VIEW>
+// row 2 e + p(e) of it.  ROWS (with VIEW): compact rows r in [range[0], range[1]) only, environment rows[r] written to
+// out[r]; a CTA whose share of the range is empty leaves before its prologue.
+template <int CPL, bool VIEW, bool ROWS = false>
 __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncLinArgs a) {
     constexpr int CS = 32 * CPL;  // columns per CTA
     extern __shared__ __align__(16) char el_smem[];
@@ -124,6 +127,12 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncL
     const int n_slices = a.n_out / CS;
     const int slice = blockIdx.x % n_slices, worker = blockIdx.x / n_slices;
     const int col0 = slice * CS;
+    long long r_beg = 0, r_end = a.n_envs;
+    if constexpr (ROWS) {
+        r_beg = max(__ldg(a.range), 0);
+        r_end = min((long long)__ldg(a.range + 1), a.n_envs);
+        if (r_beg + (long long)worker * (EL_THREADS / 32) >= r_end) return;
+    }
 
     // ---- prologue: the table slice and the per-layout constants ----
     unsigned char *tplane = reinterpret_cast<unsigned char *>(srow + a.n_layouts * 128);  // [n_layouts][256] terrain plane of a cell, 0 = none
@@ -179,7 +188,8 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncL
     const long long stride = (long long)a.n_workers * NW;
     const int max_slot_chunks = (a.S - 4 + 31) / 32;
 
-    for (long long env = (long long)worker * NW + warp; env < a.n_envs; env += stride) {
+    for (long long r = r_beg + (long long)worker * NW + warp; r < r_end; r += stride) {
+        const long long env = ROWS ? (long long)__ldg(a.rows + r) : r;
         const int32_t *__restrict__ rec = a.state + env * a.S;
         const int4 head = __ldg(reinterpret_cast<const int4 *>(rec));  // timestep, player 0, player 1, misc (same address in every lane)
         const int lid = head.w & 0xFF;
@@ -261,7 +271,7 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncL
             else *reinterpret_cast<unsigned *>(dst) = packed[0];
         };
         if constexpr (VIEW) {
-            view(a.seat ^ swap, env);
+            view(a.seat ^ swap, r);
         } else {
 #pragma unroll
             for (int p = 0; p < 2; p++) view(p, 2 * env + (swap ? 1 - p : p));
@@ -274,13 +284,17 @@ static size_t encode_linear_smem(int cpl, int n_rows, int n_layouts) {
     return (size_t)n_rows * CS * 2 + ((size_t)n_layouts + 1) * CS * 4 + (size_t)n_layouts * (16 * 4 + 2 * 4 + 128 * 2 + 256) + 16;
 }
 
-// seat < 0: both views (ovc_encode_linear); 0 / 1: one view per environment (ovc_encode_linear_view, view_swap = swap)
+// seat < 0: both views (ovc_encode_linear); 0 / 1: one view per environment (ovc_encode_linear_view, view_swap = swap);
+// with rows / range: the rows map (ovc_encode_linear_rows)
 static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const int32_t *state, const int32_t *view_swap,
                               const void *wt, const float *bias, void *out, long long n_envs, int S, int W, int H, int horizon,
-                              int n_out, float neg_slope, cudaStream_t st, int seat = -1) {
-    if (!out || !wt || !bias) return fail(OVC_E_BADARG, "null pointer argument");
+                              int n_out, float neg_slope, cudaStream_t st, int seat = -1, const int32_t *rows = nullptr,
+                              const int32_t *range = nullptr) {
+    const bool rows_map = rows || range;
+    if (!out || !wt || !bias || (rows_map && (!rows || !range))) return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)out | (uintptr_t)wt) & 15) != 0) return fail(OVC_E_BADARG, "weights and output must be 16-byte aligned");
     if (seat >= 0 && ((uintptr_t)view_swap & 3) != 0) return fail(OVC_E_BADARG, "swap must be 4-byte aligned");
+    if ((((uintptr_t)rows | (uintptr_t)range) & 3) != 0) return fail(OVC_E_BADARG, "rows and range must be 4-byte aligned");
     if (W < 1 || W > 16 || H < 1 || H > 16) return fail(OVC_E_BADARG, "grid shape out of range");
     if (n_out < 64 || n_out % 64) return fail(OVC_E_BADARG, "n_out must be a positive multiple of 64", n_out);
     if (!(neg_slope >= 0.f && neg_slope <= 1.f)) return fail(OVC_E_BADARG, "negative slope must lie in [0, 1]");
@@ -301,7 +315,7 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
     EncLinArgs a;
     a.layouts = layouts, a.state = state, a.view_swap = view_swap, a.wt = (const __nv_bfloat16 *)wt, a.bias = bias;
     a.out = (__nv_bfloat16 *)out, a.n_envs = n_envs, a.n_layouts = n_layouts, a.S = S, a.W = W, a.H = H, a.horizon = horizon;
-    a.n_out = n_out, a.neg_slope = neg_slope, a.seat = seat;
+    a.n_out = n_out, a.neg_slope = neg_slope, a.seat = seat, a.rows = rows, a.range = range;
     const int n_slices = n_out / (32 * cpl);
     const long long want = (n_envs + EL_THREADS / 32 - 1) / (EL_THREADS / 32);
     int workers = n_sm / n_slices;
@@ -310,13 +324,17 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
     a.n_workers = workers;
     const size_t smem = encode_linear_smem(cpl, n_rows, n_layouts);
     cudaError_t e;
-#define OVC_LAUNCH_EL(C, V)                                                                                           \
-    do {                                                                                                              \
-        e = cudaFuncSetAttribute(encode_linear_kernel<C, V>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                                  \
-        encode_linear_kernel<C, V><<<(unsigned)(workers * n_slices), EL_THREADS, smem, st>>>(a);                      \
+#define OVC_LAUNCH_EL(C, ...)                                                                                                 \
+    do {                                                                                                                      \
+        e = cudaFuncSetAttribute(encode_linear_kernel<C, __VA_ARGS__>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+        if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                                          \
+        encode_linear_kernel<C, __VA_ARGS__><<<(unsigned)(workers * n_slices), EL_THREADS, smem, st>>>(a);                    \
     } while (0)
-    if (seat >= 0) {
+    if (rows_map) {
+        if (cpl == 8) OVC_LAUNCH_EL(8, true, true);
+        else if (cpl == 4) OVC_LAUNCH_EL(4, true, true);
+        else OVC_LAUNCH_EL(2, true, true);
+    } else if (seat >= 0) {
         if (cpl == 8) OVC_LAUNCH_EL(8, true);
         else if (cpl == 4) OVC_LAUNCH_EL(4, true);
         else OVC_LAUNCH_EL(2, true);
@@ -389,6 +407,74 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__rest
             __threadfence();
         }
     }
+}
+
+// The rows map (ovc_sample_actions_rows): compact rows r in [range[0], range[1]) only, environment e = rows[r] at player
+// p(e) = seat ^ (swap[e] != 0): the draw uses the joint row 2 e + p(e) and writes actions[2 e + p(e)]; scores and logp stay
+// indexed by r.  Every CTA, with rows in the range or not, takes part in the counter's advance.  A kernel of its own, so
+// that sample_actions_kernel's instantiations stay as they are.
+template <bool LOGP>
+__global__ void __launch_bounds__(256) sample_actions_rows_kernel(const float *__restrict__ scores, int ld, int n_actions, long long n_rows,
+                                                                  unsigned long long seed, unsigned long long *counter,
+                                                                  int32_t *__restrict__ actions, float *__restrict__ logp,
+                                                                  const int32_t *__restrict__ swap, int seat, const int32_t *__restrict__ rows,
+                                                                  const int32_t *__restrict__ range) {
+    const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(counter);
+    const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= max(__ldg(range), 0) && row < min((long long)__ldg(range + 1), n_rows)) {
+        const float *s = scores + row * ld;
+        const long long e = __ldg(rows + row);
+        const long long g = 2 * e + (seat ^ (swap && swap[e] != 0));
+        const uint32_t c3 = (uint32_t)(step >> 32) << 1;
+        const Philox4 A = philox4x32_10(seed, (uint32_t)g, (uint32_t)((unsigned long long)g >> 32), (uint32_t)step, c3);
+        Philox4 B = A;
+        if (n_actions > 4) B = philox4x32_10(seed, (uint32_t)g, (uint32_t)((unsigned long long)g >> 32), (uint32_t)step, c3 | 1u);
+        int best = 0;
+        float best_v = -INFINITY;
+        for (int i = 0; i < n_actions; i++) {
+            const uint32_t r = i < 4 ? A.v[i] : B.v[i - 4];
+            const float u = ((float)(r >> 9) + 0.5f) * 1.1920928955078125e-7f;
+            const float v = s[i] - logf(-logf(u));
+            if (v > best_v) best_v = v, best = i;
+        }
+        actions[g] = best;
+        if constexpr (LOGP) {
+            float m = s[0];
+            for (int i = 1; i < n_actions; i++) m = fmaxf(m, s[i]);
+            float se = 0.f;
+            for (int i = 0; i < n_actions; i++) se += expf(s[i] - m);
+            logp[row] = s[best] - (m + logf(se));
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        const unsigned long long arrived = atomicAdd(counter + 1, 1ull);
+        if (arrived == (unsigned long long)gridDim.x - 1) {
+            counter[1] = 0;
+            counter[0] = step + 1;
+            __threadfence();
+        }
+    }
+}
+
+static int sample_actions_rows_impl(const float *scores, int ld, int n_actions, long long n_rows, unsigned long long seed,
+                                    unsigned long long *counter, const int32_t *swap, int seat, const int32_t *rows, const int32_t *range,
+                                    int32_t *actions, float *logp, cudaStream_t st) {
+    if (!scores || !counter || !actions || !rows || !range) return fail(OVC_E_BADARG, "null pointer argument");
+    if (seat != 0 && seat != 1) return fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
+    if (n_actions < 1 || n_actions > 8 || ld < n_actions) return fail(OVC_E_BADARG, "n_actions must be 1..8 and <= ld", n_actions);
+    if (n_rows < 0) return fail(OVC_E_BADARG, "negative row count");
+    if ((((uintptr_t)scores | (uintptr_t)actions | (uintptr_t)logp | (uintptr_t)swap | (uintptr_t)rows | (uintptr_t)range) & 3) != 0)
+        return fail(OVC_E_BADARG, "scores, actions, logp, swap, rows and range must be 4-byte aligned");
+    if (((uintptr_t)counter & 7) != 0) return fail(OVC_E_BADARG, "counter must be 8-byte aligned");
+    if (n_rows == 0) return OVC_OK;
+    const unsigned grid = (unsigned)((n_rows + 255) / 256);
+    if (logp) sample_actions_rows_kernel<true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, logp, swap, seat, rows, range);
+    else sample_actions_rows_kernel<false><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, nullptr, swap, seat, rows, range);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "sample_actions_rows kernel launch");
+    return OVC_OK;
 }
 
 // ret_sparse[e] += sparse[e];  ret_mixed[e] += sparse[e] + factor * (shaped[e][0] + shaped[e][1])   (rllib.py:328-329)

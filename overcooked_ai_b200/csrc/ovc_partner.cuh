@@ -164,4 +164,127 @@ static int assign_partners_impl(const int32_t *done, const float *bc_factor, lon
     return OVC_OK;
 }
 
+// ---- a population of partners: environments grouped by member, the member drawn per episode ----
+constexpr int GM_THREADS = 1024;  // one CTA: 32 warps, warp w owns the w-th contiguous segment of the environments
+constexpr int MAX_MEMBERS = 64;
+
+// Stable counting sort of the environments by member[e] in ONE CTA, so that nothing leaves the device between the count and
+// the scatter: (1) every warp counts its segment per member (warp-private rows of a shared histogram), (2) 64 threads
+// turn the histogram into each (warp, member) start: offsets[k] + the counts of member k in the earlier segments, (3) every
+// warp walks its segment 32 environments at a time in order; lanes with the same member find each other with
+// __match_any_sync and take consecutive slots in lane order.  Segments and chunks are visited in index order, so each group
+// is ascending.
+__global__ void __launch_bounds__(GM_THREADS, 1) group_members_kernel(const int32_t *__restrict__ member, int n_members, long long n_envs,
+                                                                      int32_t *__restrict__ order, int32_t *__restrict__ offsets) {
+    __shared__ int hist[GM_THREADS / 32][MAX_MEMBERS];
+    __shared__ int tot[MAX_MEMBERS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int i = threadIdx.x; i < (GM_THREADS / 32) * MAX_MEMBERS; i += GM_THREADS) (&hist[0][0])[i] = 0;
+    __syncthreads();
+    const long long seg = (n_envs + GM_THREADS / 32 - 1) / (GM_THREADS / 32);
+    const long long beg = warp * seg, end = beg + seg < n_envs ? beg + seg : n_envs;
+    for (long long e = beg + lane; e < end; e += 32) atomicAdd(&hist[warp][__ldg(member + e)], 1);
+    __syncthreads();
+    if (threadIdx.x < MAX_MEMBERS) {  // thread k: member k's start in every segment, relative to the group's start
+        const int k = threadIdx.x;
+        int total = 0;
+        for (int w = 0; w < GM_THREADS / 32; w++) {
+            const int c = hist[w][k];
+            hist[w][k] = total;
+            total += c;
+        }
+        tot[k] = total;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {  // the group starts: an exclusive scan of the totals
+        int run = 0;
+        for (int k = 0; k < n_members; k++) {
+            const int c = tot[k];
+            tot[k] = run;
+            run += c;
+        }
+        offsets[n_members] = run;
+    }
+    __syncthreads();
+    if (threadIdx.x < n_members) {
+        const int k = threadIdx.x, base = tot[k];
+        offsets[k] = base;
+        for (int w = 0; w < GM_THREADS / 32; w++) hist[w][k] += base;
+    }
+    __syncthreads();
+    const unsigned lt = (1u << lane) - 1u;
+    for (long long e0 = beg; e0 < end; e0 += 32) {
+        const long long e = e0 + lane;
+        const bool in = e < end;
+        const int k = in ? __ldg(member + e) : -1 - lane;  // lanes past the end match nobody
+        const unsigned peers = __match_any_sync(0xFFFFFFFFu, k);
+        const int slot = in ? hist[warp][k] + __popc(peers & lt) : 0;
+        __syncwarp();
+        if (in) {
+            order[slot] = (int32_t)e;
+            if ((peers & lt) == 0) hist[warp][k] += __popc(peers);  // the group's first lane moves the start on
+        }
+        __syncwarp();
+    }
+}
+
+static int group_members_impl(const int32_t *member, int n_members, long long n_envs, int32_t *order, int32_t *offsets, cudaStream_t st) {
+    if (!member || !order || !offsets) return fail(OVC_E_BADARG, "null pointer argument");
+    if (((uintptr_t)member | (uintptr_t)order | (uintptr_t)offsets) & 3) return fail(OVC_E_BADARG, "member, order and offsets must be 4-byte aligned");
+    if (n_members < 1 || n_members > MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+    if (n_envs < 0 || n_envs > 0x7FFFFFFFll) return fail(OVC_E_BADARG, "n_envs must be 0..2^31-1", n_envs);
+    if (n_envs == 0) return OVC_OK;
+    group_members_kernel<<<1, GM_THREADS, 0, st>>>(member, n_members, n_envs, order, offsets);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "group_members kernel launch");
+    return OVC_OK;
+}
+
+// Per environment e with done[e] (every e with done == NULL): the ending episode's member into the records' slot count[e]
+// (when done is given, rec_member non-NULL and count[e] < capacity), then, with thresholds, a new member: Philox4x32-10,
+// key = seed, counter = (e low, e high, step low, step high) -> w0;  member[e] = #{k < n_members - 1 : w0 >= thresholds[k]}.
+__global__ void __launch_bounds__(256) assign_members_kernel(const int32_t *__restrict__ done, const long long *__restrict__ thresholds,
+                                                             int n_members, long long n_envs, unsigned long long seed,
+                                                             unsigned long long *counter, int32_t *__restrict__ member,
+                                                             int32_t *__restrict__ rec_member, const int32_t *__restrict__ count, int capacity) {
+    __shared__ long long thr[MAX_MEMBERS];
+    const unsigned long long step = thresholds ? *reinterpret_cast<volatile unsigned long long *>(counter) : 0ull;
+    if (thresholds)
+        for (int i = threadIdx.x; i < n_members - 1; i += blockDim.x) thr[i] = thresholds[i];
+    __syncthreads();
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < n_envs && (!done || done[e] != 0)) {
+        if (done && rec_member) {
+            const int k = count[e];
+            if (k < capacity) rec_member[(long long)k * n_envs + e] = member[e];
+        }
+        if (thresholds) {
+            const Philox4 P = philox4x32_10(seed, (uint32_t)e, (uint32_t)((unsigned long long)e >> 32), (uint32_t)step, (uint32_t)(step >> 32));
+            const long long w0 = P.v[0];
+            int m = 0;
+            for (int k = 0; k < n_members - 1; k++) m += w0 >= thr[k];
+            member[e] = m;
+        }
+    }
+    if (thresholds) advance_step(counter, step);
+}
+
+static int assign_members_impl(const int32_t *done, const long long *thresholds, int n_members, long long n_envs, unsigned long long seed,
+                               unsigned long long *counter, int32_t *member, int32_t *rec_member, const int32_t *count, int capacity,
+                               cudaStream_t st) {
+    if (!member || (thresholds && !counter) || (rec_member && !count)) return fail(OVC_E_BADARG, "null pointer argument");
+    if (((uintptr_t)done | (uintptr_t)member | (uintptr_t)rec_member | (uintptr_t)count) & 3)
+        return fail(OVC_E_BADARG, "done, member, rec_member and count must be 4-byte aligned");
+    if (((uintptr_t)thresholds | (uintptr_t)counter) & 7) return fail(OVC_E_BADARG, "thresholds and counter must be 8-byte aligned");
+    if (n_members < 1 || n_members > MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+    if (capacity < 0) return fail(OVC_E_BADARG, "negative record capacity", capacity);
+    if (n_envs < 0) return fail(OVC_E_BADARG, "negative env count");
+    if (n_envs == 0) return OVC_OK;
+    assign_members_kernel<<<(unsigned)((n_envs + 255) / 256), 256, 0, st>>>(done, thresholds, n_members, n_envs, seed, counter, member,
+                                                                           rec_member, count, capacity);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "assign_members kernel launch");
+    return OVC_OK;
+}
+
 }  // namespace ovc

@@ -243,8 +243,11 @@ __device__ __forceinline__ void advance_step(unsigned long long *counter, unsign
 // the joint row g and writes p.actions[g]; values, logp and scores stay indexed by r.  The one-view kernel is a kernel of
 // its own (policy_tail_view_kernel, swap and seat as extra parameters): a larger PolicyTailArgs would change the code of
 // every instantiation.
-template <int KS2, bool LOGP, bool HIDDEN, bool VIEW>
-__device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const int32_t *swap, int seat) {
+// ROWS (with VIEW, policy_tail_rows_kernel): compact rows r in [range[0], range[1]) only; row r is environment rows[r]'s
+// agent, drawn on its joint row 2 rows[r] + p(rows[r]).
+template <int KS2, bool LOGP, bool HIDDEN, bool VIEW, bool ROWS = false>
+__device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const int32_t *swap, int seat, const int32_t *rows = nullptr,
+                                                 const int32_t *range = nullptr) {
     constexpr int K0 = 32 * KS2;
     extern __shared__ __align__(16) char pt_smem[];
 
@@ -255,15 +258,22 @@ __device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const 
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const float in_slope2 = p.in_slope;
-    const long long n_tiles = (p.n_rows + 15) / 16;
-    for (long long tile = (long long)blockIdx.x * (PT_THREADS / 32) + warp; tile < n_tiles; tile += (long long)gridDim.x * (PT_THREADS / 32)) {
-        const long long r0 = tile * 16 + g, r1 = r0 + 8;
+    // the rows form counts rows in 32 bits (a range of int32 entries), which keeps it within K8's registers
+    using Row = typename std::conditional<ROWS, int, long long>::type;
+    Row r_beg = 0, r_end = p.n_rows;
+    if constexpr (ROWS) {
+        r_beg = max(__ldg(range), 0);
+        r_end = max((int)min((long long)__ldg(range + 1), p.n_rows), r_beg);
+    }
+    const Row n_tiles = (r_end - r_beg + 15) / 16;
+    for (Row tile = (Row)blockIdx.x * (PT_THREADS / 32) + warp; tile < n_tiles; tile += (Row)gridDim.x * (PT_THREADS / 32)) {
+        const Row r0 = r_beg + tile * 16 + g, r1 = r0 + 8;
         // ---- first layer: A fragments straight from global memory, 16 bytes (8 inputs) per load ----
         uint4 xa[KS2], xb[KS2];
 #pragma unroll
         for (int s2 = 0; s2 < KS2; s2++) {
-            xa[s2] = r0 < p.n_rows ? __ldg(reinterpret_cast<const uint4 *>(p.x + r0 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
-            xb[s2] = r1 < p.n_rows ? __ldg(reinterpret_cast<const uint4 *>(p.x + r1 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
+            xa[s2] = r0 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r0 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
+            xb[s2] = r1 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r1 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
         }
         float acc[8][4];
         first_layer64<KS2>(acc, w, g, t, [&](int s2, unsigned a_lo[4], unsigned a_hi[4]) {
@@ -288,18 +298,24 @@ __device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const 
         float out[1][4];
         tail_layers(out, acc, w, p.n_hidden, p.slope, g, t);
         if (p.scores) {
-            if (r0 < p.n_rows) *reinterpret_cast<float2 *>(p.scores + r0 * PT_NOUT + 2 * t) = make_float2(out[0][0], out[0][1]);
-            if (r1 < p.n_rows) *reinterpret_cast<float2 *>(p.scores + r1 * PT_NOUT + 2 * t) = make_float2(out[0][2], out[0][3]);
+            if (r0 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r0 * PT_NOUT + 2 * t) = make_float2(out[0][0], out[0][1]);
+            if (r1 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r1 * PT_NOUT + 2 * t) = make_float2(out[0][2], out[0][3]);
         }
         // ---- the draw (ovc_sample_actions) ----
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-            const long long row = h ? r1 : r0;
+            const Row row = h ? r1 : r0;
             const float s0 = out[0][2 * h], s1 = out[0][2 * h + 1];
             float lp = 0.f;
-            const long long g = VIEW ? view_row(swap, seat, row, p.n_rows) : row;
+            long long g;
+            if constexpr (ROWS) {
+                const long long e = row < r_end ? (long long)__ldg(rows + row) : 0;  // rows past the end: the draw is discarded
+                g = 2 * e + (seat ^ (swap && row < r_end && __ldg(swap + e) != 0));
+            } else {
+                g = VIEW ? view_row(swap, seat, row, p.n_rows) : row;
+            }
             const int best = draw_row<LOGP>(s0, s1, p.seed, step, g, p.n_actions, lane, t, lp);
-            if (row < p.n_rows) {
+            if (row < r_end) {
                 if (t == 0) p.actions[g] = best;
                 if constexpr (LOGP) if (t == 0) p.logp[row] = lp;
                 // the value head is head n_actions: lane n_actions / 2 holds it
@@ -320,19 +336,26 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_view_kernel(const P
     policy_tail_body<KS2, LOGP, false, true>(p, swap, seat);
 }
 
+template <int KS2, bool LOGP>
+__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_rows_kernel(const PolicyTailArgs p, const int32_t *swap, int seat,
+                                                                         const int32_t *rows, const int32_t *range) {
+    policy_tail_body<KS2, LOGP, false, true, true>(p, swap, seat, rows, range);
+}
+
 // hid: the HIDDEN instantiation into a.hidden (no heads, no draw; a.w_heads / a.b_heads are staged but never read, so the
 // entry point passes the first layer's tables, which are at least as large, in their place).  seat >= 0: the one-view
 // kernel with swap (ovc_policy_tail_view); -1: the two-view ones.
 static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bool hid = false, const int32_t *swap = nullptr,
-                            int seat = -1) {
-    const bool view = seat >= 0;
+                            int seat = -1, const int32_t *rows = nullptr, const int32_t *range = nullptr) {
+    const bool view = seat >= 0, rows_map = rows || range;
     if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || (hid ? !a.hidden : (!a.counter || !a.actions)) ||
-        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)))
+        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)) || (rows_map && (!rows || !range)))
         return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)a.x | (uintptr_t)a.w_first) & 15) != 0) return fail(OVC_E_BADARG, "x and w_first must be 16-byte aligned");
     if (hid && ((uintptr_t)a.hidden & 3) != 0) return fail(OVC_E_BADARG, "hidden must be 4-byte aligned");
     if (view && (((uintptr_t)a.actions | (uintptr_t)a.values | (uintptr_t)a.logp | (uintptr_t)swap) & 3) != 0)
         return fail(OVC_E_BADARG, "actions, values, logp and swap must be 4-byte aligned");
+    if ((((uintptr_t)rows | (uintptr_t)range) & 3) != 0) return fail(OVC_E_BADARG, "rows and range must be 4-byte aligned");
     if (view && ((uintptr_t)a.scores & 7) != 0) return fail(OVC_E_BADARG, "scores must be 8-byte aligned");
     if (k0 < 32 || k0 > 256 || k0 % 32) return fail(OVC_E_BADARG, "k0 must be a multiple of 32 in 32..256", k0);
     if (a.n_hidden < 0 || a.n_hidden > 8) return fail(OVC_E_BADARG, "n_hidden must be 0..8", a.n_hidden);
@@ -355,6 +378,8 @@ static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bo
 #define OVC_LAUNCH_PT(KS2)                                                                                       \
     case KS2:                                                                                                    \
         if (hid) OVC_PT_KERNEL((a), policy_tail_kernel<KS2, false, true>);                                       \
+        else if (rows_map && a.logp) OVC_PT_KERNEL((a, swap, seat, rows, range), policy_tail_rows_kernel<KS2, true>); \
+        else if (rows_map) OVC_PT_KERNEL((a, swap, seat, rows, range), policy_tail_rows_kernel<KS2, false>);     \
         else if (view && a.logp) OVC_PT_KERNEL((a, swap, seat), policy_tail_view_kernel<KS2, true>);             \
         else if (view) OVC_PT_KERNEL((a, swap, seat), policy_tail_view_kernel<KS2, false>);                      \
         else if (a.logp) OVC_PT_KERNEL((a), policy_tail_kernel<KS2, true, false>);                               \

@@ -44,6 +44,7 @@ struct WideArgs {
     long long m;
     float slope;
     int n_tiles;
+    const int32_t *range;  // wide_layers_kernel<true>: rows [range[0], range[1]) of the m-row buffers only (device memory)
 };
 
 __device__ __forceinline__ void mbar_wait_bounded(uint64_t *bar, uint32_t parity) {
@@ -140,9 +141,19 @@ __device__ __forceinline__ uint32_t leaky_bf16x2(float x0, float x1, float slope
     return *reinterpret_cast<const uint32_t *>(&h);
 }
 
+// RANGE: 128-row tiles from row range[0], stores guarded by range[1]; every warp reads the range, so the producer and both
+// consumer warpgroups walk the same tiles and the mbarrier protocol stays balanced.  The tensor maps still span all m rows.
+template <bool RANGE = false>
 __global__ void __launch_bounds__(WL_THREADS, 1)
 wide_layers_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_w1,
                    const __grid_constant__ CUtensorMap map_w2, const WideArgs p) {
+    long long r_beg = 0, r_end = p.m;
+    int n_tiles = p.n_tiles;
+    if constexpr (RANGE) {
+        r_beg = max(__ldg(p.range), 0);
+        r_end = max(min((long long)__ldg(p.range + 1), p.m), r_beg);
+        n_tiles = (int)((r_end - r_beg + WL_BM - 1) / WL_BM);
+    }
     extern __shared__ char wl_raw[];
     char *tile = reinterpret_cast<char *>((reinterpret_cast<uintptr_t>(wl_raw) + 1023) & ~(uintptr_t)1023);
     char *w2_tile = tile + WL_STAGES * WL_STAGE;
@@ -168,8 +179,8 @@ wide_layers_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_cons
         if (warp == 8 && lane == 0) {
             // ---- TMA producer: tiles blockIdx.x, + gridDim.x, ...; the rings' use counters run on across tiles ----
             int it1 = 0, it2 = 0;
-            for (int tile_i = blockIdx.x; tile_i < p.n_tiles; tile_i += gridDim.x) {
-                const int m0 = tile_i * WL_BM;
+            for (int tile_i = blockIdx.x; tile_i < n_tiles; tile_i += gridDim.x) {
+                const int m0 = (int)(r_beg + tile_i * WL_BM);
                 for (int n = 0; n < WL_CHUNKS; n++) {
                     for (int c = 0; c < WL_KC; c++, it1++) {
                         const int s = it1 % WL_STAGES, u = it1 / WL_STAGES;
@@ -199,7 +210,7 @@ wide_layers_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_cons
 #pragma unroll
     for (int i = 0; i < 80; i++) acc2[i] = 0.f;
     int it1 = 0, it2 = 0;
-    for (int tile_i = blockIdx.x; tile_i < p.n_tiles; tile_i += gridDim.x) {
+    for (int tile_i = blockIdx.x; tile_i < n_tiles; tile_i += gridDim.x) {
         for (int n = 0; n < WL_CHUNKS; n++) {
             // layer 1, columns n*128 .. n*128+127: 8 k-chunks, one stage each; a stage is released once the wgmma
             // group after it has been issued and it has itself completed (wait_group 1)
@@ -244,14 +255,14 @@ wide_layers_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_cons
             if (lane == 0) mbar_arrive(w2_empty + s);
         }
         // epilogue 2: bias, bf16, two rows of 160 columns per quad of lanes
-        const long long row = (long long)tile_i * WL_BM + g * 64 + w * 16 + (lane >> 2);
+        const long long row = r_beg + (long long)tile_i * WL_BM + g * 64 + w * 16 + (lane >> 2);
 #pragma unroll
         for (int j = 0; j < WL_N2 / 8; j++) {
             const int col = 8 * j + 2 * (lane & 3);
             const float b0 = bias2[col], b1 = bias2[col + 1];
-            if (row < p.m)
+            if (row < r_end)
                 *reinterpret_cast<__nv_bfloat162 *>(p.z2 + row * WL_N2 + col) = __floats2bfloat162_rn(acc2[4 * j] + b0, acc2[4 * j + 1] + b1);
-            if (row + 8 < p.m)
+            if (row + 8 < r_end)
                 *reinterpret_cast<__nv_bfloat162 *>(p.z2 + (row + 8) * WL_N2 + col) = __floats2bfloat162_rn(acc2[4 * j + 2] + b0, acc2[4 * j + 3] + b1);
         }
     }
@@ -270,11 +281,15 @@ static int make_tmap_bf16(CUtensorMap *m, const void *base, long long rows, int 
     return OVC_OK;
 }
 
+// range != NULL: ovc_wide_layers_range (wide_layers_kernel<true>)
 static int wide_layers_impl(const void *a0, long long m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2,
-                            int n2, float slope, void *z2, cudaStream_t st) {
+                            int n2, float slope, void *z2, cudaStream_t st, const int32_t *range = nullptr) {
+    const bool ranged = range != nullptr;
     if (!a0 || !w1 || !b1 || !w2 || !b2 || !z2) return fail(OVC_E_BADARG, "null pointer argument");
     if (k0 != WL_K0 || n1 != WL_N1 || n2 != WL_N2) return fail(OVC_E_UNSUPPORTED, "wide_layers: built for 512 -> 512 -> 160", k0 * 1000000ll + n1 * 1000 + n2);
     if ((((uintptr_t)a0 | (uintptr_t)w1 | (uintptr_t)w2 | (uintptr_t)z2) & 15) != 0) return fail(OVC_E_BADARG, "operands must be 16-byte aligned");
+    if (((uintptr_t)range & 3) != 0) return fail(OVC_E_BADARG, "range must be 4-byte aligned");
+    if (ranged && m > 0x7FFFFFFFll) return fail(OVC_E_BADARG, "m must be below 2^31", m);
     if (!(slope >= 0.f && slope <= 1.f)) return fail(OVC_E_BADARG, "negative slope must lie in [0, 1]");
     if (m < 0) return fail(OVC_E_BADARG, "negative row count");
     if (m == 0) return OVC_OK;
@@ -283,16 +298,19 @@ static int wide_layers_impl(const void *a0, long long m, int k0, const void *w1,
     if (!rc) rc = make_tmap_bf16(&mw1, w1, WL_N1, WL_K0, WL_NC);  // one column chunk of a k-chunk per box
     if (!rc) rc = make_tmap_bf16(&mw2, w2, WL_N2, WL_N1, WL_N2);
     if (rc) return rc;
-    cudaError_t e = cudaFuncSetAttribute(wide_layers_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WL_SMEM);
+    cudaError_t e = ranged ? cudaFuncSetAttribute(wide_layers_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WL_SMEM)
+                           : cudaFuncSetAttribute(wide_layers_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WL_SMEM);
     if (e != cudaSuccess) return cuda_fail(e, "wide_layers kernel attribute");
     WideArgs p;
     int dev = 0, n_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    p.b1 = b1, p.b2 = b2, p.z2 = (__nv_bfloat16 *)z2, p.m = m, p.slope = slope;
-    p.n_tiles = (int)((m + WL_BM - 1) / WL_BM);
+    p.b1 = b1, p.b2 = b2, p.z2 = (__nv_bfloat16 *)z2, p.m = m, p.slope = slope, p.range = range;
+    p.n_tiles = (int)((m + WL_BM - 1) / WL_BM);  // with a range: the most tiles it can hold (the kernel reads its own count)
     // persistent: one CTA per SM walks tiles blockIdx.x, + gridDim.x, ... (barriers and biases are set up once)
-    wide_layers_kernel<<<(unsigned)(p.n_tiles < n_sm ? p.n_tiles : n_sm), WL_THREADS, WL_SMEM, st>>>(ma, mw1, mw2, p);
+    const unsigned grid = (unsigned)(p.n_tiles < n_sm ? p.n_tiles : n_sm);
+    if (ranged) wide_layers_kernel<true><<<grid, WL_THREADS, WL_SMEM, st>>>(ma, mw1, mw2, p);
+    else wide_layers_kernel<false><<<grid, WL_THREADS, WL_SMEM, st>>>(ma, mw1, mw2, p);
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "wide_layers kernel launch");
     return OVC_OK;

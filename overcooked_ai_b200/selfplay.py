@@ -19,6 +19,7 @@ the network ``SelfPlayRollout`` evaluates: on a 5x4 grid entirely with this libr
 """
 import copy
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -384,10 +385,11 @@ class SampleBatch(object):
     ``one_view`` (``AgentPairRollout.collect``: a learner next to a different agent): ONE row per environment, the learner's.
     Every [T, 2N] / [2N] field above is then [T, N] / [N] (row e: the learner of environment e, at player
     ``1 - partner_seat[t, e]``), ``state_h`` / ``state_c`` are [ceil(T/L), N, 256], ``partner_seat`` is agent 1's player and
-    ``learner_mask`` is all ones.
+    ``learner_mask`` is all ones.  Next to a population of partners (``members``) ``partner_member`` int8 [T, N] is the member
+    agent 1 was at transition t, and ``episodes.finished()`` has ``partner_member``; both are None / absent otherwise.
     """
 
-    def __init__(self, env, n_steps, keep_logits=False, partner=False, seq_len=None, one_view=False):
+    def __init__(self, env, n_steps, keep_logits=False, partner=False, seq_len=None, one_view=False, members=False):
         N, T, dev = env.n_envs, int(n_steps), env.device
         R = N if one_view else 2 * N
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
@@ -400,7 +402,8 @@ class SampleBatch(object):
         self.last_values = z(R, torch.float32)
         self.logits = z((T, R, 8), torch.float32) if keep_logits else None
         self.partner_seat = z((T, N), torch.int8) if partner or one_view else None
-        self.episodes = EpisodeRecords(env, -(-T // env.horizon) if env.horizon > 0 else 0)
+        self.partner_member = z((T, N), torch.int8) if members else None
+        self.episodes = EpisodeRecords(env, -(-T // env.horizon) if env.horizon > 0 else 0, members=members)
         self.seq_len = seq_len
         self.state_h = z((-(-T // seq_len), R, 256), torch.bfloat16) if seq_len else None
         self.state_c = z((-(-T // seq_len), R, 256), torch.float32) if seq_len else None
@@ -944,6 +947,155 @@ class _BCAgent(object):
             dst.copy_(src)
 
 
+# The population draw's key is seed ^ PARTNER_MEMBER_SALT: its counters (env, step) are the seat draw's, so it needs a key of
+# its own to draw numbers independent of the seats.
+PARTNER_MEMBER_SALT = 0x94D049BB133111EB
+MAX_MEMBERS = 64  # ovc_group_members / ovc_assign_members
+
+
+def member_thresholds(weights):
+    """The table ``ovc_assign_members`` draws a member from: int64 [K - 1] with entry k = floor(cdf[k] * 2^32), cdf[k] the
+    float64 share of members 0..k in ``weights`` (K non-negative floats with a positive sum).  A member of weight 0 is never
+    drawn: its entry equals the one before (or is 0 for member 0, 2^32 after the last positive weight)."""
+    w = np.asarray(weights, dtype=np.float64)
+    assert w.ndim == 1 and 1 <= w.size <= MAX_MEMBERS, "between 1 and %d member weights" % MAX_MEMBERS
+    assert np.all(np.isfinite(w)) and np.all(w >= 0) and w.sum() > 0, "member weights: finite, non-negative, a positive sum"
+    c = np.cumsum(w)
+    return np.floor(c[:-1] / c[-1] * 2.0**32).astype(np.int64)
+
+
+class _Population(object):
+    """Agent 1 of an ``AgentPairRollout`` drawn from a population: member k (an ``RllibShapedCNN`` or a ``BCPolicy``) plays
+    player ``partner_seat[e]`` in the environments e with ``member[e] == k``.  Per transition ``ovc_group_members`` sorts
+    the environments by member (``order``, ``offsets``), then each network member runs its kernels on its own range of
+    compact rows only: the rows forms of K7 / K9 / K8 (one shared set of compact buffers), or, off the fused path, the
+    library layers over all N compact rows of the observation (gathered once for all members) and the rows form of the
+    draw.  A BC member is K10 with ``partner_seat`` where ``member == k`` and -1 elsewhere.  Every member keeps its own
+    counter, advanced by one per transition whatever its share, so member k draws in environment e what the pair
+    ``(learner, m_k)`` draws there.  ``member``: fixed, or drawn per episode from ``weights`` (``ovc_assign_members``)."""
+
+    lstm = False
+
+    def __init__(self, env, members, partner_seat, seed, autocast_dtype, member=None, weights=None):
+        N, dev = env.n_envs, env.device
+        self.env, self.K, self.seed, self.partner_seat = env, len(members), int(seed), partner_seat
+        self.agents = [_BCAgent(env, m, 1, None, seed) if isinstance(m, BCPolicy)
+                       else _NetworkAgent(env, m, 0, partner_seat, seed, autocast_dtype) for m in members]
+        shared = {}
+
+        def buf(shape, dt):
+            key = (tuple(shape), dt)
+            if key not in shared:
+                shared[key] = torch.empty(key[0], dtype=dt, device=dev)
+            return shared[key]
+
+        self.obs = None  # K2's observation, set by the pair when a member runs without K7
+        nets = [a for a in self.agents if isinstance(a, _NetworkAgent)]
+        for a in nets:  # one set of compact buffers for all members: each writes its own rows only
+            a.values = buf((N,), torch.float32)
+            a._flat = None
+            if a.fused_first_layer:
+                a._act0 = buf(a._act0.shape, torch.bfloat16)
+            if a.fused_tail:
+                a._z = buf(a._z.shape, torch.bfloat16)
+            else:
+                a._scores = buf((N, 6), torch.float32)
+        self._unpaired = torch.full((N,), -1, dtype=torch.int32, device=dev)
+        for a in self.agents:
+            if isinstance(a, _BCAgent):
+                a.partner_seat = torch.full((N,), -1, dtype=torch.int32, device=dev)  # rebuilt every transition
+        self.needs_obs = any(not a.fused_first_layer for a in nets)
+        l = env.layouts[0]
+        self._cobs = torch.empty((N, l.width * l.height * 26), dtype=autocast_dtype or torch.float32, device=dev) if self.needs_obs else None
+        self._jrows = torch.empty(N, dtype=torch.int32, device=dev)
+        self.order = torch.empty(N, dtype=torch.int32, device=dev)
+        self.offsets = torch.zeros(self.K + 1, dtype=torch.int32, device=dev)
+        self._counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of the population draw
+        if member is not None:
+            assert weights is None, "member fixes each environment's member, member_weights draws it: pass one of them"
+            assert member.dtype == torch.int32 and member.is_contiguous() and member.numel() == N, "member: int32 [N]"
+            lo, hi = int(member.min()), int(member.max())
+            assert 0 <= lo and hi < self.K, "member values must lie in [0, %d): found %d..%d" % (self.K, lo, hi)
+            assert member.device == dev, "member: on the environments' device"
+            self.member, self._thresholds = member, None
+        else:
+            self.member = torch.zeros(N, dtype=torch.int32, device=dev)
+            self._thresholds = torch.zeros(max(self.K - 1, 1), dtype=torch.int64, device=dev)  # never NULL: NULL skips the draw
+            self.weights = [1.0] * self.K if weights is None else weights
+            self.assign(None, None)
+
+    @property
+    def weights(self):
+        return list(self._weights)
+
+    @weights.setter
+    def weights(self, value):
+        assert self._thresholds is not None, "member_weights: the population was built with a fixed member tensor"
+        w = [float(x) for x in value]
+        assert len(w) == self.K, "one weight per member (%d)" % self.K
+        thr = member_thresholds(w)
+        self._weights = w
+        self._thresholds[:self.K - 1].copy_(torch.from_numpy(thr))
+
+    def assign(self, done, records):
+        """After K1: the ending episodes' member into ``records``, then (drawn members) a new member; done None: every
+        environment, no record (construction)."""
+        drawn = self._thresholds is not None
+        self.env.assign_members(self.member, self.K, self._thresholds, self._counter if drawn else None,
+                                seed=self.seed ^ PARTNER_MEMBER_SALT, done=done, records=records)
+
+    def live(self):
+        out = [self.member, self._counter]
+        for a in self.agents:
+            out += a.live()
+        return out
+
+    def follow_seats(self):
+        pass  # every member reads partner_seat itself
+
+    def sync_weights(self):
+        for a in self.agents:
+            a.sync_weights()
+
+    def act(self, actions):
+        env, N = self.env, self.env.n_envs
+        lib, stream = _native.lib(), env._stream()
+        env.group_members(self.member, self.K, self.order, self.offsets)
+        if self._cobs is not None:  # the members' observation rows 2 e + p(e), in compact order, once for all members
+            torch.index_select(self.partner_seat, 0, self.order, out=self._jrows)
+            self._jrows.add_(self.order, alpha=2)
+            torch.index_select(self.obs.view(2 * N, -1), 0, self._jrows, out=self._cobs)
+        for k, a in enumerate(self.agents):
+            rng = self.offsets[k:k + 2]
+            if isinstance(a, _BCAgent):
+                torch.where(self.member == k, self.partner_seat, self._unpaired, out=a.partner_seat)
+                a.act(actions)
+                continue
+            seed = a.seed & (2**64 - 1)
+            with torch.no_grad():
+                if a.fused_first_layer:
+                    flat, first = env.encoded_linear_rows(a._wt0, a._b0, 0, self.partner_seat, self.order, rng, a._act0), 1  # K7
+                else:
+                    flat, first = self._cobs, 0
+                if a.fused_wide:
+                    w1, b1, w2, b2 = a._wide
+                    _native.check(lib.ovc_wide_layers_range(flat.data_ptr(), N, flat.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
+                                                            w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, rng.data_ptr(), a._z.data_ptr(),
+                                                            stream))
+                elif a.fused_tail:
+                    a.dense_model.trunk(flat, first, out=a._z)
+                if a.fused_tail:
+                    w1, b1, wh, bh, wo, bo = a._tail
+                    _native.check(lib.ovc_policy_tail_rows(
+                        a._z.data_ptr(), N, a._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(), wh.shape[0],
+                        wo.data_ptr(), bo.data_ptr(), 0.3, a.dense_model.n_actions, seed, a._counter.data_ptr(), self.partner_seat.data_ptr(),
+                        0, self.order.data_ptr(), rng.data_ptr(), actions.data_ptr(), 0, 0, 0, stream))
+                else:
+                    logits, _ = a.dense_model.forward_from(flat, first)
+                    a._scores.copy_(logits)
+                    env.sample_actions_rows(a._scores, a._counter, 0, self.partner_seat, self.order, rng, seed=a.seed, out=actions)
+
+
 class AgentPairRollout(object):
     """Two different agents, each evaluated on its own seat's view only: the reference's evaluation of an agent pair
     (rllib.py ``evaluate``: ``AgentEvaluator.evaluate_agent_pair(AgentPair(agent_0_policy, agent_1_policy))``) with N
@@ -952,7 +1104,8 @@ class AgentPairRollout(object):
     co-play, training against a held-out PPO, LSTM or BC partner).
 
     agents: (agent0, agent1), each an ``RllibShapedCNN``, an ``RllibLSTMShapedCNN`` or a ``BCPolicy`` (the same object twice
-    is allowed).  Agent 0 plays player ``swap[e]`` of environment e, agent 1 the other one.  A network agent runs its own
+    is allowed).  agent1 may instead be a population: a list of 1..64 members, each an ``RllibShapedCNN`` or a ``BCPolicy``
+    (fictitious co-play's second stage, training against a set of checkpoints, PPO_BC with several BC human proxies).  Agent 0 plays player ``swap[e]`` of environment e, agent 1 the other one.  A network agent runs its own
     policy on N rows (the one-view forms of K7 / K8 / K11 and the draw, with K9 on N rows, where ``fused_kernel_support``
     allows them; K2, the dense model on the agent's rows and the one-view draw elsewhere); a BC agent is K10.
     swap: int32 CUDA tensor [N] or None (no swap): both seat orders in one batch; fixed for the rollout's lifetime.
@@ -967,17 +1120,36 @@ class AgentPairRollout(object):
     autocast_dtype: as ``SelfPlayRollout``'s, for every network agent (an LSTM agent needs bfloat16).
     episode_capacity: as ``SelfPlayRollout``'s.  Every finished episode's ``partner_seat`` is agent 1's player.
     max_seq_len: as ``SelfPlayRollout``'s, for an LSTM learner's ``collect()``.
+    member (population only): int32 CUDA tensor [N] with values in [0, K): environment e plays member member[e] for the
+    rollout's lifetime (checked once here).
+    member_weights (population only; see the property): instead of ``member``, each environment's member is drawn at
+    construction and again at every episode end (``env.assign_members``, key ``seed ^ PARTNER_MEMBER_SALT``), member k with
+    probability ``member_weights[k] / sum``; default uniform.  The seats follow ``swap`` / ``random_seats`` as for a pair, so
+    a population of one draws what the pair draws.  Member k's actions in environment e are those ``AgentPairRollout(env,
+    (agent0, m_k))`` draws there.  ``episodes.finished()`` and collect()'s batches then report ``partner_member``.
 
     A transition is K2 (once, when a network agent runs without K7), agent 0's policy, agent 1's policy, K1 (auto-reset
     inside), ``record_transition`` with the episode statistics (``record_transition_view`` of agent 0's row in collect()),
-    then, with random_seats, the seat draw.  ``ret_sparse`` is the running sparse return of every environment."""
+    then, with random_seats, the seat draw.  With a population, agent 1's step is ``ovc_group_members`` and each member's
+    kernels on its own environments, and ``ovc_assign_members`` (the ending episodes' member, the new draw) runs between
+    K1 and the record.  ``ret_sparse`` is the running sparse return of every environment."""
 
     def __init__(self, env, agents, swap=None, seed=0, use_graph=True, episode_capacity=1, autocast_dtype=torch.bfloat16,
-                 random_seats=False, max_seq_len=20):
+                 random_seats=False, max_seq_len=20, member=None, member_weights=None):
         assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
         assert len(agents) == 2, "agents: (agent0, agent1)"
         assert not (random_seats and swap is not None), "random_seats draws the seats: pass no swap tensor with it"
-        for a in agents:
+        assert not isinstance(agents[0], (list, tuple)), "a population plays agent 1 only: agents = (agent0, [m_0, ..., m_K-1])"
+        self.population = isinstance(agents[1], (list, tuple))
+        members = list(agents[1]) if self.population else []
+        if self.population:
+            assert 1 <= len(members) <= MAX_MEMBERS, "a population has 1..%d members" % MAX_MEMBERS
+            for m in members:
+                assert isinstance(m, (RllibShapedCNN, BCPolicy)) and not isinstance(m, RllibLSTMShapedCNN), \
+                    "a population member is an RllibShapedCNN or a BCPolicy (an LSTM member is not supported)"
+        else:
+            assert member is None and member_weights is None, "member / member_weights go with a population in agents[1]"
+        for a in [agents[0]] + (members or [agents[1]]):
             assert isinstance(a, (RllibShapedCNN, BCPolicy)), "an agent is an RllibShapedCNN, an RllibLSTMShapedCNN or a BCPolicy"
             assert not isinstance(a, RllibLSTMShapedCNN) or autocast_dtype == torch.bfloat16, \
                 "the LSTM policy runs as ovc_lstm_head (K11), which takes bfloat16 operands: autocast_dtype=None is not supported"
@@ -1001,9 +1173,12 @@ class AgentPairRollout(object):
             self.partner_seat = (torch.ones(N, dtype=torch.int32, device=dev) if swap is None
                                  else (1 ^ (swap != 0).int()).to(torch.int32).contiguous())  # agent 1's player
         self.agents = [_BCAgent(env, a, seat, swap, seed, self.random_seats) if isinstance(a, BCPolicy)
-                       else _NetworkAgent(env, a, seat, swap, seed, autocast_dtype, self.random_seats) for seat, a in zip(seats, agents)]
-        # network agents without K7 read K2's observation, written once per transition for both of them
-        library = [a for a in self.agents if isinstance(a, _NetworkAgent) and not a.fused_first_layer]
+                       else _NetworkAgent(env, a, seat, swap, seed, autocast_dtype, self.random_seats)
+                       for seat, a in zip(seats, agents[:1] if self.population else agents)]
+        if self.population:
+            self.agents.append(_Population(env, members, self.partner_seat, seed, autocast_dtype, member, member_weights))
+        # network agents without K7 read K2's observation, written once per transition for all of them
+        library = [a for a in self.agents if (isinstance(a, _NetworkAgent) and not a.fused_first_layer) or getattr(a, "needs_obs", False)]
         l = env.layouts[0]
         self.obs = torch.empty((N, 2, l.width, l.height, 26), dtype=autocast_dtype or torch.float32, device=dev) if library else None
         for a in library:
@@ -1013,7 +1188,7 @@ class AgentPairRollout(object):
         self.factor = 1.0
         self._factor = torch.ones(1, dtype=torch.float32, device=dev)  # reward_shaping_factor, read by the captured graphs
         self.stats = EpisodeStats(env)
-        self.episodes = EpisodeRecords(env, episode_capacity)
+        self.episodes = EpisodeRecords(env, episode_capacity, members=self.population)
         self.graph = None
         self._collect_graphs = {}  # (n_steps, keep_logits) -> ((gamma, lam), CUDA graph of the window)
         self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
@@ -1033,6 +1208,24 @@ class AgentPairRollout(object):
     def reward_shaping_factor(self, value):
         self.factor = float(value)
         self._factor.fill_(self.factor)
+
+    @property
+    def member_weights(self):
+        """The population's draw weights (K non-negative floats with a positive sum).  Setting them writes the device
+        table the draw reads, so run() and collect() follow a new distribution at the next episode ends without a re-capture
+        (prioritised sampling of the population between windows)."""
+        assert self.population and self.agents[1]._thresholds is not None, "member_weights: a population drawn per episode"
+        return self.agents[1].weights
+
+    @member_weights.setter
+    def member_weights(self, value):
+        assert self.population and self.agents[1]._thresholds is not None, "member_weights: a population drawn per episode"
+        self.agents[1].weights = value
+
+    @property
+    def member(self):
+        """int32 [N]: each environment's population member in its running episode (None without a population)."""
+        return self.agents[1].member if self.population else None
 
     def _assign_seats(self, done):
         self.env.assign_partners(self.partner_seat, self._seat_factor, self._seat_counter, seed=self.seed ^ PARTNER_SEAT_SALT, done=done)
@@ -1055,8 +1248,12 @@ class AgentPairRollout(object):
             learner.act(self.actions, values=b.values[t], logp=b.logp[t], scores8=None if b.logits is None else b.logits[t], snap=snap)
             torch.index_select(self.actions.view(-1), 0, learner._rows, out=b.actions[t])
             b.partner_seat[t].copy_(self.partner_seat)
+            if self.population:
+                b.partner_member[t].copy_(partner.member)
         partner.act(self.actions)
         env.step(self.actions)  # K1 (auto-reset inside)
+        if self.population:  # before the record: both use the slot count[e] the ending episode goes to
+            partner.assign(env.done, self.episodes if b is None else b.episodes)
         if b is None:
             env.record_transition(self._factor, ret_sparse=self.ret_sparse, stats=self.stats, records=self.episodes,
                                   partner_seat=self.partner_seat)
@@ -1108,15 +1305,15 @@ class AgentPairRollout(object):
         advantages; ``partner_seat`` is agent 1's player) for a PPO update of agent 0 next to the fixed agent 1.  The batch's
         tensors are reused by the next collect() with the same n_steps / keep_logits.  With use_graph the whole window is one
         CUDA graph (captured once per n_steps / keep_logits; a new gamma or lam re-captures it).  After an update, call
-        ``sync_weights()``; a population member is swapped into agent 1 the same way (``load_state_dict`` on its model, then
-        ``sync_weights()``)."""
+        ``sync_weights()`` (it refolds every population member too).  With a population in agent 1 the batch's
+        ``partner_member`` is the member of every transition."""
         assert isinstance(self.agents[0], _NetworkAgent), "collect() trains agents[0]: an RllibShapedCNN or RllibLSTMShapedCNN, not a BCPolicy"
         assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
         key = (int(n_steps), bool(keep_logits))
         b = self._batches.get(key)
         if b is None:
             b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits, seq_len=self.max_seq_len if self.agents[0].lstm else None,
-                                                 one_view=True)
+                                                 one_view=True, members=self.population)
         if not self.use_graph:
             self._collect_window(b, n_steps, gamma, lam)
             return b

@@ -254,4 +254,23 @@ for name, agents in (("cramped_room", lambda W, H: (RllibShapedCNN(W, H), BCPoli
     assert b.dones.any() and (b.partner_seat >= 0).all()
 torch.cuda.synchronize()
 print("learner-row collect (record_transition_view, gae_view, seat draw) ok", flush=True)
+# a population of partners: ovc_group_members, ovc_assign_members and the rows forms of K7 / K9 / K8 next to K10 on a 5x4
+# grid, the library layers with the rows form of the draw on a 9x5 grid, members drawn per episode (one of weight 0) and
+# fixed; the environments follow the oracle
+for name, fixed in (("cramped_room", False), ("asymmetric_advantages", False), ("cramped_room", True)):
+    env10 = BatchedOvercookedEnv(name, 37, horizon=3, auto_reset=True)
+    l10 = env10.layouts[0]
+    W, H = l10.width, l10.height
+    kw = dict(member=torch.from_numpy(rng.randint(0, 3, 37).astype(np.int32)).cuda()) if fixed else dict(member_weights=[1.0, 0.0, 2.0])
+    pop = AgentPairRollout(env10, (RllibShapedCNN(W, H), [RllibShapedCNN(W, H), RllibShapedCNN(W, H), BCPolicy()]), seed=4,
+                           use_graph=False, random_seats=True, episode_capacity=2, **kw)
+    st = env10.state.cpu().numpy().copy()
+    for t in range(5):
+        pop.run(1)
+        cpu.step(env10._tab_host, env10._starts_host, st, pop.actions.cpu().numpy(), horizon=3, flags=1)
+    assert np.array_equal(env10.state.cpu().numpy(), st)
+    b = pop.collect(5, 0.99, 0.95)
+    assert b.dones.any() and len(b.episodes.finished()["partner_member"]) > 0
+torch.cuda.synchronize()
+print("population (group / assign members, rows forms of K7 / K9 / K8 and the draw, K10) ok", flush=True)
 print("sanitize_smoke: all ok")
