@@ -707,6 +707,36 @@ int ovc_sample_actions_rows(const float *scores, int ld, int n_actions, int64_t 
                             int seat, const int32_t *rows, const int32_t *range, int32_t *actions, float *logp, void *stream);
 
 /*
+ * Self-play mixtures: each environment is self-play (partner_seat[e] = -1: the learner plays both views) or plays a frozen
+ * partner in seat partner_seat[e] (0 or 1: the learner plays view 1 - partner_seat[e]).  The learner's policy runs on its
+ * own rows of the joint [2 n_envs] rows only, with the object part of K7 computed once per environment.
+ *
+ * ovc_learner_rows: from partner_seat int32 [n_envs] (values -1, 0, 1), in ONE CTA without host synchronisation, for every
+ *   environment e in ascending order: list[e] = e << 2 | mask (bit v: the learner plays view v; 3 for -1, 1 << (1 - seat)
+ *   otherwise), first[e] = the compact row of its first view; the compact rows of e's views are consecutive, in ascending
+ *   view order, so compact row r is joint row jrow[r] (int32 [2 n_envs]); range[0] = 0, range[1] = the row count (device
+ *   memory: K9's and K8's range).  n_envs < 2^29; n_envs = 0 writes nothing.  All pointers 4-byte aligned.
+ * ovc_encode_linear_masked: ovc_encode_linear for the views in a list: entry r < n_list is environment list[r] >> 2 with the
+ *   views of mask list[r] & 3 (mask 0: nothing), written to out rows first[r], first[r] + 1, ... in ascending view order,
+ *   each bit for bit row 2 e + v of ovc_encode_linear without view_swap.  The object part is computed once per entry.
+ *   Environments index state; out holds at least as many rows as the list's views.  At most 8 layouts.  list, first 4-byte
+ *   aligned.
+ * ovc_policy_tail_joint: ovc_policy_tail_logp on compact rows r in [range[0], range[1]) of x ([n_rows][k0], the range
+ *   clipped to [0, n_rows), n_rows < 2^31): row r is joint row jrow[r], drawn there with key seed and counter's step, and
+ *   actions, values, logp (required) and scores ([.][8], nullable) are written at jrow[r]: bit for bit what
+ *   ovc_policy_tail_logp writes at that joint row from the same x row.  Every other entry is untouched.  Every CTA
+ *   advances the counter, also for an empty range.
+ */
+int ovc_learner_rows(const int32_t *partner_seat, int64_t n_envs, int32_t *list, int32_t *first, int32_t *jrow, int32_t *range, void *stream);
+int ovc_encode_linear_masked(const void *layouts, int n_layouts, const int32_t *state, const int32_t *list, const int32_t *first,
+                             const void *wt, const float *bias, void *out, int64_t n_list, int state_words, int width, int height,
+                             int horizon, int n_out, float neg_slope, void *stream);
+int ovc_policy_tail_joint(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                          const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                          float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *jrow, const int32_t *range,
+                          int32_t *actions, float *values, float *scores, float *logp, void *stream);
+
+/*
  * featurize_state (:2579-2898) with the default planner parameters (NO_COUNTERS_PARAMS,
  * planners.py:27-34): out float32[n_envs][2][F],
  * F = 2*(num_pots*10+28), lut = ovc_feat_lut_entry_t[n_layouts][256][4].  view_swap as above.

@@ -479,6 +479,34 @@ class BatchedOvercookedEnv(object):
             0 if logp_out is None else logp_out.data_ptr(), self._stream()))
         return out
 
+    def learner_rows(self, partner_seat, lst, first, jrow, rng):
+        """A self-play mixture's learner rows (ovc_learner_rows, one CTA on the device): from ``partner_seat`` int32 [N]
+        (-1: self-play, else the partner's player) writes ``lst`` int32 [N] (``e << 2 | mask``, bit v of the mask: the learner
+        plays view v), ``first`` int32 [N] (the compact row of e's first view), ``jrow`` int32 [2N] (compact row -> joint row)
+        and ``rng`` int32 [2] = (0, the row count)."""
+        for t, n in ((partner_seat, self.n_envs), (lst, self.n_envs), (first, self.n_envs), (jrow, 2 * self.n_envs), (rng, 2)):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n
+        _native.check(self._lib.ovc_learner_rows(partner_seat.data_ptr(), self.n_envs, lst.data_ptr(), first.data_ptr(), jrow.data_ptr(),
+                                                 rng.data_ptr(), self._stream()))
+
+    def encoded_linear_masked(self, wt, bias, lst, first, out, neg_slope=0.2):
+        """``encoded_linear`` on the views of a list (ovc_encode_linear_masked): entry r of ``lst`` (int32, ``e << 2 | mask``)
+        writes the views of its mask to rows ``first[r], first[r] + 1, ...`` of ``out`` (bfloat16 ``[rows, n_out]``), each bit
+        for bit row ``2 e + v`` of ``encoded_linear``; the object part is computed once per entry."""
+        assert len({(l.width, l.height) for l in self.layouts}) == 1, "one grid shape per call (group envs by layout)"
+        W, H = self.layouts[0].width, self.layouts[0].height
+        assert wt.is_cuda and wt.dtype == torch.bfloat16 and wt.is_contiguous() and wt.shape[0] == W * H * 26, wt.shape
+        n_out = wt.shape[1]
+        assert bias.is_cuda and bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == n_out
+        for t in (lst, first):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == lst.numel()
+        assert out.is_cuda and out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape[-1] == n_out
+        _native.check(self._lib.ovc_encode_linear_masked(
+            self.tables.data_ptr(), self.n_layouts, self.state.data_ptr(), lst.data_ptr(), first.data_ptr(), wt.data_ptr(),
+            bias.data_ptr(), out.data_ptr(), lst.numel(), self.state_words, W, H, self.horizon if self.horizon > 0 else 2**31 - 1,
+            n_out, float(neg_slope), self._stream()))
+        return out
+
     def group_members(self, member, n_members, order, offsets):
         """The environments grouped by population member (ovc_group_members, a stable counting sort on the device):
         ``member`` int32 [N] with values in [0, n_members); writes ``order`` int32 [N] (environment indices by member,

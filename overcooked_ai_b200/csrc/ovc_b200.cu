@@ -930,6 +930,33 @@ int ovc_sample_actions_rows(const float *scores, int ld, int n_actions, int64_t 
                                          logp, (cudaStream_t)stream);
 }
 
+int ovc_learner_rows(const int32_t *partner_seat, int64_t n_envs, int32_t *list, int32_t *first, int32_t *jrow, int32_t *range, void *stream) {
+    return ovc::learner_rows_impl(partner_seat, n_envs, list, first, jrow, range, (cudaStream_t)stream);
+}
+
+int ovc_encode_linear_masked(const void *layouts, int n_layouts, const int32_t *state, const int32_t *list, const int32_t *first,
+                             const void *wt, const float *bias, void *out, int64_t n_list, int state_words, int width, int height,
+                             int horizon, int n_out, float neg_slope, void *stream) {
+    int rc = ovc::check_common(layouts, n_layouts, state, n_list, state_words);
+    if (rc) return rc;
+    if (!list || !first) return ovc::fail(OVC_E_BADARG, "null pointer argument");
+    return ovc::encode_linear_impl((const ovc_layout_t *)layouts, n_layouts, state, nullptr, wt, bias, out, n_list, state_words, width,
+                                   height, horizon, n_out, neg_slope, (cudaStream_t)stream, -1, nullptr, nullptr, list, first);
+}
+
+int ovc_policy_tail_joint(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                          const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                          float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *jrow, const int32_t *range,
+                          int32_t *actions, float *values, float *scores, float *logp, void *stream) {
+    ovc::PolicyTailArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
+    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
+    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
+    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    if (n_rows > 0x7FFFFFFFll) return ovc::fail(OVC_E_BADARG, "n_rows must be below 2^31", n_rows);
+    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, nullptr, -1, jrow, range, true);
+}
+
 int ovc_featurize(const void *layouts, int n_layouts, const void *lut, const int32_t *state,
                   const int32_t *view_swap, float *out, int64_t n_envs, int state_words, int num_pots, void *stream) {
     int rc = ovc::check_common(layouts, n_layouts, state, n_envs, state_words);

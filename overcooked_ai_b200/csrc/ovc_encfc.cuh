@@ -111,8 +111,11 @@ __device__ __forceinline__ void el_gather(float acc[CPL], const __nv_bfloat16 *t
 // object part and that view's gathers run in the same order as in the two-view kernel, so the row is bit-identical to
 // row 2 e + p(e) of it.  ROWS (with VIEW): compact rows r in [range[0], range[1]) only, environment rows[r] written to
 // out[r]; a CTA whose share of the range is empty leaves before its prologue.
-template <int CPL, bool VIEW, bool ROWS = false>
-__global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncLinArgs a) {
+// MASKED (encode_linear_masked_kernel, without view_swap): entry r < n_envs of the list is environment list[r] >> 2 with the
+// views of mask list[r] & 3 (bit v: view v); the object part is computed once, and the views in the mask go to consecutive
+// rows from first[r] in ascending view order, each bit for bit row 2 e + v of the two-view kernel.
+template <int CPL, bool VIEW, bool ROWS, bool MASKED>
+__device__ __forceinline__ void encode_linear_body(const EncLinArgs &a, const int32_t *list = nullptr, const int32_t *first = nullptr) {
     constexpr int CS = 32 * CPL;  // columns per CTA
     extern __shared__ __align__(16) char el_smem[];
     const int WH = a.W * a.H;
@@ -132,6 +135,9 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncL
         r_beg = max(__ldg(a.range), 0);
         r_end = min((long long)__ldg(a.range + 1), a.n_envs);
         if (r_beg + (long long)worker * (EL_THREADS / 32) >= r_end) return;
+    }
+    if constexpr (MASKED) {
+        if ((long long)worker * (EL_THREADS / 32) >= r_end) return;
     }
 
     // ---- prologue: the table slice and the per-layout constants ----
@@ -189,7 +195,16 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncL
     const int max_slot_chunks = (a.S - 4 + 31) / 32;
 
     for (long long r = r_beg + (long long)worker * NW + warp; r < r_end; r += stride) {
-        const long long env = ROWS ? (long long)__ldg(a.rows + r) : r;
+        long long env, row0 = 0;
+        int vmask = 3;
+        if constexpr (MASKED) {
+            const int entry = __ldg(list + r);
+            env = entry >> 2, vmask = entry & 3;
+            if (!vmask) continue;  // the whole warp holds entry r
+            row0 = __ldg(first + r);
+        } else {
+            env = ROWS ? (long long)__ldg(a.rows + r) : r;
+        }
         const int32_t *__restrict__ rec = a.state + env * a.S;
         const int4 head = __ldg(reinterpret_cast<const int4 *>(rec));  // timestep, player 0, player 1, misc (same address in every lane)
         const int lid = head.w & 0xFF;
@@ -270,7 +285,10 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncL
             else if constexpr (CPL == 4) *reinterpret_cast<uint2 *>(dst) = make_uint2(packed[0], packed[1]);
             else *reinterpret_cast<unsigned *>(dst) = packed[0];
         };
-        if constexpr (VIEW) {
+        if constexpr (MASKED) {
+            if (vmask & 1) view(0, row0);
+            if (vmask & 2) view(1, row0 + (vmask & 1));
+        } else if constexpr (VIEW) {
             view(a.seat ^ swap, r);
         } else {
 #pragma unroll
@@ -279,22 +297,35 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncL
     }
 }
 
+template <int CPL, bool VIEW, bool ROWS = false>
+__global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncLinArgs a) {
+    encode_linear_body<CPL, VIEW, ROWS, false>(a);
+}
+
+// A kernel of its own, so that the list and first-row pointers stay out of EncLinArgs and encode_linear_kernel's code
+template <int CPL>
+__global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_masked_kernel(const EncLinArgs a, const int32_t *list, const int32_t *first) {
+    encode_linear_body<CPL, false, false, true>(a, list, first);
+}
+
 static size_t encode_linear_smem(int cpl, int n_rows, int n_layouts) {
     const size_t CS = 32 * (size_t)cpl;
     return (size_t)n_rows * CS * 2 + ((size_t)n_layouts + 1) * CS * 4 + (size_t)n_layouts * (16 * 4 + 2 * 4 + 128 * 2 + 256) + 16;
 }
 
 // seat < 0: both views (ovc_encode_linear); 0 / 1: one view per environment (ovc_encode_linear_view, view_swap = swap);
-// with rows / range: the rows map (ovc_encode_linear_rows)
+// with rows / range: the rows map (ovc_encode_linear_rows); with list / first: n_envs list entries (ovc_encode_linear_masked)
 static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const int32_t *state, const int32_t *view_swap,
                               const void *wt, const float *bias, void *out, long long n_envs, int S, int W, int H, int horizon,
                               int n_out, float neg_slope, cudaStream_t st, int seat = -1, const int32_t *rows = nullptr,
-                              const int32_t *range = nullptr) {
-    const bool rows_map = rows || range;
-    if (!out || !wt || !bias || (rows_map && (!rows || !range))) return fail(OVC_E_BADARG, "null pointer argument");
+                              const int32_t *range = nullptr, const int32_t *list = nullptr, const int32_t *first = nullptr) {
+    const bool rows_map = rows || range, masked = list || first;
+    if (!out || !wt || !bias || (rows_map && (!rows || !range)) || (masked && (!list || !first)))
+        return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)out | (uintptr_t)wt) & 15) != 0) return fail(OVC_E_BADARG, "weights and output must be 16-byte aligned");
     if (seat >= 0 && ((uintptr_t)view_swap & 3) != 0) return fail(OVC_E_BADARG, "swap must be 4-byte aligned");
     if ((((uintptr_t)rows | (uintptr_t)range) & 3) != 0) return fail(OVC_E_BADARG, "rows and range must be 4-byte aligned");
+    if ((((uintptr_t)list | (uintptr_t)first) & 3) != 0) return fail(OVC_E_BADARG, "list and first must be 4-byte aligned");
     if (W < 1 || W > 16 || H < 1 || H > 16) return fail(OVC_E_BADARG, "grid shape out of range");
     if (n_out < 64 || n_out % 64) return fail(OVC_E_BADARG, "n_out must be a positive multiple of 64", n_out);
     if (!(neg_slope >= 0.f && neg_slope <= 1.f)) return fail(OVC_E_BADARG, "negative slope must lie in [0, 1]");
@@ -330,7 +361,17 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
         if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                                          \
         encode_linear_kernel<C, __VA_ARGS__><<<(unsigned)(workers * n_slices), EL_THREADS, smem, st>>>(a);                    \
     } while (0)
-    if (rows_map) {
+#define OVC_LAUNCH_ELM(C)                                                                                                     \
+    do {                                                                                                                      \
+        e = cudaFuncSetAttribute(encode_linear_masked_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);     \
+        if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                                          \
+        encode_linear_masked_kernel<C><<<(unsigned)(workers * n_slices), EL_THREADS, smem, st>>>(a, list, first);             \
+    } while (0)
+    if (masked) {
+        if (cpl == 8) OVC_LAUNCH_ELM(8);
+        else if (cpl == 4) OVC_LAUNCH_ELM(4);
+        else OVC_LAUNCH_ELM(2);
+    } else if (rows_map) {
         if (cpl == 8) OVC_LAUNCH_EL(8, true, true);
         else if (cpl == 4) OVC_LAUNCH_EL(4, true, true);
         else OVC_LAUNCH_EL(2, true, true);
@@ -344,6 +385,7 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
         else OVC_LAUNCH_EL(2, false);
     }
 #undef OVC_LAUNCH_EL
+#undef OVC_LAUNCH_ELM
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel launch");
     return OVC_OK;

@@ -240,6 +240,75 @@ static int group_members_impl(const int32_t *member, int n_members, long long n_
     return OVC_OK;
 }
 
+// ---- self-play mixtures: the learner's rows of the joint [2 n_envs] rows ----
+constexpr int LR_THREADS = 1024;  // one CTA: 32 warps, warp w owns the w-th contiguous segment of the environments
+constexpr long long LR_MAX_ENVS = 1ll << 29;  // list entries pack e << 2 | mask into an int32
+
+// A stable scan in ONE CTA, as group_members_kernel: (1) every warp counts its segment's learner views (2 where
+// partner_seat[e] < 0, else 1), (2) one thread turns the warp totals into segment starts and writes range = {0, total},
+// (3) every warp walks its segment 32 environments at a time in order, a warp-wide inclusive scan giving each environment
+// its first compact row.  Environment e's views go to consecutive rows in ascending view order.
+__global__ void __launch_bounds__(LR_THREADS, 1) learner_rows_kernel(const int32_t *__restrict__ partner_seat, long long n_envs,
+                                                                     int32_t *__restrict__ list, int32_t *__restrict__ first,
+                                                                     int32_t *__restrict__ jrow, int32_t *__restrict__ range) {
+    __shared__ int start[LR_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const long long seg = (n_envs + LR_THREADS / 32 - 1) / (LR_THREADS / 32);
+    const long long beg = warp * seg, end = beg + seg < n_envs ? beg + seg : n_envs;
+    int cnt = 0;
+    for (long long e = beg + lane; e < end; e += 32) cnt += __ldg(partner_seat + e) < 0 ? 2 : 1;
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) cnt += __shfl_xor_sync(0xFFFFFFFFu, cnt, d);
+    if (lane == 0) start[warp] = cnt;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int run = 0;
+        for (int w = 0; w < LR_THREADS / 32; w++) {
+            const int c = start[w];
+            start[w] = run;
+            run += c;
+        }
+        range[0] = 0;
+        range[1] = run;
+    }
+    __syncthreads();
+    int base = start[warp];
+    for (long long e0 = beg; e0 < end; e0 += 32) {
+        const long long e = e0 + lane;
+        const bool in = e < end;
+        const int s = in ? __ldg(partner_seat + e) : 0;
+        const int mask = s < 0 ? 3 : (s == 0 ? 2 : 1);  // the learner's views: both in self-play, else view 1 - seat
+        const int c = in ? (mask == 3 ? 2 : 1) : 0;
+        int x = c;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int y = __shfl_up_sync(0xFFFFFFFFu, x, d);
+            if (lane >= d) x += y;
+        }
+        if (in) {
+            const int f = base + x - c;
+            list[e] = (int32_t)(e << 2) | mask;
+            first[e] = f;
+            if (mask & 1) jrow[f] = (int32_t)(2 * e);
+            if (mask & 2) jrow[f + (mask & 1)] = (int32_t)(2 * e + 1);
+        }
+        base += __shfl_sync(0xFFFFFFFFu, x, 31);
+    }
+}
+
+static int learner_rows_impl(const int32_t *partner_seat, long long n_envs, int32_t *list, int32_t *first, int32_t *jrow, int32_t *range,
+                             cudaStream_t st) {
+    if (!partner_seat || !list || !first || !jrow || !range) return fail(OVC_E_BADARG, "null pointer argument");
+    if (((uintptr_t)partner_seat | (uintptr_t)list | (uintptr_t)first | (uintptr_t)jrow | (uintptr_t)range) & 3)
+        return fail(OVC_E_BADARG, "partner_seat, list, first, jrow and range must be 4-byte aligned");
+    if (n_envs < 0 || n_envs >= LR_MAX_ENVS) return fail(OVC_E_BADARG, "n_envs must be 0..2^29-1", n_envs);
+    if (n_envs == 0) return OVC_OK;
+    learner_rows_kernel<<<1, LR_THREADS, 0, st>>>(partner_seat, n_envs, list, first, jrow, range);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "learner_rows kernel launch");
+    return OVC_OK;
+}
+
 // Per environment e with done[e] (every e with done == NULL): the ending episode's member into the records' slot count[e]
 // (when done is given, rec_member non-NULL and count[e] < capacity), then, with thresholds, a new member: Philox4x32-10,
 // key = seed, counter = (e low, e high, step low, step high) -> w0;  member[e] = #{k < n_members - 1 : w0 >= thresholds[k]}.

@@ -245,7 +245,9 @@ __device__ __forceinline__ void advance_step(unsigned long long *counter, unsign
 // every instantiation.
 // ROWS (with VIEW, policy_tail_rows_kernel): compact rows r in [range[0], range[1]) only; row r is environment rows[r]'s
 // agent, drawn on its joint row 2 rows[r] + p(rows[r]).
-template <int KS2, bool LOGP, bool HIDDEN, bool VIEW, bool ROWS = false>
+// JOINT (policy_tail_joint_kernel): compact rows r in [range[0], range[1]) only; x row r is joint row rows[r], drawn on it,
+// and actions, values, logp and scores are written at that joint row.
+template <int KS2, bool LOGP, bool HIDDEN, bool VIEW, bool ROWS = false, bool JOINT = false>
 __device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const int32_t *swap, int seat, const int32_t *rows = nullptr,
                                                  const int32_t *range = nullptr) {
     constexpr int K0 = 32 * KS2;
@@ -259,9 +261,9 @@ __device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     const float in_slope2 = p.in_slope;
     // the rows form counts rows in 32 bits (a range of int32 entries), which keeps it within K8's registers
-    using Row = typename std::conditional<ROWS, int, long long>::type;
+    using Row = typename std::conditional<ROWS || JOINT, int, long long>::type;
     Row r_beg = 0, r_end = p.n_rows;
-    if constexpr (ROWS) {
+    if constexpr (ROWS || JOINT) {
         r_beg = max(__ldg(range), 0);
         r_end = max((int)min((long long)__ldg(range + 1), p.n_rows), r_beg);
     }
@@ -297,6 +299,26 @@ __device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const 
         // ---- hidden layers and heads: fragments in, fragments out ----
         float out[1][4];
         tail_layers(out, acc, w, p.n_hidden, p.slope, g, t);
+        if constexpr (JOINT) {  // rows past the end: their draw is discarded
+            const long long j0 = r0 < r_end ? (long long)__ldg(rows + r0) : 0, j1 = r1 < r_end ? (long long)__ldg(rows + r1) : 0;
+            if (p.scores) {
+                if (r0 < r_end) *reinterpret_cast<float2 *>(p.scores + j0 * PT_NOUT + 2 * t) = make_float2(out[0][0], out[0][1]);
+                if (r1 < r_end) *reinterpret_cast<float2 *>(p.scores + j1 * PT_NOUT + 2 * t) = make_float2(out[0][2], out[0][3]);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const long long jr = h ? j1 : j0;
+                const float s0 = out[0][2 * h], s1 = out[0][2 * h + 1];
+                float lp = 0.f;
+                const int best = draw_row<LOGP>(s0, s1, p.seed, step, jr, p.n_actions, lane, t, lp);
+                if ((h ? r1 : r0) < r_end) {
+                    if (t == 0) p.actions[jr] = best;
+                    if constexpr (LOGP) if (t == 0) p.logp[jr] = lp;
+                    if (p.values && t == (p.n_actions >> 1)) p.values[jr] = (p.n_actions & 1) ? s1 : s0;
+                }
+            }
+            continue;
+        }
         if (p.scores) {
             if (r0 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r0 * PT_NOUT + 2 * t) = make_float2(out[0][0], out[0][1]);
             if (r1 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r1 * PT_NOUT + 2 * t) = make_float2(out[0][2], out[0][3]);
@@ -342,14 +364,19 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_rows_kernel(const P
     policy_tail_body<KS2, LOGP, false, true, true>(p, swap, seat, rows, range);
 }
 
+template <int KS2>
+__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_joint_kernel(const PolicyTailArgs p, const int32_t *jrow, const int32_t *range) {
+    policy_tail_body<KS2, true, false, false, false, true>(p, nullptr, 0, jrow, range);
+}
+
 // hid: the HIDDEN instantiation into a.hidden (no heads, no draw; a.w_heads / a.b_heads are staged but never read, so the
 // entry point passes the first layer's tables, which are at least as large, in their place).  seat >= 0: the one-view
-// kernel with swap (ovc_policy_tail_view); -1: the two-view ones.
+// kernel with swap (ovc_policy_tail_view); -1: the two-view ones.  joint: rows is the joint-row map (ovc_policy_tail_joint).
 static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bool hid = false, const int32_t *swap = nullptr,
-                            int seat = -1, const int32_t *rows = nullptr, const int32_t *range = nullptr) {
-    const bool view = seat >= 0, rows_map = rows || range;
+                            int seat = -1, const int32_t *rows = nullptr, const int32_t *range = nullptr, bool joint = false) {
+    const bool view = seat >= 0 || joint, rows_map = rows || range;
     if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || (hid ? !a.hidden : (!a.counter || !a.actions)) ||
-        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)) || (rows_map && (!rows || !range)))
+        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)) || (rows_map && (!rows || !range)) || (joint && (!rows || !range || !a.logp)))
         return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)a.x | (uintptr_t)a.w_first) & 15) != 0) return fail(OVC_E_BADARG, "x and w_first must be 16-byte aligned");
     if (hid && ((uintptr_t)a.hidden & 3) != 0) return fail(OVC_E_BADARG, "hidden must be 4-byte aligned");
@@ -378,6 +405,7 @@ static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bo
 #define OVC_LAUNCH_PT(KS2)                                                                                       \
     case KS2:                                                                                                    \
         if (hid) OVC_PT_KERNEL((a), policy_tail_kernel<KS2, false, true>);                                       \
+        else if (joint) OVC_PT_KERNEL((a, rows, range), policy_tail_joint_kernel<KS2>);                          \
         else if (rows_map && a.logp) OVC_PT_KERNEL((a, swap, seat, rows, range), policy_tail_rows_kernel<KS2, true>); \
         else if (rows_map) OVC_PT_KERNEL((a, swap, seat, rows, range), policy_tail_rows_kernel<KS2, false>);     \
         else if (view && a.logp) OVC_PT_KERNEL((a, swap, seat), policy_tail_view_kernel<KS2, true>);             \

@@ -365,8 +365,10 @@ class SampleBatch(object):
     last_values   float32 [2N]       value head on the state after the window (bootstrap)
     advantages, value_targets  float32 [T, 2N]   GAE (ovc_gae)
     logits        float32 [T, 2N, 8] the policy's heads (columns 0..5 the logits), only with ``keep_logits``
-    partner_seat  int8 [T, N]        with a BC partner: its player index at transition t (-1: self-play), else None
+    partner_seat  int8 [T, N]        with a partner: its player index at transition t (-1: self-play), else None
                                      (``one_view``: agent 1's player)
+    partner_member int8 [T, N]       with a population of partners: each environment's member at transition t (in a
+                                     two-view batch meaningful where partner_seat >= 0), else None
     learner_mask  uint8 [T, 2N]      (property) the rows the learner trains on: all rows but the partner's
     episodes      EpisodeRecords     the episodes that ended in the window (``episodes.finished()``), capacity
                                      ceil(T / horizon): an environment cannot end more episodes in T transitions
@@ -527,14 +529,15 @@ def _capture_graph(env, live, warm_up, body):
 
 
 class SelfPlayRollout(_FoldedPolicy):
-    """Policy-in-the-loop rollout: both agents of every environment act from the same network, or, with a BC ``partner``,
-    one seat of an environment is the partner's in the episodes the seat draw gives it (PPO_BC).  The network evaluated is
+    """Policy-in-the-loop rollout: both agents of every environment act from the same network, or, with a ``partner``,
+    one seat of an environment is the partner's in the episodes the seat draw gives it (PPO_BC, or a self-play mixture with
+    a frozen network or a population).  The network evaluated is
     ``DenseGridPolicy`` of ``model``: K7 / K9 / K8 where they fit (``fused_kernel_support``; K7, and K9 behind it, only with
     at most 8 layouts in ``env``), library GEMMs and the draw kernel elsewhere."""
 
     def __init__(self, env, model=None, autocast_dtype=torch.bfloat16, use_graph=True, reward_shaping_factor=1.0,
                  fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0, episode_capacity=1,
-                 max_seq_len=20):
+                 max_seq_len=20, member=None, member_weights=None):
         """autocast_dtype: the dtype of the dense model (``DenseGridPolicy``, widths padded to 16-byte rows) and of the
         observation K2 writes for it: bfloat16 (the plane values are exact in bf16), or None for float32 throughout.
         fused_first_layer (default: on for the bf16 policy where ``fused_kernel_support`` allows K7): the observation is
@@ -552,6 +555,19 @@ class SelfPlayRollout(_FoldedPolicy):
         episode start (and for every environment at construction) an environment gets the partner with probability
         ``bc_factor``, in seat 0 or 1 with equal probability (``env.assign_partners``); per transition K10
         (``env.partner_actions``) overwrites that seat's action after the PPO policy drew both.
+        partner may instead be a frozen ``RllibShapedCNN`` or a population: a list of 1..63 members, each an ``RllibShapedCNN``
+        or a ``BCPolicy`` (a self-play mixture: each episode is self-play with probability ``1 - bc_factor``, else played
+        next to the partner, or next to the population member the environment holds).  The partner, or member k, then
+        evaluates only the seat it holds in the paired environments that play it (``ovc_group_members`` over the paired
+        environments; a network member runs the rows forms of K7 / K9 / K8, a BC member K10), and never writes a self-play
+        row.  A network partner draws with key ``seed`` on a counter of its own, a BC member with ``seed ^
+        PARTNER_DRAW_SALT``: ``partner=copy.deepcopy(model)`` draws exactly what self-play draws.  Where the learner runs K7,
+        K9 and K8, it evaluates only its own rows (``ovc_learner_rows``, ``ovc_encode_linear_masked``, K9 on the compact
+        rows, ``ovc_policy_tail_joint``); the partner rows' values, logp and advantages are then not written.  Other learners
+        run on all 2N rows, as without a partner.  LSTM partners and members are refused (K11 has no rows form).
+        member, member_weights: with a population only, as ``AgentPairRollout``'s: a fixed member per environment, or one
+        drawn at construction and at every episode end (uniform by default), whether or not the next episode is paired.
+        ``episodes.finished()`` and collect()'s batches then report ``partner_member``, meaningful where ``partner_seat >= 0``.
         bc_factor: see the property.
         episode_capacity: episodes per environment that ``self.episodes`` holds (an ``EpisodeRecords``): every episode that
         ends in run() is written there, up to this many per environment since ``self.episodes.clear()`` (the rest are
@@ -568,6 +584,37 @@ class SelfPlayRollout(_FoldedPolicy):
         self.env = env
         self._fold(env, model, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
         dev = env.device
+        N = env.n_envs
+        self.partner = None
+        self.bc = float(bc_factor)
+        self.population = isinstance(partner, (list, tuple))
+        self._pop = None  # the network partner or the population (a _Population)
+        if self.population:
+            assert 1 <= len(partner) <= MAX_MEMBERS - 1, \
+                "a mixture's population has 1..%d members (one of ovc_group_members' %d groups holds the self-play environments)" \
+                % (MAX_MEMBERS - 1, MAX_MEMBERS)
+        else:
+            assert member is None and member_weights is None, "member / member_weights go with a population in partner"
+        for m in (list(partner) if self.population else [partner] if partner is not None else []):
+            assert not isinstance(m, RllibLSTMShapedCNN), \
+                "an LSTM partner or member is not supported in a self-play mixture (ovc_lstm_head has no rows form)"
+            assert isinstance(m, (RllibShapedCNN, BCPolicy)), "a partner is a BCPolicy, an RllibShapedCNN or a list of them"
+        if partner is not None:
+            self._bc_factor = torch.full((1,), self.bc, dtype=torch.float32, device=dev)  # read by the seat draw
+            self.partner_seat = torch.full((N,), -1, dtype=torch.int32, device=dev)
+            self._seat_counter = torch.zeros(2, dtype=torch.int64, device=dev)     # [step, scratch] of the seat draw
+        if isinstance(partner, BCPolicy):
+            self.partner = partner.to(dev).eval()
+            self._partner_tables = self.partner.tables()
+            self._partner_n_actions = self.partner.logits.out_features
+            self._partner_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of K10's draw
+        elif partner is not None:
+            self.partner = partner
+            members = list(partner) if self.population else [partner]
+            if not self.population:  # one network partner: a population of one, its member fixed
+                member = torch.zeros(N, dtype=torch.int32, device=dev)
+            self._pop = _Population(env, members, self.partner_seat, seed, autocast_dtype, member, member_weights, mixture=True)
+        self._learner_rows = False
         self.factor = float(reward_shaping_factor)
         self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by the captured graphs
         N = env.n_envs
@@ -601,17 +648,22 @@ class SelfPlayRollout(_FoldedPolicy):
         self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
         self._boot_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # the bootstrap's draws leave _draw_counter alone
         self._boot_actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
-        self.partner = None
-        self.bc = float(bc_factor)
         if partner is not None:
-            self.partner = partner.to(dev).eval()
-            self._partner_tables = self.partner.tables()
-            self._partner_n_actions = self.partner.logits.out_features
-            self._bc_factor = torch.full((1,), self.bc, dtype=torch.float32, device=dev)  # read by the seat draw
-            self.partner_seat = torch.full((N,), -1, dtype=torch.int32, device=dev)
-            self._partner_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of K10's draw
-            self._seat_counter = torch.zeros(2, dtype=torch.int64, device=dev)     # [step, scratch] of the seat draw
             self._assign_partners(None)
+        if self._pop is not None:
+            if self._pop.needs_obs and self.obs is None:
+                self.obs = torch.empty((N, 2, self.W, self.H, 26), dtype=autocast_dtype or torch.float32, device=dev)
+            self._pop.obs = self.obs
+            # the learner on its own rows only, where it runs K7 -> K9 -> K8
+            self._learner_rows = self.fused_first_layer and self.fused_wide and self.fused_tail and not self.lstm
+            if self._learner_rows:
+                self._lst = torch.empty(N, dtype=torch.int32, device=dev)
+                self._first = torch.empty(N, dtype=torch.int32, device=dev)
+                self._jrow = torch.empty(2 * N, dtype=torch.int32, device=dev)
+                self._lrange = torch.zeros(2, dtype=torch.int32, device=dev)
+                self._logp = torch.empty(2 * N, dtype=torch.float32, device=dev)  # run()'s logp: the joint K8 always writes it
+        if self.population:
+            self.episodes = EpisodeRecords(env, episode_capacity, members=True)
 
     @property
     def reward_shaping_factor(self):
@@ -626,7 +678,7 @@ class SelfPlayRollout(_FoldedPolicy):
 
     @property
     def bc_factor(self):
-        """Probability that an episode is played with the BC partner (human_aware_rl's ``bc_factor``, annealed by its
+        """The probability that an episode is played with the partner (human_aware_rl's ``bc_factor``, annealed by its
         ``bc_schedule``).  Setting it takes effect at the next episode starts, in run() and collect() alike, without a
         re-capture (the seat draw reads a device scalar)."""
         return self.bc
@@ -637,13 +689,42 @@ class SelfPlayRollout(_FoldedPolicy):
         self.bc = float(value)
         self._bc_factor.fill_(self.bc)
 
+    @property
+    def member_weights(self):
+        """The population's draw weights, as ``AgentPairRollout.member_weights``: setting them takes effect at the next
+        episode ends without a re-capture."""
+        assert self.population and self._pop._thresholds is not None, "member_weights: a population drawn per episode"
+        return self._pop.weights
+
+    @member_weights.setter
+    def member_weights(self, value):
+        assert self.population and self._pop._thresholds is not None, "member_weights: a population drawn per episode"
+        self._pop.weights = value
+
+    @property
+    def member(self):
+        """int32 [N]: each environment's population member in its running episode (None without a population); it plays
+        only where ``partner_seat >= 0``."""
+        return self._pop.member if self.population else None
+
     def _assign_partners(self, done):
         self.env.assign_partners(self.partner_seat, self._bc_factor, self._seat_counter, seed=self.seed ^ PARTNER_SEAT_SALT, done=done)
 
     def _partner_act(self, actions):
-        """K10: the partner's seat of ``actions`` (int32 [N, 2] or [2N]) from the current state."""
+        """The partner's seat of ``actions`` (int32 [N, 2] or [2N]) in the paired environments, from the current state: K10
+        for a BC partner, else the network partner's or the population's kernels."""
+        if self._pop is not None:
+            self._pop.act(actions)
+            return
         self.env.partner_actions(self._partner_tables, self.partner_seat, self._partner_counter, seed=self.seed ^ PARTNER_DRAW_SALT,
                                  n_actions=self._partner_n_actions, out=actions)
+
+    def sync_weights(self):
+        """Re-fold the learner (``_FoldedPolicy.sync_weights``) and a network partner or every population member, in place:
+        the captured graphs use the new weights without a re-capture."""
+        _FoldedPolicy.sync_weights(self)
+        if self._pop is not None:
+            self._pop.sync_weights()
 
     def _capture(self, warm_up, body):
         """A CUDA graph of ``body``, captured after ``warm_up`` (on a side stream).  Warm-up and capture must not advance
@@ -653,7 +734,8 @@ class SelfPlayRollout(_FoldedPolicy):
         if self.lstm:
             live += [self.h, self.c, self.env.done]  # env.done: the next transition's LSTM reset
         if self.partner is not None:
-            live += [self.partner_seat, self._partner_counter, self._seat_counter]
+            live += [self.partner_seat, self._seat_counter]
+            live += self._pop.live() if self._pop is not None else [self._partner_counter]
         return _capture_graph(self.env, live, warm_up, body)
 
     def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None, state_out=None, snap=None):
@@ -703,6 +785,24 @@ class SelfPlayRollout(_FoldedPolicy):
                 _native.check(_native.lib().ovc_policy_tail_logp(*args, logp.data_ptr(), env._stream()))
         return None  # K8 has drawn the actions itself
 
+    def _policy_learner_rows(self, actions, values, logp, scores8):
+        """K7 -> K9 -> K8 on the learner's rows only: both views of a self-play environment, view 1 - partner_seat[e] of a
+        paired one.  Each row is drawn and written at its joint row, bit for bit what ``_policy`` writes there."""
+        env, rows, lib = self.env, 2 * self.env.n_envs, _native.lib()
+        env.learner_rows(self.partner_seat, self._lst, self._first, self._jrow, self._lrange)
+        env.encoded_linear_masked(self._wt0, self._b0, self._lst, self._first, self._act0, neg_slope=0.2)  # K7
+        w1, b1, w2, b2 = self._wide
+        _native.check(lib.ovc_wide_layers_range(self._act0.data_ptr(), rows, self._act0.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
+                                                w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, self._lrange.data_ptr(), self._z.data_ptr(),
+                                                env._stream()))
+        w1, b1, wh, bh, wo, bo = self._tail
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        _native.check(lib.ovc_policy_tail_joint(
+            self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(), wh.shape[0],
+            wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1), self._draw_counter.data_ptr(),
+            self._jrow.data_ptr(), self._lrange.data_ptr(), actions.data_ptr(), values.data_ptr(), ptr(scores8),
+            (self._logp if logp is None else logp).data_ptr(), env._stream()))
+
     def _lstm_head(self, actions, values, logp, scores8, counter, state_out, snap):
         """K11 on self._x and the live state, reset where the previous transition ended an episode (env.done)."""
         w, b, wo, bo = self._lstm_tables
@@ -727,12 +827,16 @@ class SelfPlayRollout(_FoldedPolicy):
             b.states[t].copy_(env.state)
             actions, values, logp, rewards, dones = b.actions[t], b.values[t], b.logp[t], b.rewards[t], b.dones[t]
             logits = None if b.logits is None else b.logits[t]
-        if not self.fused_first_layer:
+        if self.obs is not None:
             env.lossless_state_encoding(out=self.obs)  # K2
         snap = None
         if self.lstm and b is not None and t % b.seq_len == 0:
             snap = (b.state_h[t // b.seq_len], b.state_c[t // b.seq_len])
-        scores = self._policy(actions=actions, values=values, logp=logp, scores8=logits, snap=snap)
+        if self._learner_rows:
+            scores = self._policy_learner_rows(actions, self.values.view(-1) if values is None else values, logp,
+                                               self._scores8 if logits is None else logits)
+        else:
+            scores = self._policy(actions=actions, values=values, logp=logp, scores8=logits, snap=snap)
         if scores is not None:  # library layers: the separate draw kernel
             env.sample_actions(scores, self._draw_counter, seed=self.seed, out=actions, logp_out=logp)
             if logits is not None:
@@ -740,8 +844,12 @@ class SelfPlayRollout(_FoldedPolicy):
         if self.partner is not None:
             if b is not None:
                 b.partner_seat[t].copy_(self.partner_seat)
-            self._partner_act(actions)  # K10
+                if self.population:
+                    b.partner_member[t].copy_(self._pop.member)
+            self._partner_act(actions)  # K10, or the network partner / the population
         env.step(actions.view(env.n_envs, 2))  # K1 (auto-reset inside)
+        if self.population:  # before the record: both use the slot count[e] the ending episode goes to
+            self._pop.assign(env.done, self.episodes if b is None else b.episodes)
         # the seat draw below runs after this kernel, so partner_seat is still the ending episode's
         env.record_transition(self._factor, rewards=rewards, dones=dones, ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed,
                               stats=self.stats, records=self.episodes if b is None else b.episodes,
@@ -780,14 +888,16 @@ class SelfPlayRollout(_FoldedPolicy):
         reused: the next collect() with the same n_steps / keep_logits overwrites them.  With use_graph the whole window
         is one CUDA graph (captured once per n_steps / keep_logits; a new gamma or lam re-captures it); no host
         synchronisation otherwise.  With a partner, the batch's ``partner_seat`` / ``learner_mask`` say which rows were the
-        partner's; their actions are the partner's, their logp / values / advantages are the PPO network's and meaningless.
+        partner's; their actions are the partner's, their logp / values / advantages are meaningless (the PPO network's, or,
+        where the learner runs on its own rows only, not written).  With a population, ``partner_member`` is each
+        transition's member (meaningful where ``partner_seat >= 0``).
         A seat changes hands only at a done, where GAE cuts, so a learner row's advantages never read a partner step."""
         assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
         key = (int(n_steps), bool(keep_logits))
         b = self._batches.get(key)
         if b is None:
             b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits, partner=self.partner is not None,
-                                                 seq_len=self.max_seq_len if self.lstm else None)
+                                                 seq_len=self.max_seq_len if self.lstm else None, members=self.population)
         if not self.use_graph:
             self._collect_window(b, n_steps, gamma, lam)
             return b
@@ -972,11 +1082,13 @@ class _Population(object):
     library layers over all N compact rows of the observation (gathered once for all members) and the rows form of the
     draw.  A BC member is K10 with ``partner_seat`` where ``member == k`` and -1 elsewhere.  Every member keeps its own
     counter, advanced by one per transition whatever its share, so member k draws in environment e what the pair
-    ``(learner, m_k)`` draws there.  ``member``: fixed, or drawn per episode from ``weights`` (``ovc_assign_members``)."""
+    ``(learner, m_k)`` draws there.  ``member``: fixed, or drawn per episode from ``weights`` (``ovc_assign_members``).
+    ``mixture`` (``SelfPlayRollout``'s partner): ``partner_seat[e]`` is -1 in self-play environments, which no member may
+    write; the grouping key is then ``member[e]`` where ``partner_seat[e] >= 0`` and K elsewhere, and group K never runs."""
 
     lstm = False
 
-    def __init__(self, env, members, partner_seat, seed, autocast_dtype, member=None, weights=None):
+    def __init__(self, env, members, partner_seat, seed, autocast_dtype, member=None, weights=None, mixture=False):
         N, dev = env.n_envs, env.device
         self.env, self.K, self.seed, self.partner_seat = env, len(members), int(seed), partner_seat
         self.agents = [_BCAgent(env, m, 1, None, seed) if isinstance(m, BCPolicy)
@@ -1009,7 +1121,9 @@ class _Population(object):
         self._cobs = torch.empty((N, l.width * l.height * 26), dtype=autocast_dtype or torch.float32, device=dev) if self.needs_obs else None
         self._jrows = torch.empty(N, dtype=torch.int32, device=dev)
         self.order = torch.empty(N, dtype=torch.int32, device=dev)
-        self.offsets = torch.zeros(self.K + 1, dtype=torch.int32, device=dev)
+        self.offsets = torch.zeros(self.K + 1 + bool(mixture), dtype=torch.int32, device=dev)
+        self._key = torch.empty(N, dtype=torch.int32, device=dev) if mixture else None  # the grouping key of a mixture
+        self._self_play_key = torch.full((N,), self.K, dtype=torch.int32, device=dev) if mixture else None
         self._counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of the population draw
         if member is not None:
             assert weights is None, "member fixes each environment's member, member_weights draws it: pass one of them"
@@ -1060,10 +1174,16 @@ class _Population(object):
     def act(self, actions):
         env, N = self.env, self.env.n_envs
         lib, stream = _native.lib(), env._stream()
-        env.group_members(self.member, self.K, self.order, self.offsets)
+        if self._key is None:
+            env.group_members(self.member, self.K, self.order, self.offsets)
+        else:
+            torch.where(self.partner_seat >= 0, self.member, self._self_play_key, out=self._key)
+            env.group_members(self._key, self.K + 1, self.order, self.offsets)
         if self._cobs is not None:  # the members' observation rows 2 e + p(e), in compact order, once for all members
             torch.index_select(self.partner_seat, 0, self.order, out=self._jrows)
             self._jrows.add_(self.order, alpha=2)
+            if self._key is not None:  # group K's rows (2 e - 1 at seat -1) are gathered but never read: keep them in bounds
+                self._jrows.clamp_(min=0)
             torch.index_select(self.obs.view(2 * N, -1), 0, self._jrows, out=self._cobs)
         for k, a in enumerate(self.agents):
             rng = self.offsets[k:k + 2]

@@ -273,4 +273,21 @@ for name, fixed in (("cramped_room", False), ("asymmetric_advantages", False), (
     assert b.dones.any() and len(b.episodes.finished()["partner_member"]) > 0
 torch.cuda.synchronize()
 print("population (group / assign members, rows forms of K7 / K9 / K8 and the draw, K10) ok", flush=True)
+# self-play mixtures: ovc_learner_rows, the masked K7, K9 on the compact rows and the joint K8 for the learner, the rows forms
+# for a network partner and a population (a BC member among them) on the paired environments only, on a 5x4 and a 9x5 grid
+for name, partner in (("cramped_room", lambda W, H: RllibShapedCNN(W, H)), ("cramped_room", lambda W, H: [RllibShapedCNN(W, H), BCPolicy()]),
+                      ("asymmetric_advantages", lambda W, H: [RllibShapedCNN(W, H), BCPolicy()])):
+    env11 = BatchedOvercookedEnv(name, 37, horizon=3, auto_reset=True)
+    l11 = env11.layouts[0]
+    W, H = l11.width, l11.height
+    mix = SelfPlayRollout(env11, RllibShapedCNN(W, H), seed=4, use_graph=False, partner=partner(W, H), bc_factor=0.5, episode_capacity=2)
+    st = env11.state.cpu().numpy().copy()
+    for t in range(5):
+        mix.run(1)
+        cpu.step(env11._tab_host, env11._starts_host, st, mix.actions.cpu().numpy(), horizon=3, flags=1)
+    assert np.array_equal(env11.state.cpu().numpy(), st)
+    b = mix.collect(5, 0.99, 0.95)
+    assert b.dones.any() and (b.partner_seat == -1).any() and (b.partner_seat >= 0).any()
+torch.cuda.synchronize()
+print("self-play mixtures (learner rows, masked K7, joint K8, partner rows forms) ok", flush=True)
 print("sanitize_smoke: all ok")
