@@ -40,13 +40,14 @@ ap.add_argument("--vf-coef", type=float, default=1e-4)
 ap.add_argument("--entropy-coef", type=float, default=0.1)
 ap.add_argument("--shaping-horizon", type=float, default=2.5e6, help="env-steps over which the shaping factor anneals 1 -> 0")
 ap.add_argument("--seed", type=int, default=0)
+ap.add_argument("--use-phi", action="store_true", help="the potential-based dense reward (use_phi) instead of the shaped rewards")
 args = ap.parse_args()
 
 torch.manual_seed(args.seed)
 env = BatchedOvercookedEnv("cramped_room", args.envs, horizon=400, auto_reset=True)
 W, H = env.layouts[0].width, env.layouts[0].height
 model = RllibShapedCNN(W, H).cuda()
-sp = SelfPlayRollout(env, model=model, seed=args.seed)
+sp = SelfPlayRollout(env, model=model, seed=args.seed, use_phi=args.use_phi)
 opt = torch.optim.Adam(model.parameters(), lr=args.lr)
 N, T = env.n_envs, args.steps
 env_steps = 0

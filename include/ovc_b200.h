@@ -757,6 +757,35 @@ int ovc_potential(const void *layouts, int n_layouts, const void *pot_tables, co
                   int state_words, void *stream);
 size_t ovc_potential_table_size(void);
 
+/*
+ * The potential-based dense reward (human_aware_rl's use_phi, rllib.py:314-329): both agents get
+ *     reward = sparse + factor * dense,   dense = (float)(phi(s') - phi(s))
+ * with phi = potential_function at gamma 0.99 (the value get_state_transition(display_phi=True) reports, MDP:1422-1429),
+ * s the record before the transition and s' the record after it, BEFORE a finishing episode is reset.  A transition is
+ *     ovc_potential (phi_s = phi(s)) -> ovc_step without OVC_F_AUTO_RESET -> ovc_potential_shaping -> ovc_record_transition_dense
+ *
+ * ovc_potential_shaping: per environment e, with the tables and gpow of ovc_potential and the records ovc_step left:
+ *     dense[e] = (float)(phi(state[e]) - phi_s[e])     the float64 difference rounded once; float32 [n_envs]
+ *   then, where done[e] != 0 (ovc_step's int32 done), state[e] is reset as OVC_F_AUTO_RESET inside ovc_step would reset it:
+ *   the start record of its layout (word 3), or with random_start the random start of the next episode (layout drawn with
+ *   random_layout, episode counter + 1, env index e).  phi_s float64 [n_envs] (8-byte aligned), done and dense 4-byte aligned;
+ *   n_pow >= 2.
+ * ovc_record_transition_dense: ovc_record_transition (stats NULL) or ovc_record_transition_stats (stats given) with the
+ *   reward of both agents taken from dense (float32 [n_envs], 4-byte aligned) instead of shaped, each operation rounded
+ *   to float32 on its own:
+ *     r[e] = (float)sparse[e] + factor * dense[e];  rewards[2 e + i] = r[e] (one_view 0, [n_envs][2], 8-byte aligned) or
+ *     rewards[e] = r[e] (one_view 1, [n_envs], 4-byte aligned; an agent pair's learner: no seat, both rewards are equal);
+ *     ret_mixed[e] = ((ret_mixed[e] + (float)sparse[e]) + factor * dense[e]) + factor * dense[e]
+ *   rewards nullable; reward_by_agent sums r[e] for both agents; shaped feeds shaped_by_agent, and dones, ret_sparse, the
+ *   other statistics and the records are exactly what those calls write.
+ */
+int ovc_potential_shaping(const void *layouts, int n_layouts, const int32_t *start_records, const void *pot_tables, const void *cost_lut,
+                          const double *gpow, int n_pow, int32_t *state, const int32_t *done, const double *phi_s, float *dense,
+                          int64_t n_envs, int state_words, const ovc_random_start_t *random_start, void *stream);
+int ovc_record_transition_dense(const int32_t *sparse, const int32_t *shaped, const float *dense, const int32_t *done, const float *factor,
+                                int64_t n_envs, int one_view, float *rewards, uint8_t *dones, int64_t *ret_sparse, float *ret_mixed,
+                                const ovc_episode_stats_t *stats, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -109,12 +109,13 @@ class BatchedOvercookedEnv(object):
                                            int(self.random_layout), 0)
         self._lut = None
         self._segments = None
+        self._pot = {}  # gamma -> potential tables; never dropped, so a captured graph's tables stay alive
         with torch.cuda.device(self.device):
             self.reset()
 
     # ---------------------------------------------------------------------------------------------
-    def _flags(self):
-        return ((_native.F_AUTO_RESET if self.auto_reset else 0) | (_native.F_PDL if self.pdl else 0)
+    def _flags(self, auto_reset=None):
+        return ((_native.F_AUTO_RESET if (self.auto_reset if auto_reset is None else auto_reset) else 0) | (_native.F_PDL if self.pdl else 0)
                 | (self.io << _native.F_IO_SHIFT))
 
     def _rs_ptr(self):
@@ -137,11 +138,13 @@ class BatchedOvercookedEnv(object):
             self.env_layout.data_ptr(), 0 if mask is None else mask.data_ptr(), self.n_envs, self.state_words,
             self._rs_ptr(), self._stream()))
 
-    def step(self, actions, out=None):
+    def step(self, actions, out=None, auto_reset=None):
         """One joint transition of every environment.
 
         actions  int32 CUDA tensor [N, 2], action indices 0..5 (Action.INDEX_TO_ACTION order)
         out      optional (sparse[N], shaped[N,2], done[N], events[N,2]) int32 CUDA tensors to write
+        auto_reset  None: the env's own setting; False: finished episodes keep their terminal record (for
+                 ``potential_shaping``, which takes phi on it and then resets them)
         returns  (sparse, shaped, done, events); without ``out`` these are buffers owned by the env and
                  overwritten by the next call.  ``sparse`` is the summed delivery reward
                  (what OvercookedEnv.step returns), ``shaped`` is shaped_reward_by_agent,
@@ -157,7 +160,7 @@ class BatchedOvercookedEnv(object):
         _native.check(self._lib.ovc_step(
             self.tables.data_ptr(), self.n_layouts, self.start_records.data_ptr(), self.state.data_ptr(),
             actions.data_ptr(), sparse.data_ptr(), shaped.data_ptr(), done.data_ptr(),
-            events.data_ptr(), self.n_envs, self.state_words, self.horizon, self._flags(), self._rs_ptr(), self._stream()))
+            events.data_ptr(), self.n_envs, self.state_words, self.horizon, self._flags(auto_reset), self._rs_ptr(), self._stream()))
         return sparse, shaped, done, events
 
     def narrow_ok(self):
@@ -571,7 +574,7 @@ class BatchedOvercookedEnv(object):
                                                        0 if ret_mixed is None else ret_mixed.data_ptr(), self._stream()))
 
     def record_transition(self, factor, rewards=None, dones=None, ret_sparse=None, ret_mixed=None, stats=None, records=None,
-                          partner_seat=None):
+                          partner_seat=None, dense=None):
         """What a sample batch keeps of the last ``step`` (ovc_record_transition, one kernel): ``rewards`` float32 [N, 2] =
         sparse + factor * shaped[:, i] per agent (rllib.py:328-329), ``dones`` uint8 [N], and the running returns as
         ``accumulate_returns`` keeps them; each output optional.  ``factor``: float32 CUDA scalar tensor, read by the
@@ -579,23 +582,27 @@ class BatchedOvercookedEnv(object):
         ``stats`` (an ``EpisodeStats``) with ``records`` (an ``EpisodeRecords``): in the same kernel
         (ovc_record_transition_stats), fold the step into the running episode statistics and write every episode that
         ended with it into ``records``; ``partner_seat`` (int32 [N], nullable): the partner's seat each episode was played
-        with, -1 = self-play."""
+        with, -1 = self-play.
+        ``dense`` (float32 [N], ``potential_shaping``'s output): both agents' reward is ``sparse + factor * dense`` instead
+        (use_phi; ovc_record_transition_dense); the shaped rewards still go into the statistics."""
         self._record(self.sparse, self.shaped, self.done, self.events, factor, rewards, dones, ret_sparse, ret_mixed, stats, records,
-                     partner_seat)
+                     partner_seat, dense=dense)
 
     def record_transition_view(self, factor, seat, swap, rewards, dones=None, ret_sparse=None, ret_mixed=None, stats=None, records=None,
-                               partner_seat=None):
+                               partner_seat=None, dense=None):
         """``record_transition`` for ONE agent per environment (ovc_record_transition_view): ``rewards`` float32 [N] is the
         reward of the agent at player ``seat ^ (swap[e] != 0)`` (``swap`` int32 CUDA [N] or None), bit for bit the entry
-        ``record_transition`` writes for that player; everything else as ``record_transition``."""
+        ``record_transition`` writes for that player; everything else as ``record_transition``.  With ``dense`` both agents'
+        rewards are equal, so the one-view form of ovc_record_transition_dense needs no seat."""
         if swap is not None:
             assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == self.n_envs
         self._record(self.sparse, self.shaped, self.done, self.events, factor, rewards, dones, ret_sparse, ret_mixed, stats, records,
-                     partner_seat, view=(int(seat), swap))
+                     partner_seat, view=(int(seat), swap), dense=dense)
 
     def _record(self, sparse, shaped, done, events, factor, rewards=None, dones=None, ret_sparse=None, ret_mixed=None, stats=None,
-                records=None, partner_seat=None, view=None):
+                records=None, partner_seat=None, view=None, dense=None):
         assert factor.is_cuda and factor.dtype == torch.float32 and factor.numel() == 1
+        assert dense is None or (dense.is_cuda and dense.dtype == torch.float32 and dense.is_contiguous() and dense.numel() == self.n_envs)
         for t, dt, n in ((rewards, torch.float32, 1 if view else 2), (dones, torch.uint8, 1), (ret_sparse, torch.int64, 1),
                          (ret_mixed, torch.float32, 1)):
             assert t is None or (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n * self.n_envs)
@@ -619,7 +626,11 @@ class BatchedOvercookedEnv(object):
                 d.rec_event_counts, d.rec_reward_by_agent = records.game_stats.data_ptr(), records.reward_by_agent.data_ptr()
         args = (sparse.data_ptr(), shaped.data_ptr(), done.data_ptr(), factor.data_ptr(), self.n_envs)
         outs = (ptr(rewards), ptr(dones), ptr(ret_sparse), ptr(ret_mixed))
-        if view is not None:
+        if dense is not None:
+            _native.check(self._lib.ovc_record_transition_dense(sparse.data_ptr(), shaped.data_ptr(), dense.data_ptr(), done.data_ptr(),
+                                                                factor.data_ptr(), self.n_envs, int(view is not None), *outs,
+                                                                None if d is None else ctypes.byref(d), self._stream()))
+        elif view is not None:
             seat, swap = view
             _native.check(self._lib.ovc_record_transition_view(*args, ptr(swap), seat, *outs, None if d is None else ctypes.byref(d),
                                                                self._stream()))
@@ -717,23 +728,42 @@ class BatchedOvercookedEnv(object):
             self._stream()))
         return out
 
+    def potential_tables(self, gamma=0.99):
+        """The device tables ``potential`` evaluates phi with at ``gamma`` (potential tables, cost LUT, gamma powers): built
+        on first use and kept for the env's lifetime, so a CUDA graph that captured them never reads freed memory.  Build
+        them before a capture: building copies host data to the device."""
+        if gamma not in self._pot:
+            pt, cl, gpow = L.build_potential_tables(self.layouts, gamma)
+            assert pt.shape[1] == self._lib.ovc_potential_table_size()
+            self._pot[gamma] = (torch.from_numpy(pt).to(self.device), torch.from_numpy(cl).to(self.device),
+                                torch.from_numpy(gpow).to(self.device))
+        return self._pot[gamma]
+
     def potential(self, gamma=0.99, out=None):
         """potential_function (overcooked_mdp.py:2920-3250) of every environment: float64 [N], bit-identical
         to the reference's Python floats (planner costs from the default NO_COUNTERS_PARAMS planner)."""
-        if getattr(self, "_pot_gamma", None) != gamma:
-            pt, cl, gpow = L.build_potential_tables(self.layouts, gamma)
-            assert pt.shape[1] == self._lib.ovc_potential_table_size()
-            self._pot = (torch.from_numpy(pt).to(self.device), torch.from_numpy(cl).to(self.device),
-                         torch.from_numpy(gpow).to(self.device))
-            self._pot_gamma = gamma
+        pt, cl, gpow = self.potential_tables(gamma)
         if out is None:
             out = torch.empty(self.n_envs, dtype=torch.float64, device=self.device)
         assert out.dtype == torch.float64 and out.is_cuda and out.is_contiguous() and out.numel() == self.n_envs
-        pt, cl, gpow = self._pot
         _native.check(self._lib.ovc_potential(
             self.tables.data_ptr(), self.n_layouts, pt.data_ptr(), cl.data_ptr(), gpow.data_ptr(), gpow.numel(),
             self.state.data_ptr(), out.data_ptr(), self.n_envs, self.state_words, self._stream()))
         return out
+
+    def potential_shaping(self, phi_s, dense):
+        """The dense reward of the last ``step(..., auto_reset=False)`` (ovc_potential_shaping, one kernel):
+        ``dense[e] = float32(phi(s') - phi_s[e])`` with phi at gamma 0.99 on the record the step left (the terminal one where
+        an episode ended), then every environment with ``done`` is reset as ``auto_reset`` would have reset it.
+        ``phi_s``: float64 [N], ``potential(0.99)`` taken before the step; ``dense``: float32 [N], written."""
+        assert phi_s.is_cuda and phi_s.dtype == torch.float64 and phi_s.is_contiguous() and phi_s.numel() == self.n_envs
+        assert dense.is_cuda and dense.dtype == torch.float32 and dense.is_contiguous() and dense.numel() == self.n_envs
+        pt, cl, gpow = self.potential_tables(0.99)
+        _native.check(self._lib.ovc_potential_shaping(
+            self.tables.data_ptr(), self.n_layouts, self.start_records.data_ptr(), pt.data_ptr(), cl.data_ptr(), gpow.data_ptr(),
+            gpow.numel(), self.state.data_ptr(), self.done.data_ptr(), phi_s.data_ptr(), dense.data_ptr(), self.n_envs,
+            self.state_words, self._rs_ptr(), self._stream()))
+        return dense
 
     # ---------------------------------------------------------------------------------------------
     def sparse_by_agent(self, events, layout_ids=None):

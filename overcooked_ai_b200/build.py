@@ -9,7 +9,7 @@ import sys
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 SOURCES = ["ovc_b200.cu"]
-DEPS = ["ovc_b200.cu", "ovc_step.cuh", "ovc_obs.cuh", "ovc_encfc.cuh", "ovc_tail.cuh", "ovc_wide.cuh", "ovc_partner.cuh", "ovc_lstm.cuh", "ovc_potential.cuh", "ovc_rng.cuh", "ovc_host.cuh", "ovc_rollout.cuh", os.path.join("..", "..", "include", "ovc_b200.h")]
+DEPS = ["ovc_b200.cu", "ovc_step.cuh", "ovc_obs.cuh", "ovc_encfc.cuh", "ovc_tail.cuh", "ovc_wide.cuh", "ovc_partner.cuh", "ovc_lstm.cuh", "ovc_potential.cuh", "ovc_potential_phi.inc", "ovc_rng.cuh", "ovc_host.cuh", "ovc_rollout.cuh", os.path.join("..", "..", "include", "ovc_b200.h")]
 OUT = os.path.join(CSRC, "libovc_b200.so")
 
 NVCC_FLAGS = [

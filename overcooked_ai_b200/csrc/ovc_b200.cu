@@ -975,6 +975,23 @@ int ovc_potential(const void *layouts, int n_layouts, const void *pot_tables, co
 }
 size_t ovc_potential_table_size(void) { return sizeof(ovc_potential_t); }
 
+int ovc_potential_shaping(const void *layouts, int n_layouts, const int32_t *start_records, const void *pot_tables, const void *cost_lut,
+                          const double *gpow, int n_pow, int32_t *state, const int32_t *done, const double *phi_s, float *dense,
+                          int64_t n_envs, int state_words, const ovc_random_start_t *random_start, void *stream) {
+    int rc = ovc::check_common(layouts, n_layouts, state, n_envs, state_words);
+    if (rc) return rc;
+    return ovc::potential_shaping_impl((const ovc_layout_t *)layouts, n_layouts, start_records, (const ovc_potential_t *)pot_tables,
+                                       (const ovc_cost_lut_entry_t *)cost_lut, gpow, n_pow, state, done, phi_s, dense, n_envs, state_words,
+                                       random_start, (cudaStream_t)stream);
+}
+
+int ovc_record_transition_dense(const int32_t *sparse, const int32_t *shaped, const float *dense, const int32_t *done, const float *factor,
+                                int64_t n_envs, int one_view, float *rewards, uint8_t *dones, int64_t *ret_sparse, float *ret_mixed,
+                                const ovc_episode_stats_t *stats, void *stream) {
+    return ovc::record_transition_dense_impl(sparse, shaped, dense, done, factor, n_envs, one_view, rewards, dones, (long long *)ret_sparse,
+                                             ret_mixed, stats, (cudaStream_t)stream);
+}
+
 int ovc_pipeline_create(const ovc_pipeline_desc_t *desc, ovc_pipeline_t **out) { return ovc::pipeline_create(desc, out); }
 int ovc_pipeline_run(ovc_pipeline_t *p, const void *h_actions, void *h_sparse, void *h_shaped, void *h_done, void *h_events,
                      int n_steps, void *stream, int join, int64_t *ticket) {

@@ -720,6 +720,51 @@ static int record_transition_view_impl(const int32_t *sparse, const int32_t *sha
     return OVC_OK;
 }
 
+// ovc_record_transition_dense: accumulate_returns_kernel's transition with the potential-based dense reward (use_phi,
+// rllib.py:314-319): both agents get sparse + f * dense[e], every operation rounded on its own.  shaped still feeds the
+// game statistics.  ONE_VIEW: rewards [n_envs] (the agents' rewards are equal, so no seat is needed), else [n_envs][2].
+template <bool STATS, bool ONE_VIEW>
+__global__ void __launch_bounds__(256) record_transition_dense_kernel(const int32_t *__restrict__ sparse, const int32_t *__restrict__ shaped,
+                                                                      const float *__restrict__ dense, long long n_envs,
+                                                                      long long *__restrict__ ret_sparse, float *__restrict__ ret_mixed,
+                                                                      const float *__restrict__ factor_dev, const int32_t *__restrict__ done,
+                                                                      float *__restrict__ rewards, uint8_t *__restrict__ dones,
+                                                                      const ovc_episode_stats_t stats) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n_envs) return;
+    const float f = *factor_dev;
+    const int sp = sparse[e];
+    const float fd = __fmul_rn(f, dense[e]);
+    const float r = __fadd_rn((float)sp, fd);
+    if (ret_sparse) ret_sparse[e] += sp;
+    if (ret_mixed) ret_mixed[e] = __fadd_rn(__fadd_rn(__fadd_rn(ret_mixed[e], (float)sp), fd), fd);
+    if (rewards) {
+        if (ONE_VIEW) rewards[e] = r;
+        else reinterpret_cast<float2 *>(rewards)[e] = make_float2(r, r);
+    }
+    if (dones) dones[e] = done[e] != 0;
+    if constexpr (STATS) episode_stats_update(stats, e, n_envs, reinterpret_cast<const int2 *>(shaped)[e], r, r, done[e] != 0);
+}
+
+static int record_transition_dense_impl(const int32_t *sparse, const int32_t *shaped, const float *dense, const int32_t *done,
+                                        const float *factor_dev, long long n_envs, int one_view, float *rewards, uint8_t *dones,
+                                        long long *ret_sparse, float *ret_mixed, const ovc_episode_stats_t *stats, cudaStream_t st) {
+    if (!factor_dev || !dense) return fail(OVC_E_BADARG, "null pointer argument");
+    if (int rc = check_record_args(sparse, shaped, n_envs, done, dones, stats)) return rc;
+    if (one_view != 0 && one_view != 1) return fail(OVC_E_BADARG, "one_view must be 0 or 1", one_view);
+    if (((uintptr_t)dense & 3) || ((uintptr_t)rewards & (one_view ? 3 : 7)))
+        return fail(OVC_E_BADARG, "dense must be 4-byte aligned, rewards 4-byte (one view) or 8-byte (two rows)");
+    if (n_envs == 0) return OVC_OK;
+    const unsigned grid = (unsigned)((n_envs + 255) / 256);
+    const ovc_episode_stats_t s = stats ? *stats : ovc_episode_stats_t{};
+    auto kern = stats ? (one_view ? record_transition_dense_kernel<true, true> : record_transition_dense_kernel<true, false>)
+                      : (one_view ? record_transition_dense_kernel<false, true> : record_transition_dense_kernel<false, false>);
+    kern<<<grid, 256, 0, st>>>(sparse, shaped, dense, n_envs, ret_sparse, ret_mixed, factor_dev, done, rewards, dones, s);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "record_transition_dense kernel launch");
+    return OVC_OK;
+}
+
 // Generalized advantage estimation over a window of T transitions (the postprocessing of RLlib's PPO sample batches),
 // one thread per environment holding its two agent rows, walking t backwards.  Every operation is rounded on its own
 // (no FMA contraction) in the order ovc_gae documents, so a float32 loop on the host reproduces it bit for bit.  A

@@ -31,160 +31,7 @@ __global__ void __launch_bounds__(128) potential_kernel(const PotArgs a) {
     const long long env = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (env >= a.n_envs) return;
     const int32_t *__restrict__ rec = a.state + env * a.S;
-    const int4 h = __ldg(reinterpret_cast<const int4 *>(rec));
-    const int lid = h.w & 0xFF;
-    const ovc_layout_t *__restrict__ L = a.layouts + lid;
-    const ovc_potential_t *__restrict__ P = a.pt + lid;
-    const ovc_cost_lut_entry_t *__restrict__ C = a.cost + (size_t)lid * 1024;
-    const int n_pots = __ldg(&L->n_pots);
-    const int max_del = __ldg(&P->max_delivery_steps), max_pick = __ldg(&P->max_pickup_steps);
-    const unsigned pl[2] = {(unsigned)h.y, (unsigned)h.z};
-
-    // planner costs of both players: one 8-byte entry each (serve, pot[0..3])
-    unsigned long long ce[2];
-#pragma unroll
-    for (int i = 0; i < 2; i++)
-        ce[i] = __ldg(reinterpret_cast<const unsigned long long *>(C + (((pl[i] & 0xFF) << 2) | ((pl[i] >> 8) & 3))));
-    auto cost_of = [&](int player, int which) {  // which 0 = serve, 1 + k = pot k; OVC_BIG if unreachable
-        const int c = (int)((ce[player] >> (8 * which)) & 0xFF);
-        return c == OVC_COST_INF ? OVC_BIG : c;
-    };
-
-    // pot words and their classes (get_pot_states :1809-1838)
-    unsigned pw[OVC_MAX_POTS];
-    int cls[OVC_MAX_POTS];  // 0 empty, 1..3 idle with that many items, 4 cooking, 5 ready
-    int remaining[OVC_MAX_POTS], row[OVC_MAX_POTS];
-#pragma unroll
-    for (int k = 0; k < OVC_MAX_POTS; k++) {
-        pw[k] = k < n_pots ? (unsigned)__ldg(rec + 4 + k) : 0u;
-        cls[k] = 0, remaining[k] = 0, row[k] = 0;
-        if ((pw[k] & 7) == OVC_O_SOUP) {
-            const int n = (pw[k] >> 3) & 3;
-            const int tp1 = (pw[k] >> 8) & 0x3FFF;
-            row[k] = recipe_row(pw[k]);
-            if (tp1 == 0) cls[k] = n;  // n == 0 cannot persist
-            else {
-                remaining[k] = __ldg(&L->cook_time[row[k]]) - (tp1 - 1);
-                cls[k] = remaining[k] <= 0 ? 5 : 4;
-            }
-        }
-    }
-
-    double potential = __ldg(&P->steady);  // :2985-2999
-
-    // player masks by held object (:3047-3070)
-    unsigned m_soup = 0, m_dish = 0, m_tom = 0, m_oni = 0, m_none = 0;
-#pragma unroll
-    for (int i = 0; i < 2; i++) {
-        const int t = (pl[i] >> 10) & 7;
-        m_soup |= (unsigned)(t == OVC_O_SOUP) << i, m_dish |= (unsigned)(t == OVC_O_DISH) << i;
-        m_tom |= (unsigned)(t == OVC_O_TOMATO) << i, m_oni |= (unsigned)(t == OVC_O_ONION) << i;
-        m_none |= (unsigned)(t == OVC_O_NONE) << i;
-    }
-
-    // ---- step 4: players holding a soup (:3075-3084) ----
-#pragma unroll
-    for (int i = 0; i < 2; i++)
-        if ((m_soup >> i) & 1) {
-            const int v = max(__ldg(&L->deliver_value[recipe_row(pl[i] >> 10)]), 1);
-            potential = __dadd_rn(potential, __dmul_rn(gpw(a, min(cost_of(i, 0), max_del)), (double)v));
-        }
-
-    // ---- step 3: non-idle soups, cooking ones first then ready ones, each in pot order (:3026-3043) ----
-    int non[OVC_MAX_POTS], n_non = 0;
-    double val[OVC_MAX_POTS];
-    for (int pass = 4; pass <= 5; pass++)
-        for (int k = 0; k < n_pots; k++)
-            if (cls[k] == pass) {
-                const int v = max(__ldg(&L->deliver_value[row[k]]), 1);
-                val[n_non] = __dmul_rn(gpw(a, max_del + max(max_pick, remaining[k])), (double)v);
-                non[n_non++] = k;
-            }
-#pragma unroll
-    for (int i = 0; i < 2; i++)
-        if ((m_dish >> i) & 1) {  // :3089-3128
-            int best = -1;
-            double best_value = 0.0;
-            for (int j = 0; j < n_non; j++) {
-                const int k = non[j];
-                const int pd = cost_of(i, 1 + k);
-                if (pd >= OVC_BIG) continue;  // is_useful == 0: value 0, never selected
-                const int v = max(__ldg(&L->deliver_value[row[k]]), 1);
-                const double psv = __dmul_rn(gpw(a, max_del), (double)v);
-                const double disc = gpw(a, max(remaining[k], min(pd, max_pick)));
-                const double pv = __dmul_rn(__dmul_rn(disc, psv), 1.0);
-                if (pv > best_value) best = j, best_value = pv;
-            }
-            if (best >= 0 && best_value > val[best]) val[best] = best_value;
-        }
-    for (int j = 0; j < n_non; j++) potential = __dadd_rn(potential, val[j]);
-
-    // ---- step 2: idle soups (:3002-3022, :3137-3210) ----
-    int idle[OVC_MAX_POTS], n_idle = 0, code = 0, p3 = 1;
-    for (int k = 0; k < n_pots; k++) {
-        if (cls[k] == 3) idle[n_idle++] = k;
-        code += (cls[k] == 1 ? 1 : cls[k] == 2 ? 2 : 0) * p3;
-        p3 *= 3;
-    }
-    {
-        const unsigned ord = __ldg(reinterpret_cast<const unsigned *>(&P->partial_order[code][0]));
-        for (int j = 0; j < 4; j++) {
-            const int s = (ord >> (8 * j)) & 0xFF;
-            if (s == OVC_NO_SLOT) break;
-            idle[n_idle++] = s;
-        }
-    }
-    for (int i = 1; i < n_idle; i++)  // stable, descending by the discounted value of the best reachable recipe
-        for (int j = i; j > 0 && __ldg(&P->disc_value[row[idle[j - 1]]]) < __ldg(&P->disc_value[row[idle[j]]]); j--) {
-            const int t = idle[j];
-            idle[j] = idle[j - 1], idle[j - 1] = t;
-        }
-    for (int q = 0; q < n_idle; q++) {
-        const int k = idle[q];
-        const int cur = row[k], opt = __ldg(&P->opt_recipe[cur]);
-        const int miss_on = (opt >> 2) - (cur >> 2), miss_to = (opt & 3) - (cur & 3);
-        double disc = gpw(a, max(max_pick, __ldg(&L->cook_time[opt])) + max_del);
-        for (int m = 0; m < miss_on + miss_to; m++) {  // sorted ingredient tuple: onions, then tomatoes
-            const bool tom = m >= miss_on;
-            unsigned &mask = tom ? m_tom : m_oni;
-            int dist = OVC_BIG, who = -1;
-#pragma unroll
-            for (int i = 0; i < 2; i++)
-                if ((mask >> i) & 1) {
-                    const int cd = cost_of(i, 1 + k);
-                    if (cd < dist) dist = cd, who = i;
-                }
-            disc = __dmul_rn(disc, gpw(a, min(dist, tom ? __ldg(&P->pot_tomato_steps) : __ldg(&P->pot_onion_steps))));
-            if (who >= 0) mask &= ~(1u << who);  // that player's ingredient is spoken for
-        }
-        if (miss_on + miss_to > 0) {
-            disc = __dmul_rn(disc, gpw(a, 1));
-        } else {
-            int cook_dist = OVC_BIG;
-#pragma unroll
-            for (int i = 0; i < 2; i++)
-                if ((m_none >> i) & 1) cook_dist = min(cook_dist, cost_of(i, 1 + k));
-            disc = __dmul_rn(disc, gpw(a, min(cook_dist, max_pick)));
-        }
-        potential = __dadd_rn(potential, __dmul_rn(disc, (double)max(__ldg(&L->deliver_value[opt]), 1)));
-    }
-
-    // ---- step 1: left-over ingredients and the closest EMPTY pot (:3215-3247) ----
-    for (int pass = 0; pass < 2; pass++) {
-        const unsigned mask = pass == 0 ? m_tom : m_oni;
-#pragma unroll
-        for (int i = 0; i < 2; i++)
-            if ((mask >> i) & 1) {
-                int dist = OVC_BIG;
-                for (int k = 0; k < n_pots; k++)
-                    if (cls[k] == 0) dist = min(dist, cost_of(i, 1 + k));
-                const int steps = pass == 0 ? __ldg(&P->pot_tomato_steps) : __ldg(&P->pot_onion_steps);
-                const double useful = dist < OVC_BIG ? 1.0 : 0.0;
-                const double disc = __dmul_rn(gpw(a, min(steps, dist) + max_pick + max_del), useful);
-                const int value = pass == 0 ? __ldg(&P->tomato_value) : __ldg(&P->onion_value);
-                potential = __dadd_rn(potential, __dmul_rn(disc, (double)value));
-            }
-    }
+#include "ovc_potential_phi.inc"
     a.out[env] = potential;
 }
 
@@ -198,6 +45,68 @@ static int potential_impl(const ovc_layout_t *layouts, const ovc_potential_t *pt
     potential_kernel<<<(unsigned)((n_envs + 127) / 128), 128, 0, st>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "potential kernel launch");
+    return OVC_OK;
+}
+
+// ovc_potential_shaping: the potential-based dense reward of the transition ovc_step has just made with auto-reset off,
+// then that auto-reset.  K1 resets a finishing environment inside the step, where phi(s') of the terminal record would be
+// lost; here phi is taken first and the record is reset after.
+struct ShapingArgs {
+    PotArgs p;  // p.state: the records, p.out unused
+    const int32_t *start_records;
+    int32_t *state;
+    const int32_t *done;
+    const double *phi_s;
+    float *dense;
+    int n_layouts;
+    ovc_random_start_t rs;
+};
+
+// RS: compiled with the random-start draw, as K1's RS instantiation.
+template <bool RS>
+__global__ void __launch_bounds__(128) potential_shaping_kernel(const ShapingArgs s) {
+    const long long env = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= s.p.n_envs) return;
+    const int S = s.p.S;
+    const PotArgs &a = s.p;
+    const int32_t *rec = s.state + env * S;
+#include "ovc_potential_phi.inc"
+    s.dense[env] = __double2float_rn(__dsub_rn(potential, s.phi_s[env]));
+    if (s.done[env] == 0) return;
+    // The record was read through the read-only path: those reads are ordered before the reset's stores to it.
+    __threadfence_block();
+    // K1's OVC_F_AUTO_RESET (step_core): the start record of the record's layout, or a random start of the next episode
+    GlobalRec r{s.state + env * S};
+    int nl = lid;  // the layout id of word 3 (h: the record's header, read above)
+    if (RS) {
+        const unsigned episode = (((unsigned)h.w >> 16) + 1u) & 0xFFFFu;
+        if (s.rs.random_layout) nl = random_layout_id(s.rs, (uint64_t)env, episode, s.n_layouts);
+        const ovc_layout_t *Ln = s.p.layouts + nl;
+        random_start_record([&](int w, int32_t v) { r.stw(w, v); }, S, s.start_records + (size_t)nl * S, Ln->cook_time, Ln->free_pos,
+                            Ln->n_free, Ln->n_pots, nl, s.rs, (uint64_t)env, episode);
+    } else {
+        const int4 *__restrict__ src = reinterpret_cast<const int4 *>(s.start_records + (size_t)nl * S);
+#pragma unroll 4
+        for (int c = 0; c < S / 4; c++) r.st4(c, __ldg(src + c));
+    }
+}
+
+static int potential_shaping_impl(const ovc_layout_t *layouts, int n_layouts, const int32_t *start_records, const ovc_potential_t *pt,
+                                  const ovc_cost_lut_entry_t *cost, const double *gpow, int n_pow, int32_t *state, const int32_t *done,
+                                  const double *phi_s, float *dense, long long n_envs, int S, const ovc_random_start_t *rs,
+                                  cudaStream_t st) {
+    if (!start_records || !pt || !cost || !gpow || !done || !phi_s || !dense) return fail(OVC_E_BADARG, "null pointer argument");
+    if (n_pow < 2) return fail(OVC_E_BADARG, "gamma power table too short");
+    if (((uintptr_t)phi_s & 7) != 0) return fail(OVC_E_BADARG, "phi_s must be 8-byte aligned");
+    if ((((uintptr_t)dense | (uintptr_t)done) & 3) != 0) return fail(OVC_E_BADARG, "dense and done must be 4-byte aligned");
+    if (n_envs == 0) return OVC_OK;
+    ShapingArgs a{PotArgs{layouts, pt, cost, gpow, state, nullptr, n_envs, S, n_pow}, start_records, state, done, phi_s, dense, n_layouts,
+                  rs ? *rs : ovc_random_start_t{0, 0, 0}};
+    const unsigned grid = (unsigned)((n_envs + 127) / 128);
+    if (rs) potential_shaping_kernel<true><<<grid, 128, 0, st>>>(a);
+    else potential_shaping_kernel<false><<<grid, 128, 0, st>>>(a);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "potential_shaping kernel launch");
     return OVC_OK;
 }
 

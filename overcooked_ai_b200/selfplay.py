@@ -510,6 +510,32 @@ class _FoldedPolicy(object):
 
 
 
+PHI_GAMMA = 0.99  # the gamma of the reference's use_phi reward (get_state_transition(display_phi=True), MDP:1422-1429)
+
+
+class _PhiReward(object):
+    """use_phi's scratch: phi(s) (float64 [N]) and the dense reward (float32 [N]), both rewritten every transition, so
+    neither is state a captured graph has to restore.  The 0.99 potential tables are built here, never inside a capture."""
+
+    def __init__(self, env):
+        assert env.auto_reset, "use_phi needs an auto_reset environment: ovc_potential_shaping resets every episode that ends"
+        env.potential_tables(PHI_GAMMA)
+        self.phi_s = torch.empty(env.n_envs, dtype=torch.float64, device=env.device)
+        self.dense = torch.empty(env.n_envs, dtype=torch.float32, device=env.device)
+
+
+def _env_step(env, actions, phi):
+    """K1 with its auto-reset; with ``phi`` (a ``_PhiReward``), K6 on s, K1 without the reset, then
+    ovc_potential_shaping (phi(s') on the terminal records, the dense reward, the reset).  Returns the dense reward for
+    the record (None without ``phi``)."""
+    if phi is None:
+        env.step(actions)  # K1 (auto-reset inside)
+        return None
+    env.potential(PHI_GAMMA, out=phi.phi_s)  # K6
+    env.step(actions, auto_reset=False)
+    return env.potential_shaping(phi.phi_s, phi.dense)
+
+
 def _capture_graph(env, live, warm_up, body):
     """A CUDA graph of ``body``, captured after ``warm_up`` (on a side stream).  The tensors ``live`` (what warm-up and
     capture advance: the state, returns, statistics, counters...) are restored after them."""
@@ -537,7 +563,7 @@ class SelfPlayRollout(_FoldedPolicy):
 
     def __init__(self, env, model=None, autocast_dtype=torch.bfloat16, use_graph=True, reward_shaping_factor=1.0,
                  fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0, episode_capacity=1,
-                 max_seq_len=20, member=None, member_weights=None):
+                 max_seq_len=20, member=None, member_weights=None, use_phi=False):
         """autocast_dtype: the dtype of the dense model (``DenseGridPolicy``, widths padded to 16-byte rows) and of the
         observation K2 writes for it: bfloat16 (the plane values are exact in bf16), or None for float32 throughout.
         fused_first_layer (default: on for the bf16 policy where ``fused_kernel_support`` allows K7): the observation is
@@ -580,8 +606,14 @@ class SelfPlayRollout(_FoldedPolicy):
         an ``env.reset()`` outside run() / collect(), call ``reset_state()``.  It needs the bf16 policy.  The LSTM's tables
         are folded from the float32 model (the gate bias is one float32 sum of its two biases).
         max_seq_len: RLlib's model-config key for the LSTM policy: collect() records the state every ``max_seq_len``
-        transitions (``SampleBatch.state_h`` / ``state_c``)."""
+        transitions (``SampleBatch.state_h`` / ``state_c``).
+        use_phi: the reference's potential-based dense reward (rllib.py:314-329): both agents get ``sparse +
+        reward_shaping_factor * (phi(s') - phi(s))``, phi at gamma 0.99 with s' taken before an ending episode's reset,
+        instead of ``sparse + reward_shaping_factor * shaped_i``.  Only the rewards, the returns, the advantages, the value
+        targets and the episodes' reward sums change; the draws, the states and the game statistics are those without it.
+        Needs an ``auto_reset`` env."""
         self.env = env
+        self._phi = _PhiReward(env) if use_phi else None
         self._fold(env, model, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
         dev = env.device
         N = env.n_envs
@@ -847,13 +879,13 @@ class SelfPlayRollout(_FoldedPolicy):
                 if self.population:
                     b.partner_member[t].copy_(self._pop.member)
             self._partner_act(actions)  # K10, or the network partner / the population
-        env.step(actions.view(env.n_envs, 2))  # K1 (auto-reset inside)
+        dense = _env_step(env, actions.view(env.n_envs, 2), self._phi)
         if self.population:  # before the record: both use the slot count[e] the ending episode goes to
             self._pop.assign(env.done, self.episodes if b is None else b.episodes)
         # the seat draw below runs after this kernel, so partner_seat is still the ending episode's
         env.record_transition(self._factor, rewards=rewards, dones=dones, ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed,
                               stats=self.stats, records=self.episodes if b is None else b.episodes,
-                              partner_seat=None if self.partner is None else self.partner_seat)
+                              partner_seat=None if self.partner is None else self.partner_seat, dense=dense)
         if self.partner is not None:
             self._assign_partners(env.done)
 
@@ -1252,11 +1284,14 @@ class AgentPairRollout(object):
     inside), ``record_transition`` with the episode statistics (``record_transition_view`` of agent 0's row in collect()),
     then, with random_seats, the seat draw.  With a population, agent 1's step is ``ovc_group_members`` and each member's
     kernels on its own environments, and ``ovc_assign_members`` (the ending episodes' member, the new draw) runs between
-    K1 and the record.  ``ret_sparse`` is the running sparse return of every environment."""
+    K1 and the record.  ``ret_sparse`` is the running sparse return of every environment.
+    use_phi: as ``SelfPlayRollout``'s: both agents' rewards are the potential-based dense reward (K6 before K1, K1 without
+    the reset, ovc_potential_shaping after it)."""
 
     def __init__(self, env, agents, swap=None, seed=0, use_graph=True, episode_capacity=1, autocast_dtype=torch.bfloat16,
-                 random_seats=False, max_seq_len=20, member=None, member_weights=None):
+                 random_seats=False, max_seq_len=20, member=None, member_weights=None, use_phi=False):
         assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per rollout (group envs by layout)"
+        self._phi = _PhiReward(env) if use_phi else None
         assert len(agents) == 2, "agents: (agent0, agent1)"
         assert not (random_seats and swap is not None), "random_seats draws the seats: pass no swap tensor with it"
         assert not isinstance(agents[0], (list, tuple)), "a population plays agent 1 only: agents = (agent0, [m_0, ..., m_K-1])"
@@ -1371,15 +1406,15 @@ class AgentPairRollout(object):
             if self.population:
                 b.partner_member[t].copy_(partner.member)
         partner.act(self.actions)
-        env.step(self.actions)  # K1 (auto-reset inside)
+        dense = _env_step(env, self.actions, self._phi)
         if self.population:  # before the record: both use the slot count[e] the ending episode goes to
             partner.assign(env.done, self.episodes if b is None else b.episodes)
         if b is None:
             env.record_transition(self._factor, ret_sparse=self.ret_sparse, stats=self.stats, records=self.episodes,
-                                  partner_seat=self.partner_seat)
+                                  partner_seat=self.partner_seat, dense=dense)
         else:
             env.record_transition_view(self._factor, learner.seat, learner.swap, b.rewards[t], dones=b.dones[t], ret_sparse=self.ret_sparse,
-                                       stats=self.stats, records=b.episodes, partner_seat=self.partner_seat)
+                                       stats=self.stats, records=b.episodes, partner_seat=self.partner_seat, dense=dense)
         if self.random_seats:  # after the record: the ending episode's seats went into it
             self._assign_seats(env.done)
             for a in self.agents:

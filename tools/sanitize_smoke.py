@@ -290,4 +290,20 @@ for name, partner in (("cramped_room", lambda W, H: RllibShapedCNN(W, H)), ("cra
     assert b.dones.any() and (b.partner_seat == -1).any() and (b.partner_seat >= 0).any()
 torch.cuda.synchronize()
 print("self-play mixtures (learner rows, masked K7, joint K8, partner rows forms) ok", flush=True)
+# use_phi: K6 before K1, K1 without the auto-reset, ovc_potential_shaping (standard and random starts), both forms of
+# ovc_record_transition_dense with the episode statistics
+for kw in ({}, dict(random_start_pos=True, rnd_obj_prob_thresh=0.5, seed=3)):
+    env12 = BatchedOvercookedEnv("cramped_room", 37, horizon=3, auto_reset=True, **kw)
+    phi = SelfPlayRollout(env12, RllibShapedCNN(5, 4), seed=4, use_graph=False, use_phi=True, episode_capacity=2)
+    st = env12.state.cpu().numpy().copy()
+    for t in range(5):
+        phi.run(1)
+        cpu.step(env12._tab_host, env12._starts_host, st, phi.actions.cpu().numpy(), horizon=3, flags=1,
+                 rs=cpu.random_start(3, 0.5, True) if kw else None)
+    assert np.array_equal(env12.state.cpu().numpy(), st)
+    assert phi.collect(5, 0.99, 0.95).dones.any()
+    pair = AgentPairRollout(env12, (RllibShapedCNN(5, 4), BCPolicy()), seed=4, use_graph=False, random_seats=True, use_phi=True)
+    assert pair.collect(5, 0.99, 0.95).dones.any()
+torch.cuda.synchronize()
+print("use_phi (K6, K1 without auto-reset, potential shaping, dense record) ok", flush=True)
 print("sanitize_smoke: all ok")
