@@ -4,7 +4,8 @@
 The worker (``SelfPlayRollout.collect``) runs the bf16 policy kernels K7 -> K9 -> K8 and the environments on the GPU
 and returns a ``SampleBatch`` with behaviour log-probabilities, values, per-agent shaped rewards, dones and GAE
 advantages.  The learner is torch autograd on ``RllibShapedCNN`` in float32 over observations re-encoded from the stored
-records (``batch.observations``), with the clipped PPO objective and Adam.  After each iteration ``sync_weights()``
+records (``batch.observations``), with the clipped PPO objective and Adam.  ``--learner records`` trains the folded bf16
+network the rollout runs instead, straight from the records (``batch.forward``: K7 forward, K12 weight gradient).  After each iteration ``sync_weights()``
 folds the updated network back into the kernels' bf16 tables; the captured CUDA graph keeps running.
 
 The behaviour policy is the bf16 fold of the learner's float32 weights, so the importance ratio is not exactly 1 even
@@ -41,6 +42,9 @@ ap.add_argument("--entropy-coef", type=float, default=0.1)
 ap.add_argument("--shaping-horizon", type=float, default=2.5e6, help="env-steps over which the shaping factor anneals 1 -> 0")
 ap.add_argument("--seed", type=int, default=0)
 ap.add_argument("--use-phi", action="store_true", help="the potential-based dense reward (use_phi) instead of the shaped rewards")
+ap.add_argument("--learner", choices=("conv", "records"), default="conv",
+                help="conv: K2's float32 observation through RllibShapedCNN; records: batch.forward, the folded bf16 network "
+                     "evaluated from the stored records (K7 forward, K12 for the first layer's weight gradient)")
 args = ap.parse_args()
 
 torch.manual_seed(args.seed)
@@ -76,8 +80,11 @@ for it in range(args.iters):
         for k in range(0, T * N, args.minibatch):
             idx = perm[k:k + args.minibatch]
             rows = (2 * idx[:, None] + torch.arange(2, device=env.device)).view(-1)  # agent rows 2 (t N + e) + i
-            obs = batch.observations(idx).view(-1, W, H, 26).permute(0, 3, 1, 2)  # (2m, 26, W, H), agent order as rows
-            logits, value = model(obs)
+            if args.learner == "records":
+                logits, value = batch.forward(model, idx)  # rows in the same order
+            else:
+                obs = batch.observations(idx).view(-1, W, H, 26).permute(0, 3, 1, 2)  # (2m, 26, W, H), agent order as rows
+                logits, value = model(obs)
             logp_all = F.log_softmax(logits, dim=-1)
             logp = logp_all.gather(1, actions[rows, None]).squeeze(1)
             ratio = torch.exp(logp - old_logp[rows])

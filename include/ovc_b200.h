@@ -737,6 +737,24 @@ int ovc_policy_tail_joint(const void *x, int64_t n_rows, int k0, float in_slope,
                           int32_t *actions, float *values, float *scores, float *logp, void *stream);
 
 /*
+ * ovc_encode_linear_wgrad (K12): the weight gradient of ovc_encode_linear's layer, from the packed records,
+ *     dwt[f][c] += sum over rows r of enc(r)[f] * dz[r][c]
+ *   enc(r) = lossless_state_encoding of row r's record and view (never materialised), f in the observation's element order
+ *   (x*height + y)*26 + plane, i.e. dwt has the layout of ovc_encode_linear's wt; dz float32 [rows][n_out] is the gradient
+ *   at the layer's pre-activation (for a leaky ReLU layer: the output gradient times 1 or neg_slope).  Rows:
+ *     seat -1: two views, rows = 2 n_records, row 2 m + v is view v of record m (ovc_encode_linear without view_swap);
+ *     seat 0 / 1: one view, rows = n_records, row m is player seat ^ (swap[m] != 0) of record m (ovc_encode_linear_view).
+ *   states int32 [n_records][state_words] (any records, e.g. a sample batch's, gathered); urgency from horizon minus the
+ *   record's timestep, as in ovc_encode_linear.  dwt float32 [width*height*26][n_out] is added to, never overwritten; only
+ *   rows < rows of dz are read.  Accumulation in float32, summation order unspecified (it varies between calls).
+ *   dz and dwt 16-byte aligned, swap (nullable, one view only) 4-byte aligned, n_out a multiple of 64.  At most 8 layouts
+ *   (OVC_E_UNSUPPORTED), one grid shape; OVC_E_UNSUPPORTED for a grid whose 32-column gradient table (width*height*19*128 B)
+ *   does not fit 227 KB of shared memory.  n_records = 0 launches nothing.
+ */
+int ovc_encode_linear_wgrad(const void *layouts, int n_layouts, const int32_t *states, const int32_t *swap, int seat, const float *dz,
+                            float *dwt, int64_t n_records, int state_words, int width, int height, int horizon, int n_out, void *stream);
+
+/*
  * featurize_state (:2579-2898) with the default planner parameters (NO_COUNTERS_PARAMS,
  * planners.py:27-34): out float32[n_envs][2][F],
  * F = 2*(num_pots*10+28), lut = ovc_feat_lut_entry_t[n_layouts][256][4].  view_swap as above.

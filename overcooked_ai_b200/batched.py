@@ -386,47 +386,83 @@ class BatchedOvercookedEnv(object):
             outs.append(o)
         return outs[0] if len(shapes) == 1 else outs
 
-    def encoded_linear(self, wt, bias, out=None, neg_slope=0.2, view_swap=None):
+    def _records(self, states):
+        """(records, count): ``self.state`` or the int32 CUDA records ``states`` [M, S] (e.g. gathered from a sample batch)."""
+        if states is None:
+            return self.state, self.n_envs
+        assert states.dtype == torch.int32 and states.is_cuda and states.is_contiguous() and states.dim() == 2 and \
+            states.shape[1] == self.state_words, "states: int32 CUDA records [M, %d]" % self.state_words
+        return states, states.shape[0]
+
+    def encoded_linear(self, wt, bias, out=None, neg_slope=0.2, view_swap=None, states=None):
         """First policy layer on ``lossless_state_encoding`` without the observation tensor (kernel K7, ovc_encode_linear):
         ``out[2 env + view] = leaky_relu(obs[env, view].flatten() @ wt + bias, neg_slope)`` as bfloat16 ``[2N, n_out]``.
         ``wt``: bfloat16 CUDA tensor ``[W*H*26, n_out]`` (the layer's matrix TRANSPOSED, rows in the observation's own
         element order ``[x][y][plane]`` — for a convolution, the matrix ``selfplay.DenseGridPolicy`` builds), ``bias``
-        float32 ``[n_out]``, ``n_out`` a multiple of 64.  All environments must share one grid shape."""
+        float32 ``[n_out]``, ``n_out`` a multiple of 64.  All environments must share one grid shape.  ``states``: these
+        records (int32 CUDA [M, S]) instead of ``self.state``; N is then M."""
         assert len({(l.width, l.height) for l in self.layouts}) == 1, "one grid shape per call (group envs by layout)"
         W, H = self.layouts[0].width, self.layouts[0].height
+        recs, n = self._records(states)
         assert wt.is_cuda and wt.dtype == torch.bfloat16 and wt.is_contiguous() and wt.shape[0] == W * H * 26, wt.shape
         n_out = wt.shape[1]
         assert bias.is_cuda and bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == n_out
         if view_swap is not None:
-            assert view_swap.dtype == torch.int32 and view_swap.is_cuda and view_swap.is_contiguous() and view_swap.numel() == self.n_envs
+            assert view_swap.dtype == torch.int32 and view_swap.is_cuda and view_swap.is_contiguous() and view_swap.numel() == n
         if out is None:
-            out = torch.empty((2 * self.n_envs, n_out), dtype=torch.bfloat16, device=self.device)
-        assert out.is_cuda and out.dtype == torch.bfloat16 and out.is_contiguous() and out.numel() == 2 * self.n_envs * n_out
+            out = torch.empty((2 * n, n_out), dtype=torch.bfloat16, device=self.device)
+        assert out.is_cuda and out.dtype == torch.bfloat16 and out.is_contiguous() and out.numel() == 2 * n * n_out
         _native.check(self._lib.ovc_encode_linear(
-            self.tables.data_ptr(), self.n_layouts, self.state.data_ptr(), 0 if view_swap is None else view_swap.data_ptr(),
-            wt.data_ptr(), bias.data_ptr(), out.data_ptr(), self.n_envs, self.state_words, W, H,
+            self.tables.data_ptr(), self.n_layouts, recs.data_ptr(), 0 if view_swap is None else view_swap.data_ptr(),
+            wt.data_ptr(), bias.data_ptr(), out.data_ptr(), n, self.state_words, W, H,
             self.horizon if self.horizon > 0 else 2**31 - 1, n_out, float(neg_slope), self._stream()))
         return out
 
-    def encoded_linear_view(self, wt, bias, seat, swap=None, out=None, neg_slope=0.2):
+    def encoded_linear_view(self, wt, bias, seat, swap=None, out=None, neg_slope=0.2, states=None):
         """``encoded_linear`` for one view per environment (ovc_encode_linear_view): ``out[e]`` (bfloat16 ``[N, n_out]``) is
         the view of player ``seat ^ (swap[e] != 0)``, bit for bit the row ``encoded_linear`` writes for that view.  ``swap``:
-        int32 CUDA tensor [N] or None."""
+        int32 CUDA tensor [N] or None.  ``states``: as in ``encoded_linear``."""
         assert len({(l.width, l.height) for l in self.layouts}) == 1, "one grid shape per call (group envs by layout)"
         W, H = self.layouts[0].width, self.layouts[0].height
+        recs, n = self._records(states)
         assert wt.is_cuda and wt.dtype == torch.bfloat16 and wt.is_contiguous() and wt.shape[0] == W * H * 26, wt.shape
         n_out = wt.shape[1]
         assert bias.is_cuda and bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == n_out
         if swap is not None:
-            assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == self.n_envs
+            assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == n
         if out is None:
-            out = torch.empty((self.n_envs, n_out), dtype=torch.bfloat16, device=self.device)
-        assert out.is_cuda and out.dtype == torch.bfloat16 and out.is_contiguous() and out.numel() == self.n_envs * n_out
+            out = torch.empty((n, n_out), dtype=torch.bfloat16, device=self.device)
+        assert out.is_cuda and out.dtype == torch.bfloat16 and out.is_contiguous() and out.numel() == n * n_out
         _native.check(self._lib.ovc_encode_linear_view(
-            self.tables.data_ptr(), self.n_layouts, self.state.data_ptr(), 0 if swap is None else swap.data_ptr(), int(seat),
-            wt.data_ptr(), bias.data_ptr(), out.data_ptr(), self.n_envs, self.state_words, W, H,
+            self.tables.data_ptr(), self.n_layouts, recs.data_ptr(), 0 if swap is None else swap.data_ptr(), int(seat),
+            wt.data_ptr(), bias.data_ptr(), out.data_ptr(), n, self.state_words, W, H,
             self.horizon if self.horizon > 0 else 2**31 - 1, n_out, float(neg_slope), self._stream()))
         return out
+
+    def encoded_linear_wgrad(self, states, dz, dwt, seat=None, swap=None):
+        """The weight gradient of ``encoded_linear``'s layer from the records (kernel K12, ovc_encode_linear_wgrad):
+        ``dwt[f] += sum over rows r of enc(r)[f] * dz[r]``, with ``dwt`` float32 ``[W*H*26, n_out]`` in ``wt``'s layout and
+        ``dz`` float32 ``[rows, n_out]`` the gradient at the layer's pre-activation.  ``states`` int32 CUDA records [M, S].
+        ``seat`` None: both views, rows ``2 m + v`` (``encoded_linear``'s rows); 0 / 1: one view, row m is player
+        ``seat ^ (swap[m] != 0)`` (``encoded_linear_view``'s rows).  Summation order is unspecified.  Returns ``dwt``."""
+        assert len({(l.width, l.height) for l in self.layouts}) == 1, "one grid shape per call (group envs by layout)"
+        W, H = self.layouts[0].width, self.layouts[0].height
+        recs, n = self._records(states)
+        rows = n if seat is not None else 2 * n
+        assert dwt.is_cuda and dwt.dtype == torch.float32 and dwt.is_contiguous() and dwt.dim() == 2 and dwt.shape[0] == W * H * 26, dwt.shape
+        n_out = dwt.shape[1]
+        assert dz.is_cuda and dz.dtype == torch.float32 and dz.is_contiguous() and dz.dim() == 2 and dz.shape[1] == n_out and \
+            dz.shape[0] >= rows, (dz.shape, rows)
+        assert swap is None or seat is not None, "swap goes with a seat (one view)"
+        if swap is not None:
+            assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == n
+        if n == 0:  # nothing to add (an empty tensor's data pointer is null)
+            return dwt
+        _native.check(self._lib.ovc_encode_linear_wgrad(
+            self.tables.data_ptr(), self.n_layouts, recs.data_ptr(), 0 if swap is None else swap.data_ptr(),
+            -1 if seat is None else int(seat), dz.data_ptr(), dwt.data_ptr(), n, self.state_words, W, H,
+            self.horizon if self.horizon > 0 else 2**31 - 1, n_out, self._stream()))
+        return dwt
 
     def sample_actions_view(self, scores, counter, seat, swap=None, seed=0, out=None, logp_out=None):
         """``sample_actions`` for one agent per environment (ovc_sample_actions_view): ``scores`` float32 ``[N, ld]`` (row e:

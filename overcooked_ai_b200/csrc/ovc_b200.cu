@@ -944,6 +944,15 @@ int ovc_encode_linear_masked(const void *layouts, int n_layouts, const int32_t *
                                    height, horizon, n_out, neg_slope, (cudaStream_t)stream, -1, nullptr, nullptr, list, first);
 }
 
+int ovc_encode_linear_wgrad(const void *layouts, int n_layouts, const int32_t *states, const int32_t *swap, int seat, const float *dz,
+                            float *dwt, int64_t n_records, int state_words, int width, int height, int horizon, int n_out, void *stream) {
+    int rc = ovc::check_common(layouts, n_layouts, states, n_records, state_words);
+    if (rc) return rc;
+    if (seat < -1 || seat > 1) return ovc::fail(OVC_E_BADARG, "seat must be -1 (two views), 0 or 1", seat);
+    return ovc::encode_linear_wgrad_impl((const ovc_layout_t *)layouts, n_layouts, states, swap, seat, dz, dwt, n_records, state_words,
+                                         width, height, horizon, n_out, (cudaStream_t)stream);
+}
+
 int ovc_policy_tail_joint(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
                           const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                           float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *jrow, const int32_t *range,

@@ -391,6 +391,253 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
     return OVC_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// K12 encode_linear_wgrad_kernel: the weight gradient of K7's layer, from the same packed records,
+//     dwt[f][c] += sum over rows r of enc(r)[f] * dz[r][c]
+// with enc(r) the lossless encoding of row r's record and view (never materialised) and dz the gradient at the layer's
+// pre-activation.  K7's decomposition read backwards: each dynamic entry (value, feature row) of a row scatters
+// value * dz[r][:] into its row of the gradient; the object entries, held objects included, are shared by both views of a
+// record, so they scatter value * (dz[2m] + dz[2m + 1]) once; the terrain rows of layout l get the column sum of dz over
+// the rows on l, the urgency rows the column sum over the urgent rows.
+//
+// One CTA per SM holds the float32 gradient of its column slice of the 19 dynamic planes in shared memory ([W*H*19][CS],
+// 190 KB on a 5x4 grid at 128 columns; 32 columns reach K7's largest grid).  A warp takes one record at a time; lane l
+// owns columns l, l + 32, ... of the slice (conflict-free shared accesses, coalesced dz loads); lanes decode object slots
+// and pass the entries round by shuffle, as K7 does.  Warps of a CTA meet in shared memory through atomicAdd; each CTA
+// adds its non-zero sums to dwt once, with global reductions.  Summation order is unspecified (it depends on the grid and
+// on scheduling); on operands whose float32 sums are exact in any order the result is exact.
+// ------------------------------------------------------------------------------------------------
+constexpr int WG_SMEM_LIMIT = 227 * 1024;  // sm_90's opt-in shared memory per block: the grids K12 takes are checked against it
+
+struct EncWgradArgs {
+    const ovc_layout_t *layouts;
+    const int32_t *state;     // [n_rec][S]
+    const int32_t *swap;      // one view: nullable
+    const float *dz;          // [n_rec or 2 n_rec][n_out]
+    float *dwt;               // [W*H*26][n_out]
+    long long n_rec;
+    int n_layouts, S, W, H, horizon, n_out, n_workers;
+    int seat;                 // -1: two views (row 2 m + v); 0 / 1: one view (row m, player seat ^ (swap[m] != 0))
+};
+
+static size_t encode_linear_wgrad_smem(int cpl, int n_dyn_rows, int n_layouts) {
+    const size_t CS = 32 * (size_t)cpl;
+    return (size_t)n_dyn_rows * CS * 4 + ((size_t)n_layouts + 1) * CS * 4 + (size_t)n_layouts * (16 * 4 + 2 * 4 + 128 * 2 + 256) + 16;
+}
+
+template <int CPL>
+__device__ __forceinline__ void wg_scatter(float *g_lane, int row, float value, const float d[CPL]) {
+#pragma unroll
+    for (int i = 0; i < CPL; i++) atomicAdd(g_lane + row * (32 * CPL) + 32 * i, value * d[i]);
+}
+
+template <int CPL>
+__global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_wgrad_kernel(const EncWgradArgs a) {
+    constexpr int CS = 32 * CPL;
+    constexpr int NW = EL_THREADS / 32;
+    extern __shared__ __align__(16) char wg_smem[];
+    const int WH = a.W * a.H;
+    const int n_rows = WH * EL_DYN;
+    float *g = reinterpret_cast<float *>(wg_smem);                                       // [n_rows][CS]
+    float *tsum = g + (size_t)n_rows * CS;                                               // [n_layouts][CS]
+    float *urg = tsum + a.n_layouts * CS;                                                // [CS]
+    int *cook = reinterpret_cast<int *>(urg + CS);                                       // [n_layouts][16]
+    int *nslots = cook + a.n_layouts * 16;                                               // [n_layouts][2]
+    unsigned short *srow = reinterpret_cast<unsigned short *>(nslots + a.n_layouts * 2);  // [n_layouts][128]
+    unsigned char *tplane = reinterpret_cast<unsigned char *>(srow + a.n_layouts * 128);  // [n_layouts][256]
+
+    const int n_slices = a.n_out / CS;
+    const int slice = blockIdx.x % n_slices, worker = blockIdx.x / n_slices;
+    const int col0 = slice * CS;
+
+    for (int i = threadIdx.x; i < (n_rows + a.n_layouts + 1) * CS; i += EL_THREADS) g[i] = 0.f;  // g, tsum, urg
+    for (int i = threadIdx.x; i < a.n_layouts * WH; i += EL_THREADS) {
+        const int l = i / WH, cell = i - l * WH, x = cell / a.H, y = cell - x * a.H;
+        tplane[l * 256 + cell] = (unsigned char)((0x000F0A0E0D0C0B00ull >> ((a.layouts[l].cell[(y << 4) | x] & 7) * 8)) & 0xFF);
+    }
+    for (int i = threadIdx.x; i < a.n_layouts * 128; i += EL_THREADS) {
+        const ovc_layout_t *L = a.layouts + (i >> 7);
+        const int pb = L->slot_pos[i & 127];
+        srow[i] = (unsigned short)((((pb & 15) * a.H + (pb >> 4)) * EL_DYN) & 0xFFFF);
+    }
+    for (int i = threadIdx.x; i < a.n_layouts * 16; i += EL_THREADS) cook[i] = a.layouts[i >> 4].cook_time[i & 15];
+    for (int i = threadIdx.x; i < a.n_layouts; i += EL_THREADS) {
+        nslots[2 * i] = a.layouts[i].n_slots;
+        nslots[2 * i + 1] = a.layouts[i].n_pots;
+    }
+    __syncthreads();
+
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float *g_lane = g + lane;
+    const long long stride = (long long)a.n_workers * NW;
+    const int max_slot_chunks = (a.S - 4 + 31) / 32;
+    const bool two = a.seat < 0;
+    // the warp's terrain sum for layout t_lid and its urgency sum, in registers: one shared-memory add per layout change
+    float t_acc[CPL], u_acc[CPL];
+    int t_lid = -1;
+#pragma unroll
+    for (int i = 0; i < CPL; i++) t_acc[i] = 0.f, u_acc[i] = 0.f;
+
+    for (long long m = (long long)worker * NW + warp; m < a.n_rec; m += stride) {
+        const int32_t *__restrict__ rec = a.state + m * a.S;
+        const int4 head = __ldg(reinterpret_cast<const int4 *>(rec));
+        const int lid = head.w & 0xFF;
+        const int n_slots = nslots[2 * lid], n_pots = nslots[2 * lid + 1];
+        const int *ck = cook + lid * 16;
+        const unsigned short *sr = srow + lid * 128;
+        // the rows' gradients in this lane's columns: d0 (view 0, or the one view), d1 (view 1), ds = their sum
+        float d0[CPL], d1[CPL], ds[CPL];
+        const float *dz0 = a.dz + (two ? 2 * m : m) * a.n_out + col0 + lane;
+#pragma unroll
+        for (int i = 0; i < CPL; i++) d0[i] = __ldcs(dz0 + 32 * i);
+        if (two) {
+#pragma unroll
+            for (int i = 0; i < CPL; i++) d1[i] = __ldcs(dz0 + a.n_out + 32 * i), ds[i] = d0[i] + d1[i];
+        } else {
+#pragma unroll
+            for (int i = 0; i < CPL; i++) d1[i] = 0.f, ds[i] = d0[i];
+        }
+        // terrain (per layout) and urgency column sums
+        if (lid != t_lid) {
+            if (t_lid >= 0) {
+#pragma unroll
+                for (int i = 0; i < CPL; i++) atomicAdd(tsum + t_lid * CS + 32 * i + lane, t_acc[i]), t_acc[i] = 0.f;
+            }
+            t_lid = lid;
+        }
+        const bool urgent = a.horizon - head.x < 40;
+#pragma unroll
+        for (int i = 0; i < CPL; i++) {
+            t_acc[i] += ds[i];
+            if (urgent) u_acc[i] += ds[i];
+        }
+        // objects on pots / counters: lane l of chunk c decodes slot 32 c + l; entries travel by shuffle
+        for (int c = 0; c < max_slot_chunks; c++) {
+            if (c * 32 >= n_slots) break;
+            const int slot = c * 32 + lane;
+            unsigned e[4] = {0, 0, 0, 0};
+            if (slot < n_slots) {
+                const unsigned code = (unsigned)__ldg(rec + 4 + slot) & OVC_OBJ_MASK;
+                if (code) el_object(code, sr[slot], slot < n_pots, ck, e);
+            }
+            unsigned msk = __ballot_sync(0xFFFFFFFFu, (e[0] | e[1] | e[2] | e[3]) != 0);
+            while (msk) {
+                const int j = __ffs(msk) - 1;
+                msk &= msk - 1;
+#pragma unroll
+                for (int q = 0; q < 4; q++) {
+                    const unsigned w = __shfl_sync(0xFFFFFFFFu, e[q], j);
+                    if (w & 0xFFFFu) wg_scatter<CPL>(g_lane, (int)(w >> 16), (float)(short)(w & 0xFFFFu), ds);
+                }
+            }
+        }
+        // held objects, at the holder's cell in both views
+        const unsigned p0 = (unsigned)head.y, p1 = (unsigned)head.z;
+        const int cell0 = ((p0 & 15) * a.H + ((p0 >> 4) & 15)) * EL_DYN, cell1 = ((p1 & 15) * a.H + ((p1 >> 4) & 15)) * EL_DYN;
+#pragma unroll
+        for (int j = 0; j < 2; j++) {
+            const unsigned held = (j ? p1 : p0) >> 10;
+            if (held) {
+                unsigned e[4];
+                el_object(held, j ? cell1 : cell0, false, ck, e);
+#pragma unroll
+                for (int q = 0; q < 4; q++)
+                    if (e[q] & 0xFFFFu) wg_scatter<CPL>(g_lane, (int)(e[q] >> 16), (float)(short)(e[q] & 0xFFFFu), ds);
+            }
+        }
+        // each view's own cell / orientation (planes 0, 2..5) and the partner's (planes 1, 6..9)
+        const int ori0 = (p0 >> 8) & 3, ori1 = (p1 >> 8) & 3;
+        auto view = [&](int p, const float d[CPL]) {
+            const int own_cell = p ? cell1 : cell0, oth_cell = p ? cell0 : cell1;
+            const int own_ori = p ? ori1 : ori0, oth_ori = p ? ori0 : ori1;
+            wg_scatter<CPL>(g_lane, own_cell + PL_LOC, 1.f, d);
+            wg_scatter<CPL>(g_lane, own_cell + PL_ORI + own_ori, 1.f, d);
+            wg_scatter<CPL>(g_lane, oth_cell + PL_LOC + 1, 1.f, d);
+            wg_scatter<CPL>(g_lane, oth_cell + PL_ORI + 4 + oth_ori, 1.f, d);
+        };
+        if (two) {
+            view(0, d0);
+            view(1, d1);
+        } else {
+            view(a.seat ^ (a.swap ? (__ldg(a.swap + m) != 0) : 0), d0);
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < CPL; i++) {
+        if (t_lid >= 0) atomicAdd(tsum + t_lid * CS + 32 * i + lane, t_acc[i]);
+        atomicAdd(urg + 32 * i + lane, u_acc[i]);
+    }
+    __syncthreads();
+
+    // flush: the dynamic rows, then each layout's terrain sum at its terrain cells and the urgency sum at every cell
+    for (int i = threadIdx.x; i < n_rows * CS; i += EL_THREADS) {
+        const float v = g[i];
+        if (v != 0.f) {
+            const int r = i / CS, c = i - r * CS;
+            const int cell = r / EL_DYN, d = r - cell * EL_DYN;
+            const int plane = d < 10 ? d : d + 6;
+            atomicAdd(a.dwt + (size_t)(cell * N_PLANES + plane) * a.n_out + col0 + c, v);
+        }
+    }
+    for (int i = threadIdx.x; i < (a.n_layouts + 1) * WH * CS; i += EL_THREADS) {
+        const int l = i / (WH * CS), rem = i - l * WH * CS, cell = rem / CS, c = rem - cell * CS;
+        const int pl = l == a.n_layouts ? (int)PL_URGENCY : (int)tplane[l * 256 + cell];
+        const float v = l == a.n_layouts ? urg[c] : tsum[l * CS + c];
+        if (pl && v != 0.f) atomicAdd(a.dwt + (size_t)(cell * N_PLANES + pl) * a.n_out + col0 + c, v);
+    }
+}
+
+// seat < 0: two views (row 2 m + v); 0 / 1: one view per record (row m, player seat ^ (swap[m] != 0))
+static int encode_linear_wgrad_impl(const ovc_layout_t *layouts, int n_layouts, const int32_t *state, const int32_t *swap, int seat,
+                                    const float *dz, float *dwt, long long n_rec, int S, int W, int H, int horizon, int n_out,
+                                    cudaStream_t st) {
+    if (!dz || !dwt) return fail(OVC_E_BADARG, "null pointer argument");
+    if ((((uintptr_t)dz | (uintptr_t)dwt) & 15) != 0) return fail(OVC_E_BADARG, "dz and dwt must be 16-byte aligned");
+    if (((uintptr_t)swap & 3) != 0) return fail(OVC_E_BADARG, "swap must be 4-byte aligned");
+    if (W < 1 || W > 16 || H < 1 || H > 16) return fail(OVC_E_BADARG, "grid shape out of range");
+    if (n_out < 64 || n_out % 64) return fail(OVC_E_BADARG, "n_out must be a positive multiple of 64", n_out);
+    if (n_layouts > EL_MAX_LAYOUTS) return fail(OVC_E_UNSUPPORTED, "encode_linear_wgrad: more than 8 layouts per call", n_layouts);
+    const int n_rows = W * H * EL_DYN;
+    if (encode_linear_wgrad_smem(1, n_rows, n_layouts) > (size_t)WG_SMEM_LIMIT)
+        return fail(OVC_E_UNSUPPORTED, "encode_linear_wgrad: the gradient table of this grid does not fit shared memory", W * H);
+    if (n_rec == 0) return OVC_OK;
+    int dev = 0, n_sm = 0, max_smem = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    int cpl = 0;
+    for (int c = 4; c >= 1; c >>= 1)
+        if (n_out % (32 * c) == 0 && encode_linear_wgrad_smem(c, n_rows, n_layouts) <= (size_t)max_smem) {
+            cpl = c;
+            break;
+        }
+    if (!cpl) return fail(OVC_E_UNSUPPORTED, "encode_linear_wgrad: the gradient table of this grid does not fit shared memory", W * H);
+    EncWgradArgs a;
+    a.layouts = layouts, a.state = state, a.swap = seat >= 0 ? swap : nullptr, a.dz = dz, a.dwt = dwt, a.n_rec = n_rec;
+    a.n_layouts = n_layouts, a.S = S, a.W = W, a.H = H, a.horizon = horizon, a.n_out = n_out, a.seat = seat;
+    const int n_slices = n_out / (32 * cpl);
+    const long long want = (n_rec + EL_THREADS / 32 - 1) / (EL_THREADS / 32);
+    int workers = n_sm / n_slices;
+    if (workers < 1) workers = 1;
+    if (workers > want) workers = (int)want;
+    a.n_workers = workers;
+    const size_t smem = encode_linear_wgrad_smem(cpl, n_rows, n_layouts);
+    cudaError_t e;
+#define OVC_LAUNCH_WG(C)                                                                                                      \
+    do {                                                                                                                      \
+        e = cudaFuncSetAttribute(encode_linear_wgrad_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);      \
+        if (e != cudaSuccess) return cuda_fail(e, "encode_linear_wgrad kernel attribute");                                    \
+        encode_linear_wgrad_kernel<C><<<(unsigned)(workers * n_slices), EL_THREADS, smem, st>>>(a);                           \
+    } while (0)
+    if (cpl == 4) OVC_LAUNCH_WG(4);
+    else if (cpl == 2) OVC_LAUNCH_WG(2);
+    else OVC_LAUNCH_WG(1);
+#undef OVC_LAUNCH_WG
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "encode_linear_wgrad kernel launch");
+    return OVC_OK;
+}
+
 }  // namespace ovc
 
 // ------------------------------------------------------------------------------------------------

@@ -18,6 +18,8 @@ of 64, leaky ReLU, heads 6 + 1), random init, shared by both agents.  ``RllibSha
 the network ``SelfPlayRollout`` evaluates: on a 5x4 grid entirely with this library's kernels K7, K9 and K8.
 """
 import copy
+import functools
+from types import SimpleNamespace
 
 import numpy as np
 import torch
@@ -147,10 +149,17 @@ def lstm_gate_permutation(cell):
     return (q % 4) * cell + 16 * j + 8 * (q // 4) + n
 
 
-def _conv_matrix(conv, c, w, h):
+def _conv_matrix(conv, c, w, h, grad=False):
     """(matrix [n_out, n_in], (c_out, w', h')) of a convolution over a (c, x = w, y = h) image, inputs and outputs flat in
     [x][y][channel] order.  Each tap's weights are placed by index, with no arithmetic, so the matrix holds the convolution's
-    own weights on any device (a convolution of the identity would be rounded to TF32 by cuDNN's default on the GPU)."""
+    own weights on any device (a convolution of the identity would be rounded to TF32 by cuDNN's default on the GPU).
+    ``grad``: the placement stays in autograd, so a gradient on the matrix reaches ``conv.weight``."""
+    if grad:  # one gather of the weights through the placement of their indices (_tap_index), one scatter in backward
+        idx = _tap_index(tuple(conv.weight.shape), tuple(conv.padding), tuple(conv.stride), tuple(conv.dilation), w, h,
+                         conv.weight.device)
+        co, _, kx, ky = conv.weight.shape
+        return torch.cat([conv.weight.new_zeros(1), conv.weight.reshape(-1)])[idx], \
+            (co, w + 2 * conv.padding[0] - kx + 1, h + 2 * conv.padding[1] - ky + 1)
     k = conv.weight.detach()
     co, ci, kx, ky = k.shape
     px, py = conv.padding
@@ -164,6 +173,50 @@ def _conv_matrix(conv, c, w, h):
             yo = torch.arange(max(0, py - dy), min(ho, h + py - dy), device=k.device)
             m[(xo + dx - px)[:, None], (yo + dy - py)[None, :], :, xo[:, None], yo[None, :], :] = k[:, :, dx, dy].t()
     return m.reshape(w * h * c, wo * ho * co).t().contiguous(), (co, wo, ho)
+
+
+@functools.lru_cache(maxsize=None)
+def _tap_index(shape, padding, stride, dilation, w, h, device):
+    """int64 [n_out, n_in]: 1 + the flat index into a weight of ``shape`` that ``_conv_matrix`` places at each matrix
+    element, 0 where it places nothing (the placement of the weights 1, 2, ... in float64, exact far beyond these sizes)."""
+    n = int(np.prod(shape))
+    stand_in = SimpleNamespace(weight=torch.arange(1, n + 1, dtype=torch.float64, device=device).view(shape), padding=padding,
+                               stride=stride, dilation=dilation)
+    return _conv_matrix(stand_in, shape[1], w, h)[0].long()
+
+
+def _folded_mats(cnn, width, height, grad=False):
+    """The layers of ``cnn`` (``RllibShapedCNN``) as [(matrix [n_out, n_in], bias [n_out])], unpadded: the three
+    convolutions (``_conv_matrix``), the dense layers (the first one's inputs re-ordered from torch's (c, x, y) flatten to
+    [x][y][c]) and the heads (logits rows, then the value row).  ``grad``: every step stays in autograd."""
+    mats = []
+    shape = (26, width, height)  # (channels, x, y) as the conv sees it
+    for conv in (cnn.conv_initial, cnn.conv_0, cnn.conv_1):
+        m, shape = _conv_matrix(conv, *shape, grad=grad)
+        co, wo, ho = shape
+        mats.append((m, conv.bias.view(1, 1, co).expand(wo, ho, co).reshape(-1).clone()))
+    # the first dense layer consumed conv_1's NCHW flatten (c, x, y): re-order its inputs to [x][y][c]
+    co, wo, ho = shape
+    first = cnn.dense[0]
+    mats.append((first.weight.view(-1, co, wo, ho).permute(0, 2, 3, 1).reshape(first.out_features, -1), first.bias))
+    mats += [(d.weight, d.bias) for d in cnn.dense[1:]]
+    mats.append((torch.cat([cnn.logits.weight, cnn.value.weight]), torch.cat([cnn.logits.bias, cnn.value.bias])))
+    return mats
+
+
+def folded_layers(cnn, width, height, pad_to=16):
+    """``DenseGridPolicy(cnn, width, height, pad_to)``'s layers as [(weight, bias)] float tensors that stay in autograd:
+    a gradient on a folded (padded, tap-placed, re-ordered) matrix reaches ``cnn``'s parameters.  Same values, same
+    padding as the module: conv_initial, conv_0, conv_1, the dense layers, the heads."""
+    assert not hasattr(cnn, "lstm"), "the LSTM model is not folded here"
+    up = lambda n: -(-n // pad_to) * pad_to
+    out, n_in = [], None
+    for m, bias in _folded_mats(cnn, width, height, grad=True):
+        n_in = m.shape[1] if n_in is None else n_in  # the input width is K2's row: never padded
+        n_out = up(m.shape[0])
+        out.append((F.pad(m, (0, n_in - m.shape[1], 0, n_out - m.shape[0])), F.pad(bias, (0, n_out - bias.shape[0]))))
+        n_in = n_out
+    return out
 
 
 class DenseGridPolicy(nn.Module):
@@ -187,18 +240,7 @@ class DenseGridPolicy(nn.Module):
         self.W, self.H = width, height
         up = lambda n: -(-n // pad_to) * pad_to
         with torch.no_grad():
-            mats = []
-            shape = (26, width, height)  # (channels, x, y) as the conv sees it
-            for conv in (cnn.conv_initial, cnn.conv_0, cnn.conv_1):
-                m, shape = _conv_matrix(conv, *shape)
-                co, wo, ho = shape
-                mats.append((m, conv.bias.view(1, 1, co).expand(wo, ho, co).reshape(-1).clone()))
-            # the first dense layer consumed conv_1's NCHW flatten (c, x, y): re-order its inputs to [x][y][c]
-            co, wo, ho = shape
-            first = cnn.dense[0]
-            mats.append((first.weight.view(-1, co, wo, ho).permute(0, 2, 3, 1).reshape(first.out_features, -1), first.bias))
-            mats += [(d.weight, d.bias) for d in cnn.dense[1:]]
-            mats.append((torch.cat([cnn.logits.weight, cnn.value.weight]), torch.cat([cnn.logits.bias, cnn.value.bias])))
+            mats = _folded_mats(cnn, width, height)
             self.n_actions = cnn.logits.out_features
             self.dense_slope = cnn.dense_slope
             # RllibLSTMShapedCNN: the LSTM between the dense layers and the heads, kept as it is (lstm_tables folds it for K11)
@@ -300,11 +342,82 @@ def fused_kernel_support(dense_model, width, height, n_layouts=1):
     wide layers as library GEMMs, then K8."""
     l0, l1, l2 = dense_model.conv_as_linear
     d = list(dense_model.dense)
-    k7 = (l0.out_features % 64 == 0 and width * height * 19 * 64 * 2 + 4096 <= 227 * 1024
-          and n_layouts <= K7_MAX_LAYOUTS)
+    k7 = _k7_fits(l0.out_features, width, height, n_layouts)
     k9 = (l1.in_features, l1.out_features, l2.out_features) == (512, 512, 160)
     k8 = all(l.out_features == 64 for l in d) and d[0].in_features % 32 == 0 and d[0].in_features <= 256 and dense_model.n_actions <= 7
     return k7, k9, k8
+
+
+def _k7_fits(n_out, width, height, n_layouts):
+    """K7 (and K12, whose narrowest table takes the same bytes) on a first layer of width ``n_out``: see ``fused_kernel_support``."""
+    return n_out % 64 == 0 and width * height * 19 * 64 * 2 + 4096 <= 227 * 1024 and n_layouts <= K7_MAX_LAYOUTS
+
+
+class _RecordsFirstLayer(torch.autograd.Function):
+    """The first layer of the folded network on packed records: forward K7 (bf16 out, exactly what the behaviour policy's
+    K7 computed from the same weights), backward K12 for the weight gradient.  The records have no gradient."""
+
+    @staticmethod
+    def forward(ctx, w0, b0, env, recs, seat, swap):
+        wt = w0.detach().t().to(torch.bfloat16).contiguous()
+        bias = b0.detach().to(torch.bfloat16).float()  # the rollout folds into a bf16 module: its K7 bias is bf16-rounded
+        if seat is None:
+            y = env.encoded_linear(wt, bias, neg_slope=0.2, states=recs)
+        else:
+            y = env.encoded_linear_view(wt, bias, seat, swap, neg_slope=0.2, states=recs)
+        ctx.save_for_backward(y)
+        ctx.env, ctx.recs, ctx.seat, ctx.swap, ctx.n_in = env, recs, seat, swap, w0.shape[1]
+        return y
+
+    @staticmethod
+    def backward(ctx, grad):
+        y, = ctx.saved_tensors
+        # bf16 keeps float32's exponent range, so y's sign is the pre-activation's: the leaky ReLU's derivative from y
+        dz = (grad.float() * torch.where(y > 0, 1.0, 0.2)).contiguous()
+        dwt = torch.zeros((ctx.n_in, dz.shape[1]), dtype=torch.float32, device=dz.device)
+        ctx.env.encoded_linear_wgrad(ctx.recs, dz, dwt, seat=ctx.seat, swap=ctx.swap)
+        return dwt.t(), dz.sum(0), None, None, None, None
+
+
+def records_forward(model, env, recs, seat=None, swap=None, fused_first_layer=None):
+    """(logits float32 [rows, n_actions], values float32 [rows]) of ``model`` (``RllibShapedCNN``) on the packed records
+    ``recs`` (int32 CUDA [M, S]), differentiable with respect to ``model``'s parameters.  Rows as K7's: ``seat`` None, both
+    views (row 2 m + v); 0 / 1, one view (row m: player ``seat ^ (swap[m] != 0)``).
+
+    The network is ``DenseGridPolicy``'s fold (``folded_layers``, pad 16) at the rollout's precision: bf16 operands, float32
+    accumulation, float32 master weights and gradients.  The first layer runs as K7 / K12 (``_RecordsFirstLayer``) where
+    K7 takes the grid and the layout count (``fused_first_layer`` None), else as K2's bf16 observation times the same
+    matrix; the wide and dense layers are library GEMMs with bf16 outputs, and the heads are computed in float32 from the
+    bf16 activations and weights (K8 writes float32 heads too)."""
+    assert not isinstance(model, RllibLSTMShapedCNN), \
+        "the LSTM model is trained on sequences: use RllibLSTMShapedCNN.forward_sequence on batch.observations"
+    assert len({(l.width, l.height) for l in env.layouts}) == 1, "one grid shape per call (group envs by layout)"
+    W, H = env.layouts[0].width, env.layouts[0].height
+    layers = folded_layers(model, W, H, pad_to=16)
+    bf = lambda t: t.to(torch.bfloat16)
+    w0, b0 = layers[0]
+    k7 = _k7_fits(w0.shape[0], W, H, env.n_layouts)
+    if fused_first_layer is None:
+        fused_first_layer = k7
+    assert not fused_first_layer or k7, "K7 / K12 do not take this grid, layout count or first-layer width"
+    if fused_first_layer:
+        x = _RecordsFirstLayer.apply(w0, b0, env, recs, seat, swap)
+    else:
+        if seat is None:
+            obs = env.lossless_state_encoding(dtype=torch.bfloat16, states=recs)
+        else:
+            vs = torch.full((recs.shape[0],), int(seat), dtype=torch.int32, device=recs.device)
+            if swap is not None:
+                vs ^= (swap != 0).to(torch.int32)
+            obs = env.lossless_state_encoding(dtype=torch.bfloat16, states=recs, view_swap=vs.contiguous())[:, 0]
+        x = F.leaky_relu(F.linear(obs.reshape(-1, w0.shape[1]), bf(w0), bf(b0)), 0.2)
+    n_conv = 3
+    for i, (w, b) in enumerate(layers[1:-1], 1):
+        x = F.leaky_relu(F.linear(x, bf(w), bf(b)), 0.2 if i < n_conv else model.dense_slope)
+    wh, bh = layers[-1]
+    hv = F.linear(x.float(), bf(wh).float(), bf(bh).float())
+    n_act = model.logits.out_features
+    return hv[:, :n_act], hv[:, n_act]
 
 
 class BCPolicy(nn.Module):
@@ -432,6 +545,22 @@ class SampleBatch(object):
             return self.env.lossless_state_encoding(dtype=dtype, states=recs)
         learner = (1 - self.partner_seat.view(-1).index_select(0, env_steps)).to(torch.int32).contiguous()  # view_swap: this view first
         return self.env.lossless_state_encoding(dtype=dtype, states=recs, view_swap=learner)[:, 0]
+
+    def forward(self, model, env_steps, fused_first_layer=None):
+        """(logits float32 [rows, 6], values float32 [rows]) of ``model`` (``RllibShapedCNN``, e.g. the learner after some
+        updates) on the env-steps ``env_steps``, with autograd to ``model``'s parameters, in the row order of
+        ``observations(env_steps)``: both views (rows ``2 m + i``), or the learner's view in a ``one_view`` batch.
+
+        The network is the fold the rollout runs, at its precision (``records_forward``), evaluated from the stored records:
+        where K7 takes the grid and the layout count, the first layer is K7 on the records (its output bit for bit what the
+        behaviour policy's K7 computed from the same weights) and its weight gradient is K12; no observation is written.
+        Else the first layer reads K2's bf16 observation.  Not for ``RllibLSTMShapedCNN`` (use ``forward_sequence``)."""
+        recs = self.states.view(-1, self.states.shape[-1]).index_select(0, env_steps)
+        if not self.one_view:
+            return records_forward(model, self.env, recs, fused_first_layer=fused_first_layer)
+        # the learner is player 1 - partner_seat = 1 ^ partner_seat
+        swap = self.partner_seat.view(-1).index_select(0, env_steps).to(torch.int32).contiguous()
+        return records_forward(model, self.env, recs, seat=1, swap=swap, fused_first_layer=fused_first_layer)
 
 
 # The BC partner's draws use their own Philox keys: seed ^ PARTNER_DRAW_SALT for K10's action draw, seed ^ PARTNER_SEAT_SALT
