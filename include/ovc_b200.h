@@ -737,6 +737,43 @@ int ovc_policy_tail_joint(const void *x, int64_t n_rows, int k0, float in_slope,
                           int32_t *actions, float *values, float *scores, float *logp, void *stream);
 
 /*
+ * A population of self-play learners on one batch (fictitious co-play's first stage): member k of n_members (1..64,
+ * OVC_E_BADARG otherwise) plays both views of the environments of its block, a contiguous range of rows.
+ *
+ * Each grouped form is ONE launch for every member: its tables are stacked with a leading member dimension, and offsets
+ * (int32 [n_members + 1] in DEVICE memory, non-decreasing, clipped to the rows the call holds) gives the members' blocks.
+ * A CTA (encode) or a tile (wide layers, tail) never spans two members.
+ *
+ * ovc_encode_linear_grouped: ovc_encode_linear (two views, no view_swap) with member k's table on environments
+ *   [offsets[k], offsets[k + 1]) of state: wt bfloat16 [n_members][width*height*26][n_out], bias float32 [n_members][n_out].
+ *   Output row 2 e + v is bit for bit row 2 e + v of ovc_encode_linear with member k's table; rows of environments outside
+ *   every block are untouched.  The CTAs are split over (member, column slice, worker).  Same limits as ovc_encode_linear.
+ * ovc_wide_layers_grouped: ovc_wide_layers with member k's weights on rows [offsets[k], offsets[k + 1]) of a0 / z2 ([m][...],
+ *   m < 2^31): w1 bfloat16 [n_members * 512][512], w2 bfloat16 [n_members * 160][512] (one tensor map per operand serves
+ *   every member through row coordinates), b1 float32 [n_members][512], b2 float32 [n_members][160] (8-byte aligned).  Each
+ *   row is bit for bit ovc_wide_layers on that member's weights; rows outside every block are untouched.
+ * ovc_policy_tail_grouped: ovc_policy_tail_logp for every member.  The tables are stacked with a leading
+ *   member dimension: w_first bfloat16 [n_members][64][k0], b_first float32 [n_members][64], w_hidden bfloat16
+ *   [n_members][n_hidden][64][64], b_hidden float32 [n_members][n_hidden][64], w_heads bfloat16 [n_members][8][64], b_heads
+ *   float32 [n_members][8].  offsets int32 [n_members + 1] in DEVICE memory, non-decreasing: member k's rows are
+ *   [offsets[k], offsets[k + 1]) of x ([n_rows][k0], n_rows < 2^31), clipped to [0, n_rows).  Row r of member k is drawn on
+ *   row r with this call's seed and counter's step, and actions, values, scores ([.][8]) and logp (each but actions
+ *   nullable) are written at row r: bit for bit what ovc_policy_tail_logp writes at row r with member k's tables.  Rows
+ *   outside every block are untouched.  Every CTA advances the counter once per launch (one step per launch, as
+ *   ovc_sample_actions').  x and the weight tables 16-byte aligned; biases, scores and counter 8-byte aligned; actions,
+ *   values, logp and offsets 4-byte aligned.
+ */
+int ovc_encode_linear_grouped(const void *layouts, int n_layouts, const int32_t *state, const void *wt, const float *bias,
+                              const int32_t *offsets, int n_members, void *out, int64_t n_envs, int state_words, int width, int height,
+                              int horizon, int n_out, float neg_slope, void *stream);
+int ovc_wide_layers_grouped(const void *a0, int64_t m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2,
+                            int n2, float slope, const int32_t *offsets, int n_members, void *z2, void *stream);
+int ovc_policy_tail_grouped(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                            const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                            float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *offsets, int n_members,
+                            int32_t *actions, float *values, float *scores, float *logp, void *stream);
+
+/*
  * ovc_encode_linear_wgrad (K12): the weight gradient of ovc_encode_linear's layer, from the packed records,
  *     dwt[f][c] += sum over rows r of enc(r)[f] * dz[r][c]
  *   enc(r) = lossless_state_encoding of row r's record and view (never materialised), f in the observation's element order

@@ -966,6 +966,34 @@ int ovc_policy_tail_joint(const void *x, int64_t n_rows, int k0, float in_slope,
     return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, nullptr, -1, jrow, range, true);
 }
 
+int ovc_encode_linear_grouped(const void *layouts, int n_layouts, const int32_t *state, const void *wt, const float *bias,
+                              const int32_t *offsets, int n_members, void *out, int64_t n_envs, int state_words, int width, int height,
+                              int horizon, int n_out, float neg_slope, void *stream) {
+    int rc = ovc::check_common(layouts, n_layouts, state, n_envs, state_words);
+    if (rc) return rc;
+    if (n_members < 1 || n_members > ovc::EL_MAX_MEMBERS) return ovc::fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+    return ovc::encode_linear_impl((const ovc_layout_t *)layouts, n_layouts, state, nullptr, wt, bias, out, n_envs, state_words, width,
+                                   height, horizon, n_out, neg_slope, (cudaStream_t)stream, -1, nullptr, nullptr, nullptr, nullptr, offsets,
+                                   n_members);
+}
+
+int ovc_wide_layers_grouped(const void *a0, int64_t m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2,
+                            int n2, float slope, const int32_t *offsets, int n_members, void *z2, void *stream) {
+    return ovc::wide_layers_grouped_impl(a0, m, k0, w1, b1, n1, w2, b2, n2, slope, offsets, n_members, z2, (cudaStream_t)stream);
+}
+
+int ovc_policy_tail_grouped(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                            const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                            float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *offsets, int n_members,
+                            int32_t *actions, float *values, float *scores, float *logp, void *stream) {
+    ovc::PolicyTailArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
+    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
+    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
+    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    return ovc::policy_tail_grouped_impl(a, k0, offsets, n_members, (cudaStream_t)stream);
+}
+
 int ovc_featurize(const void *layouts, int n_layouts, const void *lut, const int32_t *state,
                   const int32_t *view_swap, float *out, int64_t n_envs, int state_words, int num_pots, void *stream) {
     int rc = ovc::check_common(layouts, n_layouts, state, n_envs, state_words);

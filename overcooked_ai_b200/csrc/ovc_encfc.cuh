@@ -27,6 +27,7 @@ namespace ovc {
 constexpr int EL_DYN = 19;          // dynamic planes kept in the table: 0-9 (players) and 16-24 (objects)
 constexpr int EL_THREADS = 1024;
 constexpr int EL_MAX_LAYOUTS = 8;
+constexpr int EL_MAX_MEMBERS = 64;
 
 struct EncLinArgs {
     const ovc_layout_t *layouts;
@@ -297,6 +298,208 @@ __device__ __forceinline__ void encode_linear_body(const EncLinArgs &a, const in
     }
 }
 
+// encode_linear_body with GROUPED (a copy, so that the code of the kernels above stays as it was; encode_linear_grouped_kernel,
+// two views, without view_swap): n_members members, member k's tables entry k of
+// stacked wt / bias and its environments [offsets[k], offsets[k + 1]); the CTAs are split over (member, column slice,
+// worker), a.n_workers workers per member, so a CTA loads its member's column slice once and walks only that member's
+// environments.
+template <int CPL, bool VIEW, bool ROWS, bool MASKED, bool GROUPED = false>
+__device__ __forceinline__ void encode_linear_grouped_body(const EncLinArgs &a, const int32_t *list = nullptr, const int32_t *first = nullptr,
+                                                   const int32_t *offsets = nullptr) {
+    constexpr int CS = 32 * CPL;  // columns per CTA
+    extern __shared__ __align__(16) char el_smem[];
+    const int WH = a.W * a.H;
+    const int n_rows = WH * EL_DYN;
+    __nv_bfloat16 *tab = reinterpret_cast<__nv_bfloat16 *>(el_smem);                      // [n_rows][CS]
+    float *bias_eff = reinterpret_cast<float *>(el_smem + (size_t)n_rows * CS * 2);       // [n_layouts][CS]
+    float *urg = bias_eff + a.n_layouts * CS;                                             // [CS]
+    int *cook = reinterpret_cast<int *>(urg + CS);                                        // [n_layouts][16]
+    int *nslots = cook + a.n_layouts * 16;                                                // [n_layouts][2]: n_slots, n_pots
+    unsigned short *srow = reinterpret_cast<unsigned short *>(nslots + a.n_layouts * 2);  // [n_layouts][128] slot -> row base
+
+    const int n_slices = a.n_out / CS;
+    int bx = blockIdx.x;
+    const __nv_bfloat16 *wt = a.wt;
+    const float *bias = a.bias;
+    long long r_beg = 0, r_end = a.n_envs;
+    if constexpr (GROUPED) {
+        const int per = n_slices * a.n_workers, k = bx / per;
+        bx -= k * per;
+        wt += (size_t)k * a.W * a.H * N_PLANES * a.n_out, bias += (size_t)k * a.n_out;
+        r_beg = min(max((long long)__ldg(offsets + k), 0ll), a.n_envs);
+        r_end = max(min((long long)__ldg(offsets + k + 1), a.n_envs), r_beg);
+    }
+    const int slice = bx % n_slices, worker = bx / n_slices;
+    const int col0 = slice * CS;
+    if constexpr (ROWS) {
+        r_beg = max(__ldg(a.range), 0);
+        r_end = min((long long)__ldg(a.range + 1), a.n_envs);
+        if (r_beg + (long long)worker * (EL_THREADS / 32) >= r_end) return;
+    }
+    if constexpr (MASKED) {
+        if ((long long)worker * (EL_THREADS / 32) >= r_end) return;
+    }
+    if constexpr (GROUPED) {
+        if (r_beg + (long long)worker * (EL_THREADS / 32) >= r_end) return;
+    }
+
+    // ---- prologue: the table slice and the per-layout constants ----
+    unsigned char *tplane = reinterpret_cast<unsigned char *>(srow + a.n_layouts * 128);  // [n_layouts][256] terrain plane of a cell, 0 = none
+    for (int i = threadIdx.x; i < a.n_layouts * WH; i += EL_THREADS) {  // terrain code -> plane: X 11, O 12, T 13, D 14, P 10, S 15 (:2449-2465)
+        const int l = i / WH, cell = i - l * WH, x = cell / a.H, y = cell - x * a.H;
+        tplane[l * 256 + cell] = (unsigned char)((0x000F0A0E0D0C0B00ull >> ((a.layouts[l].cell[(y << 4) | x] & 7) * 8)) & 0xFF);
+    }
+    __syncthreads();
+    {
+        constexpr int CH = CS * 2 / 16;  // 16-byte chunks per row
+        for (int i = threadIdx.x; i < n_rows * CH; i += EL_THREADS) {
+            const int r = i / CH, c = i - r * CH;
+            const int cell = r / EL_DYN, d = r - cell * EL_DYN;
+            const int plane = d < 10 ? d : d + 6;
+            const uint4 *src = reinterpret_cast<const uint4 *>(wt + (size_t)(cell * N_PLANES + plane) * a.n_out + col0) + c;
+            reinterpret_cast<uint4 *>(tab)[i] = __ldg(src);
+        }
+        // terrain and urgency sums: one thread per (layout, column); the cells' loads are independent (plane ids staged in
+        // shared memory first), issued four at a time, added in cell order
+        for (int i = threadIdx.x; i < (a.n_layouts + 1) * CS; i += EL_THREADS) {
+            const int l = i / CS, c = i - l * CS;
+            const unsigned char *tp = tplane + l * 256;
+            const __nv_bfloat16 *w = wt + col0 + c;
+            float s = l == a.n_layouts ? 0.f : bias[col0 + c];
+            for (int cell = 0; cell < WH; cell += 4) {
+                float v[4];
+#pragma unroll
+                for (int u = 0; u < 4; u++) {
+                    const int pl = cell + u < WH ? (l == a.n_layouts ? (int)PL_URGENCY : (int)tp[cell + u]) : 0;
+                    v[u] = pl ? __bfloat162float(w[(size_t)((cell + u) * N_PLANES + pl) * a.n_out]) : 0.f;
+                }
+                s = (((s + v[0]) + v[1]) + v[2]) + v[3];
+            }
+            if (l == a.n_layouts) urg[c] = s;
+            else bias_eff[i] = s;
+        }
+        for (int i = threadIdx.x; i < a.n_layouts * 128; i += EL_THREADS) {
+            const ovc_layout_t *L = a.layouts + (i >> 7);
+            const int pb = L->slot_pos[i & 127];
+            srow[i] = (unsigned short)((((pb & 15) * a.H + (pb >> 4)) * EL_DYN) & 0xFFFF);
+        }
+        for (int i = threadIdx.x; i < a.n_layouts * 16; i += EL_THREADS) cook[i] = a.layouts[i >> 4].cook_time[i & 15];
+        for (int i = threadIdx.x; i < a.n_layouts; i += EL_THREADS) {
+            nslots[2 * i] = a.layouts[i].n_slots;
+            nslots[2 * i + 1] = a.layouts[i].n_pots;
+        }
+    }
+    __syncthreads();
+
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    constexpr int NW = EL_THREADS / 32;
+    const __nv_bfloat16 *tab_lane = tab + lane * CPL;
+    const long long stride = (long long)a.n_workers * NW;
+    const int max_slot_chunks = (a.S - 4 + 31) / 32;
+
+    for (long long r = r_beg + (long long)worker * NW + warp; r < r_end; r += stride) {
+        long long env, row0 = 0;
+        int vmask = 3;
+        if constexpr (MASKED) {
+            const int entry = __ldg(list + r);
+            env = entry >> 2, vmask = entry & 3;
+            if (!vmask) continue;  // the whole warp holds entry r
+            row0 = __ldg(first + r);
+        } else {
+            env = ROWS ? (long long)__ldg(a.rows + r) : r;
+        }
+        const int32_t *__restrict__ rec = a.state + env * a.S;
+        const int4 head = __ldg(reinterpret_cast<const int4 *>(rec));  // timestep, player 0, player 1, misc (same address in every lane)
+        const int lid = head.w & 0xFF;
+        const int n_slots = nslots[2 * lid], n_pots = nslots[2 * lid + 1];
+        const int *ck = cook + lid * 16;
+        const unsigned short *sr = srow + lid * 128;
+
+        float common[CPL];
+        {   // vector loads: consecutive lanes read consecutive CPL-float pieces (conflict free)
+            const bool urgent = a.horizon - head.x < 40;
+            constexpr int V = CPL >= 4 ? 4 : 2;
+            using fv = typename std::conditional<CPL >= 4, float4, float2>::type;
+#pragma unroll
+            for (int i = 0; i < CPL / V; i++) {
+                const fv b = reinterpret_cast<const fv *>(bias_eff + lid * CS + lane * CPL)[i];
+                const fv u = reinterpret_cast<const fv *>(urg + lane * CPL)[i];
+                const float *bp = reinterpret_cast<const float *>(&b), *up = reinterpret_cast<const float *>(&u);
+#pragma unroll
+                for (int k = 0; k < V; k++) common[i * V + k] = bp[k] + (urgent ? up[k] : 0.f);
+            }
+        }
+        // objects on pots / counters: lane l of chunk c decodes slot 32 c + l; entries travel by shuffle
+        for (int c = 0; c < max_slot_chunks; c++) {
+            if (c * 32 >= n_slots) break;
+            const int slot = c * 32 + lane;
+            unsigned e[4] = {0, 0, 0, 0};
+            if (slot < n_slots) {
+                const unsigned code = (unsigned)__ldg(rec + 4 + slot) & OVC_OBJ_MASK;
+                if (code) el_object(code, sr[slot], slot < n_pots, ck, e);
+            }
+            unsigned m = __ballot_sync(0xFFFFFFFFu, (e[0] | e[1] | e[2] | e[3]) != 0);
+            while (m) {
+                const int j = __ffs(m) - 1;
+                m &= m - 1;
+#pragma unroll
+                for (int q = 0; q < 4; q++) {
+                    const unsigned w = __shfl_sync(0xFFFFFFFFu, e[q], j);
+                    if (w & 0xFFFFu) el_gather<CPL>(common, tab_lane, (int)(w >> 16), (float)(short)(w & 0xFFFFu));
+                }
+            }
+        }
+        // held objects: at the holder's cell, in both views (computed by every lane, no exchange needed)
+        const unsigned p0 = (unsigned)head.y, p1 = (unsigned)head.z;
+        const int cell0 = ((p0 & 15) * a.H + ((p0 >> 4) & 15)) * EL_DYN, cell1 = ((p1 & 15) * a.H + ((p1 >> 4) & 15)) * EL_DYN;
+#pragma unroll
+        for (int j = 0; j < 2; j++) {
+            const unsigned held = (j ? p1 : p0) >> 10;
+            if (held) {
+                unsigned e[4];
+                el_object(held, j ? cell1 : cell0, false, ck, e);
+#pragma unroll
+                for (int q = 0; q < 4; q++)
+                    if (e[q] & 0xFFFFu) el_gather<CPL>(common, tab_lane, (int)(e[q] >> 16), (float)(short)(e[q] & 0xFFFFu));
+            }
+        }
+        // the two views: own cell / orientation in planes 0, 2..5, the partner's in planes 1, 6..9 (:2468-2479)
+        const int ori0 = (p0 >> 8) & 3, ori1 = (p1 >> 8) & 3;
+        const int swap = a.view_swap ? (__ldg(a.view_swap + env) != 0) : 0;
+        auto view = [&](int p, long long row) {  // p = the player whose view this is
+            float acc[CPL];
+#pragma unroll
+            for (int i = 0; i < CPL; i++) acc[i] = common[i];
+            const int own_cell = p ? cell1 : cell0, oth_cell = p ? cell0 : cell1;
+            const int own_ori = p ? ori1 : ori0, oth_ori = p ? ori0 : ori1;
+            el_gather<CPL>(acc, tab_lane, own_cell + PL_LOC, 1.f);
+            el_gather<CPL>(acc, tab_lane, own_cell + PL_ORI + own_ori, 1.f);
+            el_gather<CPL>(acc, tab_lane, oth_cell + PL_LOC + 1, 1.f);
+            el_gather<CPL>(acc, tab_lane, oth_cell + PL_ORI + 4 + oth_ori, 1.f);
+            unsigned packed[CPL / 2];
+#pragma unroll
+            for (int i = 0; i < CPL / 2; i++) {
+                const float x0 = acc[2 * i], x1 = acc[2 * i + 1];
+                const __nv_bfloat162 h = __floats2bfloat162_rn(fmaxf(x0, x0 * a.neg_slope), fmaxf(x1, x1 * a.neg_slope));
+                packed[i] = *reinterpret_cast<const unsigned *>(&h);
+            }
+            __nv_bfloat16 *dst = a.out + row * a.n_out + col0 + lane * CPL;
+            if constexpr (CPL == 8) *reinterpret_cast<uint4 *>(dst) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
+            else if constexpr (CPL == 4) *reinterpret_cast<uint2 *>(dst) = make_uint2(packed[0], packed[1]);
+            else *reinterpret_cast<unsigned *>(dst) = packed[0];
+        };
+        if constexpr (MASKED) {
+            if (vmask & 1) view(0, row0);
+            if (vmask & 2) view(1, row0 + (vmask & 1));
+        } else if constexpr (VIEW) {
+            view(a.seat ^ swap, r);
+        } else {
+#pragma unroll
+            for (int p = 0; p < 2; p++) view(p, 2 * env + (swap ? 1 - p : p));
+        }
+    }
+}
+
 template <int CPL, bool VIEW, bool ROWS = false>
 __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_kernel(const EncLinArgs a) {
     encode_linear_body<CPL, VIEW, ROWS, false>(a);
@@ -308,20 +511,29 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_masked_kernel(con
     encode_linear_body<CPL, false, false, true>(a, list, first);
 }
 
+template <int CPL>
+__global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_grouped_kernel(const EncLinArgs a, const int32_t *offsets) {
+    encode_linear_grouped_body<CPL, false, false, false, true>(a, nullptr, nullptr, offsets);
+}
+
 static size_t encode_linear_smem(int cpl, int n_rows, int n_layouts) {
     const size_t CS = 32 * (size_t)cpl;
     return (size_t)n_rows * CS * 2 + ((size_t)n_layouts + 1) * CS * 4 + (size_t)n_layouts * (16 * 4 + 2 * 4 + 128 * 2 + 256) + 16;
 }
 
 // seat < 0: both views (ovc_encode_linear); 0 / 1: one view per environment (ovc_encode_linear_view, view_swap = swap);
-// with rows / range: the rows map (ovc_encode_linear_rows); with list / first: n_envs list entries (ovc_encode_linear_masked)
+// with rows / range: the rows map (ovc_encode_linear_rows); with list / first: n_envs list entries (ovc_encode_linear_masked);
+// n_members > 0: a population's stacked tables over its environment offsets (ovc_encode_linear_grouped)
 static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const int32_t *state, const int32_t *view_swap,
                               const void *wt, const float *bias, void *out, long long n_envs, int S, int W, int H, int horizon,
                               int n_out, float neg_slope, cudaStream_t st, int seat = -1, const int32_t *rows = nullptr,
-                              const int32_t *range = nullptr, const int32_t *list = nullptr, const int32_t *first = nullptr) {
-    const bool rows_map = rows || range, masked = list || first;
-    if (!out || !wt || !bias || (rows_map && (!rows || !range)) || (masked && (!list || !first)))
+                              const int32_t *range = nullptr, const int32_t *list = nullptr, const int32_t *first = nullptr,
+                              const int32_t *offsets = nullptr, int n_members = 0) {
+    const bool rows_map = rows || range, masked = list || first, grouped = n_members != 0;
+    if (!out || !wt || !bias || (rows_map && (!rows || !range)) || (masked && (!list || !first)) || (grouped && !offsets))
         return fail(OVC_E_BADARG, "null pointer argument");
+    if (grouped && (n_members < 1 || n_members > EL_MAX_MEMBERS)) return fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+    if (grouped && ((uintptr_t)offsets & 3) != 0) return fail(OVC_E_BADARG, "offsets must be 4-byte aligned");
     if ((((uintptr_t)out | (uintptr_t)wt) & 15) != 0) return fail(OVC_E_BADARG, "weights and output must be 16-byte aligned");
     if (seat >= 0 && ((uintptr_t)view_swap & 3) != 0) return fail(OVC_E_BADARG, "swap must be 4-byte aligned");
     if ((((uintptr_t)rows | (uintptr_t)range) & 3) != 0) return fail(OVC_E_BADARG, "rows and range must be 4-byte aligned");
@@ -350,6 +562,7 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
     const int n_slices = n_out / (32 * cpl);
     const long long want = (n_envs + EL_THREADS / 32 - 1) / (EL_THREADS / 32);
     int workers = n_sm / n_slices;
+    if (grouped) workers /= n_members;  // workers per member: one wave of CTAs in all
     if (workers < 1) workers = 1;
     if (workers > want) workers = (int)want;
     a.n_workers = workers;
@@ -367,7 +580,18 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
         if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                                          \
         encode_linear_masked_kernel<C><<<(unsigned)(workers * n_slices), EL_THREADS, smem, st>>>(a, list, first);             \
     } while (0)
-    if (masked) {
+#define OVC_LAUNCH_ELG(C)                                                                                                     \
+    do {                                                                                                                      \
+        e = cudaFuncSetAttribute(encode_linear_grouped_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);    \
+        if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                                          \
+        encode_linear_grouped_kernel<C><<<grid, EL_THREADS, smem, st>>>(a, offsets);                                          \
+    } while (0)
+    if (grouped) {
+        const unsigned grid = (unsigned)(workers * n_slices * n_members);
+        if (cpl == 8) OVC_LAUNCH_ELG(8);
+        else if (cpl == 4) OVC_LAUNCH_ELG(4);
+        else OVC_LAUNCH_ELG(2);
+    } else if (masked) {
         if (cpl == 8) OVC_LAUNCH_ELM(8);
         else if (cpl == 4) OVC_LAUNCH_ELM(4);
         else OVC_LAUNCH_ELM(2);
@@ -386,6 +610,7 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
     }
 #undef OVC_LAUNCH_EL
 #undef OVC_LAUNCH_ELM
+#undef OVC_LAUNCH_ELG
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel launch");
     return OVC_OK;

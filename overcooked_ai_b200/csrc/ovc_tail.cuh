@@ -369,6 +369,133 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_joint_kernel(const 
     policy_tail_body<KS2, true, false, false, false, true>(p, nullptr, 0, jrow, range);
 }
 
+// Grouped K8 (ovc_policy_tail_grouped): a population of K tails, member k's tables entry k of stacked tables, its rows
+// [offsets[k], offsets[k + 1]) (clipped to [0, n_rows)).  The launch's tile list is every member's 16-row tiles in member
+// order (a member's last tile partial, never shared with the next member); CTA b takes the contiguous share
+// [b T / G, (b + 1) T / G) of the T tiles, so a CTA holds at most a few members' tables, each staged once, and the work is
+// balanced whatever the block sizes.  Each row is drawn on its own row index r with the call's step, exactly as
+// ovc_policy_tail_logp draws row r, and every CTA advances the counter once.
+// 12 warps per CTA (a cap of 170 registers; ptxas uses 116 - 156 over the instantiations, no spills): under K8's 16 warps
+// (a cap of 128) the member bookkeeping on top of K8's tile spilled 8 - 44 bytes at k0 = 96..160 (K8 itself spills at that cap).
+constexpr int PT_MAX_MEMBERS = 64;
+constexpr int PTG_THREADS = 384;
+
+template <int KS2, bool LOGP>
+__global__ void __launch_bounds__(PTG_THREADS, 1) policy_tail_grouped_kernel(const PolicyTailArgs p, const int32_t *offsets, int n_members) {
+    constexpr int K0 = 32 * KS2;
+    extern __shared__ __align__(16) char pt_smem[];
+    __shared__ int tile0[PT_MAX_MEMBERS + 1], rbeg[PT_MAX_MEMBERS], rend[PT_MAX_MEMBERS];
+
+    const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(p.counter);
+    if (threadIdx.x == 0) {
+        int n = 0;
+        for (int k = 0; k < n_members; k++) {
+            const int lo = max(__ldg(offsets + k), 0), hi = max((int)min((long long)__ldg(offsets + k + 1), p.n_rows), lo);
+            tile0[k] = n, rbeg[k] = lo, rend[k] = hi;
+            n += (hi - lo + 15) / 16;
+        }
+        tile0[n_members] = n;
+    }
+    __syncthreads();
+    const int total = tile0[n_members];
+    const int t_lo = (int)((long long)blockIdx.x * total / gridDim.x), t_hi = (int)((long long)(blockIdx.x + 1) * total / gridDim.x);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
+    int tb = t_lo;
+    for (int k = 0; k < n_members && tb < t_hi; k++) {
+        const int te = min(t_hi, tile0[k + 1]);
+        if (te <= tb) continue;
+        PolicyTailArgs q = p;  // member k's tables
+        q.w_first += (size_t)k * PT_H * K0, q.b_first += (size_t)k * PT_H;
+        q.w_hidden += (size_t)k * p.n_hidden * PT_H * PT_H, q.b_hidden += (size_t)k * p.n_hidden * PT_H;
+        q.w_heads += (size_t)k * PT_NOUT * PT_H, q.b_heads += (size_t)k * PT_NOUT;
+        __syncthreads();  // the previous member's tiles no longer read the shared tables
+        const TailSmem w = tail_weights_to_smem<K0, PTG_THREADS>(pt_smem, q);
+        __syncthreads();
+        const int r_end = rend[k];
+        for (int tile = tb + warp; tile < te; tile += PTG_THREADS / 32) {
+            const int r0 = rbeg[k] + (tile - tile0[k]) * 16 + g, r1 = r0 + 8;
+            uint4 xa[KS2], xb[KS2];
+#pragma unroll
+            for (int s2 = 0; s2 < KS2; s2++) {
+                xa[s2] = r0 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r0 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
+                xb[s2] = r1 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r1 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
+            }
+            float acc[8][4];
+            first_layer64<KS2>(acc, w, g, t, [&](int s2, unsigned a_lo[4], unsigned a_hi[4]) {
+                a_lo[0] = lrelu_bf16x2(xa[s2].x, p.in_slope), a_lo[1] = lrelu_bf16x2(xb[s2].x, p.in_slope);
+                a_lo[2] = lrelu_bf16x2(xa[s2].y, p.in_slope), a_lo[3] = lrelu_bf16x2(xb[s2].y, p.in_slope);
+                a_hi[0] = lrelu_bf16x2(xa[s2].z, p.in_slope), a_hi[1] = lrelu_bf16x2(xb[s2].z, p.in_slope);
+                a_hi[2] = lrelu_bf16x2(xa[s2].w, p.in_slope), a_hi[3] = lrelu_bf16x2(xb[s2].w, p.in_slope);
+            });
+            float out[1][4];
+            tail_layers(out, acc, w, p.n_hidden, p.slope, g, t);
+            if (p.scores) {
+                if (r0 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r0 * PT_NOUT + 2 * t) = make_float2(out[0][0], out[0][1]);
+                if (r1 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r1 * PT_NOUT + 2 * t) = make_float2(out[0][2], out[0][3]);
+            }
+#pragma unroll
+            for (int h = 0; h < 2; h++) {  // rows past the member's end: their draw is discarded
+                const int row = h ? r1 : r0;
+                const float s0 = out[0][2 * h], s1 = out[0][2 * h + 1];
+                float lp = 0.f;
+                const int best = draw_row<LOGP>(s0, s1, p.seed, step, row, p.n_actions, lane, t, lp);
+                if (row < r_end) {
+                    if (t == 0) p.actions[row] = best;
+                    if constexpr (LOGP) if (t == 0) p.logp[row] = lp;
+                    if (p.values && t == (p.n_actions >> 1)) p.values[row] = (p.n_actions & 1) ? s1 : s0;
+                }
+            }
+        }
+        tb = te;
+    }
+    advance_step(p.counter, step);
+}
+
+static int policy_tail_grouped_impl(const PolicyTailArgs &a, int k0, const int32_t *offsets, int n_members, cudaStream_t st) {
+    if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || !a.counter || !a.actions || !offsets ||
+        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)))
+        return fail(OVC_E_BADARG, "null pointer argument");
+    if ((((uintptr_t)a.x | (uintptr_t)a.w_first | (uintptr_t)a.w_hidden | (uintptr_t)a.w_heads) & 15) != 0)
+        return fail(OVC_E_BADARG, "x and the weight tables must be 16-byte aligned");
+    if ((((uintptr_t)a.b_first | (uintptr_t)a.b_hidden | (uintptr_t)a.b_heads | (uintptr_t)a.scores | (uintptr_t)a.counter) & 7) != 0)
+        return fail(OVC_E_BADARG, "biases, scores and counter must be 8-byte aligned");
+    if ((((uintptr_t)a.actions | (uintptr_t)a.values | (uintptr_t)a.logp | (uintptr_t)offsets) & 3) != 0)
+        return fail(OVC_E_BADARG, "actions, values, logp and offsets must be 4-byte aligned");
+    if (n_members < 1 || n_members > PT_MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+    if (k0 < 32 || k0 > 256 || k0 % 32) return fail(OVC_E_BADARG, "k0 must be a multiple of 32 in 32..256", k0);
+    if (a.n_hidden < 0 || a.n_hidden > 8) return fail(OVC_E_BADARG, "n_hidden must be 0..8", a.n_hidden);
+    if (a.n_actions < 1 || a.n_actions > 7) return fail(OVC_E_BADARG, "n_actions must be 1..7 (head n_actions is the value)", a.n_actions);
+    if (!(a.in_slope >= 0.f && a.in_slope <= 1.f && a.slope >= 0.f && a.slope <= 1.f)) return fail(OVC_E_BADARG, "slopes must lie in [0, 1]");
+    if (a.n_rows < 0 || a.n_rows > 0x7FFFFFFFll) return fail(OVC_E_BADARG, "n_rows must lie in [0, 2^31)", a.n_rows);
+    if (a.n_rows == 0) return OVC_OK;
+    int dev = 0, n_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    const size_t smem = tail_smem_bytes(k0, a.n_hidden) + 16;
+    // at most n_rows / 16 + n_members tiles: one wave of CTAs, never more than the SMs
+    const long long n_tiles = (a.n_rows + 15) / 16 + n_members, want = (n_tiles + PTG_THREADS / 32 - 1) / (PTG_THREADS / 32);
+    const unsigned grid = (unsigned)(want < n_sm ? want : n_sm);
+    cudaError_t e = cudaSuccess;
+#define OVC_LAUNCH_PTG(KS2)                                                                                            \
+    case KS2:                                                                                                          \
+        if (a.logp) {                                                                                                  \
+            e = cudaFuncSetAttribute(policy_tail_grouped_kernel<KS2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            if (e == cudaSuccess) policy_tail_grouped_kernel<KS2, true><<<grid, PTG_THREADS, smem, st>>>(a, offsets, n_members); \
+        } else {                                                                                                       \
+            e = cudaFuncSetAttribute(policy_tail_grouped_kernel<KS2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+            if (e == cudaSuccess) policy_tail_grouped_kernel<KS2, false><<<grid, PTG_THREADS, smem, st>>>(a, offsets, n_members); \
+        }                                                                                                              \
+        break;
+    switch (k0 / 32) {
+        OVC_LAUNCH_PTG(1) OVC_LAUNCH_PTG(2) OVC_LAUNCH_PTG(3) OVC_LAUNCH_PTG(4) OVC_LAUNCH_PTG(5) OVC_LAUNCH_PTG(6) OVC_LAUNCH_PTG(7) OVC_LAUNCH_PTG(8)
+    }
+#undef OVC_LAUNCH_PTG
+    if (e != cudaSuccess) return cuda_fail(e, "policy_tail_grouped kernel attribute");
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "policy_tail_grouped kernel launch");
+    return OVC_OK;
+}
+
 // hid: the HIDDEN instantiation into a.hidden (no heads, no draw; a.w_heads / a.b_heads are staged but never read, so the
 // entry point passes the first layer's tables, which are at least as large, in their place).  seat >= 0: the one-view
 // kernel with swap (ovc_policy_tail_view); -1: the two-view ones.  joint: rows is the joint-row map (ovc_policy_tail_joint).

@@ -683,6 +683,12 @@ def _capture_graph(env, live, warm_up, body):
     return graph
 
 
+# A population of learners runs grouped K9 from this many members on; below it, K9 per member on its block is faster
+# (cramped_room, 32 768 envs, inside a CUDA graph on an H100 80GB HBM3 at 700 W: 103.1 / 109.3 us grouped against
+# 89.9 / 101.1 us for K = 1 / 2, 110.1 against 116.3 us for K = 4; tools/prof_selfplay_population.py).
+GROUPED_K9_MIN_MEMBERS = 4
+
+
 class SelfPlayRollout(_FoldedPolicy):
     """Policy-in-the-loop rollout: both agents of every environment act from the same network, or, with a ``partner``,
     one seat of an environment is the partner's in the episodes the seat draw gives it (PPO_BC, or a self-play mixture with
@@ -692,7 +698,7 @@ class SelfPlayRollout(_FoldedPolicy):
 
     def __init__(self, env, model=None, autocast_dtype=torch.bfloat16, use_graph=True, reward_shaping_factor=1.0,
                  fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0, episode_capacity=1,
-                 max_seq_len=20, member=None, member_weights=None, use_phi=False):
+                 max_seq_len=20, member=None, member_weights=None, use_phi=False, blocks=None):
         """autocast_dtype: the dtype of the dense model (``DenseGridPolicy``, widths padded to 16-byte rows) and of the
         observation K2 writes for it: bfloat16 (the plane values are exact in bf16), or None for float32 throughout.
         fused_first_layer (default: on for the bf16 policy where ``fused_kernel_support`` allows K7): the observation is
@@ -740,12 +746,37 @@ class SelfPlayRollout(_FoldedPolicy):
         reward_shaping_factor * (phi(s') - phi(s))``, phi at gamma 0.99 with s' taken before an ending episode's reset,
         instead of ``sparse + reward_shaping_factor * shaped_i``.  Only the rewards, the returns, the advantages, the value
         targets and the episodes' reward sums change; the draws, the states and the game statistics are those without it.
-        Needs an ``auto_reset`` env."""
+        Needs an ``auto_reset`` env.
+        model may instead be a population of self-play learners (fictitious co-play's first stage): a list of 1..64
+        ``RllibShapedCNN`` members of one architecture.  Member k plays both views of the environments of its block
+        ``[blocks[k], blocks[k + 1])``; blocks (argument): K positive environment counts summing to N, default equal blocks
+        (``blocks[k] = k N // K``).  ``self.blocks`` is then the offsets (int32 [K + 1]) and ``self.member`` the member of
+        each environment (int32 [N]).  The fused layers run as one grouped launch each for all members
+        (``ovc_encode_linear_grouped``, ``ovc_wide_layers_grouped`` from ``GROUPED_K9_MIN_MEMBERS`` members on,
+        ``ovc_policy_tail_grouped``), library layers per member on its block's rows; every row is drawn with key ``seed``
+        and the one counter (grouped K8, or, without K8, one ``ovc_sample_actions`` over all rows): block k is bit
+        for bit what ``SelfPlayRollout(env, model[k], seed=seed)`` does on those environments.  ``sync_weights()`` refolds
+        every member.  Not with a ``partner`` or an ``RllibLSTMShapedCNN`` member."""
         self.env = env
         self._phi = _PhiReward(env) if use_phi else None
-        self._fold(env, model, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
+        models = list(model) if isinstance(model, (list, tuple)) else None
+        if models is not None:
+            assert 1 <= len(models) <= MAX_MEMBERS, "a population of learners has 1..%d members" % MAX_MEMBERS
+            for m in models:
+                assert isinstance(m, RllibShapedCNN) and not isinstance(m, RllibLSTMShapedCNN), \
+                    "a population learner is an RllibShapedCNN (an LSTM member is not supported)"
+            arch = lambda m: (m.dense_slope,) + tuple((n, tuple(p.shape)) for n, p in m.named_parameters())
+            assert len({arch(m) for m in models}) == 1, "the members of a population of learners must share one architecture"
+            assert partner is None, "a population of learners plays self-play only: no partner with a list model"
+        else:
+            assert blocks is None, "blocks go with a population of learners (a list model)"
+        self._fold(env, models[0] if models else model, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
         dev = env.device
         N = env.n_envs
+        self._members = None  # a population of learners: the K folded members, self first
+        self._member = None
+        if models is not None:
+            self._fold_members(models, blocks, autocast_dtype)
         self.partner = None
         self.bc = float(bc_factor)
         self.population = isinstance(partner, (list, tuple))
@@ -864,9 +895,92 @@ class SelfPlayRollout(_FoldedPolicy):
 
     @property
     def member(self):
-        """int32 [N]: each environment's population member in its running episode (None without a population); it plays
-        only where ``partner_seat >= 0``."""
-        return self._pop.member if self.population else None
+        """int32 [N]: with a population of partners, each environment's member in its running episode (it plays only where
+        ``partner_seat >= 0``); with a population of learners, the member that plays environment e (fixed); else None."""
+        return self._pop.member if self.population else self._member
+
+    def _fold_members(self, models, blocks, autocast_dtype):
+        """A population of learners: fold members 1.. like member 0 (self), set the blocks, and stack the K8 tables so that
+        each member's tables are views of the stack (its ``sync_weights`` then refreshes the stack in place)."""
+        env, N, dev, K = self.env, self.env.n_envs, self.env.device, len(models)
+        if blocks is None:
+            assert N >= K, "equal blocks need at least one environment per member (%d members, %d environments)" % (K, N)
+            counts = [(k + 1) * N // K - k * N // K for k in range(K)]
+        else:
+            counts = [int(b) for b in blocks]
+            assert len(counts) == K, "blocks: one environment count per member (%d)" % K
+            assert all(c > 0 for c in counts) and sum(counts) == N, \
+                "blocks: positive environment counts summing to the %d environments, got %s" % (N, counts)
+        self._offs = [0] + np.cumsum(counts).tolist()
+        self.blocks = torch.tensor(self._offs, dtype=torch.int32, device=dev)
+        self._row_offsets = 2 * self.blocks  # K8's offsets are joint rows
+        self._member = torch.repeat_interleave(torch.arange(K, dtype=torch.int32, device=dev),
+                                               torch.tensor(counts, device=dev)).to(torch.int32)
+        self._members = [self]
+        for m in models[1:]:
+            f = _FoldedPolicy()
+            f.env = env
+            f._fold(env, m, autocast_dtype, self.fused_first_layer, self.fused_tail, self.fused_wide)
+            self._members.append(f)
+        def stack(attr):  # the grouped kernels' stacked tables; each member's tables become views of them
+            st = tuple(torch.stack([getattr(f, attr)[i] for f in self._members]) for i in range(len(getattr(self, attr))))
+            for k, f in enumerate(self._members):
+                setattr(f, attr, tuple(t[k] for t in st))
+            return st
+        if self.fused_first_layer:
+            self._k7_stack = (torch.stack([f._wt0 for f in self._members]), torch.stack([f._b0 for f in self._members]))
+            for k, f in enumerate(self._members):
+                f._wt0, f._b0 = self._k7_stack[0][k], self._k7_stack[1][k]
+        if self.fused_wide:
+            self._wide_stack = stack("_wide")
+        if self.fused_tail:
+            self._tail_stack = stack("_tail")
+
+    def _policy_members(self, actions, vals, logp, scores8, counter):
+        """``_policy`` for a population of learners: grouped K7, K9 (from ``GROUPED_K9_MIN_MEMBERS`` members on, else K9 per
+        member on its block) and grouped K8 (None returned); off the fused path, library layers per member on its block's rows
+        ``[2 o_k, 2 o_{k+1})`` and, without K8, member k's logits into its rows of self._scores (returned for the one draw
+        kernel over all rows)."""
+        env, lib, rows = self.env, _native.lib(), 2 * self.env.n_envs
+        with torch.no_grad():
+            if self.fused_first_layer:  # grouped K7
+                wt, b0 = self._k7_stack
+                _native.check(lib.ovc_encode_linear_grouped(
+                    env.tables.data_ptr(), env.n_layouts, env.state.data_ptr(), wt.data_ptr(), b0.data_ptr(), self.blocks.data_ptr(),
+                    len(self._members), self._act0.data_ptr(), env.n_envs, env.state_words, self.W, self.H,
+                    env.horizon if env.horizon > 0 else 2**31 - 1, wt.shape[2], 0.2, env._stream()))
+                flat, first = self._act0, 1
+            else:
+                flat, first = self.obs.view(rows, self.W * self.H * 26), 0
+            if self.fused_wide and len(self._members) >= GROUPED_K9_MIN_MEMBERS:  # grouped K9
+                w1, b1, w2, b2 = self._wide_stack
+                _native.check(lib.ovc_wide_layers_grouped(flat.data_ptr(), rows, flat.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[1],
+                                                          w2.data_ptr(), b2.data_ptr(), w2.shape[1], 0.2, self._row_offsets.data_ptr(),
+                                                          len(self._members), self._z.data_ptr(), env._stream()))
+            for k, f in enumerate(self._members):  # per member on its block's rows [2 o_k, 2 o_{k+1})
+                r = slice(2 * self._offs[k], 2 * self._offs[k + 1])
+                if self.fused_wide and len(self._members) < GROUPED_K9_MIN_MEMBERS:  # K9 on the block
+                    w1, b1, w2, b2 = f._wide
+                    x, z = flat[r], self._z[r]
+                    _native.check(lib.ovc_wide_layers(x.data_ptr(), x.shape[0], x.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
+                                                      w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, z.data_ptr(), env._stream()))
+                elif not self.fused_tail:  # library layers; bit for bit the member's own rollout only where cuBLAS computes a
+                    # row independently of the row count (tested at up to 2 x 300 rows per call)
+                    logits, value = f.dense_model.forward_from(flat[r], first)
+                    self._scores[r].copy_(logits)
+                    vals[r].copy_(value)
+                elif not self.fused_wide:
+                    f.dense_model.trunk(flat[r], first, out=self._z[r])
+            if not self.fused_tail:
+                return self._scores
+            w1, b1, wh, bh, wo, bo = self._tail_stack
+            ptr = lambda t: 0 if t is None else t.data_ptr()
+            _native.check(lib.ovc_policy_tail_grouped(
+                self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(), wh.shape[1],
+                wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1), counter.data_ptr(),
+                self._row_offsets.data_ptr(), len(self._members), actions.data_ptr(), vals.data_ptr(), ptr(scores8), ptr(logp),
+                env._stream()))
+        return None
 
     def _assign_partners(self, done):
         self.env.assign_partners(self.partner_seat, self._bc_factor, self._seat_counter, seed=self.seed ^ PARTNER_SEAT_SALT, done=done)
@@ -881,11 +995,13 @@ class SelfPlayRollout(_FoldedPolicy):
                                  n_actions=self._partner_n_actions, out=actions)
 
     def sync_weights(self):
-        """Re-fold the learner (``_FoldedPolicy.sync_weights``) and a network partner or every population member, in place:
-        the captured graphs use the new weights without a re-capture."""
+        """Re-fold the learner (``_FoldedPolicy.sync_weights``) and a network partner or every population member, or every
+        member of a population of learners, in place: the captured graphs use the new weights without a re-capture."""
         _FoldedPolicy.sync_weights(self)
         if self._pop is not None:
             self._pop.sync_weights()
+        for f in (self._members or [])[1:]:
+            f.sync_weights()
 
     def _capture(self, warm_up, body):
         """A CUDA graph of ``body``, captured after ``warm_up`` (on a side stream).  Warm-up and capture must not advance
@@ -910,6 +1026,8 @@ class SelfPlayRollout(_FoldedPolicy):
         vals = self.values.view(rows) if values is None else values
         scores8 = self._scores8 if scores8 is None else scores8
         counter = self._draw_counter if counter is None else counter
+        if self._members is not None:
+            return self._policy_members(actions, vals, logp, scores8, counter)
         with torch.no_grad():
             if self.fused_first_layer:
                 flat, first = env.encoded_linear(self._wt0, self._b0, out=self._act0, neg_slope=0.2), 1  # K7
