@@ -656,6 +656,37 @@ static int step_impl(const void *layouts, int n_layouts, const int32_t *start_re
 #include "ovc_potential.cuh"
 #include "ovc_host.cuh"
 
+namespace ovc {
+
+// The parameter block of K8 (ovc_policy_tail and its forms) from the C entry points' common argument list.
+static PolicyTailArgs tail_args(const void *x, int64_t n_rows, float in_slope, const void *w_first, const float *b_first,
+                                const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                                float slope, int n_actions, uint64_t seed, uint64_t *counter, int32_t *actions, float *values,
+                                float *scores, float *logp) {
+    PolicyTailArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
+    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
+    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
+    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    return a;
+}
+
+// The parameter block of K11 (ovc_lstm_head, ovc_lstm_head_view: swap / seat are read by the one-view form only).
+static LstmHeadArgs lstm_head_args(const void *x, const void *h_in, const float *c_in, const int32_t *reset, int64_t n_rows,
+                                   const void *w, const float *b, const void *w_heads, const float *b_heads, int n_actions,
+                                   uint64_t seed, uint64_t *counter, const int32_t *swap, int seat, void *h_out, float *c_out,
+                                   void *snap_h, float *snap_c, int32_t *actions, float *values, float *logp, float *scores) {
+    LstmHeadArgs a;
+    a.x = (const __nv_bfloat16 *)x, a.h_in = (const __nv_bfloat16 *)h_in, a.c_in = c_in, a.reset = reset, a.n_rows = n_rows;
+    a.w = (const __nv_bfloat16 *)w, a.b = b, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
+    a.n_actions = n_actions, a.seed = seed, a.counter = (unsigned long long *)counter;
+    a.h_out = (__nv_bfloat16 *)h_out, a.c_out = c_out, a.snap_h = (__nv_bfloat16 *)snap_h, a.snap_c = snap_c;
+    a.actions = actions, a.values = values, a.logp = logp, a.scores = scores, a.swap = swap, a.seat = seat;
+    return a;
+}
+
+}  // namespace ovc
+
 // ------------------------------------------------------------------------------------------------
 // C ABI
 // ------------------------------------------------------------------------------------------------
@@ -791,11 +822,8 @@ int ovc_policy_tail_logp(const void *x, int64_t n_rows, int k0, float in_slope, 
                          const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                          float slope, int n_actions, uint64_t seed, uint64_t *counter, int32_t *actions, float *values, float *scores,
                          float *logp, void *stream) {
-    ovc::PolicyTailArgs a;
-    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
-    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
-    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
-    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    const ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                                 n_actions, seed, counter, actions, values, scores, logp);
     return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream);
 }
 
@@ -803,23 +831,18 @@ int ovc_policy_tail_view(const void *x, int64_t n_rows, int k0, float in_slope, 
                          const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                          float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *swap, int seat, int32_t *actions,
                          float *values, float *scores, float *logp, void *stream) {
-    ovc::PolicyTailArgs a;
-    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
-    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
-    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
-    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    const ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                                 n_actions, seed, counter, actions, values, scores, logp);
     if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
     return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, swap, seat);
 }
 
 int ovc_policy_hidden(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
                       const void *w_hidden, const float *b_hidden, int n_hidden, float slope, void *hidden, void *stream) {
-    ovc::PolicyTailArgs a;
-    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
-    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden;
-    a.w_heads = (const __nv_bfloat16 *)w_first, a.b_heads = b_first;  // staged, never read (see policy_tail_impl)
-    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = 1, a.in_slope = in_slope, a.slope = slope, a.seed = 0;
-    a.counter = nullptr, a.actions = nullptr, a.values = nullptr, a.hidden = (__nv_bfloat16 *)hidden, a.logp = nullptr;
+    // w_heads / b_heads: staged, never read (see policy_tail_impl)
+    ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_first, b_first, slope, 1,
+                                           0, nullptr, nullptr, nullptr, nullptr, nullptr);
+    a.hidden = (__nv_bfloat16 *)hidden;
     return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, true);
 }
 
@@ -827,12 +850,8 @@ int ovc_lstm_head(const void *x, const void *h_in, const float *c_in, const int3
                   const float *b, const void *w_heads, const float *b_heads, int n_actions, uint64_t seed, uint64_t *counter,
                   void *h_out, float *c_out, void *snap_h, float *snap_c, int32_t *actions, float *values, float *logp,
                   float *scores, void *stream) {
-    ovc::LstmHeadArgs a;
-    a.x = (const __nv_bfloat16 *)x, a.h_in = (const __nv_bfloat16 *)h_in, a.c_in = c_in, a.reset = reset, a.n_rows = n_rows;
-    a.w = (const __nv_bfloat16 *)w, a.b = b, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
-    a.n_actions = n_actions, a.seed = seed, a.counter = (unsigned long long *)counter;
-    a.h_out = (__nv_bfloat16 *)h_out, a.c_out = c_out, a.snap_h = (__nv_bfloat16 *)snap_h, a.snap_c = snap_c;
-    a.actions = actions, a.values = values, a.logp = logp, a.scores = scores;
+    const ovc::LstmHeadArgs a = ovc::lstm_head_args(x, h_in, c_in, reset, n_rows, w, b, w_heads, b_heads, n_actions, seed, counter,
+                                                     nullptr, 0, h_out, c_out, snap_h, snap_c, actions, values, logp, scores);
     return ovc::lstm_head_impl(a, (cudaStream_t)stream);
 }
 
@@ -840,12 +859,8 @@ int ovc_lstm_head_view(const void *x, const void *h_in, const float *c_in, const
                        const float *b, const void *w_heads, const float *b_heads, int n_actions, uint64_t seed, uint64_t *counter,
                        const int32_t *swap, int seat, void *h_out, float *c_out, void *snap_h, float *snap_c, int32_t *actions,
                        float *values, float *logp, float *scores, void *stream) {
-    ovc::LstmHeadArgs a;
-    a.x = (const __nv_bfloat16 *)x, a.h_in = (const __nv_bfloat16 *)h_in, a.c_in = c_in, a.reset = reset, a.n_rows = n_rows;
-    a.w = (const __nv_bfloat16 *)w, a.b = b, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
-    a.n_actions = n_actions, a.seed = seed, a.counter = (unsigned long long *)counter;
-    a.h_out = (__nv_bfloat16 *)h_out, a.c_out = c_out, a.snap_h = (__nv_bfloat16 *)snap_h, a.snap_c = snap_c;
-    a.actions = actions, a.values = values, a.logp = logp, a.scores = scores, a.swap = swap, a.seat = seat;
+    const ovc::LstmHeadArgs a = ovc::lstm_head_args(x, h_in, c_in, reset, n_rows, w, b, w_heads, b_heads, n_actions, seed, counter,
+                                                     swap, seat, h_out, c_out, snap_h, snap_c, actions, values, logp, scores);
     if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
     return ovc::lstm_head_impl(a, (cudaStream_t)stream, true);
 }
@@ -914,11 +929,8 @@ int ovc_policy_tail_rows(const void *x, int64_t n_rows, int k0, float in_slope, 
                          const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                          float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *swap, int seat, const int32_t *rows,
                          const int32_t *range, int32_t *actions, float *values, float *scores, float *logp, void *stream) {
-    ovc::PolicyTailArgs a;
-    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
-    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
-    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
-    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    const ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                                 n_actions, seed, counter, actions, values, scores, logp);
     if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
     if (!rows || !range) return ovc::fail(OVC_E_BADARG, "null pointer argument");
     return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, swap, seat, rows, range);
@@ -957,11 +969,8 @@ int ovc_policy_tail_joint(const void *x, int64_t n_rows, int k0, float in_slope,
                           const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                           float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *jrow, const int32_t *range,
                           int32_t *actions, float *values, float *scores, float *logp, void *stream) {
-    ovc::PolicyTailArgs a;
-    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
-    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
-    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
-    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    const ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                                 n_actions, seed, counter, actions, values, scores, logp);
     if (n_rows > 0x7FFFFFFFll) return ovc::fail(OVC_E_BADARG, "n_rows must be below 2^31", n_rows);
     return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, nullptr, -1, jrow, range, true);
 }
@@ -986,11 +995,8 @@ int ovc_policy_tail_grouped(const void *x, int64_t n_rows, int k0, float in_slop
                             const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                             float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *offsets, int n_members,
                             int32_t *actions, float *values, float *scores, float *logp, void *stream) {
-    ovc::PolicyTailArgs a;
-    a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
-    a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
-    a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
-    a.counter = (unsigned long long *)counter, a.actions = actions, a.values = values, a.scores = scores, a.logp = logp;
+    const ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                                 n_actions, seed, counter, actions, values, scores, logp);
     return ovc::policy_tail_grouped_impl(a, k0, offsets, n_members, (cudaStream_t)stream);
 }
 

@@ -637,6 +637,89 @@ class _FoldedPolicy(object):
             for dst, src in pairs:
                 dst.copy_(src)
 
+    def _chain_buffers(self, rows):
+        """The buffers of ``_chain`` on ``rows`` rows: K7's output, K8's input (the last convolution's pre-activation), the
+        library layers' logits, and the LSTM's input and live state (zero at every episode start)."""
+        dev = self.env.device
+        if self.fused_first_layer:
+            self._act0 = torch.empty((rows, self._wt0.shape[1]), dtype=torch.bfloat16, device=dev)
+        if self.fused_tail:
+            self._z = torch.empty((rows, self._tail[0].shape[1]), dtype=torch.bfloat16, device=dev)
+        self._scores = torch.empty((rows, 6), dtype=torch.float32, device=dev)
+        if self.lstm:
+            cell = self.model.lstm.hidden_size
+            self._x = torch.empty((rows, self.model.lstm.input_size), dtype=torch.bfloat16, device=dev)
+            self.h = torch.zeros((rows, cell), dtype=torch.bfloat16, device=dev)
+            self.c = torch.zeros((rows, cell), dtype=torch.float32, device=dev)
+
+    def _k9_args(self, x, tables=None):
+        """``ovc_wide_layers``' arguments (and its range and grouped forms') up to the slope, on the rows of ``x``
+        [rows, k0]: ``tables`` (default this policy's) may be a member stack."""
+        w1, b1, w2, b2 = self._wide if tables is None else tables
+        return (x.data_ptr(), x.shape[0], x.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[-2], w2.data_ptr(), b2.data_ptr(),
+                w2.shape[-2], 0.2)
+
+    def _k8_args(self, x, tables=None):
+        """K8's arguments on the rows of ``x`` [rows, k0]: up to the seed for the drawing forms (``ovc_policy_tail`` and its
+        view, rows, joint and grouped forms), up to the dense slope for ``ovc_policy_hidden`` (LSTM policy).  ``tables``
+        (default this policy's) may be a member stack."""
+        w1, b1, wh, bh = (self._tail if tables is None else tables)[:4]
+        args = (x.data_ptr(), x.shape[0], x.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(), wh.shape[-3])
+        if self.lstm:
+            return args + (self.dense_model.dense_slope,)
+        wo, bo = (self._tail if tables is None else tables)[4:]
+        return args + (wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1))
+
+    def _chain(self, flat, actions, values, logp, scores8, counter, view=None, state_out=None, snap=None):
+        """The policy after its first layer, on the rows of ``flat`` (K7's output, else the observation's rows): K9 or the
+        library trunk, then K8's draw; or K8's hidden output (or the library layers) and K11 on the live state, which it
+        writes to ``state_out`` (h, c) (default in place) and, as it used it, to ``snap``; or the library layers to
+        ``self._scores`` and ``values``.  ``view`` None: both views of every environment (the two-view entry points), and
+        the library path returns the logits for the caller to draw from.  ``view`` (seat, swap): one view per environment
+        (the ``_view`` entry points, ``sample_actions_view``).  Returns None once the actions are drawn."""
+        env, lib, stream = self.env, _native.lib(), self.env._stream()
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        first = 1 if self.fused_first_layer else 0
+        with torch.no_grad():
+            if self.fused_wide:
+                _native.check(lib.ovc_wide_layers(*self._k9_args(flat), self._z.data_ptr(), stream))
+            elif self.fused_tail:
+                self.dense_model.trunk(flat, first, out=self._z)
+            if self.lstm:
+                if self.fused_tail:
+                    _native.check(lib.ovc_policy_hidden(*self._k8_args(self._z), self._x.data_ptr(), stream))
+                else:
+                    self._x.copy_(self.dense_model.hidden_from(flat, first))
+                w, b, wo, bo = self._lstm_tables
+                h_out, c_out = state_out or (self.h, self.c)
+                snap_h, snap_c = snap or (None, None)
+                head = (self._x.data_ptr(), self.h.data_ptr(), self.c.data_ptr(), env.done.data_ptr(), self._x.shape[0], w.data_ptr(),
+                        b.data_ptr(), wo.data_ptr(), bo.data_ptr(), self.dense_model.n_actions, self.seed & (2**64 - 1),
+                        counter.data_ptr()) + (() if view is None else (ptr(view[1]), view[0]))
+                out = (h_out.data_ptr(), c_out.data_ptr(), ptr(snap_h), ptr(snap_c), actions.data_ptr(), ptr(values), ptr(logp),
+                       ptr(scores8), stream)
+                _native.check((lib.ovc_lstm_head if view is None else lib.ovc_lstm_head_view)(*head, *out))
+                return None
+            if self.fused_tail:
+                args = self._k8_args(self._z) + (counter.data_ptr(),)
+                if view is not None:
+                    _native.check(lib.ovc_policy_tail_view(*args, ptr(view[1]), view[0], actions.data_ptr(), values.data_ptr(),
+                                                           ptr(scores8), ptr(logp), stream))
+                elif logp is None:
+                    _native.check(lib.ovc_policy_tail(*args, actions.data_ptr(), values.data_ptr(), ptr(scores8), stream))
+                else:
+                    _native.check(lib.ovc_policy_tail_logp(*args, actions.data_ptr(), values.data_ptr(), ptr(scores8), logp.data_ptr(),
+                                                           stream))
+                return None
+            logits, value = self.dense_model.forward_from(flat, first)
+            self._scores.copy_(logits)
+            values.copy_(value)
+            if view is None:
+                return self._scores
+            env.sample_actions_view(self._scores, counter, view[0], view[1], seed=self.seed, out=actions, logp_out=logp)
+            if scores8 is not None:
+                scores8[:, :self._scores.shape[1]].copy_(self._scores)
+        return None
 
 
 PHI_GAMMA = 0.99  # the gamma of the reference's use_phi reward (get_state_transition(display_phi=True), MDP:1422-1429)
@@ -689,7 +772,140 @@ def _capture_graph(env, live, warm_up, body):
 GROUPED_K9_MIN_MEMBERS = 4
 
 
-class SelfPlayRollout(_FoldedPolicy):
+def _check_members(members, most, kinds, count_msg, kind_msg):
+    """The checks on a population of models: 1..``most`` members, each an instance of ``kinds`` and none an
+    ``RllibLSTMShapedCNN`` (K11 has no rows or grouped form)."""
+    assert 1 <= len(members) <= most, count_msg
+    for m in members:
+        assert isinstance(m, kinds) and not isinstance(m, RllibLSTMShapedCNN), kind_msg
+
+
+class _Rollout(object):
+    """The rollout driver of ``SelfPlayRollout`` and ``AgentPairRollout``: run() and collect() over the subclass's
+    ``_transition(b, t)``, their CUDA graphs, the bootstrap step's scratch and GAE, the returns, the episode statistics and
+    records, the shaping factor, the seat draw and the population's members.  A subclass provides ``_transition``,
+    ``_live()`` (the tensors a transition advances besides the state, the returns, the statistics and the records),
+    ``_bootstrap(b)`` (the learner's value of the state after a window into ``b.last_values``), ``_new_batch(n_steps,
+    keep_logits)`` and ``_agents()`` (its policies); it sets ``population``, ``_pop`` (the population, or None) and
+    ``_member``."""
+
+    def _init_rollout(self, env, learner, use_graph, reward_shaping_factor, episode_capacity, max_seq_len):
+        """The shared state; ``learner`` is the policy whose LSTM state (if any) the bootstrap step leaves alone."""
+        N, dev = env.n_envs, env.device
+        self.use_graph = use_graph
+        self.actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
+        self.ret_sparse = torch.zeros(N, dtype=torch.int64, device=dev)  # running episode return (sparse)
+        self.factor = float(reward_shaping_factor)
+        self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by the captured graphs
+        self.stats = EpisodeStats(env)
+        self.episodes = EpisodeRecords(env, episode_capacity, members=self.population)
+        self.max_seq_len = int(max_seq_len)
+        assert self.max_seq_len >= 1
+        self.graph = None          # run()'s CUDA graph of one transition
+        self._collect_graphs = {}  # (n_steps, keep_logits) -> ((gamma, lam), CUDA graph of the window)
+        self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
+        self._boot_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # the bootstrap's draws leave the learner's counter alone
+        self._boot_actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
+        if learner.lstm:  # the bootstrap's (discarded) LSTM state: the next window continues from the live state
+            self._h_boot, self._c_boot = torch.empty_like(learner.h), torch.empty_like(learner.c)
+
+    @property
+    def reward_shaping_factor(self):
+        """The factor of the shaped rewards (rllib.py:328-329) in the rewards, the returns and the episode records'
+        ``ep_reward_by_agent``.  Setting it takes effect in run() and collect() alike, without a re-capture (their graphs
+        read a device scalar)."""
+        return self.factor
+
+    @reward_shaping_factor.setter
+    def reward_shaping_factor(self, value):
+        self.factor = float(value)
+        self._factor.fill_(self.factor)
+
+    @property
+    def member_weights(self):
+        """The population's draw weights (K non-negative floats with a positive sum).  Setting them writes the device
+        table the draw reads, so run() and collect() follow a new distribution at the next episode ends without a re-capture
+        (prioritised sampling of the population between windows)."""
+        assert self._pop is not None and self._pop._thresholds is not None, "member_weights: a population drawn per episode"
+        return self._pop.weights
+
+    @member_weights.setter
+    def member_weights(self, value):
+        assert self._pop is not None and self._pop._thresholds is not None, "member_weights: a population drawn per episode"
+        self._pop.weights = value
+
+    @property
+    def member(self):
+        """int32 [N]: with a population of partners, each environment's member in its running episode (in a self-play
+        mixture it plays only where ``partner_seat >= 0``); with a population of learners, the member that plays environment
+        e (fixed); else None."""
+        return self._member if self._pop is None else self._pop.member
+
+    def _assign_seats(self, done):
+        """The seat draw (``env.assign_partners``): ``partner_seat`` for every environment whose episode ended (done None:
+        every environment), paired with probability ``_bc_factor``."""
+        self.env.assign_partners(self.partner_seat, self._bc_factor, self._seat_counter, seed=self.seed ^ PARTNER_SEAT_SALT, done=done)
+
+    def _capture(self, warm_up, body):
+        """A CUDA graph of ``body``, captured after ``warm_up`` (on a side stream).  Warm-up and capture must not advance
+        the environments: the state, the returns, the episode statistics and records, the draw counters and the seats are
+        restored after them."""
+        live = [self.env.state, self.ret_sparse] + self.stats.state_tensors() + self.episodes.tensors() + self._live()
+        return _capture_graph(self.env, live, warm_up, body)
+
+    def run(self, n_steps):
+        """Advance every environment n_steps transitions (one CUDA graph per transition with use_graph); returns the number
+        of env-steps done."""
+        if self.use_graph and self.graph is None:
+            def warm_up():
+                for _ in range(3):
+                    self._transition()
+            self.graph = self._capture(warm_up, self._transition)
+        step = self._transition if self.graph is None else self.graph.replay
+        for _ in range(n_steps):
+            step()
+        return n_steps * self.env.n_envs
+
+    def _collect_window(self, b, n_steps, gamma, lam):
+        """n_steps transitions into slots 0.. of ``b``, then the bootstrap value of the state after them and GAE over the
+        whole batch."""
+        b.episodes.clear()
+        for t in range(n_steps):
+            self._transition(b, t)
+        self._bootstrap(b)
+        gae = self.env.gae_view if b.one_view else self.env.gae
+        gae(b.rewards, b.values, b.dones, b.last_values, gamma, lam, b.advantages, b.value_targets)
+
+    def collect(self, n_steps, gamma, lam, keep_logits=False):
+        """Advance every environment n_steps transitions, as run() does (the same kernels and the same draws from the same
+        seed and counters), and return them as a ``SampleBatch`` with GAE(gamma, lam) advantages.  The batch's tensors are
+        reused: the next collect() with the same n_steps / keep_logits overwrites them.  With use_graph the whole window
+        is one CUDA graph (captured once per n_steps / keep_logits; a new gamma or lam re-captures it); no host
+        synchronisation otherwise.  With a population, the batch's ``partner_member`` is each transition's member."""
+        assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
+        key = (int(n_steps), bool(keep_logits))
+        b = self._batches.get(key)
+        if b is None:
+            b = self._batches[key] = self._new_batch(n_steps, keep_logits)
+        if not self.use_graph:
+            self._collect_window(b, n_steps, gamma, lam)
+            return b
+        g = self._collect_graphs.get(key)
+        if g is None or g[0] != (gamma, lam):
+            g = self._collect_graphs[key] = ((gamma, lam), self._capture(lambda: self._collect_window(b, 1, gamma, lam),
+                                                                         lambda: self._collect_window(b, n_steps, gamma, lam)))
+        g[1].replay()
+        return b
+
+    def reset_state(self):
+        """Zero the LSTM policies' live state.  run() and collect() zero it at every auto-reset (through ``env.done``); call
+        this after resetting the environments directly (``env.reset()``), so that the new episodes start from zero state."""
+        for a in self._agents():
+            if a.lstm:
+                a.h.zero_(), a.c.zero_()
+
+
+class SelfPlayRollout(_FoldedPolicy, _Rollout):
     """Policy-in-the-loop rollout: both agents of every environment act from the same network, or, with a ``partner``,
     one seat of an environment is the partner's in the episodes the seat draw gives it (PPO_BC, or a self-play mixture with
     a frozen network or a population).  The network evaluated is
@@ -761,10 +977,8 @@ class SelfPlayRollout(_FoldedPolicy):
         self._phi = _PhiReward(env) if use_phi else None
         models = list(model) if isinstance(model, (list, tuple)) else None
         if models is not None:
-            assert 1 <= len(models) <= MAX_MEMBERS, "a population of learners has 1..%d members" % MAX_MEMBERS
-            for m in models:
-                assert isinstance(m, RllibShapedCNN) and not isinstance(m, RllibLSTMShapedCNN), \
-                    "a population learner is an RllibShapedCNN (an LSTM member is not supported)"
+            _check_members(models, MAX_MEMBERS, RllibShapedCNN, "a population of learners has 1..%d members" % MAX_MEMBERS,
+                           "a population learner is an RllibShapedCNN (an LSTM member is not supported)")
             arch = lambda m: (m.dense_slope,) + tuple((n, tuple(p.shape)) for n, p in m.named_parameters())
             assert len({arch(m) for m in models}) == 1, "the members of a population of learners must share one architecture"
             assert partner is None, "a population of learners plays self-play only: no partner with a list model"
@@ -773,79 +987,52 @@ class SelfPlayRollout(_FoldedPolicy):
         self._fold(env, models[0] if models else model, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
         dev = env.device
         N = env.n_envs
-        self._members = None  # a population of learners: the K folded members, self first
+        self.seed = int(seed)
+        self._others = None  # a population of learners: members 1.. folded (member 0 is self)
         self._member = None
         if models is not None:
             self._fold_members(models, blocks, autocast_dtype)
-        self.partner = None
+        self.partner = partner
         self.bc = float(bc_factor)
         self.population = isinstance(partner, (list, tuple))
-        self._pop = None  # the network partner or the population (a _Population)
-        if self.population:
-            assert 1 <= len(partner) <= MAX_MEMBERS - 1, \
-                "a mixture's population has 1..%d members (one of ovc_group_members' %d groups holds the self-play environments)" \
-                % (MAX_MEMBERS - 1, MAX_MEMBERS)
-        else:
+        if partner is not None:
+            _check_members(partner if self.population else [partner], MAX_MEMBERS - 1, (RllibShapedCNN, BCPolicy),
+                           "a mixture's population has 1..%d members (one of ovc_group_members' %d groups holds the self-play "
+                           "environments)" % (MAX_MEMBERS - 1, MAX_MEMBERS),
+                           "a partner is a BCPolicy, an RllibShapedCNN or a list of them (an LSTM partner or member is not "
+                           "supported in a self-play mixture: ovc_lstm_head has no rows form)")
+        if not self.population:
             assert member is None and member_weights is None, "member / member_weights go with a population in partner"
-        for m in (list(partner) if self.population else [partner] if partner is not None else []):
-            assert not isinstance(m, RllibLSTMShapedCNN), \
-                "an LSTM partner or member is not supported in a self-play mixture (ovc_lstm_head has no rows form)"
-            assert isinstance(m, (RllibShapedCNN, BCPolicy)), "a partner is a BCPolicy, an RllibShapedCNN or a list of them"
+        self._partner = None  # the partner's agent: a _BCAgent, or a _Population (of one for a network partner)
+        self._pop = None      # the population of partners
         if partner is not None:
             self._bc_factor = torch.full((1,), self.bc, dtype=torch.float32, device=dev)  # read by the seat draw
             self.partner_seat = torch.full((N,), -1, dtype=torch.int32, device=dev)
             self._seat_counter = torch.zeros(2, dtype=torch.int64, device=dev)     # [step, scratch] of the seat draw
         if isinstance(partner, BCPolicy):
-            self.partner = partner.to(dev).eval()
-            self._partner_tables = self.partner.tables()
-            self._partner_n_actions = self.partner.logits.out_features
-            self._partner_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of K10's draw
+            self._partner = _BCAgent(env, partner, self.partner_seat, seed)
+            self._partner_counter = self._partner._counter  # [step, scratch] of K10's draw
         elif partner is not None:
-            self.partner = partner
             members = list(partner) if self.population else [partner]
             if not self.population:  # one network partner: a population of one, its member fixed
                 member = torch.zeros(N, dtype=torch.int32, device=dev)
-            self._pop = _Population(env, members, self.partner_seat, seed, autocast_dtype, member, member_weights, mixture=True)
+            self._partner = _Population(env, members, self.partner_seat, seed, autocast_dtype, member, member_weights, mixture=True)
+            self._pop = self._partner if self.population else None
         self._learner_rows = False
-        self.factor = float(reward_shaping_factor)
-        self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by the captured graphs
-        N = env.n_envs
         self.obs = None if self.fused_first_layer else torch.empty((N, 2, self.W, self.H, 26), dtype=autocast_dtype or torch.float32, device=dev)
-        if self.fused_first_layer:
-            self._act0 = torch.empty((2 * N, self._wt0.shape[1]), dtype=torch.bfloat16, device=dev)
-        self.actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
-        self.ret_sparse = torch.zeros(N, dtype=torch.int64, device=dev)      # running episode return (sparse)
+        self._chain_buffers(2 * N)
         self.ret_mixed = torch.zeros(N, dtype=torch.float32, device=dev)    # sparse + factor * shaped (rllib.py:328-329)
         self.values = torch.zeros((N, 2), dtype=torch.float32, device=dev)
-        self.stats = EpisodeStats(env)
-        self.episodes = EpisodeRecords(env, episode_capacity)
         self.native_glue = True  # the draw and the returns are always native kernels; bench.py's launch count reads this
-        if self.fused_tail:
-            self._z = torch.empty((2 * N, self._tail[0].shape[1]), dtype=torch.bfloat16, device=dev)  # last convolution, pre-activation
-        if self.lstm:
-            self.max_seq_len = int(max_seq_len)
-            assert self.max_seq_len >= 1
-            cell =self.model.lstm.hidden_size
-            self._x = torch.empty((2 * N, self.model.lstm.input_size), dtype=torch.bfloat16, device=dev)  # the LSTM's input
-            self.h = torch.zeros((2 * N, cell), dtype=torch.bfloat16, device=dev)  # the live state, zero at every episode start
-            self.c = torch.zeros((2 * N, cell), dtype=torch.float32, device=dev)
-            self._h_boot, self._c_boot = torch.empty_like(self.h), torch.empty_like(self.c)  # the bootstrap's (discarded) state
-        self.seed = int(seed)
+        self._init_rollout(env, self, use_graph, reward_shaping_factor, episode_capacity, max_seq_len)
         self._draw_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of ovc_sample_actions
         self._scores8 = None  # set to a float32 [2N, 8] tensor to make K8 also write the heads (tests)
-        self._scores = torch.empty((2 * N, 6), dtype=torch.float32, device=dev)
-        self.graph = None          # run()'s CUDA graph of one transition
-        self.use_graph = use_graph
-        self._collect_graphs = {}  # (n_steps, keep_logits) -> ((gamma, lam), CUDA graph of the window)
-        self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
-        self._boot_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # the bootstrap's draws leave _draw_counter alone
-        self._boot_actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
         if partner is not None:
-            self._assign_partners(None)
-        if self._pop is not None:
-            if self._pop.needs_obs and self.obs is None:
+            self._assign_seats(None)
+        if isinstance(self._partner, _Population):
+            if self._partner.needs_obs and self.obs is None:
                 self.obs = torch.empty((N, 2, self.W, self.H, 26), dtype=autocast_dtype or torch.float32, device=dev)
-            self._pop.obs = self.obs
+            self._partner.obs = self.obs
             # the learner on its own rows only, where it runs K7 -> K9 -> K8
             self._learner_rows = self.fused_first_layer and self.fused_wide and self.fused_tail and not self.lstm
             if self._learner_rows:
@@ -854,19 +1041,6 @@ class SelfPlayRollout(_FoldedPolicy):
                 self._jrow = torch.empty(2 * N, dtype=torch.int32, device=dev)
                 self._lrange = torch.zeros(2, dtype=torch.int32, device=dev)
                 self._logp = torch.empty(2 * N, dtype=torch.float32, device=dev)  # run()'s logp: the joint K8 always writes it
-        if self.population:
-            self.episodes = EpisodeRecords(env, episode_capacity, members=True)
-
-    @property
-    def reward_shaping_factor(self):
-        """The factor of the shaped rewards (rllib.py:328-329).  Setting it takes effect in run() and collect() alike,
-        without a re-capture (their graphs read a device scalar)."""
-        return self.factor
-
-    @reward_shaping_factor.setter
-    def reward_shaping_factor(self, value):
-        self.factor = float(value)
-        self._factor.fill_(self.factor)
 
     @property
     def bc_factor(self):
@@ -882,22 +1056,11 @@ class SelfPlayRollout(_FoldedPolicy):
         self._bc_factor.fill_(self.bc)
 
     @property
-    def member_weights(self):
-        """The population's draw weights, as ``AgentPairRollout.member_weights``: setting them takes effect at the next
-        episode ends without a re-capture."""
-        assert self.population and self._pop._thresholds is not None, "member_weights: a population drawn per episode"
-        return self._pop.weights
-
-    @member_weights.setter
-    def member_weights(self, value):
-        assert self.population and self._pop._thresholds is not None, "member_weights: a population drawn per episode"
-        self._pop.weights = value
-
-    @property
-    def member(self):
-        """int32 [N]: with a population of partners, each environment's member in its running episode (it plays only where
-        ``partner_seat >= 0``); with a population of learners, the member that plays environment e (fixed); else None."""
-        return self._pop.member if self.population else self._member
+    def _members(self):
+        """A population of learners: the K folded members, self first; else None.  Built on access: a list holding self
+        would make the rollout a reference cycle, freed by the garbage collector at any later point, possibly inside
+        another rollout's graph capture, which its graphs' destruction would then invalidate."""
+        return None if self._others is None else [self] + self._others
 
     def _fold_members(self, models, blocks, autocast_dtype):
         """A population of learners: fold members 1.. like member 0 (self), set the blocks, and stack the K8 tables so that
@@ -916,12 +1079,12 @@ class SelfPlayRollout(_FoldedPolicy):
         self._row_offsets = 2 * self.blocks  # K8's offsets are joint rows
         self._member = torch.repeat_interleave(torch.arange(K, dtype=torch.int32, device=dev),
                                                torch.tensor(counts, device=dev)).to(torch.int32)
-        self._members = [self]
+        self._others = []
         for m in models[1:]:
             f = _FoldedPolicy()
             f.env = env
             f._fold(env, m, autocast_dtype, self.fused_first_layer, self.fused_tail, self.fused_wide)
-            self._members.append(f)
+            self._others.append(f)
         def stack(attr):  # the grouped kernels' stacked tables; each member's tables become views of them
             st = tuple(torch.stack([getattr(f, attr)[i] for f in self._members]) for i in range(len(getattr(self, attr))))
             for k, f in enumerate(self._members):
@@ -953,17 +1116,12 @@ class SelfPlayRollout(_FoldedPolicy):
             else:
                 flat, first = self.obs.view(rows, self.W * self.H * 26), 0
             if self.fused_wide and len(self._members) >= GROUPED_K9_MIN_MEMBERS:  # grouped K9
-                w1, b1, w2, b2 = self._wide_stack
-                _native.check(lib.ovc_wide_layers_grouped(flat.data_ptr(), rows, flat.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[1],
-                                                          w2.data_ptr(), b2.data_ptr(), w2.shape[1], 0.2, self._row_offsets.data_ptr(),
+                _native.check(lib.ovc_wide_layers_grouped(*self._k9_args(flat, self._wide_stack), self._row_offsets.data_ptr(),
                                                           len(self._members), self._z.data_ptr(), env._stream()))
             for k, f in enumerate(self._members):  # per member on its block's rows [2 o_k, 2 o_{k+1})
                 r = slice(2 * self._offs[k], 2 * self._offs[k + 1])
                 if self.fused_wide and len(self._members) < GROUPED_K9_MIN_MEMBERS:  # K9 on the block
-                    w1, b1, w2, b2 = f._wide
-                    x, z = flat[r], self._z[r]
-                    _native.check(lib.ovc_wide_layers(x.data_ptr(), x.shape[0], x.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
-                                                      w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, z.data_ptr(), env._stream()))
+                    _native.check(lib.ovc_wide_layers(*f._k9_args(flat[r]), self._z[r].data_ptr(), env._stream()))
                 elif not self.fused_tail:  # library layers; bit for bit the member's own rollout only where cuBLAS computes a
                     # row independently of the row count (tested at up to 2 x 300 rows per call)
                     logits, value = f.dense_model.forward_from(flat[r], first)
@@ -973,47 +1131,32 @@ class SelfPlayRollout(_FoldedPolicy):
                     f.dense_model.trunk(flat[r], first, out=self._z[r])
             if not self.fused_tail:
                 return self._scores
-            w1, b1, wh, bh, wo, bo = self._tail_stack
             ptr = lambda t: 0 if t is None else t.data_ptr()
             _native.check(lib.ovc_policy_tail_grouped(
-                self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(), wh.shape[1],
-                wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1), counter.data_ptr(),
-                self._row_offsets.data_ptr(), len(self._members), actions.data_ptr(), vals.data_ptr(), ptr(scores8), ptr(logp),
-                env._stream()))
+                *self._k8_args(self._z, self._tail_stack), counter.data_ptr(), self._row_offsets.data_ptr(), len(self._members),
+                actions.data_ptr(), vals.data_ptr(), ptr(scores8), ptr(logp), env._stream()))
         return None
 
-    def _assign_partners(self, done):
-        self.env.assign_partners(self.partner_seat, self._bc_factor, self._seat_counter, seed=self.seed ^ PARTNER_SEAT_SALT, done=done)
-
-    def _partner_act(self, actions):
-        """The partner's seat of ``actions`` (int32 [N, 2] or [2N]) in the paired environments, from the current state: K10
-        for a BC partner, else the network partner's or the population's kernels."""
-        if self._pop is not None:
-            self._pop.act(actions)
-            return
-        self.env.partner_actions(self._partner_tables, self.partner_seat, self._partner_counter, seed=self.seed ^ PARTNER_DRAW_SALT,
-                                 n_actions=self._partner_n_actions, out=actions)
-
     def sync_weights(self):
-        """Re-fold the learner (``_FoldedPolicy.sync_weights``) and a network partner or every population member, or every
-        member of a population of learners, in place: the captured graphs use the new weights without a re-capture."""
+        """Re-fold the learner (``_FoldedPolicy.sync_weights``), the partner (a network partner, every population member, or
+        a BC partner's K10 tables) and every member of a population of learners, in place: the captured graphs use the new
+        weights without a re-capture."""
         _FoldedPolicy.sync_weights(self)
-        if self._pop is not None:
-            self._pop.sync_weights()
-        for f in (self._members or [])[1:]:
+        if self._partner is not None:
+            self._partner.sync_weights()
+        for f in self._others or []:
             f.sync_weights()
 
-    def _capture(self, warm_up, body):
-        """A CUDA graph of ``body``, captured after ``warm_up`` (on a side stream).  Warm-up and capture must not advance
-        the environments: the state, the returns, the episode statistics and records and the draw counters are restored after
-        them."""
-        live = [self.env.state, self.ret_sparse, self.ret_mixed, self._draw_counter] + self.stats.state_tensors() + self.episodes.tensors()
+    def _agents(self):
+        return [self]
+
+    def _live(self):
+        live = [self.ret_mixed, self._draw_counter]
         if self.lstm:
             live += [self.h, self.c, self.env.done]  # env.done: the next transition's LSTM reset
         if self.partner is not None:
-            live += [self.partner_seat, self._seat_counter]
-            live += self._pop.live() if self._pop is not None else [self._partner_counter]
-        return _capture_graph(self.env, live, warm_up, body)
+            live += [self.partner_seat, self._seat_counter] + self._partner.live()
+        return live
 
     def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None, state_out=None, snap=None):
         """(scores float32 [2N, 6] = logits, values written to ``values``) for the observations in self.obs, or None when
@@ -1030,69 +1173,22 @@ class SelfPlayRollout(_FoldedPolicy):
             return self._policy_members(actions, vals, logp, scores8, counter)
         with torch.no_grad():
             if self.fused_first_layer:
-                flat, first = env.encoded_linear(self._wt0, self._b0, out=self._act0, neg_slope=0.2), 1  # K7
+                flat = env.encoded_linear(self._wt0, self._b0, out=self._act0, neg_slope=0.2)  # K7
             else:
-                flat, first = self.obs.view(rows, self.W * self.H * 26), 0
-            lstm_head = lambda: self._lstm_head(actions, vals, logp, scores8, counter, state_out or (self.h, self.c), snap)
-            if self.lstm and not self.fused_tail:
-                self._x.copy_(self.dense_model.hidden_from(flat, first))
-                return lstm_head()
-            if not self.fused_tail:
-                logits, value = self.dense_model.forward_from(flat, first)
-                self._scores.copy_(logits)
-                vals.copy_(value)
-                return self._scores
-            if self.fused_wide:
-                w1, b1, w2, b2 = self._wide
-                _native.check(_native.lib().ovc_wide_layers(flat.data_ptr(), rows, flat.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
-                                                            w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, self._z.data_ptr(), env._stream()))
-            else:
-                self.dense_model.trunk(flat, first, out=self._z)
-            if self.lstm:
-                w1, b1, wh, bh = self._tail
-                _native.check(_native.lib().ovc_policy_hidden(self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(),
-                                                              wh.data_ptr(), bh.data_ptr(), wh.shape[0], self.dense_model.dense_slope,
-                                                              self._x.data_ptr(), env._stream()))
-                return lstm_head()
-            w1, b1, wh, bh, wo, bo = self._tail
-            args = (self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
-                    wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1),
-                    counter.data_ptr(), actions.data_ptr(), vals.data_ptr(), scores8.data_ptr() if scores8 is not None else 0)
-            if logp is None:
-                _native.check(_native.lib().ovc_policy_tail(*args, env._stream()))
-            else:
-                _native.check(_native.lib().ovc_policy_tail_logp(*args, logp.data_ptr(), env._stream()))
-        return None  # K8 has drawn the actions itself
+                flat = self.obs.view(rows, self.W * self.H * 26)
+        return self._chain(flat, actions, vals, logp, scores8, counter, state_out=state_out, snap=snap)
 
     def _policy_learner_rows(self, actions, values, logp, scores8):
         """K7 -> K9 -> K8 on the learner's rows only: both views of a self-play environment, view 1 - partner_seat[e] of a
         paired one.  Each row is drawn and written at its joint row, bit for bit what ``_policy`` writes there."""
-        env, rows, lib = self.env, 2 * self.env.n_envs, _native.lib()
+        env, lib = self.env, _native.lib()
         env.learner_rows(self.partner_seat, self._lst, self._first, self._jrow, self._lrange)
         env.encoded_linear_masked(self._wt0, self._b0, self._lst, self._first, self._act0, neg_slope=0.2)  # K7
-        w1, b1, w2, b2 = self._wide
-        _native.check(lib.ovc_wide_layers_range(self._act0.data_ptr(), rows, self._act0.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
-                                                w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, self._lrange.data_ptr(), self._z.data_ptr(),
-                                                env._stream()))
-        w1, b1, wh, bh, wo, bo = self._tail
-        ptr = lambda t: 0 if t is None else t.data_ptr()
+        _native.check(lib.ovc_wide_layers_range(*self._k9_args(self._act0), self._lrange.data_ptr(), self._z.data_ptr(), env._stream()))
         _native.check(lib.ovc_policy_tail_joint(
-            self._z.data_ptr(), rows, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(), wh.shape[0],
-            wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, self.seed & (2**64 - 1), self._draw_counter.data_ptr(),
-            self._jrow.data_ptr(), self._lrange.data_ptr(), actions.data_ptr(), values.data_ptr(), ptr(scores8),
-            (self._logp if logp is None else logp).data_ptr(), env._stream()))
-
-    def _lstm_head(self, actions, values, logp, scores8, counter, state_out, snap):
-        """K11 on self._x and the live state, reset where the previous transition ended an episode (env.done)."""
-        w, b, wo, bo = self._lstm_tables
-        ptr = lambda t: 0 if t is None else t.data_ptr()
-        snap_h, snap_c = snap or (None, None)
-        _native.check(_native.lib().ovc_lstm_head(
-            self._x.data_ptr(), self.h.data_ptr(), self.c.data_ptr(), self.env.done.data_ptr(), self._x.shape[0], w.data_ptr(),
-            b.data_ptr(), wo.data_ptr(), bo.data_ptr(), self.dense_model.n_actions, self.seed & (2**64 - 1), counter.data_ptr(),
-            state_out[0].data_ptr(), state_out[1].data_ptr(), ptr(snap_h), ptr(snap_c), actions.data_ptr(), ptr(values), ptr(logp),
-            ptr(scores8), self.env._stream()))
-        return None  # K11 has drawn the actions
+            *self._k8_args(self._z), self._draw_counter.data_ptr(), self._jrow.data_ptr(), self._lrange.data_ptr(), actions.data_ptr(),
+            values.data_ptr(), 0 if scores8 is None else scores8.data_ptr(), (self._logp if logp is None else logp).data_ptr(),
+            env._stream()))
 
     def _transition(self, b=None, t=0):
         """One transition: K2 or K7, the policy, the draw, K10 for the partner, K1 (auto-reset inside), the returns and the
@@ -1125,7 +1221,7 @@ class SelfPlayRollout(_FoldedPolicy):
                 b.partner_seat[t].copy_(self.partner_seat)
                 if self.population:
                     b.partner_member[t].copy_(self._pop.member)
-            self._partner_act(actions)  # K10, or the network partner / the population
+            self._partner.act(actions)  # K10, or the network partner / the population
         dense = _env_step(env, actions.view(env.n_envs, 2), self._phi)
         if self.population:  # before the record: both use the slot count[e] the ending episode goes to
             self._pop.assign(env.done, self.episodes if b is None else b.episodes)
@@ -1134,64 +1230,22 @@ class SelfPlayRollout(_FoldedPolicy):
                               stats=self.stats, records=self.episodes if b is None else b.episodes,
                               partner_seat=None if self.partner is None else self.partner_seat, dense=dense)
         if self.partner is not None:
-            self._assign_partners(env.done)
+            self._assign_seats(env.done)
 
-    def run(self, n_steps):
-        """Advance every environment n_steps transitions; returns the number of env-steps done."""
-        if self.use_graph and self.graph is None:
-            def warm_up():
-                for _ in range(3):
-                    self._transition()
-            self.graph = self._capture(warm_up, self._transition)
-        step = self._transition if self.graph is None else self.graph.replay
-        for _ in range(n_steps):
-            step()
-        return n_steps * self.env.n_envs
-
-    def _collect_window(self, b, n_steps, gamma, lam):
-        """n_steps transitions into slots 0.. of ``b``, then the bootstrap value of the state after them and GAE over the
-        whole batch."""
-        b.episodes.clear()
-        for t in range(n_steps):
-            self._transition(b, t)
+    def _bootstrap(self, b):
         if not self.fused_first_layer:
             self.env.lossless_state_encoding(out=self.obs)
         # the LSTM's bootstrap step writes its state to scratch: the next window continues from the live state
         self._policy(actions=self._boot_actions, values=b.last_values, counter=self._boot_counter,
                      state_out=(self._h_boot, self._c_boot) if self.lstm else None)
-        self.env.gae(b.rewards, b.values, b.dones, b.last_values, gamma, lam, b.advantages, b.value_targets)
 
-    def collect(self, n_steps, gamma, lam, keep_logits=False):
-        """Advance every environment n_steps transitions, as run() does (the same kernels and the same draws from the same
-        seed and counter), and return them as a ``SampleBatch`` with GAE(gamma, lam) advantages.  The batch's tensors are
-        reused: the next collect() with the same n_steps / keep_logits overwrites them.  With use_graph the whole window
-        is one CUDA graph (captured once per n_steps / keep_logits; a new gamma or lam re-captures it); no host
-        synchronisation otherwise.  With a partner, the batch's ``partner_seat`` / ``learner_mask`` say which rows were the
+    def _new_batch(self, n_steps, keep_logits):
+        """collect()'s two-view batch.  With a partner, its ``partner_seat`` / ``learner_mask`` say which rows were the
         partner's; their actions are the partner's, their logp / values / advantages are meaningless (the PPO network's, or,
-        where the learner runs on its own rows only, not written).  With a population, ``partner_member`` is each
-        transition's member (meaningful where ``partner_seat >= 0``).
-        A seat changes hands only at a done, where GAE cuts, so a learner row's advantages never read a partner step."""
-        assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
-        key = (int(n_steps), bool(keep_logits))
-        b = self._batches.get(key)
-        if b is None:
-            b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits, partner=self.partner is not None,
-                                                 seq_len=self.max_seq_len if self.lstm else None, members=self.population)
-        if not self.use_graph:
-            self._collect_window(b, n_steps, gamma, lam)
-            return b
-        g = self._collect_graphs.get(key)
-        if g is None or g[0] != (gamma, lam):
-            g = self._collect_graphs[key] = ((gamma, lam), self._capture(lambda: self._collect_window(b, 1, gamma, lam),
-                                                                         lambda: self._collect_window(b, n_steps, gamma, lam)))
-        g[1].replay()
-        return b
-
-    def reset_state(self):
-        """Zero the LSTM policy's live state.  run() and collect() zero it at every auto-reset (through ``env.done``); call
-        this after resetting the environments directly (``env.reset()``), so that the new episodes start from zero state."""
-        assert self.lstm, "only the LSTM policy has a recurrent state"
-        self.h.zero_(), self.c.zero_()
+        where the learner runs on its own rows only, not written); ``partner_member`` is meaningful where ``partner_seat >=
+        0``.  A seat changes hands only at a done, where GAE cuts, so a learner row's advantages never read a partner step."""
+        return SampleBatch(self.env, n_steps, keep_logits, partner=self.partner is not None,
+                           seq_len=self.max_seq_len if self.lstm else None, members=self.population)
 
     def env_only(self, n_steps):
         """The same transitions without the policy: encode + step with the last sampled actions
@@ -1227,19 +1281,9 @@ class _NetworkAgent(_FoldedPolicy):
         self.obs = None  # [N, 2, W, H, 26] without K7, shared with the other agent of the pair
         self._base = 2 * torch.arange(N, device=dev) + self.seat
         self._rows = 2 * torch.arange(N, device=dev) + (self.seat if swap is None else self.seat ^ (swap != 0).long())  # 2 e + p(e)
-        if self.fused_first_layer:
-            self._act0 = torch.empty((N, self._wt0.shape[1]), dtype=torch.bfloat16, device=dev)
-        else:
+        self._chain_buffers(N)
+        if not self.fused_first_layer:
             self._flat = torch.empty((N, self.W * self.H * 26), dtype=autocast_dtype or torch.float32, device=dev)
-        if not self.fused_tail and not self.lstm:  # library layers: the logits the draw reads
-            self._scores = torch.empty((N, 6), dtype=torch.float32, device=dev)
-        if self.fused_tail:
-            self._z = torch.empty((N, self._tail[0].shape[1]), dtype=torch.bfloat16, device=dev)
-        if self.lstm:
-            cell = self.model.lstm.hidden_size
-            self._x = torch.empty((N, self.model.lstm.input_size), dtype=torch.bfloat16, device=dev)
-            self.h = torch.zeros((N, cell), dtype=torch.bfloat16, device=dev)  # the live state, zero at every episode start
-            self.c = torch.zeros((N, cell), dtype=torch.float32, device=dev)
 
     def live(self):
         """The tensors a transition advances (restored around graph capture)."""
@@ -1256,76 +1300,38 @@ class _NetworkAgent(_FoldedPolicy):
         agent's).  The LSTM state is zeroed where the previous transition ended an episode (``env.done``); K11 writes the new
         state to ``state_out`` (h, c) (default: in place) and the state it used to ``snap`` (h, c) when given."""
         env, N = self.env, self.env.n_envs
-        lib, seed = _native.lib(), self.seed & (2**64 - 1)
-        ptr = lambda t: 0 if t is None else t.data_ptr()
         values = self.values if values is None else values
         scores8 = self._scores8 if scores8 is None else scores8
         counter = self._counter if counter is None else counter
         with torch.no_grad():
             if self.fused_first_layer:
-                flat, first = env.encoded_linear_view(self._wt0, self._b0, self.seat, self.swap, out=self._act0, neg_slope=0.2), 1  # K7
+                flat = env.encoded_linear_view(self._wt0, self._b0, self.seat, self.swap, out=self._act0, neg_slope=0.2)  # K7
             else:
-                flat, first = torch.index_select(self.obs.view(2 * N, -1), 0, self._rows, out=self._flat), 0
-            if self.fused_wide:
-                w1, b1, w2, b2 = self._wide
-                _native.check(lib.ovc_wide_layers(flat.data_ptr(), N, flat.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
-                                                  w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, self._z.data_ptr(), env._stream()))
-            elif self.fused_tail:
-                self.dense_model.trunk(flat, first, out=self._z)
-            if self.lstm:
-                if self.fused_tail:
-                    w1, b1, wh, bh = self._tail
-                    _native.check(lib.ovc_policy_hidden(self._z.data_ptr(), N, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(),
-                                                        wh.data_ptr(), bh.data_ptr(), wh.shape[0], self.dense_model.dense_slope,
-                                                        self._x.data_ptr(), env._stream()))
-                else:
-                    self._x.copy_(self.dense_model.hidden_from(flat, first))
-                w, b, wo, bo = self._lstm_tables
-                h_out, c_out = state_out or (self.h, self.c)
-                snap_h, snap_c = snap or (None, None)
-                _native.check(lib.ovc_lstm_head_view(
-                    self._x.data_ptr(), self.h.data_ptr(), self.c.data_ptr(), env.done.data_ptr(), N, w.data_ptr(), b.data_ptr(),
-                    wo.data_ptr(), bo.data_ptr(), self.dense_model.n_actions, seed, counter.data_ptr(), ptr(self.swap), self.seat,
-                    h_out.data_ptr(), c_out.data_ptr(), ptr(snap_h), ptr(snap_c), actions.data_ptr(), values.data_ptr(), ptr(logp),
-                    ptr(scores8), env._stream()))
-            elif self.fused_tail:
-                w1, b1, wh, bh, wo, bo = self._tail
-                _native.check(lib.ovc_policy_tail_view(
-                    self._z.data_ptr(), N, self._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(),
-                    wh.shape[0], wo.data_ptr(), bo.data_ptr(), 0.3, self.dense_model.n_actions, seed, counter.data_ptr(),
-                    ptr(self.swap), self.seat, actions.data_ptr(), values.data_ptr(), ptr(scores8), ptr(logp), env._stream()))
-            else:
-                logits, value = self.dense_model.forward_from(flat, first)
-                self._scores.copy_(logits)
-                values.copy_(value)
-                env.sample_actions_view(self._scores, counter, self.seat, self.swap, seed=self.seed, out=actions, logp_out=logp)
-                if scores8 is not None:
-                    scores8[:, :self._scores.shape[1]].copy_(self._scores)
+                flat = torch.index_select(self.obs.view(2 * N, -1), 0, self._rows, out=self._flat)
+        self._chain(flat, actions, values, logp, scores8, counter, view=(self.seat, self.swap), state_out=state_out, snap=snap)
 
 
 class _BCAgent(object):
-    """A ``BCPolicy`` agent of an ``AgentPairRollout``: K10 with ``partner_seat[e] = p(e)`` in every environment, its draws
-    keyed by ``seed ^ PARTNER_DRAW_SALT`` on a counter of its own (the draws of PPO_BC's partner).  ``live_seats``: ``swap``
-    (0 / 1 only) changes between transitions; ``follow_seats()`` recomputes ``partner_seat`` from it."""
+    """A ``BCPolicy`` agent: K10 with ``partner_seat`` (int32 [N]: the player it plays in environment e, -1 where it does
+    not play), its draws keyed by ``seed ^ PARTNER_DRAW_SALT`` on a counter of its own (the draws of PPO_BC's partner).
+    ``complement_of``: seats (0 / 1 only) that change between transitions; ``follow_seats()`` then sets ``partner_seat``
+    to their complement."""
 
-    def __init__(self, env, policy, seat, swap, seed, live_seats=False):
+    lstm = False
+
+    def __init__(self, env, policy, partner_seat, seed, complement_of=None):
         self.env, self.policy = env, policy.to(env.device).eval()
-        self.seat, self.seed, self.swap, self.live_seats = int(seat), int(seed), swap, live_seats
+        self.partner_seat, self.seed, self._complement_of = partner_seat, int(seed), complement_of
         self._tables = self.policy.tables()
         self._n_actions = self.policy.logits.out_features
-        if live_seats and self.seat == 0:
-            self.partner_seat = swap  # p(e) = swap[e]: the live seats themselves
-        else:
-            self.partner_seat = (torch.full((env.n_envs,), self.seat, dtype=torch.int32, device=env.device) if swap is None
-                                 else (self.seat ^ (swap != 0).int()).to(torch.int32).contiguous())
         self._counter = torch.zeros(2, dtype=torch.int64, device=env.device)
 
     def live(self):
-        return [self._counter] + ([self.partner_seat] if self.live_seats and self.seat else [])
+        return [self._counter] + ([self.partner_seat] if self._complement_of is not None else [])
 
     def follow_seats(self):
-        if self.seat:
-            torch.bitwise_xor(self.swap, 1, out=self.partner_seat)
+        if self._complement_of is not None:
+            torch.bitwise_xor(self._complement_of, 1, out=self.partner_seat)
 
     def act(self, actions):
         self.env.partner_actions(self._tables, self.partner_seat, self._counter, seed=self.seed ^ PARTNER_DRAW_SALT,
@@ -1370,7 +1376,8 @@ class _Population(object):
     def __init__(self, env, members, partner_seat, seed, autocast_dtype, member=None, weights=None, mixture=False):
         N, dev = env.n_envs, env.device
         self.env, self.K, self.seed, self.partner_seat = env, len(members), int(seed), partner_seat
-        self.agents = [_BCAgent(env, m, 1, None, seed) if isinstance(m, BCPolicy)
+        # a BC member plays partner_seat where member == k, -1 elsewhere (rebuilt every transition)
+        self.agents = [_BCAgent(env, m, torch.full((N,), -1, dtype=torch.int32, device=dev), seed) if isinstance(m, BCPolicy)
                        else _NetworkAgent(env, m, 0, partner_seat, seed, autocast_dtype) for m in members]
         shared = {}
 
@@ -1392,9 +1399,6 @@ class _Population(object):
             else:
                 a._scores = buf((N, 6), torch.float32)
         self._unpaired = torch.full((N,), -1, dtype=torch.int32, device=dev)
-        for a in self.agents:
-            if isinstance(a, _BCAgent):
-                a.partner_seat = torch.full((N,), -1, dtype=torch.int32, device=dev)  # rebuilt every transition
         self.needs_obs = any(not a.fused_first_layer for a in nets)
         l = env.layouts[0]
         self._cobs = torch.empty((N, l.width * l.height * 26), dtype=autocast_dtype or torch.float32, device=dev) if self.needs_obs else None
@@ -1470,32 +1474,26 @@ class _Population(object):
                 torch.where(self.member == k, self.partner_seat, self._unpaired, out=a.partner_seat)
                 a.act(actions)
                 continue
-            seed = a.seed & (2**64 - 1)
             with torch.no_grad():
                 if a.fused_first_layer:
                     flat, first = env.encoded_linear_rows(a._wt0, a._b0, 0, self.partner_seat, self.order, rng, a._act0), 1  # K7
                 else:
                     flat, first = self._cobs, 0
                 if a.fused_wide:
-                    w1, b1, w2, b2 = a._wide
-                    _native.check(lib.ovc_wide_layers_range(flat.data_ptr(), N, flat.shape[1], w1.data_ptr(), b1.data_ptr(), w1.shape[0],
-                                                            w2.data_ptr(), b2.data_ptr(), w2.shape[0], 0.2, rng.data_ptr(), a._z.data_ptr(),
-                                                            stream))
+                    _native.check(lib.ovc_wide_layers_range(*a._k9_args(flat), rng.data_ptr(), a._z.data_ptr(), stream))
                 elif a.fused_tail:
                     a.dense_model.trunk(flat, first, out=a._z)
                 if a.fused_tail:
-                    w1, b1, wh, bh, wo, bo = a._tail
                     _native.check(lib.ovc_policy_tail_rows(
-                        a._z.data_ptr(), N, a._z.shape[1], 0.2, w1.data_ptr(), b1.data_ptr(), wh.data_ptr(), bh.data_ptr(), wh.shape[0],
-                        wo.data_ptr(), bo.data_ptr(), 0.3, a.dense_model.n_actions, seed, a._counter.data_ptr(), self.partner_seat.data_ptr(),
-                        0, self.order.data_ptr(), rng.data_ptr(), actions.data_ptr(), 0, 0, 0, stream))
+                        *a._k8_args(a._z), a._counter.data_ptr(), self.partner_seat.data_ptr(), 0, self.order.data_ptr(), rng.data_ptr(),
+                        actions.data_ptr(), 0, 0, 0, stream))
                 else:
                     logits, _ = a.dense_model.forward_from(flat, first)
                     a._scores.copy_(logits)
                     env.sample_actions_rows(a._scores, a._counter, 0, self.partner_seat, self.order, rng, seed=a.seed, out=actions)
 
 
-class AgentPairRollout(object):
+class AgentPairRollout(_Rollout):
     """Two different agents, each evaluated on its own seat's view only: the reference's evaluation of an agent pair
     (rllib.py ``evaluate``: ``AgentEvaluator.evaluate_agent_pair(AgentPair(agent_0_policy, agent_1_policy))``) with N
     environments on the device — PPO against a held-out BC human proxy, cross-play of two PPO agents, BC against BC — and,
@@ -1543,94 +1541,67 @@ class AgentPairRollout(object):
         assert not (random_seats and swap is not None), "random_seats draws the seats: pass no swap tensor with it"
         assert not isinstance(agents[0], (list, tuple)), "a population plays agent 1 only: agents = (agent0, [m_0, ..., m_K-1])"
         self.population = isinstance(agents[1], (list, tuple))
-        members = list(agents[1]) if self.population else []
         if self.population:
-            assert 1 <= len(members) <= MAX_MEMBERS, "a population has 1..%d members" % MAX_MEMBERS
-            for m in members:
-                assert isinstance(m, (RllibShapedCNN, BCPolicy)) and not isinstance(m, RllibLSTMShapedCNN), \
-                    "a population member is an RllibShapedCNN or a BCPolicy (an LSTM member is not supported)"
+            _check_members(agents[1], MAX_MEMBERS, (RllibShapedCNN, BCPolicy), "a population has 1..%d members" % MAX_MEMBERS,
+                           "a population member is an RllibShapedCNN or a BCPolicy (an LSTM member is not supported)")
         else:
             assert member is None and member_weights is None, "member / member_weights go with a population in agents[1]"
-        for a in [agents[0]] + (members or [agents[1]]):
+        for a in agents[:1] if self.population else agents:
             assert isinstance(a, (RllibShapedCNN, BCPolicy)), "an agent is an RllibShapedCNN, an RllibLSTMShapedCNN or a BCPolicy"
-            assert not isinstance(a, RllibLSTMShapedCNN) or autocast_dtype == torch.bfloat16, \
-                "the LSTM policy runs as ovc_lstm_head (K11), which takes bfloat16 operands: autocast_dtype=None is not supported"
-        N, dev = env.n_envs, env.device
         if swap is not None:
-            assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == N, "swap: int32 CUDA [N]"
-        self.env, self.swap, self.seed, self.use_graph = env, swap, int(seed), use_graph
+            assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == env.n_envs, \
+                "swap: int32 CUDA [N]"
+        self.env, self.swap, self.seed = env, swap, int(seed)
         self.random_seats = bool(random_seats)
-        self.max_seq_len = int(max_seq_len)
-        assert self.max_seq_len >= 1
         if self.random_seats:
             # agent 1's player, drawn for every environment now and at every episode end; agent k then sits at player
             # (1 - k) ^ partner_seat[e], i.e. it is passed seat 1 - k and swap = partner_seat
-            self.partner_seat = torch.full((N,), -1, dtype=torch.int32, device=dev)
-            self._seat_factor = torch.ones(1, dtype=torch.float32, device=dev)
-            self._seat_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of the seat draw
+            self.partner_seat = torch.full((env.n_envs,), -1, dtype=torch.int32, device=env.device)
+            self._bc_factor = torch.ones(1, dtype=torch.float32, device=env.device)  # every episode is paired
+            self._seat_counter = torch.zeros(2, dtype=torch.int64, device=env.device)  # [step, scratch] of the seat draw
             self._assign_seats(None)
             seats, swap = (1, 0), self.partner_seat
         else:
             seats = (0, 1)
-            self.partner_seat = (torch.ones(N, dtype=torch.int32, device=dev) if swap is None
-                                 else (1 ^ (swap != 0).int()).to(torch.int32).contiguous())  # agent 1's player
-        self.agents = [_BCAgent(env, a, seat, swap, seed, self.random_seats) if isinstance(a, BCPolicy)
-                       else _NetworkAgent(env, a, seat, swap, seed, autocast_dtype, self.random_seats)
-                       for seat, a in zip(seats, agents[:1] if self.population else agents)]
+
+        def player(seat):  # int32 [N]: seat ^ (swap[e] != 0), the player of the agent passed seat
+            if swap is None:
+                return torch.full((env.n_envs,), seat, dtype=torch.int32, device=env.device)
+            return (seat ^ (swap != 0).int()).to(torch.int32).contiguous()
+        # with fixed seats partner_seat is made after the agents: a network agent's fold checks its model first
+        self.agents = []
+        for seat, a in zip(seats, agents[:1] if self.population else agents):
+            if not isinstance(a, BCPolicy):
+                self.agents.append(_NetworkAgent(env, a, seat, swap, seed, autocast_dtype, self.random_seats))
+            elif self.random_seats and seat == 0:  # agent 1 plays the drawn seats themselves
+                self.agents.append(_BCAgent(env, a, self.partner_seat, seed))
+            else:  # under random_seats, agent 0 plays their complement
+                self.agents.append(_BCAgent(env, a, player(seat), seed, self.partner_seat if self.random_seats else None))
+        if not self.random_seats:
+            self.partner_seat = player(1)  # agent 1's player
         if self.population:
-            self.agents.append(_Population(env, members, self.partner_seat, seed, autocast_dtype, member, member_weights))
+            self.agents.append(_Population(env, list(agents[1]), self.partner_seat, seed, autocast_dtype, member, member_weights))
+        self._pop = self.agents[1] if self.population else None
+        self._member = None
         # network agents without K7 read K2's observation, written once per transition for all of them
         library = [a for a in self.agents if (isinstance(a, _NetworkAgent) and not a.fused_first_layer) or getattr(a, "needs_obs", False)]
         l = env.layouts[0]
-        self.obs = torch.empty((N, 2, l.width, l.height, 26), dtype=autocast_dtype or torch.float32, device=dev) if library else None
+        self.obs = torch.empty((env.n_envs, 2, l.width, l.height, 26), dtype=autocast_dtype or torch.float32, device=env.device) \
+            if library else None
         for a in library:
             a.obs = self.obs
-        self.actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
-        self.ret_sparse = torch.zeros(N, dtype=torch.int64, device=dev)
-        self.factor = 1.0
-        self._factor = torch.ones(1, dtype=torch.float32, device=dev)  # reward_shaping_factor, read by the captured graphs
-        self.stats = EpisodeStats(env)
-        self.episodes = EpisodeRecords(env, episode_capacity, members=self.population)
-        self.graph = None
-        self._collect_graphs = {}  # (n_steps, keep_logits) -> ((gamma, lam), CUDA graph of the window)
-        self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
-        self._boot_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # the bootstrap's draws leave the learner's counter alone
-        self._boot_actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
-        learner = self.agents[0]
-        if getattr(learner, "lstm", False):  # the bootstrap's (discarded) LSTM state
-            self._h_boot, self._c_boot = torch.empty_like(learner.h), torch.empty_like(learner.c)
+        self._init_rollout(env, self.agents[0], use_graph, 1.0, episode_capacity, max_seq_len)
 
-    @property
-    def reward_shaping_factor(self):
-        """The factor of the shaped rewards in collect()'s rewards and in the episode records' ``ep_reward_by_agent``
-        (rllib.py:328-329; default 1).  Setting it takes effect without a re-capture (the graphs read a device scalar)."""
-        return self.factor
+    def _agents(self):
+        return self.agents
 
-    @reward_shaping_factor.setter
-    def reward_shaping_factor(self, value):
-        self.factor = float(value)
-        self._factor.fill_(self.factor)
-
-    @property
-    def member_weights(self):
-        """The population's draw weights (K non-negative floats with a positive sum).  Setting them writes the device
-        table the draw reads, so run() and collect() follow a new distribution at the next episode ends without a re-capture
-        (prioritised sampling of the population between windows)."""
-        assert self.population and self.agents[1]._thresholds is not None, "member_weights: a population drawn per episode"
-        return self.agents[1].weights
-
-    @member_weights.setter
-    def member_weights(self, value):
-        assert self.population and self.agents[1]._thresholds is not None, "member_weights: a population drawn per episode"
-        self.agents[1].weights = value
-
-    @property
-    def member(self):
-        """int32 [N]: each environment's population member in its running episode (None without a population)."""
-        return self.agents[1].member if self.population else None
-
-    def _assign_seats(self, done):
-        self.env.assign_partners(self.partner_seat, self._seat_factor, self._seat_counter, seed=self.seed ^ PARTNER_SEAT_SALT, done=done)
+    def _live(self):
+        live = [self.env.done]
+        if self.random_seats:
+            live += [self.partner_seat, self._seat_counter]
+        for a in self.agents:
+            live += a.live()
+        return live
 
     def _transition(self, b=None, t=0):
         """One transition.  Without ``b`` (run()) finished episodes go to self.episodes; with a one-view ``SampleBatch`` ``b``
@@ -1667,73 +1638,25 @@ class AgentPairRollout(object):
             for a in self.agents:
                 a.follow_seats()
 
-    def _capture(self, warm_up, body):
-        """A CUDA graph of ``body``; the state, the returns, the statistics, the counters and the seats are restored after
-        warm-up and capture."""
-        live = [self.env.state, self.env.done, self.ret_sparse] + self.stats.state_tensors() + self.episodes.tensors()
-        if self.random_seats:
-            live += [self.partner_seat, self._seat_counter]
-        for a in self.agents:
-            live += a.live()
-        return _capture_graph(self.env, live, warm_up, body)
-
-    def run(self, n_steps):
-        """Advance every environment n_steps transitions (one CUDA graph per transition with use_graph); returns the number
-        of env-steps done."""
-        if self.use_graph and self.graph is None:
-            def warm_up():
-                for _ in range(3):
-                    self._transition()
-            self.graph = self._capture(warm_up, self._transition)
-        step = self._transition if self.graph is None else self.graph.replay
-        for _ in range(n_steps):
-            step()
-        return n_steps * self.env.n_envs
-
-    def _collect_window(self, b, n_steps, gamma, lam):
-        b.episodes.clear()
-        for t in range(n_steps):
-            self._transition(b, t)
+    def _bootstrap(self, b):
         if self.obs is not None:
             self.env.lossless_state_encoding(out=self.obs)
         # the learner's bootstrap value at the seats after the window; its LSTM state goes to scratch
-        self.agents[0].act(self._boot_actions, values=b.last_values, counter=self._boot_counter,
-                           state_out=(self._h_boot, self._c_boot) if self.agents[0].lstm else None)
-        self.env.gae_view(b.rewards, b.values, b.dones, b.last_values, gamma, lam, b.advantages, b.value_targets)
+        learner = self.agents[0]
+        learner.act(self._boot_actions, values=b.last_values, counter=self._boot_counter,
+                    state_out=(self._h_boot, self._c_boot) if learner.lstm else None)
 
-    def collect(self, n_steps, gamma, lam, keep_logits=False):
-        """Advance every environment n_steps transitions, as run() does (the same kernels and draws), and return agent 0's
-        side of them as a one-view ``SampleBatch`` (one row per environment: agent 0's action, logp, value, reward and GAE
-        advantages; ``partner_seat`` is agent 1's player) for a PPO update of agent 0 next to the fixed agent 1.  The batch's
-        tensors are reused by the next collect() with the same n_steps / keep_logits.  With use_graph the whole window is one
-        CUDA graph (captured once per n_steps / keep_logits; a new gamma or lam re-captures it).  After an update, call
-        ``sync_weights()`` (it refolds every population member too).  With a population in agent 1 the batch's
-        ``partner_member`` is the member of every transition."""
+    def _new_batch(self, n_steps, keep_logits):
+        """collect()'s batch: agent 0's side of the transitions as a one-view ``SampleBatch`` (one row per environment:
+        agent 0's action, logp, value, reward and GAE advantages; ``partner_seat`` is agent 1's player), for a PPO update of
+        agent 0 next to the fixed agent 1.  After an update, call ``sync_weights()`` (it refolds every population member
+        too)."""
         assert isinstance(self.agents[0], _NetworkAgent), "collect() trains agents[0]: an RllibShapedCNN or RllibLSTMShapedCNN, not a BCPolicy"
-        assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
-        key = (int(n_steps), bool(keep_logits))
-        b = self._batches.get(key)
-        if b is None:
-            b = self._batches[key] = SampleBatch(self.env, n_steps, keep_logits, seq_len=self.max_seq_len if self.agents[0].lstm else None,
-                                                 one_view=True, members=self.population)
-        if not self.use_graph:
-            self._collect_window(b, n_steps, gamma, lam)
-            return b
-        g = self._collect_graphs.get(key)
-        if g is None or g[0] != (gamma, lam):
-            g = self._collect_graphs[key] = ((gamma, lam), self._capture(lambda: self._collect_window(b, 1, gamma, lam),
-                                                                         lambda: self._collect_window(b, n_steps, gamma, lam)))
-        g[1].replay()
-        return b
+        return SampleBatch(self.env, n_steps, keep_logits, seq_len=self.max_seq_len if self.agents[0].lstm else None,
+                           one_view=True, members=self.population)
 
     def sync_weights(self):
         """Re-fold every agent's network (e.g. a learner's after an update) in place: the captured graphs use the new weights
         without a re-capture."""
         for a in self.agents:
             a.sync_weights()
-
-    def reset_state(self):
-        """Zero the LSTM agents' live state; call it after resetting the environments directly (``env.reset()``)."""
-        for a in self.agents:
-            if getattr(a, "lstm", False):
-                a.h.zero_(), a.c.zero_()
