@@ -988,7 +988,7 @@ int ovc_encode_linear_grouped(const void *layouts, int n_layouts, const int32_t 
 
 int ovc_wide_layers_grouped(const void *a0, int64_t m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2,
                             int n2, float slope, const int32_t *offsets, int n_members, void *z2, void *stream) {
-    return ovc::wide_layers_grouped_impl(a0, m, k0, w1, b1, n1, w2, b2, n2, slope, offsets, n_members, z2, (cudaStream_t)stream);
+    return ovc::wide_layers_impl(a0, m, k0, w1, b1, n1, w2, b2, n2, slope, z2, (cudaStream_t)stream, offsets, true, n_members);
 }
 
 int ovc_policy_tail_grouped(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,

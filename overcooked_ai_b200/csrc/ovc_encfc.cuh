@@ -115,196 +115,12 @@ __device__ __forceinline__ void el_gather(float acc[CPL], const __nv_bfloat16 *t
 // MASKED (encode_linear_masked_kernel, without view_swap): entry r < n_envs of the list is environment list[r] >> 2 with the
 // views of mask list[r] & 3 (bit v: view v); the object part is computed once, and the views in the mask go to consecutive
 // rows from first[r] in ascending view order, each bit for bit row 2 e + v of the two-view kernel.
-template <int CPL, bool VIEW, bool ROWS, bool MASKED>
-__device__ __forceinline__ void encode_linear_body(const EncLinArgs &a, const int32_t *list = nullptr, const int32_t *first = nullptr) {
-    constexpr int CS = 32 * CPL;  // columns per CTA
-    extern __shared__ __align__(16) char el_smem[];
-    const int WH = a.W * a.H;
-    const int n_rows = WH * EL_DYN;
-    __nv_bfloat16 *tab = reinterpret_cast<__nv_bfloat16 *>(el_smem);                      // [n_rows][CS]
-    float *bias_eff = reinterpret_cast<float *>(el_smem + (size_t)n_rows * CS * 2);       // [n_layouts][CS]
-    float *urg = bias_eff + a.n_layouts * CS;                                             // [CS]
-    int *cook = reinterpret_cast<int *>(urg + CS);                                        // [n_layouts][16]
-    int *nslots = cook + a.n_layouts * 16;                                                // [n_layouts][2]: n_slots, n_pots
-    unsigned short *srow = reinterpret_cast<unsigned short *>(nslots + a.n_layouts * 2);  // [n_layouts][128] slot -> row base
-
-    const int n_slices = a.n_out / CS;
-    const int slice = blockIdx.x % n_slices, worker = blockIdx.x / n_slices;
-    const int col0 = slice * CS;
-    long long r_beg = 0, r_end = a.n_envs;
-    if constexpr (ROWS) {
-        r_beg = max(__ldg(a.range), 0);
-        r_end = min((long long)__ldg(a.range + 1), a.n_envs);
-        if (r_beg + (long long)worker * (EL_THREADS / 32) >= r_end) return;
-    }
-    if constexpr (MASKED) {
-        if ((long long)worker * (EL_THREADS / 32) >= r_end) return;
-    }
-
-    // ---- prologue: the table slice and the per-layout constants ----
-    unsigned char *tplane = reinterpret_cast<unsigned char *>(srow + a.n_layouts * 128);  // [n_layouts][256] terrain plane of a cell, 0 = none
-    for (int i = threadIdx.x; i < a.n_layouts * WH; i += EL_THREADS) {  // terrain code -> plane: X 11, O 12, T 13, D 14, P 10, S 15 (:2449-2465)
-        const int l = i / WH, cell = i - l * WH, x = cell / a.H, y = cell - x * a.H;
-        tplane[l * 256 + cell] = (unsigned char)((0x000F0A0E0D0C0B00ull >> ((a.layouts[l].cell[(y << 4) | x] & 7) * 8)) & 0xFF);
-    }
-    __syncthreads();
-    {
-        constexpr int CH = CS * 2 / 16;  // 16-byte chunks per row
-        for (int i = threadIdx.x; i < n_rows * CH; i += EL_THREADS) {
-            const int r = i / CH, c = i - r * CH;
-            const int cell = r / EL_DYN, d = r - cell * EL_DYN;
-            const int plane = d < 10 ? d : d + 6;
-            const uint4 *src = reinterpret_cast<const uint4 *>(a.wt + (size_t)(cell * N_PLANES + plane) * a.n_out + col0) + c;
-            reinterpret_cast<uint4 *>(tab)[i] = __ldg(src);
-        }
-        // terrain and urgency sums: one thread per (layout, column); the cells' loads are independent (plane ids staged in
-        // shared memory first), issued four at a time, added in cell order
-        for (int i = threadIdx.x; i < (a.n_layouts + 1) * CS; i += EL_THREADS) {
-            const int l = i / CS, c = i - l * CS;
-            const unsigned char *tp = tplane + l * 256;
-            const __nv_bfloat16 *w = a.wt + col0 + c;
-            float s = l == a.n_layouts ? 0.f : a.bias[col0 + c];
-            for (int cell = 0; cell < WH; cell += 4) {
-                float v[4];
-#pragma unroll
-                for (int u = 0; u < 4; u++) {
-                    const int pl = cell + u < WH ? (l == a.n_layouts ? (int)PL_URGENCY : (int)tp[cell + u]) : 0;
-                    v[u] = pl ? __bfloat162float(w[(size_t)((cell + u) * N_PLANES + pl) * a.n_out]) : 0.f;
-                }
-                s = (((s + v[0]) + v[1]) + v[2]) + v[3];
-            }
-            if (l == a.n_layouts) urg[c] = s;
-            else bias_eff[i] = s;
-        }
-        for (int i = threadIdx.x; i < a.n_layouts * 128; i += EL_THREADS) {
-            const ovc_layout_t *L = a.layouts + (i >> 7);
-            const int pb = L->slot_pos[i & 127];
-            srow[i] = (unsigned short)((((pb & 15) * a.H + (pb >> 4)) * EL_DYN) & 0xFFFF);
-        }
-        for (int i = threadIdx.x; i < a.n_layouts * 16; i += EL_THREADS) cook[i] = a.layouts[i >> 4].cook_time[i & 15];
-        for (int i = threadIdx.x; i < a.n_layouts; i += EL_THREADS) {
-            nslots[2 * i] = a.layouts[i].n_slots;
-            nslots[2 * i + 1] = a.layouts[i].n_pots;
-        }
-    }
-    __syncthreads();
-
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    constexpr int NW = EL_THREADS / 32;
-    const __nv_bfloat16 *tab_lane = tab + lane * CPL;
-    const long long stride = (long long)a.n_workers * NW;
-    const int max_slot_chunks = (a.S - 4 + 31) / 32;
-
-    for (long long r = r_beg + (long long)worker * NW + warp; r < r_end; r += stride) {
-        long long env, row0 = 0;
-        int vmask = 3;
-        if constexpr (MASKED) {
-            const int entry = __ldg(list + r);
-            env = entry >> 2, vmask = entry & 3;
-            if (!vmask) continue;  // the whole warp holds entry r
-            row0 = __ldg(first + r);
-        } else {
-            env = ROWS ? (long long)__ldg(a.rows + r) : r;
-        }
-        const int32_t *__restrict__ rec = a.state + env * a.S;
-        const int4 head = __ldg(reinterpret_cast<const int4 *>(rec));  // timestep, player 0, player 1, misc (same address in every lane)
-        const int lid = head.w & 0xFF;
-        const int n_slots = nslots[2 * lid], n_pots = nslots[2 * lid + 1];
-        const int *ck = cook + lid * 16;
-        const unsigned short *sr = srow + lid * 128;
-
-        float common[CPL];
-        {   // vector loads: consecutive lanes read consecutive CPL-float pieces (conflict free)
-            const bool urgent = a.horizon - head.x < 40;
-            constexpr int V = CPL >= 4 ? 4 : 2;
-            using fv = typename std::conditional<CPL >= 4, float4, float2>::type;
-#pragma unroll
-            for (int i = 0; i < CPL / V; i++) {
-                const fv b = reinterpret_cast<const fv *>(bias_eff + lid * CS + lane * CPL)[i];
-                const fv u = reinterpret_cast<const fv *>(urg + lane * CPL)[i];
-                const float *bp = reinterpret_cast<const float *>(&b), *up = reinterpret_cast<const float *>(&u);
-#pragma unroll
-                for (int k = 0; k < V; k++) common[i * V + k] = bp[k] + (urgent ? up[k] : 0.f);
-            }
-        }
-        // objects on pots / counters: lane l of chunk c decodes slot 32 c + l; entries travel by shuffle
-        for (int c = 0; c < max_slot_chunks; c++) {
-            if (c * 32 >= n_slots) break;
-            const int slot = c * 32 + lane;
-            unsigned e[4] = {0, 0, 0, 0};
-            if (slot < n_slots) {
-                const unsigned code = (unsigned)__ldg(rec + 4 + slot) & OVC_OBJ_MASK;
-                if (code) el_object(code, sr[slot], slot < n_pots, ck, e);
-            }
-            unsigned m = __ballot_sync(0xFFFFFFFFu, (e[0] | e[1] | e[2] | e[3]) != 0);
-            while (m) {
-                const int j = __ffs(m) - 1;
-                m &= m - 1;
-#pragma unroll
-                for (int q = 0; q < 4; q++) {
-                    const unsigned w = __shfl_sync(0xFFFFFFFFu, e[q], j);
-                    if (w & 0xFFFFu) el_gather<CPL>(common, tab_lane, (int)(w >> 16), (float)(short)(w & 0xFFFFu));
-                }
-            }
-        }
-        // held objects: at the holder's cell, in both views (computed by every lane, no exchange needed)
-        const unsigned p0 = (unsigned)head.y, p1 = (unsigned)head.z;
-        const int cell0 = ((p0 & 15) * a.H + ((p0 >> 4) & 15)) * EL_DYN, cell1 = ((p1 & 15) * a.H + ((p1 >> 4) & 15)) * EL_DYN;
-#pragma unroll
-        for (int j = 0; j < 2; j++) {
-            const unsigned held = (j ? p1 : p0) >> 10;
-            if (held) {
-                unsigned e[4];
-                el_object(held, j ? cell1 : cell0, false, ck, e);
-#pragma unroll
-                for (int q = 0; q < 4; q++)
-                    if (e[q] & 0xFFFFu) el_gather<CPL>(common, tab_lane, (int)(e[q] >> 16), (float)(short)(e[q] & 0xFFFFu));
-            }
-        }
-        // the two views: own cell / orientation in planes 0, 2..5, the partner's in planes 1, 6..9 (:2468-2479)
-        const int ori0 = (p0 >> 8) & 3, ori1 = (p1 >> 8) & 3;
-        const int swap = a.view_swap ? (__ldg(a.view_swap + env) != 0) : 0;
-        auto view = [&](int p, long long row) {  // p = the player whose view this is
-            float acc[CPL];
-#pragma unroll
-            for (int i = 0; i < CPL; i++) acc[i] = common[i];
-            const int own_cell = p ? cell1 : cell0, oth_cell = p ? cell0 : cell1;
-            const int own_ori = p ? ori1 : ori0, oth_ori = p ? ori0 : ori1;
-            el_gather<CPL>(acc, tab_lane, own_cell + PL_LOC, 1.f);
-            el_gather<CPL>(acc, tab_lane, own_cell + PL_ORI + own_ori, 1.f);
-            el_gather<CPL>(acc, tab_lane, oth_cell + PL_LOC + 1, 1.f);
-            el_gather<CPL>(acc, tab_lane, oth_cell + PL_ORI + 4 + oth_ori, 1.f);
-            unsigned packed[CPL / 2];
-#pragma unroll
-            for (int i = 0; i < CPL / 2; i++) {
-                const float x0 = acc[2 * i], x1 = acc[2 * i + 1];
-                const __nv_bfloat162 h = __floats2bfloat162_rn(fmaxf(x0, x0 * a.neg_slope), fmaxf(x1, x1 * a.neg_slope));
-                packed[i] = *reinterpret_cast<const unsigned *>(&h);
-            }
-            __nv_bfloat16 *dst = a.out + row * a.n_out + col0 + lane * CPL;
-            if constexpr (CPL == 8) *reinterpret_cast<uint4 *>(dst) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-            else if constexpr (CPL == 4) *reinterpret_cast<uint2 *>(dst) = make_uint2(packed[0], packed[1]);
-            else *reinterpret_cast<unsigned *>(dst) = packed[0];
-        };
-        if constexpr (MASKED) {
-            if (vmask & 1) view(0, row0);
-            if (vmask & 2) view(1, row0 + (vmask & 1));
-        } else if constexpr (VIEW) {
-            view(a.seat ^ swap, r);
-        } else {
-#pragma unroll
-            for (int p = 0; p < 2; p++) view(p, 2 * env + (swap ? 1 - p : p));
-        }
-    }
-}
-
-// encode_linear_body with GROUPED (a copy, so that the code of the kernels above stays as it was; encode_linear_grouped_kernel,
-// two views, without view_swap): n_members members, member k's tables entry k of
+// GROUPED (encode_linear_grouped_kernel, two views, without view_swap): n_members members, member k's tables entry k of
 // stacked wt / bias and its environments [offsets[k], offsets[k + 1]); the CTAs are split over (member, column slice,
 // worker), a.n_workers workers per member, so a CTA loads its member's column slice once and walks only that member's
 // environments.
 template <int CPL, bool VIEW, bool ROWS, bool MASKED, bool GROUPED = false>
-__device__ __forceinline__ void encode_linear_grouped_body(const EncLinArgs &a, const int32_t *list = nullptr, const int32_t *first = nullptr,
+__device__ __forceinline__ void encode_linear_body(const EncLinArgs &a, const int32_t *list = nullptr, const int32_t *first = nullptr,
                                                    const int32_t *offsets = nullptr) {
     constexpr int CS = 32 * CPL;  // columns per CTA
     extern __shared__ __align__(16) char el_smem[];
@@ -318,18 +134,19 @@ __device__ __forceinline__ void encode_linear_grouped_body(const EncLinArgs &a, 
     unsigned short *srow = reinterpret_cast<unsigned short *>(nslots + a.n_layouts * 2);  // [n_layouts][128] slot -> row base
 
     const int n_slices = a.n_out / CS;
-    int bx = blockIdx.x;
     const __nv_bfloat16 *wt = a.wt;
     const float *bias = a.bias;
     long long r_beg = 0, r_end = a.n_envs;
+    int slice = blockIdx.x % n_slices, worker = blockIdx.x / n_slices;
     if constexpr (GROUPED) {
+        int bx = blockIdx.x;
         const int per = n_slices * a.n_workers, k = bx / per;
         bx -= k * per;
         wt += (size_t)k * a.W * a.H * N_PLANES * a.n_out, bias += (size_t)k * a.n_out;
         r_beg = min(max((long long)__ldg(offsets + k), 0ll), a.n_envs);
         r_end = max(min((long long)__ldg(offsets + k + 1), a.n_envs), r_beg);
+        slice = bx % n_slices, worker = bx / n_slices;
     }
-    const int slice = bx % n_slices, worker = bx / n_slices;
     const int col0 = slice * CS;
     if constexpr (ROWS) {
         r_beg = max(__ldg(a.range), 0);
@@ -513,7 +330,7 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_masked_kernel(con
 
 template <int CPL>
 __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_grouped_kernel(const EncLinArgs a, const int32_t *offsets) {
-    encode_linear_grouped_body<CPL, false, false, false, true>(a, nullptr, nullptr, offsets);
+    encode_linear_body<CPL, false, false, false, true>(a, nullptr, nullptr, offsets);
 }
 
 static size_t encode_linear_smem(int cpl, int n_rows, int n_layouts) {
@@ -1061,6 +878,29 @@ __device__ __forceinline__ void episode_stats_update(const ovc_episode_stats_t &
     s.layout_id[e] = new_lid;
 }
 
+// The transition both record kernels write.  VIEW (record_transition_view_kernel): ONE reward per environment, the
+// agent's at player p(e) = seat ^ (swap[e] != 0), bit for bit rewards[2 e + p(e)] of the two-row store.
+template <bool STATS, bool VIEW>
+__device__ __forceinline__ void record_body(long long e, const int32_t *__restrict__ sparse, const int32_t *__restrict__ shaped, float f,
+                                            long long n_envs, long long *__restrict__ ret_sparse, float *__restrict__ ret_mixed,
+                                            const int32_t *__restrict__ done, const int32_t *__restrict__ swap, int seat,
+                                            float *__restrict__ rewards, uint8_t *__restrict__ dones, const ovc_episode_stats_t &stats) {
+    const int sp = sparse[e];
+    const int2 sh = reinterpret_cast<const int2 *>(shaped)[e];
+    if (ret_sparse) ret_sparse[e] += sp;
+    if (ret_mixed) ret_mixed[e] = ((ret_mixed[e] + (float)sp) + f * (float)sh.x) + f * (float)sh.y;
+    if constexpr (VIEW) {
+        const int p = seat ^ (swap && swap[e] != 0);
+        rewards[e] = __fadd_rn((float)sp, __fmul_rn(f, (float)(p ? sh.y : sh.x)));
+    } else if (rewards) {
+        reinterpret_cast<float2 *>(rewards)[e] = make_float2(__fadd_rn((float)sp, __fmul_rn(f, (float)sh.x)), __fadd_rn((float)sp, __fmul_rn(f, (float)sh.y)));
+    }
+    if (dones) dones[e] = done[e] != 0;
+    if constexpr (STATS)
+        episode_stats_update(stats, e, n_envs, sh, __fadd_rn((float)sp, __fmul_rn(f, (float)sh.x)), __fadd_rn((float)sp, __fmul_rn(f, (float)sh.y)),
+                             done[e] != 0);
+}
+
 template <bool STATS>
 __global__ void __launch_bounds__(256) accumulate_returns_kernel(const int32_t *__restrict__ sparse, const int32_t *__restrict__ shaped,
                                                                  float factor, long long n_envs, long long *__restrict__ ret_sparse,
@@ -1069,17 +909,8 @@ __global__ void __launch_bounds__(256) accumulate_returns_kernel(const int32_t *
                                                                  uint8_t *__restrict__ dones, const ovc_episode_stats_t stats) {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n_envs) return;
-    const float f = factor_dev ? *factor_dev : factor;
-    const int sp = sparse[e];
-    const int2 sh = reinterpret_cast<const int2 *>(shaped)[e];
-    if (ret_sparse) ret_sparse[e] += sp;
-    if (ret_mixed) ret_mixed[e] = ((ret_mixed[e] + (float)sp) + f * (float)sh.x) + f * (float)sh.y;
-    if (rewards)
-        reinterpret_cast<float2 *>(rewards)[e] = make_float2(__fadd_rn((float)sp, __fmul_rn(f, (float)sh.x)), __fadd_rn((float)sp, __fmul_rn(f, (float)sh.y)));
-    if (dones) dones[e] = done[e] != 0;
-    if constexpr (STATS)
-        episode_stats_update(stats, e, n_envs, sh, __fadd_rn((float)sp, __fmul_rn(f, (float)sh.x)), __fadd_rn((float)sp, __fmul_rn(f, (float)sh.y)),
-                             done[e] != 0);
+    record_body<STATS, false>(e, sparse, shaped, factor_dev ? *factor_dev : factor, n_envs, ret_sparse, ret_mixed, done, nullptr, 0, rewards,
+                              dones, stats);
 }
 
 // seat < 0: rows are joint rows (ovc_sample_actions[_logp]); 0 / 1: one agent's rows (ovc_sample_actions_view)
@@ -1147,9 +978,7 @@ static int accumulate_returns_impl(const int32_t *sparse, const int32_t *shaped,
     return OVC_OK;
 }
 
-// ovc_record_transition_view: accumulate_returns_kernel's transition with ONE reward per environment, the agent's at player
-// p(e) = seat ^ (swap[e] != 0): rewards[e] is bit for bit rewards[2 e + p(e)] of ovc_record_transition.  A kernel of its own:
-// an extra parameter in accumulate_returns_kernel would change the code of its existing instantiations.
+// ovc_record_transition_view: accumulate_returns_kernel's transition with ONE reward per environment (record_body's VIEW)
 template <bool STATS>
 __global__ void __launch_bounds__(256) record_transition_view_kernel(const int32_t *__restrict__ sparse, const int32_t *__restrict__ shaped,
                                                                      long long n_envs, long long *__restrict__ ret_sparse,
@@ -1159,17 +988,7 @@ __global__ void __launch_bounds__(256) record_transition_view_kernel(const int32
                                                                      const ovc_episode_stats_t stats) {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n_envs) return;
-    const float f = *factor_dev;
-    const int sp = sparse[e];
-    const int2 sh = reinterpret_cast<const int2 *>(shaped)[e];
-    if (ret_sparse) ret_sparse[e] += sp;
-    if (ret_mixed) ret_mixed[e] = ((ret_mixed[e] + (float)sp) + f * (float)sh.x) + f * (float)sh.y;
-    const int p = seat ^ (swap && swap[e] != 0);
-    rewards[e] = __fadd_rn((float)sp, __fmul_rn(f, (float)(p ? sh.y : sh.x)));
-    if (dones) dones[e] = done[e] != 0;
-    if constexpr (STATS)
-        episode_stats_update(stats, e, n_envs, sh, __fadd_rn((float)sp, __fmul_rn(f, (float)sh.x)), __fadd_rn((float)sp, __fmul_rn(f, (float)sh.y)),
-                             done[e] != 0);
+    record_body<STATS, true>(e, sparse, shaped, *factor_dev, n_envs, ret_sparse, ret_mixed, done, swap, seat, rewards, dones, stats);
 }
 
 static int record_transition_view_impl(const int32_t *sparse, const int32_t *shaped, const int32_t *done, const float *factor_dev,

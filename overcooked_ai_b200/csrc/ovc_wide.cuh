@@ -45,7 +45,7 @@ struct WideArgs {
     float slope;
     int n_tiles;
     const int32_t *range;  // wide_layers_kernel<true>: rows [range[0], range[1]) of the m-row buffers only (device memory);
-                           // wide_layers_grouped_kernel<false, true>: the members' row offsets [n_tiles + 1] (device memory)
+                           // wide_layers_kernel<false, true>: the members' row offsets [n_tiles + 1] (device memory)
 };
 
 constexpr int WL_MAX_MEMBERS = 64;
@@ -146,134 +146,6 @@ __device__ __forceinline__ uint32_t leaky_bf16x2(float x0, float x1, float slope
 
 // RANGE: 128-row tiles from row range[0], stores guarded by range[1]; every warp reads the range, so the producer and both
 // consumer warpgroups walk the same tiles and the mbarrier protocol stays balanced.  The tensor maps still span all m rows.
-template <bool RANGE = false>
-__global__ void __launch_bounds__(WL_THREADS, 1)
-wide_layers_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_w1,
-                   const __grid_constant__ CUtensorMap map_w2, const WideArgs p) {
-    long long r_beg = 0, r_end = p.m;
-    int n_tiles = p.n_tiles;
-    if constexpr (RANGE) {
-        r_beg = max(__ldg(p.range), 0);
-        r_end = max(min((long long)__ldg(p.range + 1), p.m), r_beg);
-        n_tiles = (int)((r_end - r_beg + WL_BM - 1) / WL_BM);
-    }
-    extern __shared__ char wl_raw[];
-    char *tile = reinterpret_cast<char *>((reinterpret_cast<uintptr_t>(wl_raw) + 1023) & ~(uintptr_t)1023);
-    char *w2_tile = tile + WL_STAGES * WL_STAGE;
-    float *bias1 = reinterpret_cast<float *>(tile + WL_TILE_BYTES);
-    float *bias2 = bias1 + WL_N1;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(bias2 + WL_N2);
-    uint64_t *full = bars, *empty = bars + WL_STAGES, *w2_full = bars + 2 * WL_STAGES, *w2_empty = w2_full + 2;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (threadIdx.x == 0) {
-        // a stage is free again when all 8 consumer warps have seen their wgmma reading it complete
-        for (int i = 0; i < WL_STAGES; i++) mbar_init(full + i, 1), mbar_init(empty + i, 8);
-        for (int i = 0; i < 2; i++) mbar_init(w2_full + i, 1), mbar_init(w2_empty + i, 8);
-        prefetch_tmap(&map_a0), prefetch_tmap(&map_w1), prefetch_tmap(&map_w2);
-    }
-    for (int i = threadIdx.x; i < WL_N1; i += WL_THREADS) bias1[i] = p.b1[i];
-    for (int i = threadIdx.x; i < WL_N2; i += WL_THREADS) bias2[i] = p.b2[i];
-    __syncthreads();
-
-    if (warp >= 8) {
-        regs_dealloc<40>();
-        if (warp == 8 && lane == 0) {
-            // ---- TMA producer: tiles blockIdx.x, + gridDim.x, ...; the rings' use counters run on across tiles ----
-            int it1 = 0, it2 = 0;
-            for (int tile_i = blockIdx.x; tile_i < n_tiles; tile_i += gridDim.x) {
-                const int m0 = (int)(r_beg + tile_i * WL_BM);
-                for (int n = 0; n < WL_CHUNKS; n++) {
-                    for (int c = 0; c < WL_KC; c++, it1++) {
-                        const int s = it1 % WL_STAGES, u = it1 / WL_STAGES;
-                        mbar_wait_bounded(empty + s, (u & 1) ^ 1);
-                        char *st = tile + s * WL_STAGE;
-                        mbar_expect_tx(full + s, WL_STAGE);
-                        tma_load_2d(st, &map_a0, c * WL_BK, m0, full + s);  // rows past M: zero fill, still counted
-                        tma_load_2d(st + WL_A_BYTES, &map_w1, c * WL_BK, n * WL_NC, full + s);
-                    }
-                    const int s = it2 & 1, u = it2 >> 1;
-                    it2++;
-                    mbar_wait_bounded(w2_empty + s, (u & 1) ^ 1);
-                    mbar_expect_tx(w2_full + s, WL_B2_STAGE);
-                    for (int h = 0; h < WL_NC / WL_BK; h++)
-                        tma_load_2d(w2_tile + s * WL_B2_STAGE + h * WL_B2_BOX, &map_w2, n * WL_NC + h * WL_BK, 0, w2_full + s);
-                }
-            }
-        }
-        return;
-    }
-
-    // ---- consumer warpgroup g: rows 64 g .. 64 g + 63 of the tile; warp w of the group owns 16 of them ----
-    regs_alloc<232>();
-    const int g = warp >> 2, w = warp & 3;
-    float acc1[64], acc2[80];
-    uint32_t a1[WL_NC / 16][4];  // the activation chunk as layer 2's A fragments, one [4] per k-step of 16
-#pragma unroll
-    for (int i = 0; i < 80; i++) acc2[i] = 0.f;
-    int it1 = 0, it2 = 0;
-    for (int tile_i = blockIdx.x; tile_i < n_tiles; tile_i += gridDim.x) {
-        for (int n = 0; n < WL_CHUNKS; n++) {
-            // layer 1, columns n*128 .. n*128+127: 8 k-chunks, one stage each; a stage is released once the wgmma
-            // group after it has been issued and it has itself completed (wait_group 1)
-#pragma unroll
-            for (int i = 0; i < 64; i++) acc1[i] = 0.f;
-            int prev = 0;
-            for (int c = 0; c < WL_KC; c++, it1++) {
-                const int s = it1 % WL_STAGES, u = it1 / WL_STAGES;
-                mbar_wait_bounded(full + s, u & 1);
-                const uint32_t a_addr = smem_u32(tile + s * WL_STAGE) + g * (WL_A_BYTES / 2);
-                const uint64_t da = wgmma_desc_sw128(a_addr), db = wgmma_desc_sw128(smem_u32(tile + s * WL_STAGE + WL_A_BYTES));
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < WL_BK / 16; k++) wgmma_m64n128_ss(acc1, da + 2 * k, db + 2 * k, (c | k) != 0);
-                wgmma_commit();
-                wgmma_wait<1>();
-                if (c && lane == 0) mbar_arrive(empty + prev);
-                prev = s;
-            }
-            wgmma_wait<0>();
-            if (lane == 0) mbar_arrive(empty + prev);
-            // epilogue 1: bias, leaky ReLU, bf16.  Accumulator n8-group j holds (row l/4, columns 8j + 2(l%4) + {0,1}) in
-            // [4j], [4j+1] and row l/4 + 8 in [4j+2], [4j+3]; k-step q's A fragment is groups 2q (registers 0, 1) and 2q+1 (2, 3).
-            const float *bn = bias1 + n * WL_NC + 2 * (lane & 3);
-#pragma unroll
-            for (int j = 0; j < WL_NC / 8; j++) {
-                const float b0 = bn[8 * j], b1 = bn[8 * j + 1];
-                a1[j >> 1][(j & 1) * 2] = leaky_bf16x2(acc1[4 * j] + b0, acc1[4 * j + 1] + b1, p.slope);
-                a1[j >> 1][(j & 1) * 2 + 1] = leaky_bf16x2(acc1[4 * j + 2] + b0, acc1[4 * j + 3] + b1, p.slope);
-            }
-            // layer 2: z2 += a1[:, n*128 .. n*128+127] . W2[:, n*128 .. n*128+127]^T
-            const int s = it2 & 1, u = it2 >> 1;
-            it2++;
-            mbar_wait_bounded(w2_full + s, u & 1);
-            const uint32_t b_addr = smem_u32(w2_tile + s * WL_B2_STAGE);
-            wgmma_fence();
-#pragma unroll
-            for (int q = 0; q < WL_NC / 16; q++)
-                wgmma_m64n160_rs(acc2, a1[q], wgmma_desc_sw128(b_addr + (q >> 2) * WL_B2_BOX) + 2 * (q & 3), (n | q) != 0);
-            wgmma_commit();
-            wgmma_wait<0>();
-            if (lane == 0) mbar_arrive(w2_empty + s);
-        }
-        // epilogue 2: bias, bf16, two rows of 160 columns per quad of lanes
-        const long long row = r_beg + (long long)tile_i * WL_BM + g * 64 + w * 16 + (lane >> 2);
-#pragma unroll
-        for (int j = 0; j < WL_N2 / 8; j++) {
-            const int col = 8 * j + 2 * (lane & 3);
-            const float b0 = bias2[col], b1 = bias2[col + 1];
-            if (row < r_end)
-                *reinterpret_cast<__nv_bfloat162 *>(p.z2 + row * WL_N2 + col) = __floats2bfloat162_rn(acc2[4 * j] + b0, acc2[4 * j + 1] + b1);
-            if (row + 8 < r_end)
-                *reinterpret_cast<__nv_bfloat162 *>(p.z2 + (row + 8) * WL_N2 + col) = __floats2bfloat162_rn(acc2[4 * j + 2] + b0, acc2[4 * j + 3] + b1);
-        }
-    }
-}
-
-// wide_layers_kernel with GROUPED (a copy, so that the code of wide_layers_kernel stays as it was).
-// RANGE: 128-row tiles from row range[0], stores guarded by range[1]; every warp reads the range, so the producer and both
-// consumer warpgroups walk the same tiles and the mbarrier protocol stays balanced.  The tensor maps still span all m rows.
 // GROUPED (ovc_wide_layers_grouped): p.n_tiles members, member k's rows [p.range[k], p.range[k + 1]) and weights rows
 // k n1.. of W1 / k n2.. of W2 (stacked: one tensor map per operand serves every member through its row coordinate), biases
 // [k][...] read from global memory.  The tile list is every member's 128-row tiles in member order, a member's last tile
@@ -281,8 +153,9 @@ wide_layers_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_cons
 // shared table, so the mbarrier protocol stays balanced.
 template <bool RANGE = false, bool GROUPED = false>
 __global__ void __launch_bounds__(WL_THREADS, 1)
-wide_layers_grouped_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_w1,
+wide_layers_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_w1,
                    const __grid_constant__ CUtensorMap map_w2, const WideArgs p) {
+    static_assert(!(RANGE && GROUPED), "a grouped launch reads its members' offsets, not a range");
     long long r_beg = 0, r_end = p.m;
     int n_tiles = p.n_tiles;
     if constexpr (RANGE) {
@@ -452,69 +325,49 @@ static int make_tmap_bf16(CUtensorMap *m, const void *base, long long rows, int 
     return OVC_OK;
 }
 
-// range != NULL: ovc_wide_layers_range (wide_layers_kernel<true>)
+// range != NULL: ovc_wide_layers_range (wide_layers_kernel<true>).  grouped: ovc_wide_layers_grouped
+// (wide_layers_kernel<false, true>) with w1 [n_members * 512][512], w2 [n_members * 160][512], b1 [n_members][512],
+// b2 [n_members][160] and range = the offsets [n_members + 1] rows of a0 / z2 (device memory).
 static int wide_layers_impl(const void *a0, long long m, int k0, const void *w1, const float *b1, int n1, const void *w2, const float *b2,
-                            int n2, float slope, void *z2, cudaStream_t st, const int32_t *range = nullptr) {
-    const bool ranged = range != nullptr;
-    if (!a0 || !w1 || !b1 || !w2 || !b2 || !z2) return fail(OVC_E_BADARG, "null pointer argument");
+                            int n2, float slope, void *z2, cudaStream_t st, const int32_t *range = nullptr, bool grouped = false,
+                            int n_members = 1) {
+    if (!a0 || !w1 || !b1 || !w2 || !b2 || !z2 || (grouped && !range)) return fail(OVC_E_BADARG, "null pointer argument");
     if (k0 != WL_K0 || n1 != WL_N1 || n2 != WL_N2) return fail(OVC_E_UNSUPPORTED, "wide_layers: built for 512 -> 512 -> 160", k0 * 1000000ll + n1 * 1000 + n2);
     if ((((uintptr_t)a0 | (uintptr_t)w1 | (uintptr_t)w2 | (uintptr_t)z2) & 15) != 0) return fail(OVC_E_BADARG, "operands must be 16-byte aligned");
-    if (((uintptr_t)range & 3) != 0) return fail(OVC_E_BADARG, "range must be 4-byte aligned");
-    if (ranged && m > 0x7FFFFFFFll) return fail(OVC_E_BADARG, "m must be below 2^31", m);
+    if (grouped) {
+        if ((((uintptr_t)b1 | (uintptr_t)b2) & 7) != 0) return fail(OVC_E_BADARG, "biases must be 8-byte aligned");
+        if (((uintptr_t)range & 3) != 0) return fail(OVC_E_BADARG, "offsets must be 4-byte aligned");
+        if (n_members < 1 || n_members > WL_MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+        if (m < 0 || m > 0x7FFFFFFFll) return fail(OVC_E_BADARG, "m must lie in [0, 2^31)", m);
+    } else {
+        if (((uintptr_t)range & 3) != 0) return fail(OVC_E_BADARG, "range must be 4-byte aligned");
+        if (range && m > 0x7FFFFFFFll) return fail(OVC_E_BADARG, "m must be below 2^31", m);
+    }
     if (!(slope >= 0.f && slope <= 1.f)) return fail(OVC_E_BADARG, "negative slope must lie in [0, 1]");
     if (m < 0) return fail(OVC_E_BADARG, "negative row count");
     if (m == 0) return OVC_OK;
     CUtensorMap ma, mw1, mw2;
     int rc = make_tmap_bf16(&ma, a0, m, WL_K0, WL_BM);
-    if (!rc) rc = make_tmap_bf16(&mw1, w1, WL_N1, WL_K0, WL_NC);  // one column chunk of a k-chunk per box
-    if (!rc) rc = make_tmap_bf16(&mw2, w2, WL_N2, WL_N1, WL_N2);
+    if (!rc) rc = make_tmap_bf16(&mw1, w1, (long long)n_members * WL_N1, WL_K0, WL_NC);  // one column chunk of a k-chunk per box
+    if (!rc) rc = make_tmap_bf16(&mw2, w2, (long long)n_members * WL_N2, WL_N1, WL_N2);
     if (rc) return rc;
-    cudaError_t e = ranged ? cudaFuncSetAttribute(wide_layers_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WL_SMEM)
-                           : cudaFuncSetAttribute(wide_layers_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WL_SMEM);
+    void (*kern)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const WideArgs) =
+        grouped ? wide_layers_kernel<false, true> : range ? wide_layers_kernel<true> : wide_layers_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WL_SMEM);
     if (e != cudaSuccess) return cuda_fail(e, "wide_layers kernel attribute");
     WideArgs p;
     int dev = 0, n_sm = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
     p.b1 = b1, p.b2 = b2, p.z2 = (__nv_bfloat16 *)z2, p.m = m, p.slope = slope, p.range = range;
-    p.n_tiles = (int)((m + WL_BM - 1) / WL_BM);  // with a range: the most tiles it can hold (the kernel reads its own count)
-    // persistent: one CTA per SM walks tiles blockIdx.x, + gridDim.x, ... (barriers and biases are set up once)
-    const unsigned grid = (unsigned)(p.n_tiles < n_sm ? p.n_tiles : n_sm);
-    if (ranged) wide_layers_kernel<true><<<grid, WL_THREADS, WL_SMEM, st>>>(ma, mw1, mw2, p);
-    else wide_layers_kernel<false><<<grid, WL_THREADS, WL_SMEM, st>>>(ma, mw1, mw2, p);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "wide_layers kernel launch");
-    return OVC_OK;
-}
-
-// ovc_wide_layers_grouped: w1 [n_members * 512][512], w2 [n_members * 160][512], b1 [n_members][512], b2 [n_members][160],
-// offsets [n_members + 1] rows of a0 / z2 (device memory)
-static int wide_layers_grouped_impl(const void *a0, long long m, int k0, const void *w1, const float *b1, int n1, const void *w2,
-                                    const float *b2, int n2, float slope, const int32_t *offsets, int n_members, void *z2, cudaStream_t st) {
-    if (!a0 || !w1 || !b1 || !w2 || !b2 || !z2 || !offsets) return fail(OVC_E_BADARG, "null pointer argument");
-    if (k0 != WL_K0 || n1 != WL_N1 || n2 != WL_N2) return fail(OVC_E_UNSUPPORTED, "wide_layers: built for 512 -> 512 -> 160", k0 * 1000000ll + n1 * 1000 + n2);
-    if ((((uintptr_t)a0 | (uintptr_t)w1 | (uintptr_t)w2 | (uintptr_t)z2) & 15) != 0) return fail(OVC_E_BADARG, "operands must be 16-byte aligned");
-    if ((((uintptr_t)b1 | (uintptr_t)b2) & 7) != 0) return fail(OVC_E_BADARG, "biases must be 8-byte aligned");
-    if (((uintptr_t)offsets & 3) != 0) return fail(OVC_E_BADARG, "offsets must be 4-byte aligned");
-    if (n_members < 1 || n_members > WL_MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
-    if (m < 0 || m > 0x7FFFFFFFll) return fail(OVC_E_BADARG, "m must lie in [0, 2^31)", m);
-    if (!(slope >= 0.f && slope <= 1.f)) return fail(OVC_E_BADARG, "negative slope must lie in [0, 1]");
-    if (m == 0) return OVC_OK;
-    CUtensorMap ma, mw1, mw2;
-    int rc = make_tmap_bf16(&ma, a0, m, WL_K0, WL_BM);
-    if (!rc) rc = make_tmap_bf16(&mw1, w1, (long long)n_members * WL_N1, WL_K0, WL_NC);
-    if (!rc) rc = make_tmap_bf16(&mw2, w2, (long long)n_members * WL_N2, WL_N1, WL_N2);
-    if (rc) return rc;
-    cudaError_t e = cudaFuncSetAttribute(wide_layers_grouped_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WL_SMEM);
-    if (e != cudaSuccess) return cuda_fail(e, "wide_layers kernel attribute");
-    WideArgs p;
-    int dev = 0, n_sm = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    p.b1 = b1, p.b2 = b2, p.z2 = (__nv_bfloat16 *)z2, p.m = m, p.slope = slope, p.range = offsets, p.n_tiles = n_members;
-    const long long most = (m + WL_BM - 1) / WL_BM + n_members;  // the tile list's largest length
+    // grouped: the member count (the kernel builds its tile list); otherwise the tiles of m rows (with a range: the most
+    // tiles it can hold, the kernel reads its own count)
+    p.n_tiles = grouped ? n_members : (int)((m + WL_BM - 1) / WL_BM);
+    // persistent: one CTA per SM walks tiles blockIdx.x, + gridDim.x, ... (barriers and biases are set up once); a grouped
+    // tile list holds at most one partial tile per member more than m rows do
+    const long long most = (m + WL_BM - 1) / WL_BM + (grouped ? n_members : 0);
     const unsigned grid = (unsigned)(most < n_sm ? most : n_sm);
-    wide_layers_grouped_kernel<false, true><<<grid, WL_THREADS, WL_SMEM, st>>>(ma, mw1, mw2, p);
+    kern<<<grid, WL_THREADS, WL_SMEM, st>>>(ma, mw1, mw2, p);
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "wide_layers kernel launch");
     return OVC_OK;
