@@ -663,7 +663,7 @@ static PolicyTailArgs tail_args(const void *x, int64_t n_rows, float in_slope, c
                                 const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                                 float slope, int n_actions, uint64_t seed, uint64_t *counter, int32_t *actions, float *values,
                                 float *scores, float *logp) {
-    PolicyTailArgs a;
+    PolicyTailArgs a = {};
     a.x = (const __nv_bfloat16 *)x, a.w_first = (const __nv_bfloat16 *)w_first, a.b_first = b_first;
     a.w_hidden = (const __nv_bfloat16 *)w_hidden, a.b_hidden = b_hidden, a.w_heads = (const __nv_bfloat16 *)w_heads, a.b_heads = b_heads;
     a.n_rows = n_rows, a.n_hidden = n_hidden, a.n_actions = n_actions, a.in_slope = in_slope, a.slope = slope, a.seed = seed;
@@ -765,7 +765,7 @@ int ovc_sample_actions_view(const float *scores, int ld, int n_actions, int64_t 
                             const int32_t *swap, int seat, int32_t *actions, float *logp, void *stream) {
     if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
     return ovc::sample_actions_impl(scores, ld, n_actions, n_rows, seed, (unsigned long long *)counter, actions, logp, (cudaStream_t)stream,
-                                    swap, seat);
+                                    ovc::RowMap::View, swap, seat);
 }
 
 int ovc_sample_actions(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter,
@@ -814,8 +814,8 @@ int ovc_record_transition_view(const int32_t *sparse, const int32_t *shaped, con
 
 int ovc_gae_view(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, int64_t n_steps,
                  int64_t n_envs, float gamma, float lambda, float *advantages, float *value_targets, void *stream) {
-    return ovc::gae_view_impl(rewards, values, dones, last_values, n_steps, n_envs, gamma, lambda, advantages, value_targets,
-                              (cudaStream_t)stream);
+    return ovc::gae_impl(rewards, values, dones, last_values, n_steps, n_envs, gamma, lambda, advantages, value_targets,
+                         (cudaStream_t)stream, true);
 }
 
 int ovc_policy_tail_logp(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
@@ -831,10 +831,11 @@ int ovc_policy_tail_view(const void *x, int64_t n_rows, int k0, float in_slope, 
                          const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                          float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *swap, int seat, int32_t *actions,
                          float *values, float *scores, float *logp, void *stream) {
-    const ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
-                                                 n_actions, seed, counter, actions, values, scores, logp);
+    ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                           n_actions, seed, counter, actions, values, scores, logp);
+    a.swap = swap, a.seat = seat;
     if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
-    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, swap, seat);
+    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, ovc::RowMap::View);
 }
 
 int ovc_policy_hidden(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
@@ -843,7 +844,7 @@ int ovc_policy_hidden(const void *x, int64_t n_rows, int k0, float in_slope, con
     ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_first, b_first, slope, 1,
                                            0, nullptr, nullptr, nullptr, nullptr, nullptr);
     a.hidden = (__nv_bfloat16 *)hidden;
-    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, true);
+    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, ovc::RowMap::Identity, true);
 }
 
 int ovc_lstm_head(const void *x, const void *h_in, const float *c_in, const int32_t *reset, int64_t n_rows, const void *w,
@@ -929,17 +930,18 @@ int ovc_policy_tail_rows(const void *x, int64_t n_rows, int k0, float in_slope, 
                          const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                          float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *swap, int seat, const int32_t *rows,
                          const int32_t *range, int32_t *actions, float *values, float *scores, float *logp, void *stream) {
-    const ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
-                                                 n_actions, seed, counter, actions, values, scores, logp);
+    ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                           n_actions, seed, counter, actions, values, scores, logp);
+    a.swap = swap, a.seat = seat, a.rows = rows, a.range = range;
     if (seat != 0 && seat != 1) return ovc::fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
     if (!rows || !range) return ovc::fail(OVC_E_BADARG, "null pointer argument");
-    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, swap, seat, rows, range);
+    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, ovc::RowMap::Rows);
 }
 
 int ovc_sample_actions_rows(const float *scores, int ld, int n_actions, int64_t n_rows, uint64_t seed, uint64_t *counter, const int32_t *swap,
                             int seat, const int32_t *rows, const int32_t *range, int32_t *actions, float *logp, void *stream) {
-    return ovc::sample_actions_rows_impl(scores, ld, n_actions, n_rows, seed, (unsigned long long *)counter, swap, seat, rows, range, actions,
-                                         logp, (cudaStream_t)stream);
+    return ovc::sample_actions_impl(scores, ld, n_actions, n_rows, seed, (unsigned long long *)counter, actions, logp, (cudaStream_t)stream,
+                                    ovc::RowMap::Rows, swap, seat, rows, range);
 }
 
 int ovc_learner_rows(const int32_t *partner_seat, int64_t n_envs, int32_t *list, int32_t *first, int32_t *jrow, int32_t *range, void *stream) {
@@ -969,10 +971,11 @@ int ovc_policy_tail_joint(const void *x, int64_t n_rows, int k0, float in_slope,
                           const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                           float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *jrow, const int32_t *range,
                           int32_t *actions, float *values, float *scores, float *logp, void *stream) {
-    const ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
-                                                 n_actions, seed, counter, actions, values, scores, logp);
+    ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                           n_actions, seed, counter, actions, values, scores, logp);
+    a.rows = jrow, a.range = range;
     if (n_rows > 0x7FFFFFFFll) return ovc::fail(OVC_E_BADARG, "n_rows must be below 2^31", n_rows);
-    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, false, nullptr, -1, jrow, range, true);
+    return ovc::policy_tail_impl(a, k0, (cudaStream_t)stream, ovc::RowMap::Joint);
 }
 
 int ovc_encode_linear_grouped(const void *layouts, int n_layouts, const int32_t *state, const void *wt, const float *bias,
@@ -995,9 +998,10 @@ int ovc_policy_tail_grouped(const void *x, int64_t n_rows, int k0, float in_slop
                             const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
                             float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *offsets, int n_members,
                             int32_t *actions, float *values, float *scores, float *logp, void *stream) {
-    const ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
-                                                 n_actions, seed, counter, actions, values, scores, logp);
-    return ovc::policy_tail_grouped_impl(a, k0, offsets, n_members, (cudaStream_t)stream);
+    ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                           n_actions, seed, counter, actions, values, scores, logp);
+    a.offsets = offsets, a.n_members = n_members;
+    return ovc::policy_tail_grouped_impl(a, k0, (cudaStream_t)stream);
 }
 
 int ovc_featurize(const void *layouts, int n_layouts, const void *lut, const int32_t *state,

@@ -694,19 +694,52 @@ namespace ovc {
 // (seed, step, row) alone.  counter[0] = the step; counter[1] = arrival count of the CTAs of the current launch: the
 // last CTA to finish advances the step (every CTA has read it by then), so a captured CUDA graph draws fresh numbers at
 // every replay without any host involvement.
+
+// u = (k + 0.5) / 2^23 from the top 23 bits k of a Philox word: exact in float32, never 0 or 1
+__device__ __forceinline__ float draw_uniform(uint32_t r) { return ((float)(r >> 9) + 0.5f) * 1.1920928955078125e-7f; }
+
+// The last CTA of a launch to get here advances the draw step (every CTA has read it by then): counter[1] counts arrivals.
+__device__ __forceinline__ void advance_step(unsigned long long *counter, unsigned long long step) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        const unsigned long long arrived = atomicAdd(counter + 1, 1ull);
+        if (arrived == (unsigned long long)gridDim.x - 1) {
+            counter[1] = 0;
+            counter[0] = step + 1;
+            __threadfence();
+        }
+    }
+}
+
+// Where a row of a draw's input goes (the draw kernel below, K8):
+//   Identity: row r is joint row r;
+//   View: row r is one agent's row of environment r, at player p(r) = seat ^ (swap[r] != 0) (swap nullable): drawn on the
+//     joint row 2 r + p(r), which indexes actions; every other output stays indexed by r;
+//   Rows: compact rows r in [range[0], range[1]) only, environment e = rows[r] at player p(e): drawn on the joint row
+//     2 e + p(e), which indexes actions; every other output stays indexed by r;
+//   Joint (K8 only): compact rows r in [range[0], range[1]) only, drawn on the joint row rows[r], which indexes every output.
+enum class RowMap { Identity, View, Rows, Joint };
+
 // LOGP: also logp[row] = scores[row][a] - (m + log(sum_i exp(scores[row][i] - m))), m = max_i scores[row][i], at the drawn a.
-// VIEW: row r is one agent's row of environment r, at player p(r) = seat ^ (swap[r] != 0) (swap nullable): the draw uses
-// the joint row g = 2 r + p(r) and writes actions[g]; scores and logp stay indexed by r.
-template <bool LOGP, bool VIEW = false>
+// Every CTA, with rows in the range or not, takes part in the counter's advance.
+template <bool LOGP, RowMap MAP>
 __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__restrict__ scores, int ld, int n_actions, long long n_rows,
                                                              unsigned long long seed, unsigned long long *counter,
                                                              int32_t *__restrict__ actions, float *__restrict__ logp,
-                                                             const int32_t *__restrict__ swap = nullptr, int seat = 0) {
+                                                             const int32_t *__restrict__ swap, int seat, const int32_t *__restrict__ rows,
+                                                             const int32_t *__restrict__ range) {
+    static_assert(MAP != RowMap::Joint, "the draw has no joint-rows form");
     const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(counter);
     const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (row < n_rows) {
+    const bool in = MAP == RowMap::Rows ? row >= max(__ldg(range), 0) && row < min((long long)__ldg(range + 1), n_rows) : row < n_rows;
+    if (in) {
         const float *s = scores + row * ld;
-        const long long g = VIEW ? 2 * row + (seat ^ (swap && swap[row] != 0)) : row;
+        long long g = row;
+        if constexpr (MAP != RowMap::Identity) {
+            const long long e = MAP == RowMap::Rows ? (long long)__ldg(rows + row) : row;
+            g = 2 * e + (seat ^ (swap && swap[e] != 0));
+        }
         const uint32_t c3 = (uint32_t)(step >> 32) << 1;
         const Philox4 A = philox4x32_10(seed, (uint32_t)g, (uint32_t)((unsigned long long)g >> 32), (uint32_t)step, c3);
         Philox4 B = A;
@@ -715,8 +748,7 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__rest
         float best_v = -INFINITY;
         for (int i = 0; i < n_actions; i++) {
             const uint32_t r = i < 4 ? A.v[i] : B.v[i - 4];
-            const float u = ((float)(r >> 9) + 0.5f) * 1.1920928955078125e-7f;  // (k + 0.5) / 2^23, exact in float32: never 0 or 1
-            const float v = s[i] - logf(-logf(u));
+            const float v = s[i] - logf(-logf(draw_uniform(r)));
             if (v > best_v) best_v = v, best = i;
         }
         actions[g] = best;
@@ -728,84 +760,7 @@ __global__ void __launch_bounds__(256) sample_actions_kernel(const float *__rest
             logp[row] = s[best] - (m + logf(se));
         }
     }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        const unsigned long long arrived = atomicAdd(counter + 1, 1ull);
-        if (arrived == (unsigned long long)gridDim.x - 1) {
-            counter[1] = 0;
-            counter[0] = step + 1;
-            __threadfence();
-        }
-    }
-}
-
-// The rows map (ovc_sample_actions_rows): compact rows r in [range[0], range[1]) only, environment e = rows[r] at player
-// p(e) = seat ^ (swap[e] != 0): the draw uses the joint row 2 e + p(e) and writes actions[2 e + p(e)]; scores and logp stay
-// indexed by r.  Every CTA, with rows in the range or not, takes part in the counter's advance.  A kernel of its own, so
-// that sample_actions_kernel's instantiations stay as they are.
-template <bool LOGP>
-__global__ void __launch_bounds__(256) sample_actions_rows_kernel(const float *__restrict__ scores, int ld, int n_actions, long long n_rows,
-                                                                  unsigned long long seed, unsigned long long *counter,
-                                                                  int32_t *__restrict__ actions, float *__restrict__ logp,
-                                                                  const int32_t *__restrict__ swap, int seat, const int32_t *__restrict__ rows,
-                                                                  const int32_t *__restrict__ range) {
-    const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(counter);
-    const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (row >= max(__ldg(range), 0) && row < min((long long)__ldg(range + 1), n_rows)) {
-        const float *s = scores + row * ld;
-        const long long e = __ldg(rows + row);
-        const long long g = 2 * e + (seat ^ (swap && swap[e] != 0));
-        const uint32_t c3 = (uint32_t)(step >> 32) << 1;
-        const Philox4 A = philox4x32_10(seed, (uint32_t)g, (uint32_t)((unsigned long long)g >> 32), (uint32_t)step, c3);
-        Philox4 B = A;
-        if (n_actions > 4) B = philox4x32_10(seed, (uint32_t)g, (uint32_t)((unsigned long long)g >> 32), (uint32_t)step, c3 | 1u);
-        int best = 0;
-        float best_v = -INFINITY;
-        for (int i = 0; i < n_actions; i++) {
-            const uint32_t r = i < 4 ? A.v[i] : B.v[i - 4];
-            const float u = ((float)(r >> 9) + 0.5f) * 1.1920928955078125e-7f;
-            const float v = s[i] - logf(-logf(u));
-            if (v > best_v) best_v = v, best = i;
-        }
-        actions[g] = best;
-        if constexpr (LOGP) {
-            float m = s[0];
-            for (int i = 1; i < n_actions; i++) m = fmaxf(m, s[i]);
-            float se = 0.f;
-            for (int i = 0; i < n_actions; i++) se += expf(s[i] - m);
-            logp[row] = s[best] - (m + logf(se));
-        }
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        const unsigned long long arrived = atomicAdd(counter + 1, 1ull);
-        if (arrived == (unsigned long long)gridDim.x - 1) {
-            counter[1] = 0;
-            counter[0] = step + 1;
-            __threadfence();
-        }
-    }
-}
-
-static int sample_actions_rows_impl(const float *scores, int ld, int n_actions, long long n_rows, unsigned long long seed,
-                                    unsigned long long *counter, const int32_t *swap, int seat, const int32_t *rows, const int32_t *range,
-                                    int32_t *actions, float *logp, cudaStream_t st) {
-    if (!scores || !counter || !actions || !rows || !range) return fail(OVC_E_BADARG, "null pointer argument");
-    if (seat != 0 && seat != 1) return fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
-    if (n_actions < 1 || n_actions > 8 || ld < n_actions) return fail(OVC_E_BADARG, "n_actions must be 1..8 and <= ld", n_actions);
-    if (n_rows < 0) return fail(OVC_E_BADARG, "negative row count");
-    if ((((uintptr_t)scores | (uintptr_t)actions | (uintptr_t)logp | (uintptr_t)swap | (uintptr_t)rows | (uintptr_t)range) & 3) != 0)
-        return fail(OVC_E_BADARG, "scores, actions, logp, swap, rows and range must be 4-byte aligned");
-    if (((uintptr_t)counter & 7) != 0) return fail(OVC_E_BADARG, "counter must be 8-byte aligned");
-    if (n_rows == 0) return OVC_OK;
-    const unsigned grid = (unsigned)((n_rows + 255) / 256);
-    if (logp) sample_actions_rows_kernel<true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, logp, swap, seat, rows, range);
-    else sample_actions_rows_kernel<false><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, nullptr, swap, seat, rows, range);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "sample_actions_rows kernel launch");
-    return OVC_OK;
+    advance_step(counter, step);
 }
 
 // ret_sparse[e] += sparse[e];  ret_mixed[e] += sparse[e] + factor * (shaped[e][0] + shaped[e][1])   (rllib.py:328-329)
@@ -913,27 +868,32 @@ __global__ void __launch_bounds__(256) accumulate_returns_kernel(const int32_t *
                               dones, stats);
 }
 
-// seat < 0: rows are joint rows (ovc_sample_actions[_logp]); 0 / 1: one agent's rows (ovc_sample_actions_view)
+// map Identity: rows are joint rows (ovc_sample_actions[_logp]); View: one agent's rows (ovc_sample_actions_view, which
+// checks the seat); Rows: the rows map (ovc_sample_actions_rows)
 static int sample_actions_impl(const float *scores, int ld, int n_actions, long long n_rows, unsigned long long seed,
-                               unsigned long long *counter, int32_t *actions, float *logp, cudaStream_t st,
-                               const int32_t *swap = nullptr, int seat = -1) {
-    if (!scores || !counter || !actions) return fail(OVC_E_BADARG, "null pointer argument");
+                               unsigned long long *counter, int32_t *actions, float *logp, cudaStream_t st, RowMap map = RowMap::Identity,
+                               const int32_t *swap = nullptr, int seat = 0, const int32_t *rows = nullptr, const int32_t *range = nullptr) {
+    const bool listed = map == RowMap::Rows;
+    if (!scores || !counter || !actions || (listed && (!rows || !range))) return fail(OVC_E_BADARG, "null pointer argument");
+    if (listed && seat != 0 && seat != 1) return fail(OVC_E_BADARG, "seat must be 0 or 1", seat);
     if (n_actions < 1 || n_actions > 8 || ld < n_actions) return fail(OVC_E_BADARG, "n_actions must be 1..8 and <= ld", n_actions);
     if (n_rows < 0) return fail(OVC_E_BADARG, "negative row count");
-    if (seat >= 0 && (((uintptr_t)scores | (uintptr_t)actions | (uintptr_t)logp | (uintptr_t)swap) & 3) != 0)
+    if (listed) {
+        if ((((uintptr_t)scores | (uintptr_t)actions | (uintptr_t)logp | (uintptr_t)swap | (uintptr_t)rows | (uintptr_t)range) & 3) != 0)
+            return fail(OVC_E_BADARG, "scores, actions, logp, swap, rows and range must be 4-byte aligned");
+        if (((uintptr_t)counter & 7) != 0) return fail(OVC_E_BADARG, "counter must be 8-byte aligned");
+    } else if (map == RowMap::View && (((uintptr_t)scores | (uintptr_t)actions | (uintptr_t)logp | (uintptr_t)swap) & 3) != 0) {
         return fail(OVC_E_BADARG, "scores, actions, logp and swap must be 4-byte aligned");
+    }
     if (n_rows == 0) return OVC_OK;
     const unsigned grid = (unsigned)((n_rows + 255) / 256);
-    if (seat >= 0) {
-        if (logp) sample_actions_kernel<true, true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, logp, swap, seat);
-        else sample_actions_kernel<false, true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, nullptr, swap, seat);
-    } else if (logp) {
-        sample_actions_kernel<true><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, logp);
-    } else {
-        sample_actions_kernel<false><<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, nullptr);
-    }
+    auto kern = listed                ? (logp ? sample_actions_kernel<true, RowMap::Rows> : sample_actions_kernel<false, RowMap::Rows>)
+                : map == RowMap::View ? (logp ? sample_actions_kernel<true, RowMap::View> : sample_actions_kernel<false, RowMap::View>)
+                : logp                ? sample_actions_kernel<true, RowMap::Identity>
+                                      : sample_actions_kernel<false, RowMap::Identity>;
+    kern<<<grid, 256, 0, st>>>(scores, ld, n_actions, n_rows, seed, counter, actions, logp, swap, seat, rows, range);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "sample_actions kernel launch");
+    if (e != cudaSuccess) return cuda_fail(e, listed ? "sample_actions_rows kernel launch" : "sample_actions kernel launch");
     return OVC_OK;
 }
 
@@ -1057,23 +1017,36 @@ static int record_transition_dense_impl(const int32_t *sparse, const int32_t *sh
 }
 
 // Generalized advantage estimation over a window of T transitions (the postprocessing of RLlib's PPO sample batches),
-// one thread per environment holding its two agent rows, walking t backwards.  Every operation is rounded on its own
-// (no FMA contraction) in the order ovc_gae documents, so a float32 loop on the host reproduces it bit for bit.  A
-// thread's chain is serial in t, so GAE_UNROLL timesteps of loads are issued before they are consumed: with one thread
-// per environment there are too few threads per SM to cover the memory latency otherwise.
+// one thread per environment holding its rows (V = float2: both agents' rows, ovc_gae; V = float: one row, ovc_gae_view),
+// walking t backwards.  Every operation is rounded on its own (no FMA contraction) in the order ovc_gae documents, so a
+// float32 loop on the host reproduces it bit for bit.  A thread's chain is serial in t, so GAE_UNROLL timesteps of loads
+// are issued before they are consumed: with one thread per environment there are too few threads per SM to cover the
+// memory latency otherwise.  Without a minimum of 5 CTAs per SM ptxas gives both forms 255 registers (2 CTAs per SM);
+// with it, 96 (two rows) and 64 (one row), no spills.
 constexpr int GAE_THREADS = 128;
 constexpr int GAE_UNROLL = 16;
 
-__global__ void __launch_bounds__(GAE_THREADS) gae_kernel(const float2 *__restrict__ rewards, const float2 *__restrict__ values,
-                                                          const uint8_t *__restrict__ dones, const float2 *__restrict__ last_values,
-                                                          long long T, long long n_envs, float gamma, float lambda,
-                                                          float2 *__restrict__ adv, float2 *__restrict__ targets) {
+// a row's advantage at step t from the one at t + 1 (a), its reward r, value v, the next value nv and not-done nt
+__device__ __forceinline__ float gae_step(float a, float r, float v, float nv, float nt, float gamma, float gl) {
+    const float d = __fsub_rn(__fadd_rn(r, __fmul_rn(__fmul_rn(gamma, nv), nt)), v);
+    return __fadd_rn(d, __fmul_rn(__fmul_rn(gl, nt), a));
+}
+__device__ __forceinline__ float2 gae_step(float2 a, float2 r, float2 v, float2 nv, float nt, float gamma, float gl) {
+    return make_float2(gae_step(a.x, r.x, v.x, nv.x, nt, gamma, gl), gae_step(a.y, r.y, v.y, nv.y, nt, gamma, gl));
+}
+__device__ __forceinline__ float gae_target(float a, float v) { return __fadd_rn(a, v); }
+__device__ __forceinline__ float2 gae_target(float2 a, float2 v) { return make_float2(__fadd_rn(a.x, v.x), __fadd_rn(a.y, v.y)); }
+
+template <class V>
+__global__ void __launch_bounds__(GAE_THREADS, 5)
+    gae_kernel(const V *__restrict__ rewards, const V *__restrict__ values, const uint8_t *__restrict__ dones, const V *__restrict__ last_values,
+               long long T, long long n_envs, float gamma, float lambda, V *__restrict__ adv, V *__restrict__ targets) {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= n_envs) return;
     const float gl = __fmul_rn(gamma, lambda);
-    float2 a = make_float2(0.f, 0.f), nv = last_values[e];
+    V a = {}, nv = last_values[e];
     for (long long t0 = T - 1; t0 >= 0; t0 -= GAE_UNROLL) {
-        float2 r[GAE_UNROLL], v[GAE_UNROLL];
+        V r[GAE_UNROLL], v[GAE_UNROLL];
         float nt[GAE_UNROLL];
 #pragma unroll
         for (int k = 0; k < GAE_UNROLL; k++)
@@ -1085,76 +1058,32 @@ __global__ void __launch_bounds__(GAE_THREADS) gae_kernel(const float2 *__restri
         for (int k = 0; k < GAE_UNROLL; k++)
             if (t0 - k >= 0) {
                 const long long i = (t0 - k) * n_envs + e;
-                const float dx = __fsub_rn(__fadd_rn(r[k].x, __fmul_rn(__fmul_rn(gamma, nv.x), nt[k])), v[k].x);
-                const float dy = __fsub_rn(__fadd_rn(r[k].y, __fmul_rn(__fmul_rn(gamma, nv.y), nt[k])), v[k].y);
-                a.x = __fadd_rn(dx, __fmul_rn(__fmul_rn(gl, nt[k]), a.x));
-                a.y = __fadd_rn(dy, __fmul_rn(__fmul_rn(gl, nt[k]), a.y));
+                a = gae_step(a, r[k], v[k], nv, nt[k], gamma, gl);
                 __stcs(adv + i, a);
-                __stcs(targets + i, make_float2(__fadd_rn(a.x, v[k].x), __fadd_rn(a.y, v[k].y)));
+                __stcs(targets + i, gae_target(a, v[k]));
                 nv = v[k];
             }
     }
 }
 
-static int gae_impl(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, long long T,
-                    long long n_rows, float gamma, float lambda, float *adv, float *targets, cudaStream_t st) {
+// one_row: ovc_gae_view, n environments of one row each; otherwise ovc_gae, n rows, two per environment
+static int gae_impl(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, long long T, long long n,
+                    float gamma, float lambda, float *adv, float *targets, cudaStream_t st, bool one_row = false) {
     if (!rewards || !values || !dones || !last_values || !adv || !targets) return fail(OVC_E_BADARG, "null pointer argument");
-    if (T < 0 || n_rows < 0 || n_rows % 2) return fail(OVC_E_BADARG, "T must be >= 0 and n_rows even and >= 0");
-    if (((uintptr_t)rewards | (uintptr_t)values | (uintptr_t)last_values | (uintptr_t)adv | (uintptr_t)targets) & 7)
-        return fail(OVC_E_BADARG, "float buffers must be 8-byte aligned");
-    const long long n_envs = n_rows / 2;
+    if (T < 0 || n < 0 || (!one_row && n % 2))
+        return fail(OVC_E_BADARG, one_row ? "T and n_envs must be >= 0" : "T must be >= 0 and n_rows even and >= 0");
+    if (((uintptr_t)rewards | (uintptr_t)values | (uintptr_t)last_values | (uintptr_t)adv | (uintptr_t)targets) & (one_row ? 3 : 7))
+        return fail(OVC_E_BADARG, one_row ? "float buffers must be 4-byte aligned" : "float buffers must be 8-byte aligned");
+    const long long n_envs = one_row ? n : n / 2;
     if (T == 0 || n_envs == 0) return OVC_OK;
-    gae_kernel<<<(unsigned)((n_envs + GAE_THREADS - 1) / GAE_THREADS), GAE_THREADS, 0, st>>>(
-        (const float2 *)rewards, (const float2 *)values, dones, (const float2 *)last_values, T, n_envs, gamma, lambda, (float2 *)adv,
-        (float2 *)targets);
+    const unsigned grid = (unsigned)((n_envs + GAE_THREADS - 1) / GAE_THREADS);
+    if (one_row)
+        gae_kernel<float><<<grid, GAE_THREADS, 0, st>>>(rewards, values, dones, last_values, T, n_envs, gamma, lambda, adv, targets);
+    else
+        gae_kernel<float2><<<grid, GAE_THREADS, 0, st>>>((const float2 *)rewards, (const float2 *)values, dones, (const float2 *)last_values, T,
+                                                         n_envs, gamma, lambda, (float2 *)adv, (float2 *)targets);
     cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "gae kernel launch");
-    return OVC_OK;
-}
-
-// ovc_gae_view: gae_kernel on ONE row per environment (an agent pair's learner), the same recurrence, rounding order and
-// load unroll; a kernel of its own so that gae_kernel's code stays as it is.  Without a minimum of 4 CTAs per SM ptxas gives it
-// 255 registers (2 CTAs per SM); with it, 64 and no spill, the 16 timesteps' loads still issued before they are consumed.
-__global__ void __launch_bounds__(GAE_THREADS, 4) gae_view_kernel(const float *__restrict__ rewards, const float *__restrict__ values,
-                                                               const uint8_t *__restrict__ dones, const float *__restrict__ last_values,
-                                                               long long T, long long n_envs, float gamma, float lambda,
-                                                               float *__restrict__ adv, float *__restrict__ targets) {
-    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= n_envs) return;
-    const float gl = __fmul_rn(gamma, lambda);
-    float a = 0.f, nv = last_values[e];
-    for (long long t0 = T - 1; t0 >= 0; t0 -= GAE_UNROLL) {
-        float r[GAE_UNROLL], v[GAE_UNROLL], nt[GAE_UNROLL];
-#pragma unroll
-        for (int k = 0; k < GAE_UNROLL; k++)
-            if (t0 - k >= 0) {
-                const long long i = (t0 - k) * n_envs + e;
-                r[k] = __ldcs(rewards + i), v[k] = __ldcs(values + i), nt[k] = dones[i] ? 0.f : 1.f;
-            }
-#pragma unroll
-        for (int k = 0; k < GAE_UNROLL; k++)
-            if (t0 - k >= 0) {
-                const long long i = (t0 - k) * n_envs + e;
-                const float d = __fsub_rn(__fadd_rn(r[k], __fmul_rn(__fmul_rn(gamma, nv), nt[k])), v[k]);
-                a = __fadd_rn(d, __fmul_rn(__fmul_rn(gl, nt[k]), a));
-                __stcs(adv + i, a);
-                __stcs(targets + i, __fadd_rn(a, v[k]));
-                nv = v[k];
-            }
-    }
-}
-
-static int gae_view_impl(const float *rewards, const float *values, const uint8_t *dones, const float *last_values, long long T,
-                         long long n_envs, float gamma, float lambda, float *adv, float *targets, cudaStream_t st) {
-    if (!rewards || !values || !dones || !last_values || !adv || !targets) return fail(OVC_E_BADARG, "null pointer argument");
-    if (T < 0 || n_envs < 0) return fail(OVC_E_BADARG, "T and n_envs must be >= 0");
-    if (((uintptr_t)rewards | (uintptr_t)values | (uintptr_t)last_values | (uintptr_t)adv | (uintptr_t)targets) & 3)
-        return fail(OVC_E_BADARG, "float buffers must be 4-byte aligned");
-    if (T == 0 || n_envs == 0) return OVC_OK;
-    gae_view_kernel<<<(unsigned)((n_envs + GAE_THREADS - 1) / GAE_THREADS), GAE_THREADS, 0, st>>>(rewards, values, dones, last_values, T,
-                                                                                                   n_envs, gamma, lambda, adv, targets);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "gae_view kernel launch");
+    if (e != cudaSuccess) return cuda_fail(e, one_row ? "gae_view kernel launch" : "gae kernel launch");
     return OVC_OK;
 }
 

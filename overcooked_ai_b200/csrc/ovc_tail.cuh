@@ -40,11 +40,14 @@ struct PolicyTailArgs {
     unsigned long long *counter;   // [2]: step, arrival scratch (as ovc_sample_actions)
     int32_t *actions;              // [n_rows]
     float *values;                 // [n_rows] or null
-    union {                        // (a union: the parameter block, and so the code, of the drawing kernels stays as it was)
-        float *scores;             // [n_rows][8] or null
-        __nv_bfloat16 *hidden;     // [n_rows][64]: the last 64-wide activation (policy_tail_kernel<KS2, false, true>)
-    };
-    float *logp;                   // [n_rows] or null: log-probability of the drawn action (policy_tail_kernel<KS2, true, false>)
+    float *scores;                 // [n_rows][8] or null
+    float *logp;                   // [n_rows] or null: log-probability of the drawn action (LOGP)
+    __nv_bfloat16 *hidden;         // [n_rows][64]: the last 64-wide activation (HIDDEN)
+    const int32_t *swap;           // View, Rows: per-environment seat swap, nullable
+    int seat;                      // View, Rows: the agent's player
+    const int32_t *rows, *range;   // Rows, Joint: the row map and its compact range [range[0], range[1])
+    const int32_t *offsets;        // grouped: member k's rows [offsets[k], offsets[k + 1])
+    int n_members;                 // grouped
 };
 
 __device__ __forceinline__ void mma_bf16_16816(float c[4], const unsigned a[4], unsigned b0, unsigned b1) {
@@ -190,8 +193,7 @@ __device__ __forceinline__ int draw_row(float s0, float s1, unsigned long long s
                                         int lane, int t, float &lp) {
     const Philox4 P = philox4x32_10(seed, (uint32_t)row, (uint32_t)((unsigned long long)row >> 32), (uint32_t)step,
                                     ((uint32_t)(step >> 32) << 1) | (uint32_t)(t >> 1));
-    const uint32_t d0 = P.v[(2 * t) & 3], d1 = P.v[(2 * t + 1) & 3];
-    const float u0 = ((float)(d0 >> 9) + 0.5f) * 1.1920928955078125e-7f, u1 = ((float)(d1 >> 9) + 0.5f) * 1.1920928955078125e-7f;
+    const float u0 = draw_uniform(P.v[(2 * t) & 3]), u1 = draw_uniform(P.v[(2 * t + 1) & 3]);
     float v0 = 2 * t < n_actions ? s0 - logf(-logf(u0)) : -INFINITY;
     const float v1 = 2 * t + 1 < n_actions ? s1 - logf(-logf(u1)) : -INFINITY;
     int best = 2 * t;
@@ -223,33 +225,74 @@ __device__ __forceinline__ long long view_row(const int32_t *swap, int seat, lon
     return 2 * r + (seat ^ (swap && r < n_rows && __ldg(swap + r) != 0));
 }
 
-// The last CTA of a launch to get here advances the draw step (every CTA has read it by then): counter[1] counts arrivals.
-__device__ __forceinline__ void advance_step(unsigned long long *counter, unsigned long long step) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        const unsigned long long arrived = atomicAdd(counter + 1, 1ull);
-        if (arrived == (unsigned long long)gridDim.x - 1) {
-            counter[1] = 0;
-            counter[0] = step + 1;
-            __threadfence();
+// K8's tile: rows r0 and r0 + 8 of x (g = r0 mod 8 within the warp's 16 rows; rows from r_end on read as zeros) through the
+// first layer, the hidden layers and the heads into out; without HEADS, the last 64-wide layer's A fragments into a_out.
+template <int KS2, bool HEADS = true, class Row>
+__device__ __forceinline__ void tail_tile(float out[1][4], const PolicyTailArgs &p, const TailSmem &w, Row r0, Row r_end, int g, int t,
+                                          unsigned (*a_out)[4] = nullptr) {
+    constexpr int K0 = 32 * KS2;
+    const Row r1 = r0 + 8;
+    const float in_slope = p.in_slope;
+    // ---- first layer: A fragments straight from global memory, 16 bytes (8 inputs) per load ----
+    // The loads of PRE k-steps are issued before the first layer, the rest as it reaches them.  PRE is KS2 except at
+    // KS2 = 6: holding all 48 registers of x under the 128-register cap made every drawing form spill 20 - 44 bytes
+    // there, and with 4 up front none spills.
+    constexpr int PRE = KS2 == 6 ? 4 : KS2;
+    uint4 xa[KS2], xb[KS2];
+    auto load = [&](int s2) {
+        xa[s2] = r0 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r0 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
+        xb[s2] = r1 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r1 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
+    };
+#pragma unroll
+    for (int s2 = 0; s2 < PRE; s2++) load(s2);
+    float acc[8][4];
+    first_layer64<KS2>(acc, w, g, t, [&](int s2, unsigned a_lo[4], unsigned a_hi[4]) {
+        if (s2 >= PRE) load(s2);
+        a_lo[0] = lrelu_bf16x2(xa[s2].x, in_slope), a_lo[1] = lrelu_bf16x2(xb[s2].x, in_slope);
+        a_lo[2] = lrelu_bf16x2(xa[s2].y, in_slope), a_lo[3] = lrelu_bf16x2(xb[s2].y, in_slope);
+        a_hi[0] = lrelu_bf16x2(xa[s2].z, in_slope), a_hi[1] = lrelu_bf16x2(xb[s2].z, in_slope);
+        a_hi[2] = lrelu_bf16x2(xa[s2].w, in_slope), a_hi[3] = lrelu_bf16x2(xb[s2].w, in_slope);
+    });
+    // ---- hidden layers and heads: fragments in, fragments out ----
+    tail_layers<HEADS>(out, acc, w, p.n_hidden, p.slope, g, t, a_out);
+}
+
+// K8's epilogue on rows r0 and r0 + 8 of a tile (heads in out): per row the scores, the draw (ovc_sample_actions) and the
+// action, logp and value, placed by MAP (RowMap): row r is drawn on joint row d, which indexes actions, and the other
+// outputs are indexed by o.  Rows from r_end on are drawn with the others (the shuffles need all 32 lanes) and discarded.
+template <bool LOGP, RowMap MAP, class Row>
+__device__ __forceinline__ void tail_epilogue(const PolicyTailArgs &p, const float out[1][4], unsigned long long step, Row r0, Row r_end,
+                                              int lane, int t) {
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        const Row r = h ? r0 + 8 : r0;
+        const bool in = r < r_end;
+        const float s0 = out[0][2 * h], s1 = out[0][2 * h + 1];
+        long long d = r, o = r;
+        if constexpr (MAP == RowMap::View) d = view_row(p.swap, p.seat, r, p.n_rows);
+        if constexpr (MAP == RowMap::Rows) {
+            const long long e = in ? (long long)__ldg(p.rows + r) : 0;
+            d = 2 * e + (p.seat ^ (p.swap && in && __ldg(p.swap + e) != 0));
+        }
+        if constexpr (MAP == RowMap::Joint) d = o = in ? (long long)__ldg(p.rows + r) : 0;
+        if (p.scores && in) *reinterpret_cast<float2 *>(p.scores + o * PT_NOUT + 2 * t) = make_float2(s0, s1);
+        float lp = 0.f;
+        const int best = draw_row<LOGP>(s0, s1, p.seed, step, d, p.n_actions, lane, t, lp);
+        if (in) {
+            if (t == 0) p.actions[d] = best;
+            if constexpr (LOGP) if (t == 0) p.logp[o] = lp;
+            // the value head is head n_actions: lane n_actions / 2 holds it
+            if (p.values && t == (p.n_actions >> 1)) p.values[o] = (p.n_actions & 1) ? s1 : s0;
         }
     }
 }
 
-// K0 = 32 * KS2; LOGP: also write p.logp (a separate instantiation, so the plain draw is untouched); HIDDEN: stop after the
-// last 64-wide layer and write its activations to p.hidden instead of the heads and the draw (the LSTM policy's input;
-// the counter is neither read nor advanced).  VIEW: row r is one agent's row of environment r (view_row): the draw uses
-// the joint row g and writes p.actions[g]; values, logp and scores stay indexed by r.  The one-view kernel is a kernel of
-// its own (policy_tail_view_kernel, swap and seat as extra parameters): a larger PolicyTailArgs would change the code of
-// every instantiation.
-// ROWS (with VIEW, policy_tail_rows_kernel): compact rows r in [range[0], range[1]) only; row r is environment rows[r]'s
-// agent, drawn on its joint row 2 rows[r] + p(rows[r]).
-// JOINT (policy_tail_joint_kernel): compact rows r in [range[0], range[1]) only; x row r is joint row rows[r], drawn on it,
-// and actions, values, logp and scores are written at that joint row.
-template <int KS2, bool LOGP, bool HIDDEN, bool VIEW, bool ROWS = false, bool JOINT = false>
-__device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const int32_t *swap, int seat, const int32_t *rows = nullptr,
-                                                 const int32_t *range = nullptr) {
+// K8, K0 = 32 * KS2, over the rows MAP names (Rows, Joint: the compact range).  LOGP: also write p.logp; HIDDEN: stop after
+// the last 64-wide layer and write its activations to p.hidden instead of the heads and the draw (the LSTM policy's input;
+// the counter is neither read nor advanced).
+template <int KS2, RowMap MAP, bool LOGP, bool HIDDEN = false>
+__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const PolicyTailArgs p) {
+    static_assert(!HIDDEN || (MAP == RowMap::Identity && !LOGP), "the hidden form has no draw");
     constexpr int K0 = 32 * KS2;
     extern __shared__ __align__(16) char pt_smem[];
 
@@ -259,114 +302,34 @@ __device__ __forceinline__ void policy_tail_body(const PolicyTailArgs &p, const 
     __syncthreads();
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
-    const float in_slope2 = p.in_slope;
-    // the rows form counts rows in 32 bits (a range of int32 entries), which keeps it within K8's registers
-    using Row = typename std::conditional<ROWS || JOINT, int, long long>::type;
+    // the forms over a range count rows in 32 bits (a range of int32 entries), which keeps them within K8's registers
+    constexpr bool RANGED = MAP == RowMap::Rows || MAP == RowMap::Joint;
+    using Row = typename std::conditional<RANGED, int, long long>::type;
     Row r_beg = 0, r_end = p.n_rows;
-    if constexpr (ROWS || JOINT) {
-        r_beg = max(__ldg(range), 0);
-        r_end = max((int)min((long long)__ldg(range + 1), p.n_rows), r_beg);
+    if constexpr (RANGED) {
+        r_beg = max(__ldg(p.range), 0);
+        r_end = max((int)min((long long)__ldg(p.range + 1), p.n_rows), r_beg);
     }
     const Row n_tiles = (r_end - r_beg + 15) / 16;
     for (Row tile = (Row)blockIdx.x * (PT_THREADS / 32) + warp; tile < n_tiles; tile += (Row)gridDim.x * (PT_THREADS / 32)) {
         const Row r0 = r_beg + tile * 16 + g, r1 = r0 + 8;
-        // ---- first layer: A fragments straight from global memory, 16 bytes (8 inputs) per load ----
-        uint4 xa[KS2], xb[KS2];
-#pragma unroll
-        for (int s2 = 0; s2 < KS2; s2++) {
-            xa[s2] = r0 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r0 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
-            xb[s2] = r1 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r1 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
-        }
-        float acc[8][4];
-        first_layer64<KS2>(acc, w, g, t, [&](int s2, unsigned a_lo[4], unsigned a_hi[4]) {
-            a_lo[0] = lrelu_bf16x2(xa[s2].x, in_slope2), a_lo[1] = lrelu_bf16x2(xb[s2].x, in_slope2);
-            a_lo[2] = lrelu_bf16x2(xa[s2].y, in_slope2), a_lo[3] = lrelu_bf16x2(xb[s2].y, in_slope2);
-            a_hi[0] = lrelu_bf16x2(xa[s2].z, in_slope2), a_hi[1] = lrelu_bf16x2(xb[s2].z, in_slope2);
-            a_hi[2] = lrelu_bf16x2(xa[s2].w, in_slope2), a_hi[3] = lrelu_bf16x2(xb[s2].w, in_slope2);
-        });
         if constexpr (HIDDEN) {  // the A fragments of the last layer's activations, written as [row][64]
             unsigned a[4][4];
-            tail_layers<false>(nullptr, acc, w, p.n_hidden, p.slope, g, t, a);
+            tail_tile<KS2, false>(nullptr, p, w, r0, r_end, g, t, a);
 #pragma unroll
             for (int s = 0; s < 4; s++) {
                 unsigned *h0 = reinterpret_cast<unsigned *>(p.hidden + r0 * PT_H + 16 * s + 2 * t);
                 unsigned *h1 = reinterpret_cast<unsigned *>(p.hidden + r1 * PT_H + 16 * s + 2 * t);
-                if (r0 < p.n_rows) h0[0] = a[s][0], h0[4] = a[s][2];
-                if (r1 < p.n_rows) h1[0] = a[s][1], h1[4] = a[s][3];
+                if (r0 < r_end) h0[0] = a[s][0], h0[4] = a[s][2];
+                if (r1 < r_end) h1[0] = a[s][1], h1[4] = a[s][3];
             }
-            continue;
-        }
-        // ---- hidden layers and heads: fragments in, fragments out ----
-        float out[1][4];
-        tail_layers(out, acc, w, p.n_hidden, p.slope, g, t);
-        if constexpr (JOINT) {  // rows past the end: their draw is discarded
-            const long long j0 = r0 < r_end ? (long long)__ldg(rows + r0) : 0, j1 = r1 < r_end ? (long long)__ldg(rows + r1) : 0;
-            if (p.scores) {
-                if (r0 < r_end) *reinterpret_cast<float2 *>(p.scores + j0 * PT_NOUT + 2 * t) = make_float2(out[0][0], out[0][1]);
-                if (r1 < r_end) *reinterpret_cast<float2 *>(p.scores + j1 * PT_NOUT + 2 * t) = make_float2(out[0][2], out[0][3]);
-            }
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-                const long long jr = h ? j1 : j0;
-                const float s0 = out[0][2 * h], s1 = out[0][2 * h + 1];
-                float lp = 0.f;
-                const int best = draw_row<LOGP>(s0, s1, p.seed, step, jr, p.n_actions, lane, t, lp);
-                if ((h ? r1 : r0) < r_end) {
-                    if (t == 0) p.actions[jr] = best;
-                    if constexpr (LOGP) if (t == 0) p.logp[jr] = lp;
-                    if (p.values && t == (p.n_actions >> 1)) p.values[jr] = (p.n_actions & 1) ? s1 : s0;
-                }
-            }
-            continue;
-        }
-        if (p.scores) {
-            if (r0 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r0 * PT_NOUT + 2 * t) = make_float2(out[0][0], out[0][1]);
-            if (r1 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r1 * PT_NOUT + 2 * t) = make_float2(out[0][2], out[0][3]);
-        }
-        // ---- the draw (ovc_sample_actions) ----
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const Row row = h ? r1 : r0;
-            const float s0 = out[0][2 * h], s1 = out[0][2 * h + 1];
-            float lp = 0.f;
-            long long g;
-            if constexpr (ROWS) {
-                const long long e = row < r_end ? (long long)__ldg(rows + row) : 0;  // rows past the end: the draw is discarded
-                g = 2 * e + (seat ^ (swap && row < r_end && __ldg(swap + e) != 0));
-            } else {
-                g = VIEW ? view_row(swap, seat, row, p.n_rows) : row;
-            }
-            const int best = draw_row<LOGP>(s0, s1, p.seed, step, g, p.n_actions, lane, t, lp);
-            if (row < r_end) {
-                if (t == 0) p.actions[g] = best;
-                if constexpr (LOGP) if (t == 0) p.logp[row] = lp;
-                // the value head is head n_actions: lane n_actions / 2 holds it
-                if (p.values && t == (p.n_actions >> 1)) p.values[row] = (p.n_actions & 1) ? s1 : s0;
-            }
+        } else {
+            float out[1][4];
+            tail_tile<KS2>(out, p, w, r0, r_end, g, t);
+            tail_epilogue<LOGP, MAP>(p, out, step, r0, r_end, lane, t);
         }
     }
     if constexpr (!HIDDEN) advance_step(p.counter, step);
-}
-
-template <int KS2, bool LOGP, bool HIDDEN>
-__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const PolicyTailArgs p) {
-    policy_tail_body<KS2, LOGP, HIDDEN, false>(p, nullptr, 0);
-}
-
-template <int KS2, bool LOGP>
-__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_view_kernel(const PolicyTailArgs p, const int32_t *swap, int seat) {
-    policy_tail_body<KS2, LOGP, false, true>(p, swap, seat);
-}
-
-template <int KS2, bool LOGP>
-__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_rows_kernel(const PolicyTailArgs p, const int32_t *swap, int seat,
-                                                                         const int32_t *rows, const int32_t *range) {
-    policy_tail_body<KS2, LOGP, false, true, true>(p, swap, seat, rows, range);
-}
-
-template <int KS2>
-__global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_joint_kernel(const PolicyTailArgs p, const int32_t *jrow, const int32_t *range) {
-    policy_tail_body<KS2, true, false, false, false, true>(p, nullptr, 0, jrow, range);
 }
 
 // Grouped K8 (ovc_policy_tail_grouped): a population of K tails, member k's tables entry k of stacked tables, its rows
@@ -375,13 +338,13 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_joint_kernel(const 
 // [b T / G, (b + 1) T / G) of the T tiles, so a CTA holds at most a few members' tables, each staged once, and the work is
 // balanced whatever the block sizes.  Each row is drawn on its own row index r with the call's step, exactly as
 // ovc_policy_tail_logp draws row r, and every CTA advances the counter once.
-// 12 warps per CTA (a cap of 170 registers; ptxas uses 116 - 156 over the instantiations, no spills): under K8's 16 warps
-// (a cap of 128) the member bookkeeping on top of K8's tile spilled 8 - 44 bytes at k0 = 96..160 (K8 itself spills at that cap).
+// 12 warps per CTA (a cap of 170 registers; ptxas uses 112 - 159 over the instantiations, no spills): under K8's 16 warps
+// (a cap of 128) the member bookkeeping on top of K8's tile spilled.
 constexpr int PT_MAX_MEMBERS = 64;
 constexpr int PTG_THREADS = 384;
 
 template <int KS2, bool LOGP>
-__global__ void __launch_bounds__(PTG_THREADS, 1) policy_tail_grouped_kernel(const PolicyTailArgs p, const int32_t *offsets, int n_members) {
+__global__ void __launch_bounds__(PTG_THREADS, 1) policy_tail_grouped_kernel(const PolicyTailArgs p) {
     constexpr int K0 = 32 * KS2;
     extern __shared__ __align__(16) char pt_smem[];
     __shared__ int tile0[PT_MAX_MEMBERS + 1], rbeg[PT_MAX_MEMBERS], rend[PT_MAX_MEMBERS];
@@ -389,19 +352,19 @@ __global__ void __launch_bounds__(PTG_THREADS, 1) policy_tail_grouped_kernel(con
     const unsigned long long step = *reinterpret_cast<volatile unsigned long long *>(p.counter);
     if (threadIdx.x == 0) {
         int n = 0;
-        for (int k = 0; k < n_members; k++) {
-            const int lo = max(__ldg(offsets + k), 0), hi = max((int)min((long long)__ldg(offsets + k + 1), p.n_rows), lo);
+        for (int k = 0; k < p.n_members; k++) {
+            const int lo = max(__ldg(p.offsets + k), 0), hi = max((int)min((long long)__ldg(p.offsets + k + 1), p.n_rows), lo);
             tile0[k] = n, rbeg[k] = lo, rend[k] = hi;
             n += (hi - lo + 15) / 16;
         }
-        tile0[n_members] = n;
+        tile0[p.n_members] = n;
     }
     __syncthreads();
-    const int total = tile0[n_members];
+    const int total = tile0[p.n_members];
     const int t_lo = (int)((long long)blockIdx.x * total / gridDim.x), t_hi = (int)((long long)(blockIdx.x + 1) * total / gridDim.x);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
     int tb = t_lo;
-    for (int k = 0; k < n_members && tb < t_hi; k++) {
+    for (int k = 0; k < p.n_members && tb < t_hi; k++) {
         const int te = min(t_hi, tile0[k + 1]);
         if (te <= tb) continue;
         PolicyTailArgs q = p;  // member k's tables
@@ -413,103 +376,88 @@ __global__ void __launch_bounds__(PTG_THREADS, 1) policy_tail_grouped_kernel(con
         __syncthreads();
         const int r_end = rend[k];
         for (int tile = tb + warp; tile < te; tile += PTG_THREADS / 32) {
-            const int r0 = rbeg[k] + (tile - tile0[k]) * 16 + g, r1 = r0 + 8;
-            uint4 xa[KS2], xb[KS2];
-#pragma unroll
-            for (int s2 = 0; s2 < KS2; s2++) {
-                xa[s2] = r0 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r0 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
-                xb[s2] = r1 < r_end ? __ldg(reinterpret_cast<const uint4 *>(p.x + (long long)r1 * K0 + 32 * s2 + 8 * t)) : make_uint4(0, 0, 0, 0);
-            }
-            float acc[8][4];
-            first_layer64<KS2>(acc, w, g, t, [&](int s2, unsigned a_lo[4], unsigned a_hi[4]) {
-                a_lo[0] = lrelu_bf16x2(xa[s2].x, p.in_slope), a_lo[1] = lrelu_bf16x2(xb[s2].x, p.in_slope);
-                a_lo[2] = lrelu_bf16x2(xa[s2].y, p.in_slope), a_lo[3] = lrelu_bf16x2(xb[s2].y, p.in_slope);
-                a_hi[0] = lrelu_bf16x2(xa[s2].z, p.in_slope), a_hi[1] = lrelu_bf16x2(xb[s2].z, p.in_slope);
-                a_hi[2] = lrelu_bf16x2(xa[s2].w, p.in_slope), a_hi[3] = lrelu_bf16x2(xb[s2].w, p.in_slope);
-            });
+            const int r0 = rbeg[k] + (tile - tile0[k]) * 16 + g;
             float out[1][4];
-            tail_layers(out, acc, w, p.n_hidden, p.slope, g, t);
-            if (p.scores) {
-                if (r0 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r0 * PT_NOUT + 2 * t) = make_float2(out[0][0], out[0][1]);
-                if (r1 < r_end) *reinterpret_cast<float2 *>(p.scores + (long long)r1 * PT_NOUT + 2 * t) = make_float2(out[0][2], out[0][3]);
-            }
-#pragma unroll
-            for (int h = 0; h < 2; h++) {  // rows past the member's end: their draw is discarded
-                const int row = h ? r1 : r0;
-                const float s0 = out[0][2 * h], s1 = out[0][2 * h + 1];
-                float lp = 0.f;
-                const int best = draw_row<LOGP>(s0, s1, p.seed, step, row, p.n_actions, lane, t, lp);
-                if (row < r_end) {
-                    if (t == 0) p.actions[row] = best;
-                    if constexpr (LOGP) if (t == 0) p.logp[row] = lp;
-                    if (p.values && t == (p.n_actions >> 1)) p.values[row] = (p.n_actions & 1) ? s1 : s0;
-                }
-            }
+            tail_tile<KS2>(out, p, w, r0, r_end, g, t);
+            tail_epilogue<LOGP, RowMap::Identity>(p, out, step, r0, r_end, lane, t);
         }
         tb = te;
     }
     advance_step(p.counter, step);
 }
 
-static int policy_tail_grouped_impl(const PolicyTailArgs &a, int k0, const int32_t *offsets, int n_members, cudaStream_t st) {
-    if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || !a.counter || !a.actions || !offsets ||
+using PolicyTailKernel = void (*)(PolicyTailArgs);
+
+template <int KS2>
+static PolicyTailKernel policy_tail_pick(RowMap map, bool logp, bool hid, bool grouped) {
+    if (grouped) return logp ? policy_tail_grouped_kernel<KS2, true> : policy_tail_grouped_kernel<KS2, false>;
+    if (hid) return policy_tail_kernel<KS2, RowMap::Identity, false, true>;
+    switch (map) {
+    case RowMap::View: return logp ? policy_tail_kernel<KS2, RowMap::View, true> : policy_tail_kernel<KS2, RowMap::View, false>;
+    case RowMap::Rows: return logp ? policy_tail_kernel<KS2, RowMap::Rows, true> : policy_tail_kernel<KS2, RowMap::Rows, false>;
+    case RowMap::Joint: return policy_tail_kernel<KS2, RowMap::Joint, true>;
+    default: return logp ? policy_tail_kernel<KS2, RowMap::Identity, true> : policy_tail_kernel<KS2, RowMap::Identity, false>;
+    }
+}
+
+// The launch of every K8 form, its arguments checked: one wave of CTAs at most, never more than the SMs.  The grouped form
+// runs 12 warps per CTA over at most n_rows / 16 + n_members tiles (a member's last tile partial).
+static int policy_tail_launch(const PolicyTailArgs &a, int k0, cudaStream_t st, RowMap map, bool hid, bool grouped) {
+    int dev = 0, n_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+    const int threads = grouped ? PTG_THREADS : PT_THREADS;
+    const size_t smem = tail_smem_bytes(k0, a.n_hidden) + 16;
+    const long long n_tiles = (a.n_rows + 15) / 16 + (grouped ? a.n_members : 0), want = (n_tiles + threads / 32 - 1) / (threads / 32);
+    const unsigned grid = (unsigned)(want < n_sm ? want : n_sm);
+    PolicyTailKernel kern = nullptr;
+#define OVC_PT_CASE(KS2) \
+    case KS2: kern = policy_tail_pick<KS2>(map, a.logp, hid, grouped); break;
+    switch (k0 / 32) {
+        OVC_PT_CASE(1) OVC_PT_CASE(2) OVC_PT_CASE(3) OVC_PT_CASE(4) OVC_PT_CASE(5) OVC_PT_CASE(6) OVC_PT_CASE(7) OVC_PT_CASE(8)
+    }
+#undef OVC_PT_CASE
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return cuda_fail(e, grouped ? "policy_tail_grouped kernel attribute" : "policy_tail kernel attribute");
+    kern<<<grid, threads, smem, st>>>(a);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, grouped ? "policy_tail_grouped kernel launch" : "policy_tail kernel launch");
+    return OVC_OK;
+}
+
+static int policy_tail_grouped_impl(const PolicyTailArgs &a, int k0, cudaStream_t st) {
+    if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || !a.counter || !a.actions || !a.offsets ||
         (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)))
         return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)a.x | (uintptr_t)a.w_first | (uintptr_t)a.w_hidden | (uintptr_t)a.w_heads) & 15) != 0)
         return fail(OVC_E_BADARG, "x and the weight tables must be 16-byte aligned");
     if ((((uintptr_t)a.b_first | (uintptr_t)a.b_hidden | (uintptr_t)a.b_heads | (uintptr_t)a.scores | (uintptr_t)a.counter) & 7) != 0)
         return fail(OVC_E_BADARG, "biases, scores and counter must be 8-byte aligned");
-    if ((((uintptr_t)a.actions | (uintptr_t)a.values | (uintptr_t)a.logp | (uintptr_t)offsets) & 3) != 0)
+    if ((((uintptr_t)a.actions | (uintptr_t)a.values | (uintptr_t)a.logp | (uintptr_t)a.offsets) & 3) != 0)
         return fail(OVC_E_BADARG, "actions, values, logp and offsets must be 4-byte aligned");
-    if (n_members < 1 || n_members > PT_MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+    if (a.n_members < 1 || a.n_members > PT_MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", a.n_members);
     if (k0 < 32 || k0 > 256 || k0 % 32) return fail(OVC_E_BADARG, "k0 must be a multiple of 32 in 32..256", k0);
     if (a.n_hidden < 0 || a.n_hidden > 8) return fail(OVC_E_BADARG, "n_hidden must be 0..8", a.n_hidden);
     if (a.n_actions < 1 || a.n_actions > 7) return fail(OVC_E_BADARG, "n_actions must be 1..7 (head n_actions is the value)", a.n_actions);
     if (!(a.in_slope >= 0.f && a.in_slope <= 1.f && a.slope >= 0.f && a.slope <= 1.f)) return fail(OVC_E_BADARG, "slopes must lie in [0, 1]");
     if (a.n_rows < 0 || a.n_rows > 0x7FFFFFFFll) return fail(OVC_E_BADARG, "n_rows must lie in [0, 2^31)", a.n_rows);
     if (a.n_rows == 0) return OVC_OK;
-    int dev = 0, n_sm = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    const size_t smem = tail_smem_bytes(k0, a.n_hidden) + 16;
-    // at most n_rows / 16 + n_members tiles: one wave of CTAs, never more than the SMs
-    const long long n_tiles = (a.n_rows + 15) / 16 + n_members, want = (n_tiles + PTG_THREADS / 32 - 1) / (PTG_THREADS / 32);
-    const unsigned grid = (unsigned)(want < n_sm ? want : n_sm);
-    cudaError_t e = cudaSuccess;
-#define OVC_LAUNCH_PTG(KS2)                                                                                            \
-    case KS2:                                                                                                          \
-        if (a.logp) {                                                                                                  \
-            e = cudaFuncSetAttribute(policy_tail_grouped_kernel<KS2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (e == cudaSuccess) policy_tail_grouped_kernel<KS2, true><<<grid, PTG_THREADS, smem, st>>>(a, offsets, n_members); \
-        } else {                                                                                                       \
-            e = cudaFuncSetAttribute(policy_tail_grouped_kernel<KS2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (e == cudaSuccess) policy_tail_grouped_kernel<KS2, false><<<grid, PTG_THREADS, smem, st>>>(a, offsets, n_members); \
-        }                                                                                                              \
-        break;
-    switch (k0 / 32) {
-        OVC_LAUNCH_PTG(1) OVC_LAUNCH_PTG(2) OVC_LAUNCH_PTG(3) OVC_LAUNCH_PTG(4) OVC_LAUNCH_PTG(5) OVC_LAUNCH_PTG(6) OVC_LAUNCH_PTG(7) OVC_LAUNCH_PTG(8)
-    }
-#undef OVC_LAUNCH_PTG
-    if (e != cudaSuccess) return cuda_fail(e, "policy_tail_grouped kernel attribute");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "policy_tail_grouped kernel launch");
-    return OVC_OK;
+    return policy_tail_launch(a, k0, st, RowMap::Identity, false, true);
 }
 
-// hid: the HIDDEN instantiation into a.hidden (no heads, no draw; a.w_heads / a.b_heads are staged but never read, so the
-// entry point passes the first layer's tables, which are at least as large, in their place).  seat >= 0: the one-view
-// kernel with swap (ovc_policy_tail_view); -1: the two-view ones.  joint: rows is the joint-row map (ovc_policy_tail_joint).
-static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bool hid = false, const int32_t *swap = nullptr,
-                            int seat = -1, const int32_t *rows = nullptr, const int32_t *range = nullptr, bool joint = false) {
-    const bool view = seat >= 0 || joint, rows_map = rows || range;
+// map: ovc_policy_tail[_logp] Identity, ovc_policy_tail_view View, ovc_policy_tail_rows Rows, ovc_policy_tail_joint Joint.
+// hid: the HIDDEN form into a.hidden (no heads, no draw; a.w_heads / a.b_heads are staged but never read, so the entry
+// point passes the first layer's tables, which are at least as large, in their place).
+static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, RowMap map = RowMap::Identity, bool hid = false) {
+    const bool view = map != RowMap::Identity, ranged = map == RowMap::Rows || map == RowMap::Joint;
     if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || (hid ? !a.hidden : (!a.counter || !a.actions)) ||
-        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)) || (rows_map && (!rows || !range)) || (joint && (!rows || !range || !a.logp)))
+        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)) || (ranged && (!a.rows || !a.range)) || (map == RowMap::Joint && !a.logp))
         return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)a.x | (uintptr_t)a.w_first) & 15) != 0) return fail(OVC_E_BADARG, "x and w_first must be 16-byte aligned");
     if (hid && ((uintptr_t)a.hidden & 3) != 0) return fail(OVC_E_BADARG, "hidden must be 4-byte aligned");
-    if (view && (((uintptr_t)a.actions | (uintptr_t)a.values | (uintptr_t)a.logp | (uintptr_t)swap) & 3) != 0)
+    if (view && (((uintptr_t)a.actions | (uintptr_t)a.values | (uintptr_t)a.logp | (uintptr_t)a.swap) & 3) != 0)
         return fail(OVC_E_BADARG, "actions, values, logp and swap must be 4-byte aligned");
-    if ((((uintptr_t)rows | (uintptr_t)range) & 3) != 0) return fail(OVC_E_BADARG, "rows and range must be 4-byte aligned");
+    if ((((uintptr_t)a.rows | (uintptr_t)a.range) & 3) != 0) return fail(OVC_E_BADARG, "rows and range must be 4-byte aligned");
     if (view && ((uintptr_t)a.scores & 7) != 0) return fail(OVC_E_BADARG, "scores must be 8-byte aligned");
     if (k0 < 32 || k0 > 256 || k0 % 32) return fail(OVC_E_BADARG, "k0 must be a multiple of 32 in 32..256", k0);
     if (a.n_hidden < 0 || a.n_hidden > 8) return fail(OVC_E_BADARG, "n_hidden must be 0..8", a.n_hidden);
@@ -517,38 +465,7 @@ static int policy_tail_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, bo
     if (!(a.in_slope >= 0.f && a.in_slope <= 1.f && a.slope >= 0.f && a.slope <= 1.f)) return fail(OVC_E_BADARG, "slopes must lie in [0, 1]");
     if (a.n_rows < 0) return fail(OVC_E_BADARG, "negative row count");
     if (a.n_rows == 0) return OVC_OK;
-    int dev = 0, n_sm = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-    const size_t smem = tail_smem_bytes(k0, a.n_hidden) + 16;
-    const long long n_tiles = (a.n_rows + 15) / 16, want = (n_tiles + PT_THREADS / 32 - 1) / (PT_THREADS / 32);
-    const unsigned grid = (unsigned)(want < n_sm ? want : n_sm);
-    cudaError_t e = cudaSuccess;
-#define OVC_PT_KERNEL(ARGS, ...)                                                                                 \
-    do {                                                                                                         \
-        e = cudaFuncSetAttribute(__VA_ARGS__, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);           \
-        if (e == cudaSuccess) __VA_ARGS__<<<grid, PT_THREADS, smem, st>>> ARGS;                                  \
-    } while (0)
-#define OVC_LAUNCH_PT(KS2)                                                                                       \
-    case KS2:                                                                                                    \
-        if (hid) OVC_PT_KERNEL((a), policy_tail_kernel<KS2, false, true>);                                       \
-        else if (joint) OVC_PT_KERNEL((a, rows, range), policy_tail_joint_kernel<KS2>);                          \
-        else if (rows_map && a.logp) OVC_PT_KERNEL((a, swap, seat, rows, range), policy_tail_rows_kernel<KS2, true>); \
-        else if (rows_map) OVC_PT_KERNEL((a, swap, seat, rows, range), policy_tail_rows_kernel<KS2, false>);     \
-        else if (view && a.logp) OVC_PT_KERNEL((a, swap, seat), policy_tail_view_kernel<KS2, true>);             \
-        else if (view) OVC_PT_KERNEL((a, swap, seat), policy_tail_view_kernel<KS2, false>);                      \
-        else if (a.logp) OVC_PT_KERNEL((a), policy_tail_kernel<KS2, true, false>);                               \
-        else OVC_PT_KERNEL((a), policy_tail_kernel<KS2, false, false>);                                          \
-        break;
-    switch (k0 / 32) {
-        OVC_LAUNCH_PT(1) OVC_LAUNCH_PT(2) OVC_LAUNCH_PT(3) OVC_LAUNCH_PT(4) OVC_LAUNCH_PT(5) OVC_LAUNCH_PT(6) OVC_LAUNCH_PT(7) OVC_LAUNCH_PT(8)
-    }
-#undef OVC_LAUNCH_PT
-#undef OVC_PT_KERNEL
-    if (e != cudaSuccess) return cuda_fail(e, "policy_tail kernel attribute");
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "policy_tail kernel launch");
-    return OVC_OK;
+    return policy_tail_launch(a, k0, st, map, hid, false);
 }
 
 }  // namespace ovc
