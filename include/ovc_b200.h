@@ -774,6 +774,52 @@ int ovc_policy_tail_grouped(const void *x, int64_t n_rows, int k0, float in_slop
                             int32_t *actions, float *values, float *scores, float *logp, void *stream);
 
 /*
+ * Population play: member pair[e][0] of a population of n_members learners (1..64, OVC_E_BADARG otherwise) plays player 0
+ * of environment e and member pair[e][1] player 1 (pair int32 [n_envs][2], 8-byte aligned, every value in [0, n_members);
+ * other values are undefined behaviour).  Every row of the joint [2 n_envs] rows is a learner's row.
+ *
+ * ovc_assign_pairs: ovc_assign_members for ordered pairs.  For every environment e with done[e] != 0 (done = NULL: every
+ *   environment), in this order:
+ *     record  if done != NULL, rec_pair != NULL and count[e] < capacity: rec_pair[count[e]][e][0..1] = pair[e][0..1]
+ *             (rec_pair int32 [capacity][n_envs][2], the slot the ending episode's record goes to, as rec_member)
+ *     draw    if thresholds != NULL: Philox4x32-10, key = seed, counter = (e low, e high, step low, step high) -> word w0;
+ *             p = #{q < n_members^2 - 1 : w0 >= thresholds[q]};  pair[e] = (p / n_members, p % n_members)
+ *   thresholds int64 [n_members^2 - 1] in DEVICE memory: ovc_assign_members' table of the row-major flattened n_members x
+ *   n_members weights (non-decreasing; a pair of weight 0 is never drawn).  counter uint64[2], one step per launch, used and
+ *   advanced only with thresholds.  done and count 4-byte aligned; pair, rec_pair, thresholds and counter 8-byte aligned.
+ * ovc_group_pairs: the compact layout of the pairs, in ONE CTA without host synchronisation.  Environment e contributes the
+ *   list entry e << 2 | 3 (both views) to member i where pair[e] = (i, i), else e << 2 | 1 (view 0) to member pair[e][0]
+ *   and e << 2 | 2 (view 1) to member pair[e][1].  list int32 [2 n_envs] holds the entries grouped by member, ascending in
+ *   e within a member: member k's are list[entry_offsets[k] .. entry_offsets[k + 1]) (entry_offsets int32 [n_members + 1]).
+ *   Each entry's views take consecutive compact rows in ascending view order, the members' rows in member order: first int32
+ *   [2 n_envs] is the compact row of entry r's first view, jrow int32 [2 n_envs] maps compact row -> joint row 2 e + v, and
+ *   member k's rows are [row_offsets[k], row_offsets[k + 1]) (row_offsets int32 [n_members + 1], row_offsets[n_members] =
+ *   2 n_envs).  n_envs < 2^29; n_envs = 0 writes nothing.  The int32 outputs 4-byte aligned.
+ * ovc_encode_linear_grouped_masked: ovc_encode_linear_masked with member k's table (wt / bias stacked as in
+ *   ovc_encode_linear_grouped) on list entries [entry_offsets[k], entry_offsets[k + 1]) (device memory, clipped to
+ *   [0, n_list)): each output row first[r] + i is bit for bit row 2 e + v of ovc_encode_linear with member k's table.  The
+ *   object part is computed once per entry; the CTAs are split over (member, column slice, worker).  Same limits as
+ *   ovc_encode_linear_masked.
+ * ovc_policy_tail_grouped_joint: ovc_policy_tail_grouped on compact rows with ovc_policy_tail_joint's placement: member k's
+ *   rows [row_offsets[k], row_offsets[k + 1]) of x ([n_rows][k0], n_rows < 2^31, clipped) use its stacked tables, row r is
+ *   drawn on joint row jrow[r] with the call's step, and actions, values, logp (required) and scores ([.][8], nullable) are
+ *   written at jrow[r]: bit for bit what ovc_policy_tail_logp writes at that joint row with member k's tables.  Every other
+ *   entry is untouched.  Every CTA advances the counter once per launch.  Alignment as ovc_policy_tail_grouped; jrow 4-byte
+ *   aligned.
+ */
+int ovc_assign_pairs(const int32_t *done, const int64_t *thresholds, int n_members, int64_t n_envs, uint64_t seed, uint64_t *counter,
+                     int32_t *pair, int32_t *rec_pair, const int32_t *count, int capacity, void *stream);
+int ovc_group_pairs(const int32_t *pair, int n_members, int64_t n_envs, int32_t *list, int32_t *first, int32_t *jrow, int32_t *entry_offsets,
+                    int32_t *row_offsets, void *stream);
+int ovc_encode_linear_grouped_masked(const void *layouts, int n_layouts, const int32_t *state, const int32_t *list, const int32_t *first,
+                                     const void *wt, const float *bias, const int32_t *entry_offsets, int n_members, void *out, int64_t n_list,
+                                     int state_words, int width, int height, int horizon, int n_out, float neg_slope, void *stream);
+int ovc_policy_tail_grouped_joint(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                                  const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                                  float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *jrow, const int32_t *row_offsets,
+                                  int n_members, int32_t *actions, float *values, float *scores, float *logp, void *stream);
+
+/*
  * ovc_encode_linear_wgrad (K12): the weight gradient of ovc_encode_linear's layer, from the packed records,
  *     dwt[f][c] += sum over rows r of enc(r)[f] * dz[r][c]
  *   enc(r) = lossless_state_encoding of row r's record and view (never materialised), f in the observation's element order

@@ -113,6 +113,10 @@ def lib():
     L.ovc_policy_tail_grouped.argtypes = L.ovc_policy_tail.argtypes[:15] + [vp, i32, vp, vp, vp, vp, vp]
     L.ovc_encode_linear_grouped.argtypes = [vp, i32, vp, vp, vp, vp, i32, vp, i64, i32, i32, i32, i32, i32, ctypes.c_float, vp]
     L.ovc_wide_layers_grouped.argtypes = L.ovc_wide_layers.argtypes[:10] + [vp, i32, vp, vp]
+    L.ovc_assign_pairs.argtypes = L.ovc_assign_members.argtypes
+    L.ovc_group_pairs.argtypes = [vp, i32, i64, vp, vp, vp, vp, vp, vp]
+    L.ovc_encode_linear_grouped_masked.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, vp, i64, i32, i32, i32, i32, i32, ctypes.c_float, vp]
+    L.ovc_policy_tail_grouped_joint.argtypes = L.ovc_policy_tail.argtypes[:15] + [vp, vp, i32, vp, vp, vp, vp, vp]
     L.ovc_potential.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, i64, i32, vp]
     L.ovc_potential_table_size.restype = ctypes.c_size_t
     L.ovc_potential_shaping.argtypes = [vp, i32, vp, vp, vp, vp, i32, vp, vp, vp, vp, i64, i32, vp, vp]
@@ -129,7 +133,7 @@ def lib():
               L.ovc_policy_tail_logp, L.ovc_policy_hidden, L.ovc_lstm_head,
               L.ovc_encode_linear_view, L.ovc_sample_actions_view, L.ovc_policy_tail_view, L.ovc_lstm_head_view, L.ovc_sample_actions_logp, L.ovc_record_transition, L.ovc_record_transition_stats, L.ovc_gae, L.ovc_record_transition_view, L.ovc_gae_view, L.ovc_partner_policy, L.ovc_assign_partners,
               L.ovc_group_members, L.ovc_assign_members, L.ovc_encode_linear_rows, L.ovc_wide_layers_range, L.ovc_policy_tail_rows, L.ovc_sample_actions_rows,
-              L.ovc_learner_rows, L.ovc_encode_linear_masked, L.ovc_policy_tail_joint, L.ovc_potential_shaping, L.ovc_record_transition_dense, L.ovc_encode_linear_wgrad, L.ovc_policy_tail_grouped, L.ovc_encode_linear_grouped, L.ovc_wide_layers_grouped, L.ovc_expand_codes_host, L.ovc_expand_stream_host, L.ovc_pipeline_create, L.ovc_pipeline_run, L.ovc_pipeline_wait, L.ovc_pipeline_join):
+              L.ovc_learner_rows, L.ovc_encode_linear_masked, L.ovc_policy_tail_joint, L.ovc_potential_shaping, L.ovc_record_transition_dense, L.ovc_encode_linear_wgrad, L.ovc_policy_tail_grouped, L.ovc_encode_linear_grouped, L.ovc_wide_layers_grouped, L.ovc_assign_pairs, L.ovc_group_pairs, L.ovc_encode_linear_grouped_masked, L.ovc_policy_tail_grouped_joint, L.ovc_expand_codes_host, L.ovc_expand_stream_host, L.ovc_pipeline_create, L.ovc_pipeline_run, L.ovc_pipeline_wait, L.ovc_pipeline_join):
         f.restype = i32
     if L.ovc_abi_version() != ABI_VERSION:
         raise NativeLibraryError("ABI version mismatch: library %d, binding %d" % (L.ovc_abi_version(), ABI_VERSION))
@@ -148,7 +152,8 @@ EXPORTED_SYMBOLS = (
     "ovc_group_members", "ovc_assign_members", "ovc_encode_linear_rows", "ovc_wide_layers_range", "ovc_policy_tail_rows",
     "ovc_sample_actions_rows", "ovc_learner_rows", "ovc_encode_linear_masked", "ovc_policy_tail_joint",
     "ovc_potential_shaping", "ovc_record_transition_dense", "ovc_encode_linear_wgrad", "ovc_policy_tail_grouped",
-    "ovc_encode_linear_grouped", "ovc_wide_layers_grouped",
+    "ovc_encode_linear_grouped", "ovc_wide_layers_grouped", "ovc_assign_pairs", "ovc_group_pairs", "ovc_encode_linear_grouped_masked",
+    "ovc_policy_tail_grouped_joint",
     "ovc_pipeline_create", "ovc_pipeline_run", "ovc_pipeline_wait", "ovc_pipeline_join", "ovc_pipeline_destroy",
 )
 

@@ -581,6 +581,40 @@ class BatchedOvercookedEnv(object):
             0 if rec is None else rec.capacity, self._stream()))
         return member
 
+    def group_pairs(self, pair, n_members, lst, first, jrow, entry_offsets, row_offsets):
+        """Population play's compact layout (ovc_group_pairs, one CTA on the device): from ``pair`` int32 [N, 2] (values in
+        [0, n_members)) writes ``lst`` int32 [2N] (entries ``e << 2 | mask`` grouped by member, ascending in e: mask 3 for a
+        self-play pair, 1 / 2 for view 0 / 1 of a cross pair), ``first`` int32 [2N] (each entry's first compact row), ``jrow``
+        int32 [2N] (compact row -> joint row ``2 e + v``), ``entry_offsets`` and ``row_offsets`` int32 [n_members + 1]."""
+        assert 1 <= n_members <= 64
+        assert pair.is_cuda and pair.dtype == torch.int32 and pair.is_contiguous() and pair.shape == (self.n_envs, 2)
+        for t, n in ((lst, 2 * self.n_envs), (first, 2 * self.n_envs), (jrow, 2 * self.n_envs), (entry_offsets, n_members + 1),
+                     (row_offsets, n_members + 1)):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n
+        _native.check(self._lib.ovc_group_pairs(pair.data_ptr(), int(n_members), self.n_envs, lst.data_ptr(), first.data_ptr(),
+                                                jrow.data_ptr(), entry_offsets.data_ptr(), row_offsets.data_ptr(), self._stream()))
+
+    def assign_pairs(self, pair, n_members, thresholds=None, counter=None, seed=0, done=None, records=None):
+        """``assign_members`` for population play's ordered pairs (ovc_assign_pairs): for every environment whose episode
+        ended (``done`` int32 [N]; None = every environment), the ending pair into ``records.pair`` (an ``EpisodeRecords``
+        built with ``pairs=True``), then, with ``thresholds`` (int64 CUDA [n_members^2 - 1], ``member_thresholds`` of the
+        row-major flattened pair weights), a new pair ``(p // n_members, p % n_members)`` into ``pair`` int32 [N, 2]."""
+        assert pair.is_cuda and pair.dtype == torch.int32 and pair.is_contiguous() and pair.shape == (self.n_envs, 2)
+        if thresholds is not None:
+            assert thresholds.is_cuda and thresholds.dtype == torch.int64 and thresholds.is_contiguous()
+            assert thresholds.numel() >= n_members * n_members - 1
+            assert counter.is_cuda and counter.dtype == torch.int64 and counter.numel() == 2 and counter.is_contiguous()
+        if done is not None:
+            assert done.is_cuda and done.dtype == torch.int32 and done.is_contiguous() and done.numel() == self.n_envs
+        if records is not None:
+            assert records.env is self and records.pair is not None, "records built with pairs=True"
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        _native.check(self._lib.ovc_assign_pairs(
+            ptr(done), ptr(thresholds), int(n_members), self.n_envs, int(seed) & (2**64 - 1), ptr(counter), pair.data_ptr(),
+            0 if records is None or records.capacity == 0 else records.pair.data_ptr(), 0 if records is None else records.count.data_ptr(),
+            0 if records is None else records.capacity, self._stream()))
+        return pair
+
     def sample_actions(self, scores, counter, seed=0, out=None, logp_out=None):
         """Joint actions drawn from the policy's logits (ovc_sample_actions: Gumbel-max on Philox draws, one kernel).
         ``scores`` float32 ``[2N, ld]`` (rows ordered [env][agent], the first 6 columns are the logits), ``counter`` an
@@ -1037,9 +1071,11 @@ class EpisodeRecords(object):
     reference's game_stats lists), reward_by_agent float32 [.., 2] (the sum of the per-agent rewards of the episode);
     count int32 [N] (episodes written per environment), dropped int32 [N] (episodes that ended with the buffer full,
     not written).  ``members=True`` (a population of partners): also partner_member int32 [capacity, N], the member each
-    episode was played with (written by ``env.assign_members``); None otherwise."""
+    episode was played with (written by ``env.assign_members``); None otherwise.  ``pairs=True`` (population play): also
+    pair int32 [capacity, N, 2], the members on players 0 / 1 of each episode (written by ``env.assign_pairs``); None
+    otherwise."""
 
-    def __init__(self, env, capacity, members=False):
+    def __init__(self, env, capacity, members=False, pairs=False):
         self.env = env
         self.capacity = int(capacity)
         assert self.capacity >= 0
@@ -1052,10 +1088,11 @@ class EpisodeRecords(object):
         self._counters = z((2, N), torch.int32)  # count and dropped: one memset clears both
         self.count, self.dropped = self._counters[0], self._counters[1]
         self.partner_member = z((C, N), torch.int32) if members else None
+        self.pair = z((C, N, 2), torch.int32) if pairs else None
 
     def tensors(self):
         return [self.length, self.layout, self.partner_seat, self.sparse_r_by_agent, self.shaped_r_by_agent, self.game_stats,
-                self.reward_by_agent, self._counters] + ([] if self.partner_member is None else [self.partner_member])
+                self.reward_by_agent, self._counters] + [t for t in (self.partner_member, self.pair) if t is not None]
 
     def clear(self):
         """Forget every record (stream ordered, one memset: capturable in a CUDA graph)."""
@@ -1064,7 +1101,7 @@ class EpisodeRecords(object):
     def finished(self):
         """The records as a dict of tensors in the keys of the reference's episode info (overcooked_env.py:363-401) and of
         ``EpisodeStats.update``: env_index, ep_game_stats, ep_sparse_r(_by_agent), ep_shaped_r(_by_agent), ep_length, plus
-        ep_reward_by_agent, layout and partner_seat (and partner_member with ``members=True``).  Rows are ordered by (slot,
+        ep_reward_by_agent, layout and partner_seat (and partner_member with ``members=True``, pair with ``pairs=True``).  Rows are ordered by (slot,
         env).  Synchronises with the host."""
         k, e = torch.nonzero(torch.arange(self.capacity, device=self.env.device)[:, None] < self.count[None, :], as_tuple=True)
         sp, sh = self.sparse_r_by_agent[k, e], self.shaped_r_by_agent[k, e]
@@ -1073,4 +1110,6 @@ class EpisodeRecords(object):
                "ep_reward_by_agent": self.reward_by_agent[k, e], "layout": self.layout[k, e], "partner_seat": self.partner_seat[k, e]}
         if self.partner_member is not None:
             out["partner_member"] = self.partner_member[k, e]
+        if self.pair is not None:
+            out["pair"] = self.pair[k, e]
         return out

@@ -1004,6 +1004,39 @@ int ovc_policy_tail_grouped(const void *x, int64_t n_rows, int k0, float in_slop
     return ovc::policy_tail_grouped_impl(a, k0, (cudaStream_t)stream);
 }
 
+int ovc_assign_pairs(const int32_t *done, const int64_t *thresholds, int n_members, int64_t n_envs, uint64_t seed, uint64_t *counter,
+                     int32_t *pair, int32_t *rec_pair, const int32_t *count, int capacity, void *stream) {
+    return ovc::assign_pairs_impl(done, (const long long *)thresholds, n_members, n_envs, seed, (unsigned long long *)counter, pair, rec_pair,
+                                  count, capacity, (cudaStream_t)stream);
+}
+
+int ovc_group_pairs(const int32_t *pair, int n_members, int64_t n_envs, int32_t *list, int32_t *first, int32_t *jrow, int32_t *entry_offsets,
+                    int32_t *row_offsets, void *stream) {
+    return ovc::group_pairs_impl(pair, n_members, n_envs, list, first, jrow, entry_offsets, row_offsets, (cudaStream_t)stream);
+}
+
+int ovc_encode_linear_grouped_masked(const void *layouts, int n_layouts, const int32_t *state, const int32_t *list, const int32_t *first,
+                                     const void *wt, const float *bias, const int32_t *entry_offsets, int n_members, void *out, int64_t n_list,
+                                     int state_words, int width, int height, int horizon, int n_out, float neg_slope, void *stream) {
+    int rc = ovc::check_common(layouts, n_layouts, state, n_list, state_words);
+    if (rc) return rc;
+    if (!list || !first || !entry_offsets) return ovc::fail(OVC_E_BADARG, "null pointer argument");
+    if (n_members < 1 || n_members > ovc::EL_MAX_MEMBERS) return ovc::fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+    return ovc::encode_linear_impl((const ovc_layout_t *)layouts, n_layouts, state, nullptr, wt, bias, out, n_list, state_words, width,
+                                   height, horizon, n_out, neg_slope, (cudaStream_t)stream, -1, nullptr, nullptr, list, first, entry_offsets,
+                                   n_members);
+}
+
+int ovc_policy_tail_grouped_joint(const void *x, int64_t n_rows, int k0, float in_slope, const void *w_first, const float *b_first,
+                                  const void *w_hidden, const float *b_hidden, int n_hidden, const void *w_heads, const float *b_heads,
+                                  float slope, int n_actions, uint64_t seed, uint64_t *counter, const int32_t *jrow, const int32_t *row_offsets,
+                                  int n_members, int32_t *actions, float *values, float *scores, float *logp, void *stream) {
+    ovc::PolicyTailArgs a = ovc::tail_args(x, n_rows, in_slope, w_first, b_first, w_hidden, b_hidden, n_hidden, w_heads, b_heads, slope,
+                                           n_actions, seed, counter, actions, values, scores, logp);
+    a.rows = jrow, a.offsets = row_offsets, a.n_members = n_members;
+    return ovc::policy_tail_grouped_impl(a, k0, (cudaStream_t)stream, ovc::RowMap::Joint);
+}
+
 int ovc_featurize(const void *layouts, int n_layouts, const void *lut, const int32_t *state,
                   const int32_t *view_swap, float *out, int64_t n_envs, int state_words, int num_pots, void *stream) {
     int rc = ovc::check_common(layouts, n_layouts, state, n_envs, state_words);

@@ -333,6 +333,13 @@ __global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_grouped_kernel(co
     encode_linear_body<CPL, false, false, false, true>(a, nullptr, nullptr, offsets);
 }
 
+// MASKED and GROUPED together (population play): member k walks list entries [offsets[k], offsets[k + 1]) with its table
+template <int CPL>
+__global__ void __launch_bounds__(EL_THREADS, 1) encode_linear_grouped_masked_kernel(const EncLinArgs a, const int32_t *list,
+                                                                                     const int32_t *first, const int32_t *offsets) {
+    encode_linear_body<CPL, false, false, true, true>(a, list, first, offsets);
+}
+
 static size_t encode_linear_smem(int cpl, int n_rows, int n_layouts) {
     const size_t CS = 32 * (size_t)cpl;
     return (size_t)n_rows * CS * 2 + ((size_t)n_layouts + 1) * CS * 4 + (size_t)n_layouts * (16 * 4 + 2 * 4 + 128 * 2 + 256) + 16;
@@ -340,7 +347,8 @@ static size_t encode_linear_smem(int cpl, int n_rows, int n_layouts) {
 
 // seat < 0: both views (ovc_encode_linear); 0 / 1: one view per environment (ovc_encode_linear_view, view_swap = swap);
 // with rows / range: the rows map (ovc_encode_linear_rows); with list / first: n_envs list entries (ovc_encode_linear_masked);
-// n_members > 0: a population's stacked tables over its environment offsets (ovc_encode_linear_grouped)
+// n_members > 0: a population's stacked tables over its environment offsets (ovc_encode_linear_grouped), or with list / first
+// over its list entry offsets (ovc_encode_linear_grouped_masked)
 static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const int32_t *state, const int32_t *view_swap,
                               const void *wt, const float *bias, void *out, long long n_envs, int S, int W, int H, int horizon,
                               int n_out, float neg_slope, cudaStream_t st, int seat = -1, const int32_t *rows = nullptr,
@@ -403,7 +411,18 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
         if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                                          \
         encode_linear_grouped_kernel<C><<<grid, EL_THREADS, smem, st>>>(a, offsets);                                          \
     } while (0)
-    if (grouped) {
+#define OVC_LAUNCH_ELGM(C)                                                                                                    \
+    do {                                                                                                                      \
+        e = cudaFuncSetAttribute(encode_linear_grouped_masked_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
+        if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel attribute");                                          \
+        encode_linear_grouped_masked_kernel<C><<<grid, EL_THREADS, smem, st>>>(a, list, first, offsets);                      \
+    } while (0)
+    if (grouped && masked) {
+        const unsigned grid = (unsigned)(workers * n_slices * n_members);
+        if (cpl == 8) OVC_LAUNCH_ELGM(8);
+        else if (cpl == 4) OVC_LAUNCH_ELGM(4);
+        else OVC_LAUNCH_ELGM(2);
+    } else if (grouped) {
         const unsigned grid = (unsigned)(workers * n_slices * n_members);
         if (cpl == 8) OVC_LAUNCH_ELG(8);
         else if (cpl == 4) OVC_LAUNCH_ELG(4);
@@ -428,6 +447,7 @@ static int encode_linear_impl(const ovc_layout_t *layouts, int n_layouts, const 
 #undef OVC_LAUNCH_EL
 #undef OVC_LAUNCH_ELM
 #undef OVC_LAUNCH_ELG
+#undef OVC_LAUNCH_ELGM
     e = cudaGetLastError();
     if (e != cudaSuccess) return cuda_fail(e, "encode_linear kernel launch");
     return OVC_OK;

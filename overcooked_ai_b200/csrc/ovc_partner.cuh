@@ -356,4 +356,152 @@ static int assign_members_impl(const int32_t *done, const long long *thresholds,
     return OVC_OK;
 }
 
+// ---- population play: an ordered pair of learners per environment ----
+constexpr int MAX_PAIR_THRESHOLDS = MAX_MEMBERS * MAX_MEMBERS - 1;
+
+// assign_members_kernel for ordered pairs: the ending pair into rec_pair[count[e]][e], then, with thresholds, a new pair.
+// The n_members^2 - 1 thresholds of the row-major pair weights are non-decreasing, so #{q : w0 >= thresholds[q]} is an
+// upper bound found by binary search (at most 12 cached loads, for done environments only).
+__global__ void __launch_bounds__(256) assign_pairs_kernel(const int32_t *__restrict__ done, const long long *__restrict__ thresholds,
+                                                           int n_members, long long n_envs, unsigned long long seed,
+                                                           unsigned long long *counter, int2 *__restrict__ pair, int2 *__restrict__ rec_pair,
+                                                           const int32_t *__restrict__ count, int capacity) {
+    const unsigned long long step = thresholds ? *reinterpret_cast<volatile unsigned long long *>(counter) : 0ull;
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < n_envs && (!done || done[e] != 0)) {
+        if (done && rec_pair) {
+            const int k = count[e];
+            if (k < capacity) rec_pair[(long long)k * n_envs + e] = pair[e];
+        }
+        if (thresholds) {
+            const Philox4 P = philox4x32_10(seed, (uint32_t)e, (uint32_t)((unsigned long long)e >> 32), (uint32_t)step, (uint32_t)(step >> 32));
+            const long long w0 = P.v[0];
+            int lo = 0, hi = n_members * n_members - 1;
+            while (lo < hi) {
+                const int mid = (lo + hi) >> 1;
+                if (w0 >= __ldg(thresholds + mid)) lo = mid + 1;
+                else hi = mid;
+            }
+            pair[e] = make_int2(lo / n_members, lo % n_members);
+        }
+    }
+    if (thresholds) advance_step(counter, step);
+}
+
+static int assign_pairs_impl(const int32_t *done, const long long *thresholds, int n_members, long long n_envs, unsigned long long seed,
+                             unsigned long long *counter, int32_t *pair, int32_t *rec_pair, const int32_t *count, int capacity, cudaStream_t st) {
+    if (!pair || (thresholds && !counter) || (rec_pair && !count)) return fail(OVC_E_BADARG, "null pointer argument");
+    if (((uintptr_t)done | (uintptr_t)count) & 3) return fail(OVC_E_BADARG, "done and count must be 4-byte aligned");
+    if (((uintptr_t)pair | (uintptr_t)rec_pair | (uintptr_t)thresholds | (uintptr_t)counter) & 7)
+        return fail(OVC_E_BADARG, "pair, rec_pair, thresholds and counter must be 8-byte aligned");
+    if (n_members < 1 || n_members > MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+    if (capacity < 0) return fail(OVC_E_BADARG, "negative record capacity", capacity);
+    if (n_envs < 0) return fail(OVC_E_BADARG, "negative env count");
+    if (n_envs == 0) return OVC_OK;
+    assign_pairs_kernel<<<(unsigned)((n_envs + 255) / 256), 256, 0, st>>>(done, thresholds, n_members, n_envs, seed, counter, (int2 *)pair,
+                                                                         (int2 *)rec_pair, count, capacity);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "assign_pairs kernel launch");
+    return OVC_OK;
+}
+
+// The pairs grouped by member: group_members_kernel's stable counting sort in ONE CTA, over the 2 n_envs items (e, s) in
+// index order 2 e + s.  Item (e, 0) is the entry of member pair[e][0]: e << 2 | 3 (two rows) where pair[e] = (i, i), else
+// e << 2 | 1 (view 0); item (e, 1) is the entry e << 2 | 2 (view 1) of member pair[e][1], or nothing where the pair is a
+// self-play one.  An environment has at most one entry per member, so each group is ascending in e.  Warps count entries
+// and rows per member (warp-private histograms), 64 threads and then one thread turn them into starts, and every warp
+// walks its segment 32 items at a time: lanes of one member find each other with __match_any_sync and take consecutive
+// entries in lane order, their rows after the earlier lanes' rows (a self-play entry holds two).
+__global__ void __launch_bounds__(GM_THREADS, 1) group_pairs_kernel(const int32_t *__restrict__ pair, int n_members, long long n_envs,
+                                                                    int32_t *__restrict__ list, int32_t *__restrict__ first,
+                                                                    int32_t *__restrict__ jrow, int32_t *__restrict__ entry_offsets,
+                                                                    int32_t *__restrict__ row_offsets) {
+    constexpr int NW = GM_THREADS / 32;
+    __shared__ int hent[NW][MAX_MEMBERS], hrow[NW][MAX_MEMBERS];
+    __shared__ int tent[MAX_MEMBERS], trow[MAX_MEMBERS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int i = threadIdx.x; i < NW * MAX_MEMBERS; i += GM_THREADS) (&hent[0][0])[i] = 0, (&hrow[0][0])[i] = 0;
+    __syncthreads();
+    const long long n_items = 2 * n_envs;
+    const long long seg = (n_items + NW - 1) / NW;
+    const long long beg = warp * seg, end = beg + seg < n_items ? beg + seg : n_items;
+    // item v's member (-1: no entry) and its row count
+    auto item = [&](long long v, int &rows) {
+        const int2 p = __ldg(reinterpret_cast<const int2 *>(pair) + (v >> 1));
+        rows = (v & 1) == 0 && p.x == p.y ? 2 : 1;
+        return (v & 1) == 0 ? p.x : (p.x == p.y ? -1 : p.y);
+    };
+    for (long long v = beg + lane; v < end; v += 32) {
+        int rows;
+        const int k = item(v, rows);
+        if (k >= 0) atomicAdd(&hent[warp][k], 1), atomicAdd(&hrow[warp][k], rows);
+    }
+    __syncthreads();
+    if (threadIdx.x < MAX_MEMBERS) {  // thread k: member k's start in every segment, relative to the group's start
+        const int k = threadIdx.x;
+        int te = 0, tr = 0;
+        for (int w = 0; w < NW; w++) {
+            const int ce = hent[w][k], cr = hrow[w][k];
+            hent[w][k] = te, hrow[w][k] = tr;
+            te += ce, tr += cr;
+        }
+        tent[k] = te, trow[k] = tr;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {  // the group starts: exclusive scans of the totals
+        int re = 0, rr = 0;
+        for (int k = 0; k < n_members; k++) {
+            const int ce = tent[k], cr = trow[k];
+            tent[k] = re, trow[k] = rr;
+            re += ce, rr += cr;
+        }
+        entry_offsets[n_members] = re, row_offsets[n_members] = rr;
+    }
+    __syncthreads();
+    if (threadIdx.x < n_members) {
+        const int k = threadIdx.x, be = tent[k], br = trow[k];
+        entry_offsets[k] = be, row_offsets[k] = br;
+        for (int w = 0; w < NW; w++) hent[w][k] += be, hrow[w][k] += br;
+    }
+    __syncthreads();
+    const unsigned lt = (1u << lane) - 1u;
+    for (long long v0 = beg; v0 < end; v0 += 32) {
+        const long long v = v0 + lane;
+        int rows = 0;
+        int k = v < end ? item(v, rows) : -1;
+        const bool in = k >= 0;
+        if (!in) k = -1 - lane;  // lanes without an entry match nobody
+        const unsigned peers = __match_any_sync(0xFFFFFFFFu, k);
+        const unsigned twos = __ballot_sync(0xFFFFFFFFu, in && rows == 2);
+        const int slot = in ? hent[warp][k] + __popc(peers & lt) : 0;
+        const int row = in ? hrow[warp][k] + __popc(peers & lt) + __popc(peers & twos & lt) : 0;
+        __syncwarp();
+        if (in) {
+            const long long e = v >> 1;
+            const int mask = rows == 2 ? 3 : (v & 1) ? 2 : 1;
+            list[slot] = (int32_t)(e << 2) | mask;
+            first[slot] = row;
+            jrow[row] = (int32_t)(2 * e + (mask == 2));
+            if (mask == 3) jrow[row + 1] = (int32_t)(2 * e + 1);
+            if ((peers & lt) == 0) hent[warp][k] += __popc(peers), hrow[warp][k] += __popc(peers) + __popc(peers & twos);
+        }
+        __syncwarp();
+    }
+}
+
+static int group_pairs_impl(const int32_t *pair, int n_members, long long n_envs, int32_t *list, int32_t *first, int32_t *jrow,
+                            int32_t *entry_offsets, int32_t *row_offsets, cudaStream_t st) {
+    if (!pair || !list || !first || !jrow || !entry_offsets || !row_offsets) return fail(OVC_E_BADARG, "null pointer argument");
+    if ((uintptr_t)pair & 7) return fail(OVC_E_BADARG, "pair must be 8-byte aligned");
+    if (((uintptr_t)list | (uintptr_t)first | (uintptr_t)jrow | (uintptr_t)entry_offsets | (uintptr_t)row_offsets) & 3)
+        return fail(OVC_E_BADARG, "list, first, jrow, entry_offsets and row_offsets must be 4-byte aligned");
+    if (n_members < 1 || n_members > MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", n_members);
+    if (n_envs < 0 || n_envs >= LR_MAX_ENVS) return fail(OVC_E_BADARG, "n_envs must be 0..2^29-1", n_envs);
+    if (n_envs == 0) return OVC_OK;
+    group_pairs_kernel<<<1, GM_THREADS, 0, st>>>(pair, n_members, n_envs, list, first, jrow, entry_offsets, row_offsets);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "group_pairs kernel launch");
+    return OVC_OK;
+}
+
 }  // namespace ovc

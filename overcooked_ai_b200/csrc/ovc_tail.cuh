@@ -337,14 +337,16 @@ __global__ void __launch_bounds__(PT_THREADS, 1) policy_tail_kernel(const Policy
 // order (a member's last tile partial, never shared with the next member); CTA b takes the contiguous share
 // [b T / G, (b + 1) T / G) of the T tiles, so a CTA holds at most a few members' tables, each staged once, and the work is
 // balanced whatever the block sizes.  Each row is drawn on its own row index r with the call's step, exactly as
-// ovc_policy_tail_logp draws row r, and every CTA advances the counter once.
+// ovc_policy_tail_logp draws row r, and every CTA advances the counter once.  MAP Joint (ovc_policy_tail_grouped_joint,
+// population play): the rows are compact rows, row r drawn on and written at joint row rows[r], as in the joint form.
 // 12 warps per CTA (a cap of 170 registers; ptxas uses 112 - 159 over the instantiations, no spills): under K8's 16 warps
 // (a cap of 128) the member bookkeeping on top of K8's tile spilled.
 constexpr int PT_MAX_MEMBERS = 64;
 constexpr int PTG_THREADS = 384;
 
-template <int KS2, bool LOGP>
+template <int KS2, bool LOGP, RowMap MAP = RowMap::Identity>
 __global__ void __launch_bounds__(PTG_THREADS, 1) policy_tail_grouped_kernel(const PolicyTailArgs p) {
+    static_assert(MAP == RowMap::Identity || (MAP == RowMap::Joint && LOGP), "the grouped forms: Identity, or Joint with logp");
     constexpr int K0 = 32 * KS2;
     extern __shared__ __align__(16) char pt_smem[];
     __shared__ int tile0[PT_MAX_MEMBERS + 1], rbeg[PT_MAX_MEMBERS], rend[PT_MAX_MEMBERS];
@@ -379,7 +381,7 @@ __global__ void __launch_bounds__(PTG_THREADS, 1) policy_tail_grouped_kernel(con
             const int r0 = rbeg[k] + (tile - tile0[k]) * 16 + g;
             float out[1][4];
             tail_tile<KS2>(out, p, w, r0, r_end, g, t);
-            tail_epilogue<LOGP, RowMap::Identity>(p, out, step, r0, r_end, lane, t);
+            tail_epilogue<LOGP, MAP>(p, out, step, r0, r_end, lane, t);
         }
         tb = te;
     }
@@ -390,6 +392,7 @@ using PolicyTailKernel = void (*)(PolicyTailArgs);
 
 template <int KS2>
 static PolicyTailKernel policy_tail_pick(RowMap map, bool logp, bool hid, bool grouped) {
+    if (grouped && map == RowMap::Joint) return policy_tail_grouped_kernel<KS2, true, RowMap::Joint>;
     if (grouped) return logp ? policy_tail_grouped_kernel<KS2, true> : policy_tail_grouped_kernel<KS2, false>;
     if (hid) return policy_tail_kernel<KS2, RowMap::Identity, false, true>;
     switch (map) {
@@ -425,9 +428,10 @@ static int policy_tail_launch(const PolicyTailArgs &a, int k0, cudaStream_t st, 
     return OVC_OK;
 }
 
-static int policy_tail_grouped_impl(const PolicyTailArgs &a, int k0, cudaStream_t st) {
+// map Identity: ovc_policy_tail_grouped; Joint: ovc_policy_tail_grouped_joint (a.rows = jrow, logp required)
+static int policy_tail_grouped_impl(const PolicyTailArgs &a, int k0, cudaStream_t st, RowMap map = RowMap::Identity) {
     if (!a.x || !a.w_first || !a.b_first || !a.w_heads || !a.b_heads || !a.counter || !a.actions || !a.offsets ||
-        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)))
+        (a.n_hidden > 0 && (!a.w_hidden || !a.b_hidden)) || (map == RowMap::Joint && (!a.rows || !a.logp)))
         return fail(OVC_E_BADARG, "null pointer argument");
     if ((((uintptr_t)a.x | (uintptr_t)a.w_first | (uintptr_t)a.w_hidden | (uintptr_t)a.w_heads) & 15) != 0)
         return fail(OVC_E_BADARG, "x and the weight tables must be 16-byte aligned");
@@ -435,6 +439,7 @@ static int policy_tail_grouped_impl(const PolicyTailArgs &a, int k0, cudaStream_
         return fail(OVC_E_BADARG, "biases, scores and counter must be 8-byte aligned");
     if ((((uintptr_t)a.actions | (uintptr_t)a.values | (uintptr_t)a.logp | (uintptr_t)a.offsets) & 3) != 0)
         return fail(OVC_E_BADARG, "actions, values, logp and offsets must be 4-byte aligned");
+    if (((uintptr_t)a.rows & 3) != 0) return fail(OVC_E_BADARG, "jrow must be 4-byte aligned");
     if (a.n_members < 1 || a.n_members > PT_MAX_MEMBERS) return fail(OVC_E_BADARG, "n_members must be 1..64", a.n_members);
     if (k0 < 32 || k0 > 256 || k0 % 32) return fail(OVC_E_BADARG, "k0 must be a multiple of 32 in 32..256", k0);
     if (a.n_hidden < 0 || a.n_hidden > 8) return fail(OVC_E_BADARG, "n_hidden must be 0..8", a.n_hidden);
@@ -442,7 +447,7 @@ static int policy_tail_grouped_impl(const PolicyTailArgs &a, int k0, cudaStream_
     if (!(a.in_slope >= 0.f && a.in_slope <= 1.f && a.slope >= 0.f && a.slope <= 1.f)) return fail(OVC_E_BADARG, "slopes must lie in [0, 1]");
     if (a.n_rows < 0 || a.n_rows > 0x7FFFFFFFll) return fail(OVC_E_BADARG, "n_rows must lie in [0, 2^31)", a.n_rows);
     if (a.n_rows == 0) return OVC_OK;
-    return policy_tail_launch(a, k0, st, RowMap::Identity, false, true);
+    return policy_tail_launch(a, k0, st, map, false, true);
 }
 
 // map: ovc_policy_tail[_logp] Identity, ovc_policy_tail_view View, ovc_policy_tail_rows Rows, ovc_policy_tail_joint Joint.

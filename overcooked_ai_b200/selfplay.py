@@ -482,6 +482,8 @@ class SampleBatch(object):
                                      (``one_view``: agent 1's player)
     partner_member int8 [T, N]       with a population of partners: each environment's member at transition t (in a
                                      two-view batch meaningful where partner_seat >= 0), else None
+    pair          int8 [T, N, 2]     population play: the members on players 0 / 1 of each environment at transition t, so
+                                     ``pair.view(T, 2N)[t, r]`` is the member that acted on row r; else None
     learner_mask  uint8 [T, 2N]      (property) the rows the learner trains on: all rows but the partner's
     episodes      EpisodeRecords     the episodes that ended in the window (``episodes.finished()``), capacity
                                      ceil(T / horizon): an environment cannot end more episodes in T transitions
@@ -504,7 +506,7 @@ class SampleBatch(object):
     agent 1 was at transition t, and ``episodes.finished()`` has ``partner_member``; both are None / absent otherwise.
     """
 
-    def __init__(self, env, n_steps, keep_logits=False, partner=False, seq_len=None, one_view=False, members=False):
+    def __init__(self, env, n_steps, keep_logits=False, partner=False, seq_len=None, one_view=False, members=False, pairs=False):
         N, T, dev = env.n_envs, int(n_steps), env.device
         R = N if one_view else 2 * N
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)
@@ -518,7 +520,8 @@ class SampleBatch(object):
         self.logits = z((T, R, 8), torch.float32) if keep_logits else None
         self.partner_seat = z((T, N), torch.int8) if partner or one_view else None
         self.partner_member = z((T, N), torch.int8) if members else None
-        self.episodes = EpisodeRecords(env, -(-T // env.horizon) if env.horizon > 0 else 0, members=members)
+        self.pair = z((T, N, 2), torch.int8) if pairs else None
+        self.episodes = EpisodeRecords(env, -(-T // env.horizon) if env.horizon > 0 else 0, members=members, pairs=pairs)
         self.seq_len = seq_len
         self.state_h = z((-(-T // seq_len), R, 256), torch.bfloat16) if seq_len else None
         self.state_c = z((-(-T // seq_len), R, 256), torch.float32) if seq_len else None
@@ -789,6 +792,8 @@ class _Rollout(object):
     keep_logits)`` and ``_agents()`` (its policies); it sets ``population``, ``_pop`` (the population, or None) and
     ``_member``."""
 
+    _pair_play = False  # SelfPlayRollout's population play: its episode records hold each episode's pair
+
     def _init_rollout(self, env, learner, use_graph, reward_shaping_factor, episode_capacity, max_seq_len):
         """The shared state; ``learner`` is the policy whose LSTM state (if any) the bootstrap step leaves alone."""
         N, dev = env.n_envs, env.device
@@ -798,7 +803,7 @@ class _Rollout(object):
         self.factor = float(reward_shaping_factor)
         self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by the captured graphs
         self.stats = EpisodeStats(env)
-        self.episodes = EpisodeRecords(env, episode_capacity, members=self.population)
+        self.episodes = EpisodeRecords(env, episode_capacity, members=self.population, pairs=self._pair_play)
         self.max_seq_len = int(max_seq_len)
         assert self.max_seq_len >= 1
         self.graph = None          # run()'s CUDA graph of one transition
@@ -914,7 +919,7 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
 
     def __init__(self, env, model=None, autocast_dtype=torch.bfloat16, use_graph=True, reward_shaping_factor=1.0,
                  fused_first_layer=None, seed=0, fused_tail=None, fused_wide=None, partner=None, bc_factor=0.0, episode_capacity=1,
-                 max_seq_len=20, member=None, member_weights=None, use_phi=False, blocks=None):
+                 max_seq_len=20, member=None, member_weights=None, use_phi=False, blocks=None, pairs=None, pair_weights=None):
         """autocast_dtype: the dtype of the dense model (``DenseGridPolicy``, widths padded to 16-byte rows) and of the
         observation K2 writes for it: bfloat16 (the plane values are exact in bf16), or None for float32 throughout.
         fused_first_layer (default: on for the bf16 policy where ``fused_kernel_support`` allows K7): the observation is
@@ -972,10 +977,44 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         ``ovc_policy_tail_grouped``), library layers per member on its block's rows; every row is drawn with key ``seed``
         and the one counter (grouped K8, or, without K8, one ``ovc_sample_actions`` over all rows): block k is bit
         for bit what ``SelfPlayRollout(env, model[k], seed=seed)`` does on those environments.  ``sync_weights()`` refolds
-        every member.  Not with a ``partner`` or an ``RllibLSTMShapedCNN`` member."""
+        every member.  Not with a ``partner`` or an ``RllibLSTMShapedCNN`` member.
+        pairs, pair_weights: population play for a list model instead of blocks: member ``pair[e, 0]`` plays player 0 of
+        environment e and member ``pair[e, 1]`` player 1, and every row is a learner's row.  ``pairs`` (int32 [N, 2] on the
+        environments' device) fixes the pairing (the evaluation form: a cross-play matrix through run()); ``pair_weights``
+        (K x K non-negative floats with a positive sum; see the property) draws the ordered pair (i, j) with probability
+        proportional to ``pair_weights[i][j]`` at construction and at every episode end (the training form: uniform weights
+        are PBT-style population play, a zero diagonal excludes self-play).  ``self.pair`` (int32 [N, 2]) is the live pairing.
+        Per transition ``ovc_group_pairs`` groups the entries by member on the device, then ``ovc_encode_linear_grouped_masked``
+        (the object part once per environment), K9 (grouped from ``GROUPED_K9_MIN_MEMBERS`` members on, else per member on
+        its compact rows; off K9 each member's library layers on all compact rows, its own rows selected on the device) and
+        ``ovc_policy_tail_grouped_joint`` (off K8: the library heads and one ``ovc_sample_actions`` over the joint rows).
+        Every row is drawn with key ``seed`` on the one counter at its joint row ``2 e + v``, so copies of one model draw
+        exactly what ``SelfPlayRollout(env, model)`` draws; the pair draw uses key ``seed ^ PAIR_SALT`` and a counter of its
+        own.  collect()'s batches carry ``pair`` and ``episodes.finished()`` reports each episode's ``pair``.  Needs K7 (at
+        most 8 layouts, a grid within its shared memory) and the bf16 policy; not with ``blocks``, a ``partner`` or an LSTM
+        member."""
         self.env = env
-        self._phi = _PhiReward(env) if use_phi else None
         models = list(model) if isinstance(model, (list, tuple)) else None
+        pair_play = pairs is not None or pair_weights is not None
+        if pair_play:
+            assert models is not None, "pairs / pair_weights go with a population of learners (a list model)"
+            assert pairs is None or pair_weights is None, "pairs fixes each environment's pair, pair_weights draws it: pass one of them"
+            assert blocks is None, "population play pairs the members per environment: pass no blocks with pairs / pair_weights"
+            assert partner is None, "population play has no partner: every row is a learner's"
+            assert autocast_dtype == torch.bfloat16, "population play runs K7 and K8 on the bf16 policy: autocast_dtype=None is not supported"
+            _check_members(models, MAX_MEMBERS, RllibShapedCNN, "a population of learners has 1..%d members" % MAX_MEMBERS,
+                           "a population learner is an RllibShapedCNN (an LSTM member is not supported)")
+            K, N = len(models), env.n_envs
+            if pairs is not None:
+                assert isinstance(pairs, torch.Tensor) and pairs.dtype == torch.int32 and tuple(pairs.shape) == (N, 2) and \
+                    pairs.is_contiguous(), "pairs: a contiguous int32 tensor [N, 2] (N = %d environments)" % N
+                assert pairs.device == env.device, "pairs: on the environments' device (%s), got %s" % (env.device, pairs.device)
+                lo, hi = int(pairs.min()), int(pairs.max())
+                assert 0 <= lo and hi < K, "pairs values must lie in [0, %d): found %d..%d" % (K, lo, hi)
+            else:
+                pair_thresholds(pair_weights, K)
+        self._pair_play = pair_play
+        self._phi = _PhiReward(env) if use_phi else None
         if models is not None:
             _check_members(models, MAX_MEMBERS, RllibShapedCNN, "a population of learners has 1..%d members" % MAX_MEMBERS,
                            "a population learner is an RllibShapedCNN (an LSTM member is not supported)")
@@ -985,6 +1024,10 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         else:
             assert blocks is None, "blocks go with a population of learners (a list model)"
         self._fold(env, models[0] if models else model, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
+        if pair_play:
+            assert self.fused_first_layer, \
+                "population play needs K7: a first layer width a multiple of 64, a grid whose table fits shared memory, and at " \
+                "most %d layouts (this environment has %d layouts on a %dx%d grid)" % (K7_MAX_LAYOUTS, env.n_layouts, self.W, self.H)
         dev = env.device
         N = env.n_envs
         self.seed = int(seed)
@@ -992,6 +1035,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         self._member = None
         if models is not None:
             self._fold_members(models, blocks, autocast_dtype)
+        if pair_play:
+            self._init_pairs(pairs, pair_weights)
         self.partner = partner
         self.bc = float(bc_factor)
         self.population = isinstance(partner, (list, tuple))
@@ -1029,6 +1074,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         self._scores8 = None  # set to a float32 [2N, 8] tensor to make K8 also write the heads (tests)
         if partner is not None:
             self._assign_seats(None)
+        if pair_play and pairs is None:
+            self._assign_pairs(None, None)
         if isinstance(self._partner, _Population):
             if self._partner.needs_obs and self.obs is None:
                 self.obs = torch.empty((N, 2, self.W, self.H, 26), dtype=autocast_dtype or torch.float32, device=dev)
@@ -1066,19 +1113,20 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         """A population of learners: fold members 1.. like member 0 (self), set the blocks, and stack the K8 tables so that
         each member's tables are views of the stack (its ``sync_weights`` then refreshes the stack in place)."""
         env, N, dev, K = self.env, self.env.n_envs, self.env.device, len(models)
-        if blocks is None:
-            assert N >= K, "equal blocks need at least one environment per member (%d members, %d environments)" % (K, N)
-            counts = [(k + 1) * N // K - k * N // K for k in range(K)]
-        else:
-            counts = [int(b) for b in blocks]
-            assert len(counts) == K, "blocks: one environment count per member (%d)" % K
-            assert all(c > 0 for c in counts) and sum(counts) == N, \
-                "blocks: positive environment counts summing to the %d environments, got %s" % (N, counts)
-        self._offs = [0] + np.cumsum(counts).tolist()
-        self.blocks = torch.tensor(self._offs, dtype=torch.int32, device=dev)
-        self._row_offsets = 2 * self.blocks  # K8's offsets are joint rows
-        self._member = torch.repeat_interleave(torch.arange(K, dtype=torch.int32, device=dev),
-                                               torch.tensor(counts, device=dev)).to(torch.int32)
+        if not self._pair_play:
+            if blocks is None:
+                assert N >= K, "equal blocks need at least one environment per member (%d members, %d environments)" % (K, N)
+                counts = [(k + 1) * N // K - k * N // K for k in range(K)]
+            else:
+                counts = [int(b) for b in blocks]
+                assert len(counts) == K, "blocks: one environment count per member (%d)" % K
+                assert all(c > 0 for c in counts) and sum(counts) == N, \
+                    "blocks: positive environment counts summing to the %d environments, got %s" % (N, counts)
+            self._offs = [0] + np.cumsum(counts).tolist()
+            self.blocks = torch.tensor(self._offs, dtype=torch.int32, device=dev)
+            self._row_offsets = 2 * self.blocks  # K8's offsets are joint rows
+            self._member = torch.repeat_interleave(torch.arange(K, dtype=torch.int32, device=dev),
+                                                   torch.tensor(counts, device=dev)).to(torch.int32)
         self._others = []
         for m in models[1:]:
             f = _FoldedPolicy()
@@ -1137,6 +1185,94 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
                 actions.data_ptr(), vals.data_ptr(), ptr(scores8), ptr(logp), env._stream()))
         return None
 
+    def _init_pairs(self, pairs, pair_weights):
+        """Population play's state: the live pairing, its draw, and the compact layout ``ovc_group_pairs`` writes."""
+        N, dev, K = self.env.n_envs, self.env.device, len(self._members)
+        i32 = lambda n: torch.zeros(n, dtype=torch.int32, device=dev)
+        self._pair_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of the pair draw
+        if pairs is not None:
+            self.pair, self._pair_thresholds = pairs, None
+        else:
+            self.pair = torch.zeros((N, 2), dtype=torch.int32, device=dev)
+            self._pair_thresholds = torch.zeros(max(K * K - 1, 1), dtype=torch.int64, device=dev)  # never NULL: NULL skips the draw
+            self.pair_weights = [[1.0] * K for _ in range(K)] if pair_weights is None else pair_weights
+        self._plist, self._pfirst, self._pjrow = i32(2 * N), i32(2 * N), i32(2 * N)
+        self._entry_offsets, self._pair_row_offsets = i32(K + 1), i32(K + 1)
+        self._logp = torch.empty(2 * N, dtype=torch.float32, device=dev)  # run()'s logp: the joint K8 always writes it
+        if not self.fused_wide:  # the member of each compact row, for the library layers' selection
+            self._rmember = torch.empty(2 * N, dtype=torch.int64, device=dev)
+            self._rindex = torch.arange(2 * N, device=dev)
+        if not self.fused_tail:  # the library heads on compact rows, scattered to the joint rows for the draw kernel
+            self._jrow64 = torch.empty(2 * N, dtype=torch.int64, device=dev)
+            self._cscores = torch.zeros((2 * N, self.dense_model.n_actions), dtype=torch.float32, device=dev)
+            self._cvalues = torch.zeros(2 * N, dtype=torch.float32, device=dev)
+
+    @property
+    def pair_weights(self):
+        """Population play's pair weights (K x K non-negative floats with a positive sum; entry [i][j] weighs member i on
+        player 0 next to member j on player 1).  Setting them rewrites the device thresholds the pair draw reads, so run() and
+        collect() follow the new weights at the next episode ends without a re-capture."""
+        assert self._pair_play and self._pair_thresholds is not None, "pair_weights: population play with drawn pairs"
+        return [list(r) for r in self._pair_weights]
+
+    @pair_weights.setter
+    def pair_weights(self, value):
+        assert self._pair_play and self._pair_thresholds is not None, "pair_weights: population play with drawn pairs"
+        K = len(self._members)
+        thr = pair_thresholds(value, K)
+        self._pair_weights = np.asarray(value, dtype=np.float64).tolist()
+        self._pair_thresholds[:K * K - 1].copy_(torch.from_numpy(thr))
+
+    def _assign_pairs(self, done, records):
+        """After K1: the ending episodes' pair into ``records``, then (drawn pairs) a new pair; done None: every environment,
+        no record (construction)."""
+        drawn = self._pair_thresholds is not None
+        self.env.assign_pairs(self.pair, len(self._members), self._pair_thresholds, self._pair_counter if drawn else None,
+                              seed=self.seed ^ PAIR_SALT, done=done, records=records)
+
+    def _policy_pairs(self, actions, vals, logp, scores8, counter):
+        """``_policy`` for population play: ``ovc_group_pairs``, grouped masked K7 into compact rows, K9 (grouped from
+        ``GROUPED_K9_MIN_MEMBERS`` members on, else per member on its compact rows), grouped joint K8 (None returned).  Off
+        K9, each member's library layers run on all compact rows and its rows are selected by the row's member (no host
+        synchronisation); off K8, the heads are scattered to the joint rows of self._scores (returned for the draw kernel)."""
+        env, lib, st, K, rows = self.env, _native.lib(), self.env._stream(), len(self._members), 2 * self.env.n_envs
+        with torch.no_grad():
+            env.group_pairs(self.pair, K, self._plist, self._pfirst, self._pjrow, self._entry_offsets, self._pair_row_offsets)
+            wt, b0 = self._k7_stack
+            _native.check(lib.ovc_encode_linear_grouped_masked(
+                env.tables.data_ptr(), env.n_layouts, env.state.data_ptr(), self._plist.data_ptr(), self._pfirst.data_ptr(),
+                wt.data_ptr(), b0.data_ptr(), self._entry_offsets.data_ptr(), K, self._act0.data_ptr(), rows, env.state_words, self.W,
+                self.H, env.horizon if env.horizon > 0 else 2**31 - 1, wt.shape[2], 0.2, st))
+            flat = self._act0
+            if self.fused_wide and K >= GROUPED_K9_MIN_MEMBERS:
+                _native.check(lib.ovc_wide_layers_grouped(*self._k9_args(flat, self._wide_stack), self._pair_row_offsets.data_ptr(), K,
+                                                          self._z.data_ptr(), st))
+            elif self.fused_wide:
+                for k, f in enumerate(self._members):
+                    _native.check(lib.ovc_wide_layers_range(*f._k9_args(flat), self._pair_row_offsets[k:k + 2].data_ptr(),
+                                                            self._z.data_ptr(), st))
+            else:  # library layers per member on every compact row; bit for bit the member's own rollout only where cuBLAS
+                # computes a row independently of the other rows
+                torch.searchsorted(self._pair_row_offsets[1:], self._rindex, right=True, out=self._rmember)
+                for k, f in enumerate(self._members):
+                    mine = (self._rmember == k).unsqueeze(1)
+                    if self.fused_tail:
+                        torch.where(mine, f.dense_model.trunk(flat, 1), self._z, out=self._z)
+                    else:
+                        logits, value = f.dense_model.forward_from(flat, 1)
+                        torch.where(mine, logits.float(), self._cscores, out=self._cscores)
+                        torch.where(mine[:, 0], value.float(), self._cvalues, out=self._cvalues)
+            if not self.fused_tail:
+                self._jrow64.copy_(self._pjrow)
+                self._scores.index_copy_(0, self._jrow64, self._cscores)
+                vals.index_copy_(0, self._jrow64, self._cvalues)
+                return self._scores
+            _native.check(lib.ovc_policy_tail_grouped_joint(
+                *self._k8_args(self._z, self._tail_stack), counter.data_ptr(), self._pjrow.data_ptr(), self._pair_row_offsets.data_ptr(), K,
+                actions.data_ptr(), vals.data_ptr(), 0 if scores8 is None else scores8.data_ptr(),
+                (self._logp if logp is None else logp).data_ptr(), st))
+        return None
+
     def sync_weights(self):
         """Re-fold the learner (``_FoldedPolicy.sync_weights``), the partner (a network partner, every population member, or
         a BC partner's K10 tables) and every member of a population of learners, in place: the captured graphs use the new
@@ -1156,6 +1292,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
             live += [self.h, self.c, self.env.done]  # env.done: the next transition's LSTM reset
         if self.partner is not None:
             live += [self.partner_seat, self._seat_counter] + self._partner.live()
+        if self._pair_play:
+            live += [self.pair, self._pair_counter]
         return live
 
     def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None, state_out=None, snap=None):
@@ -1169,6 +1307,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         vals = self.values.view(rows) if values is None else values
         scores8 = self._scores8 if scores8 is None else scores8
         counter = self._draw_counter if counter is None else counter
+        if self._pair_play:
+            return self._policy_pairs(actions, vals, logp, scores8, counter)
         if self._members is not None:
             return self._policy_members(actions, vals, logp, scores8, counter)
         with torch.no_grad():
@@ -1202,6 +1342,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
             b.states[t].copy_(env.state)
             actions, values, logp, rewards, dones = b.actions[t], b.values[t], b.logp[t], b.rewards[t], b.dones[t]
             logits = None if b.logits is None else b.logits[t]
+            if self._pair_play:
+                b.pair[t].copy_(self.pair)
         if self.obs is not None:
             env.lossless_state_encoding(out=self.obs)  # K2
         snap = None
@@ -1225,6 +1367,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         dense = _env_step(env, actions.view(env.n_envs, 2), self._phi)
         if self.population:  # before the record: both use the slot count[e] the ending episode goes to
             self._pop.assign(env.done, self.episodes if b is None else b.episodes)
+        if self._pair_play:  # before the record, likewise
+            self._assign_pairs(env.done, self.episodes if b is None else b.episodes)
         # the seat draw below runs after this kernel, so partner_seat is still the ending episode's
         env.record_transition(self._factor, rewards=rewards, dones=dones, ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed,
                               stats=self.stats, records=self.episodes if b is None else b.episodes,
@@ -1245,7 +1389,7 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         where the learner runs on its own rows only, not written); ``partner_member`` is meaningful where ``partner_seat >=
         0``.  A seat changes hands only at a done, where GAE cuts, so a learner row's advantages never read a partner step."""
         return SampleBatch(self.env, n_steps, keep_logits, partner=self.partner is not None,
-                           seq_len=self.max_seq_len if self.lstm else None, members=self.population)
+                           seq_len=self.max_seq_len if self.lstm else None, members=self.population, pairs=self._pair_play)
 
     def env_only(self, n_steps):
         """The same transitions without the policy: encode + step with the last sampled actions
@@ -1356,6 +1500,22 @@ def member_thresholds(weights):
     assert w.ndim == 1 and 1 <= w.size <= MAX_MEMBERS, "between 1 and %d member weights" % MAX_MEMBERS
     assert np.all(np.isfinite(w)) and np.all(w >= 0) and w.sum() > 0, "member weights: finite, non-negative, a positive sum"
     c = np.cumsum(w)
+    return np.floor(c[:-1] / c[-1] * 2.0**32).astype(np.int64)
+
+
+# The pair draw's key is seed ^ PAIR_SALT: its counters (env, step) are those of the other per-episode draws
+PAIR_SALT = 0xBF58476D1CE4E5B9
+
+
+def pair_thresholds(weights, n_members):
+    """The table ``ovc_assign_pairs`` draws an ordered pair from: ``member_thresholds``' rule on the row-major flattened
+    ``n_members`` x ``n_members`` weights (int64 [K^2 - 1]); entry [i][j] weighs member i on player 0 next to member j on
+    player 1, and a pair of weight 0 is never drawn."""
+    w = np.asarray(weights, dtype=np.float64)
+    K = int(n_members)
+    assert w.shape == (K, K), "pair_weights: a %d x %d array (one weight per ordered pair of members), got shape %s" % (K, K, w.shape)
+    assert np.all(np.isfinite(w)) and np.all(w >= 0) and w.sum() > 0, "pair weights: finite, non-negative, a positive sum"
+    c = np.cumsum(w.ravel())
     return np.floor(c[:-1] / c[-1] * 2.0**32).astype(np.int64)
 
 
