@@ -183,9 +183,10 @@ def philox4x32_10(key, c):
     return np.stack(c, 1).astype(np.uint32)
 
 
-def gumbel_scores(scores, seed, step, n_actions=6):
-    """scores[:, i] - log(-log u_i) of the ovc_sample_actions definition: counter (row lo, row hi, step lo, 2 step hi + i / 4)."""
-    rows = np.arange(len(scores), dtype=np.uint64)
+def gumbel_scores(scores, seed, step, n_actions=6, rows=None):
+    """scores[:, i] - log(-log u_i) of the ovc_sample_actions definition: counter (row lo, row hi, step lo, 2 step hi + i / 4).
+    ``rows``: the row id each score row is drawn on (the joint row of a row map); default 0, 1, ..."""
+    rows = np.arange(len(scores), dtype=np.uint64) if rows is None else np.asarray(rows).astype(np.uint64)
     step = int(step)
     ctr = np.stack([rows & np.uint64(0xFFFFFFFF), rows >> np.uint64(32), np.full_like(rows, step & 0xFFFFFFFF),
                     np.full_like(rows, (step >> 32) << 1)], 1).astype(np.uint32)
@@ -194,15 +195,22 @@ def gumbel_scores(scores, seed, step, n_actions=6):
     return np.asarray(scores)[:, :n_actions] - np.log(-np.log(u))
 
 
-def check_draw(actions, scores, seed, step, n_actions=6):
-    """actions == the ovc_sample_actions definition applied to ``scores`` at ``step`` (near-ties exempt)."""
+def check_draw(actions, scores, seed, step, n_actions=6, rows=None, row_sensitive=False):
+    """actions == the ovc_sample_actions definition applied to ``scores`` at ``step``, row i drawn on row id ``rows[i]``
+    (default i) (near-ties exempt).  ``row_sensitive``: also require that the definition at row ids rows + 1 draws another
+    action on some clear row, so that scores whose spread leaves no room for the noise cannot hide a draw on the wrong
+    row id."""
     if n_actions == 1:
         assert (actions == 0).all()
         return
-    v = gumbel_scores(scores, seed, step, n_actions)
+    v = gumbel_scores(scores, seed, step, n_actions, rows)
     top2 = np.sort(v, 1)[:, -2:]
     clear = top2[:, 1] - top2[:, 0] > 1e-4  # libm and the device logf differ in the last bits: near-ties may flip
     assert clear.mean() > 0.995 and np.array_equal(actions[clear], v.argmax(1)[clear])
+    if row_sensitive:
+        ids = (np.arange(len(scores)) if rows is None else np.asarray(rows, np.int64)) + 1
+        other = gumbel_scores(scores, seed, step, n_actions, ids).argmax(1)
+        assert (other[clear] != v.argmax(1)[clear]).any(), "the draw does not depend on the row id"
     assert actions.min() >= 0 and actions.max() < n_actions
 
 

@@ -65,11 +65,25 @@ K11_CASES = [  # (n_rows, n_actions, reset, in_place)
 
 @pytest.mark.parametrize("n_rows,n_actions,reset,in_place", K11_CASES)
 def test_k11_exact(n_rows, n_actions, reset, in_place):
+    _k11_check(n_rows, n_actions, reset, in_place)
+
+
+@pytest.mark.parametrize("n_rows,n_actions,reset,in_place", K11_CASES)
+def test_k11_view_exact(n_rows, n_actions, reset, in_place):
+    """ovc_lstm_head_view: row r is one agent's row of environment r, reset by reset[r], drawn on its joint row
+    2 r + seat ^ (swap[r] != 0) (actions [2 n_rows]: the other seat untouched); the state and the other outputs at r."""
+    _k11_check(n_rows, n_actions, reset, in_place, seat=n_rows % 2)
+
+
+def _k11_check(n_rows, n_actions, reset, in_place, seat=None):
     rng = np.random.RandomState(n_rows + 7 * n_actions)
     x, h, c, w, b, wo, bo = _k11_operands(rng, n_rows)
-    n_envs = (n_rows + 1) // 2
+    n_envs = (n_rows + 1) // 2 if seat is None else n_rows
     rs = {None: None, "none": np.zeros(n_envs), "all": np.ones(n_envs), "mixed": rng.rand(n_envs) < 0.4}[reset]
-    zero = np.zeros(n_rows, bool) if rs is None else np.repeat(rs != 0, 2)[:n_rows]
+    zero = np.zeros(n_rows, bool) if rs is None else (rs != 0 if seat is not None else np.repeat(rs != 0, 2)[:n_rows])
+    swap = None if seat is None or n_rows % 3 == 0 else rng.randint(0, 3, size=n_rows).astype(np.int32)
+    r = np.arange(n_rows)
+    d = r if seat is None else 2 * r + (seat ^ (0 if swap is None else (swap != 0).astype(np.int64)))
     hu, cu = np.where(zero[:, None], 0, h), np.where(zero[:, None], 0, c)
     z, cert = P.linear(np.concatenate([x, hu], 1), w, b)
     assert cert.holds(), "premise: the gate accumulations are not exact in float32"
@@ -91,7 +105,7 @@ def test_k11_exact(n_rows, n_actions, reset, in_place):
         co, fco = _guarded(n_rows, torch.float32, float("nan"), (CELL,))
     sh, fsh = _guarded(n_rows, torch.bfloat16, float("nan"), (CELL,))
     sc_, fsc = _guarded(n_rows, torch.float32, float("nan"), (CELL,))
-    acts, fa = _guarded(n_rows, torch.int32, -7)
+    acts, fa = _guarded(n_rows if seat is None else 2 * n_rows, torch.int32, -7)
     vals, fv = _guarded(n_rows, torch.float32, float("nan"))
     lp, fl = _guarded(n_rows, torch.float32, float("nan"))
     s8, fs8 = _guarded(n_rows, torch.float32, float("nan"), (8,))
@@ -100,15 +114,23 @@ def test_k11_exact(n_rows, n_actions, reset, in_place):
     seed = 0xABCD + n_rows
     step0 = 2 ** 32 - 1 if n_rows == 129 else 5  # the draw step crossing 2^32
     counter = torch.tensor([step0, 0], dtype=torch.int64, device="cuda")
-    _native.check(_native.lib().ovc_lstm_head(
-        tx.data_ptr(), th.data_ptr(), tc.data_ptr(), 0 if treset is None else treset.data_ptr(), n_rows, tw.data_ptr(), tb.data_ptr(),
-        two.data_ptr(), tbo.data_ptr(), n_actions, seed, counter.data_ptr(), ho.data_ptr(), co.data_ptr(), sh.data_ptr(), sc_.data_ptr(),
-        acts.data_ptr(), vals.data_ptr(), lp.data_ptr(), s8.data_ptr(), 0))
+    head = (tx.data_ptr(), th.data_ptr(), tc.data_ptr(), 0 if treset is None else treset.data_ptr(), n_rows, tw.data_ptr(), tb.data_ptr(),
+            two.data_ptr(), tbo.data_ptr(), n_actions, seed, counter.data_ptr())
+    tail = (ho.data_ptr(), co.data_ptr(), sh.data_ptr(), sc_.data_ptr(), acts.data_ptr(), vals.data_ptr(), lp.data_ptr(), s8.data_ptr(), 0)
+    if seat is None:
+        _native.check(_native.lib().ovc_lstm_head(*head, *tail))
+    else:
+        tswap = None if swap is None else _dev(swap, torch.int32)
+        _native.check(_native.lib().ovc_lstm_head_view(*head, 0 if tswap is None else tswap.data_ptr(), seat, *tail))
     torch.cuda.synchronize()
     assert _np(counter).tolist() == [step0 + 1, 0]
-    for full, fill in ((fho, float("nan")), (fco, float("nan")), (fsh, float("nan")), (fsc, float("nan")), (fa, -7), (fv, float("nan")),
+    for full, fill in ((fho, float("nan")), (fco, float("nan")), (fsh, float("nan")), (fsc, float("nan")), (fv, float("nan")),
                        (fl, float("nan")), (fs8, float("nan"))):
         assert _untouched(full, n_rows, fill)
+    a_all = _np(fa)
+    rest = np.ones(len(a_all), bool)
+    rest[d] = False
+    assert (a_all[rest] == -7).all(), "an action outside the rows' joint rows was written"
     if not in_place:
         assert torch.equal(th, h_in0) and torch.equal(tc, c_in0)
     # snapshots: the state the row used
@@ -131,8 +153,8 @@ def test_k11_exact(n_rows, n_actions, reset, in_place):
     ex = hc.exact()
     assert np.array_equal(s[ex], s_want[ex]) and (np.abs(s - s_want) <= 2.0 ** -20 * hc.abs_sum).all()
     assert np.array_equal(_np(vals), _np(s8)[:, n_actions])
-    P.check_draw(_np(acts), s, seed, step0, n_actions)
-    P.check_logp(_np(lp), s, _np(acts), n_actions)
+    P.check_draw(a_all[d], s, seed, step0, n_actions, rows=d)
+    P.check_logp(_np(lp), s, a_all[d], n_actions)
 
 
 def _gate_columns():
