@@ -792,10 +792,9 @@ class _Rollout(object):
     keep_logits)`` and ``_agents()`` (its policies); it sets ``population``, ``_pop`` (the population, or None) and
     ``_member``."""
 
-    _pair_play = False  # SelfPlayRollout's population play: its episode records hold each episode's pair
-
-    def _init_rollout(self, env, learner, use_graph, reward_shaping_factor, episode_capacity, max_seq_len):
-        """The shared state; ``learner`` is the policy whose LSTM state (if any) the bootstrap step leaves alone."""
+    def _init_rollout(self, env, learner, use_graph, reward_shaping_factor, episode_capacity, max_seq_len, pairs=False):
+        """The shared state; ``learner`` is the policy whose LSTM state (if any) the bootstrap step leaves alone, ``pairs``
+        (population play) makes the episode records hold each episode's pair."""
         N, dev = env.n_envs, env.device
         self.use_graph = use_graph
         self.actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
@@ -803,7 +802,7 @@ class _Rollout(object):
         self.factor = float(reward_shaping_factor)
         self._factor = torch.full((1,), self.factor, dtype=torch.float32, device=dev)  # read by the captured graphs
         self.stats = EpisodeStats(env)
-        self.episodes = EpisodeRecords(env, episode_capacity, members=self.population, pairs=self._pair_play)
+        self.episodes = EpisodeRecords(env, episode_capacity, members=self.population, pairs=pairs)
         self.max_seq_len = int(max_seq_len)
         assert self.max_seq_len >= 1
         self.graph = None          # run()'s CUDA graph of one transition
@@ -968,75 +967,28 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         instead of ``sparse + reward_shaping_factor * shaped_i``.  Only the rewards, the returns, the advantages, the value
         targets and the episodes' reward sums change; the draws, the states and the game statistics are those without it.
         Needs an ``auto_reset`` env.
-        model may instead be a population of self-play learners (fictitious co-play's first stage): a list of 1..64
-        ``RllibShapedCNN`` members of one architecture.  Member k plays both views of the environments of its block
-        ``[blocks[k], blocks[k + 1])``; blocks (argument): K positive environment counts summing to N, default equal blocks
-        (``blocks[k] = k N // K``).  ``self.blocks`` is then the offsets (int32 [K + 1]) and ``self.member`` the member of
-        each environment (int32 [N]).  The fused layers run as one grouped launch each for all members
-        (``ovc_encode_linear_grouped``, ``ovc_wide_layers_grouped`` from ``GROUPED_K9_MIN_MEMBERS`` members on,
-        ``ovc_policy_tail_grouped``), library layers per member on its block's rows; every row is drawn with key ``seed``
-        and the one counter (grouped K8, or, without K8, one ``ovc_sample_actions`` over all rows): block k is bit
-        for bit what ``SelfPlayRollout(env, model[k], seed=seed)`` does on those environments.  ``sync_weights()`` refolds
-        every member.  Not with a ``partner`` or an ``RllibLSTMShapedCNN`` member.
-        pairs, pair_weights: population play for a list model instead of blocks: member ``pair[e, 0]`` plays player 0 of
-        environment e and member ``pair[e, 1]`` player 1, and every row is a learner's row.  ``pairs`` (int32 [N, 2] on the
-        environments' device) fixes the pairing (the evaluation form: a cross-play matrix through run()); ``pair_weights``
-        (K x K non-negative floats with a positive sum; see the property) draws the ordered pair (i, j) with probability
-        proportional to ``pair_weights[i][j]`` at construction and at every episode end (the training form: uniform weights
-        are PBT-style population play, a zero diagonal excludes self-play).  ``self.pair`` (int32 [N, 2]) is the live pairing.
-        Per transition ``ovc_group_pairs`` groups the entries by member on the device, then ``ovc_encode_linear_grouped_masked``
-        (the object part once per environment), K9 (grouped from ``GROUPED_K9_MIN_MEMBERS`` members on, else per member on
-        its compact rows; off K9 each member's library layers on all compact rows, its own rows selected on the device) and
-        ``ovc_policy_tail_grouped_joint`` (off K8: the library heads and one ``ovc_sample_actions`` over the joint rows).
-        Every row is drawn with key ``seed`` on the one counter at its joint row ``2 e + v``, so copies of one model draw
-        exactly what ``SelfPlayRollout(env, model)`` draws; the pair draw uses key ``seed ^ PAIR_SALT`` and a counter of its
-        own.  collect()'s batches carry ``pair`` and ``episodes.finished()`` reports each episode's ``pair``.  Needs K7 (at
-        most 8 layouts, a grid within its shared memory) and the bf16 policy; not with ``blocks``, a ``partner`` or an LSTM
-        member."""
+        model may instead be a population of self-play learners: a list of 1..64 ``RllibShapedCNN`` members of one
+        architecture, each playing both views of its block of environments (``blocks``), or paired per environment
+        (population play: ``pairs`` or ``pair_weights``).  See ``_Learners`` for both forms; ``self.blocks``, ``self.member``,
+        ``self.pair`` and ``self.pair_weights`` describe the population, and ``sync_weights()`` refolds every member.  Not
+        with a ``partner`` or an ``RllibLSTMShapedCNN`` member."""
         self.env = env
+        self.seed = int(seed)
         models = list(model) if isinstance(model, (list, tuple)) else None
-        pair_play = pairs is not None or pair_weights is not None
-        if pair_play:
-            assert models is not None, "pairs / pair_weights go with a population of learners (a list model)"
-            assert pairs is None or pair_weights is None, "pairs fixes each environment's pair, pair_weights draws it: pass one of them"
-            assert blocks is None, "population play pairs the members per environment: pass no blocks with pairs / pair_weights"
-            assert partner is None, "population play has no partner: every row is a learner's"
-            assert autocast_dtype == torch.bfloat16, "population play runs K7 and K8 on the bf16 policy: autocast_dtype=None is not supported"
-            _check_members(models, MAX_MEMBERS, RllibShapedCNN, "a population of learners has 1..%d members" % MAX_MEMBERS,
-                           "a population learner is an RllibShapedCNN (an LSTM member is not supported)")
-            K, N = len(models), env.n_envs
-            if pairs is not None:
-                assert isinstance(pairs, torch.Tensor) and pairs.dtype == torch.int32 and tuple(pairs.shape) == (N, 2) and \
-                    pairs.is_contiguous(), "pairs: a contiguous int32 tensor [N, 2] (N = %d environments)" % N
-                assert pairs.device == env.device, "pairs: on the environments' device (%s), got %s" % (env.device, pairs.device)
-                lo, hi = int(pairs.min()), int(pairs.max())
-                assert 0 <= lo and hi < K, "pairs values must lie in [0, %d): found %d..%d" % (K, lo, hi)
-            else:
-                pair_thresholds(pair_weights, K)
-        self._pair_play = pair_play
         self._phi = _PhiReward(env) if use_phi else None
-        if models is not None:
-            _check_members(models, MAX_MEMBERS, RllibShapedCNN, "a population of learners has 1..%d members" % MAX_MEMBERS,
-                           "a population learner is an RllibShapedCNN (an LSTM member is not supported)")
-            arch = lambda m: (m.dense_slope,) + tuple((n, tuple(p.shape)) for n, p in m.named_parameters())
-            assert len({arch(m) for m in models}) == 1, "the members of a population of learners must share one architecture"
-            assert partner is None, "a population of learners plays self-play only: no partner with a list model"
-        else:
+        if models is None:
+            assert pairs is None and pair_weights is None, "pairs / pair_weights go with a population of learners (a list model)"
             assert blocks is None, "blocks go with a population of learners (a list model)"
-        self._fold(env, models[0] if models else model, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
-        if pair_play:
-            assert self.fused_first_layer, \
-                "population play needs K7: a first layer width a multiple of 64, a grid whose table fits shared memory, and at " \
-                "most %d layouts (this environment has %d layouts on a %dx%d grid)" % (K7_MAX_LAYOUTS, env.n_layouts, self.W, self.H)
+            self._fold(env, model, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
+            self._learners = None
+        else:
+            assert partner is None, "population play has no partner: every row is a learner's" \
+                if pairs is not None or pair_weights is not None else "a population of learners plays self-play only: no partner with a list model"
+            self._learners = _Learners(self, models, blocks, pairs, pair_weights, autocast_dtype, fused_first_layer, fused_tail, fused_wide)
+        L = self._learners  # the block offsets and each environment's member (blocks), the live pairing (population play)
+        self.blocks, self._member, self.pair = (None, None, None) if L is None else (L.blocks, L.member, L.pair)
         dev = env.device
         N = env.n_envs
-        self.seed = int(seed)
-        self._others = None  # a population of learners: members 1.. folded (member 0 is self)
-        self._member = None
-        if models is not None:
-            self._fold_members(models, blocks, autocast_dtype)
-        if pair_play:
-            self._init_pairs(pairs, pair_weights)
         self.partner = partner
         self.bc = float(bc_factor)
         self.population = isinstance(partner, (list, tuple))
@@ -1069,13 +1021,11 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         self.ret_mixed = torch.zeros(N, dtype=torch.float32, device=dev)    # sparse + factor * shaped (rllib.py:328-329)
         self.values = torch.zeros((N, 2), dtype=torch.float32, device=dev)
         self.native_glue = True  # the draw and the returns are always native kernels; bench.py's launch count reads this
-        self._init_rollout(env, self, use_graph, reward_shaping_factor, episode_capacity, max_seq_len)
+        self._init_rollout(env, self, use_graph, reward_shaping_factor, episode_capacity, max_seq_len, pairs=self.pair is not None)
         self._draw_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of ovc_sample_actions
         self._scores8 = None  # set to a float32 [2N, 8] tensor to make K8 also write the heads (tests)
         if partner is not None:
             self._assign_seats(None)
-        if pair_play and pairs is None:
-            self._assign_pairs(None, None)
         if isinstance(self._partner, _Population):
             if self._partner.needs_obs and self.obs is None:
                 self.obs = torch.empty((N, 2, self.W, self.H, 26), dtype=autocast_dtype or torch.float32, device=dev)
@@ -1103,175 +1053,17 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         self._bc_factor.fill_(self.bc)
 
     @property
-    def _members(self):
-        """A population of learners: the K folded members, self first; else None.  Built on access: a list holding self
-        would make the rollout a reference cycle, freed by the garbage collector at any later point, possibly inside
-        another rollout's graph capture, which its graphs' destruction would then invalidate."""
-        return None if self._others is None else [self] + self._others
-
-    def _fold_members(self, models, blocks, autocast_dtype):
-        """A population of learners: fold members 1.. like member 0 (self), set the blocks, and stack the K8 tables so that
-        each member's tables are views of the stack (its ``sync_weights`` then refreshes the stack in place)."""
-        env, N, dev, K = self.env, self.env.n_envs, self.env.device, len(models)
-        if not self._pair_play:
-            if blocks is None:
-                assert N >= K, "equal blocks need at least one environment per member (%d members, %d environments)" % (K, N)
-                counts = [(k + 1) * N // K - k * N // K for k in range(K)]
-            else:
-                counts = [int(b) for b in blocks]
-                assert len(counts) == K, "blocks: one environment count per member (%d)" % K
-                assert all(c > 0 for c in counts) and sum(counts) == N, \
-                    "blocks: positive environment counts summing to the %d environments, got %s" % (N, counts)
-            self._offs = [0] + np.cumsum(counts).tolist()
-            self.blocks = torch.tensor(self._offs, dtype=torch.int32, device=dev)
-            self._row_offsets = 2 * self.blocks  # K8's offsets are joint rows
-            self._member = torch.repeat_interleave(torch.arange(K, dtype=torch.int32, device=dev),
-                                                   torch.tensor(counts, device=dev)).to(torch.int32)
-        self._others = []
-        for m in models[1:]:
-            f = _FoldedPolicy()
-            f.env = env
-            f._fold(env, m, autocast_dtype, self.fused_first_layer, self.fused_tail, self.fused_wide)
-            self._others.append(f)
-        def stack(attr):  # the grouped kernels' stacked tables; each member's tables become views of them
-            st = tuple(torch.stack([getattr(f, attr)[i] for f in self._members]) for i in range(len(getattr(self, attr))))
-            for k, f in enumerate(self._members):
-                setattr(f, attr, tuple(t[k] for t in st))
-            return st
-        if self.fused_first_layer:
-            self._k7_stack = (torch.stack([f._wt0 for f in self._members]), torch.stack([f._b0 for f in self._members]))
-            for k, f in enumerate(self._members):
-                f._wt0, f._b0 = self._k7_stack[0][k], self._k7_stack[1][k]
-        if self.fused_wide:
-            self._wide_stack = stack("_wide")
-        if self.fused_tail:
-            self._tail_stack = stack("_tail")
-
-    def _policy_members(self, actions, vals, logp, scores8, counter):
-        """``_policy`` for a population of learners: grouped K7, K9 (from ``GROUPED_K9_MIN_MEMBERS`` members on, else K9 per
-        member on its block) and grouped K8 (None returned); off the fused path, library layers per member on its block's rows
-        ``[2 o_k, 2 o_{k+1})`` and, without K8, member k's logits into its rows of self._scores (returned for the one draw
-        kernel over all rows)."""
-        env, lib, rows = self.env, _native.lib(), 2 * self.env.n_envs
-        with torch.no_grad():
-            if self.fused_first_layer:  # grouped K7
-                wt, b0 = self._k7_stack
-                _native.check(lib.ovc_encode_linear_grouped(
-                    env.tables.data_ptr(), env.n_layouts, env.state.data_ptr(), wt.data_ptr(), b0.data_ptr(), self.blocks.data_ptr(),
-                    len(self._members), self._act0.data_ptr(), env.n_envs, env.state_words, self.W, self.H,
-                    env.horizon if env.horizon > 0 else 2**31 - 1, wt.shape[2], 0.2, env._stream()))
-                flat, first = self._act0, 1
-            else:
-                flat, first = self.obs.view(rows, self.W * self.H * 26), 0
-            if self.fused_wide and len(self._members) >= GROUPED_K9_MIN_MEMBERS:  # grouped K9
-                _native.check(lib.ovc_wide_layers_grouped(*self._k9_args(flat, self._wide_stack), self._row_offsets.data_ptr(),
-                                                          len(self._members), self._z.data_ptr(), env._stream()))
-            for k, f in enumerate(self._members):  # per member on its block's rows [2 o_k, 2 o_{k+1})
-                r = slice(2 * self._offs[k], 2 * self._offs[k + 1])
-                if self.fused_wide and len(self._members) < GROUPED_K9_MIN_MEMBERS:  # K9 on the block
-                    _native.check(lib.ovc_wide_layers(*f._k9_args(flat[r]), self._z[r].data_ptr(), env._stream()))
-                elif not self.fused_tail:  # library layers; bit for bit the member's own rollout only where cuBLAS computes a
-                    # row independently of the row count (tested at up to 2 x 300 rows per call)
-                    logits, value = f.dense_model.forward_from(flat[r], first)
-                    self._scores[r].copy_(logits)
-                    vals[r].copy_(value)
-                elif not self.fused_wide:
-                    f.dense_model.trunk(flat[r], first, out=self._z[r])
-            if not self.fused_tail:
-                return self._scores
-            ptr = lambda t: 0 if t is None else t.data_ptr()
-            _native.check(lib.ovc_policy_tail_grouped(
-                *self._k8_args(self._z, self._tail_stack), counter.data_ptr(), self._row_offsets.data_ptr(), len(self._members),
-                actions.data_ptr(), vals.data_ptr(), ptr(scores8), ptr(logp), env._stream()))
-        return None
-
-    def _init_pairs(self, pairs, pair_weights):
-        """Population play's state: the live pairing, its draw, and the compact layout ``ovc_group_pairs`` writes."""
-        N, dev, K = self.env.n_envs, self.env.device, len(self._members)
-        i32 = lambda n: torch.zeros(n, dtype=torch.int32, device=dev)
-        self._pair_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of the pair draw
-        if pairs is not None:
-            self.pair, self._pair_thresholds = pairs, None
-        else:
-            self.pair = torch.zeros((N, 2), dtype=torch.int32, device=dev)
-            self._pair_thresholds = torch.zeros(max(K * K - 1, 1), dtype=torch.int64, device=dev)  # never NULL: NULL skips the draw
-            self.pair_weights = [[1.0] * K for _ in range(K)] if pair_weights is None else pair_weights
-        self._plist, self._pfirst, self._pjrow = i32(2 * N), i32(2 * N), i32(2 * N)
-        self._entry_offsets, self._pair_row_offsets = i32(K + 1), i32(K + 1)
-        self._logp = torch.empty(2 * N, dtype=torch.float32, device=dev)  # run()'s logp: the joint K8 always writes it
-        if not self.fused_wide:  # the member of each compact row, for the library layers' selection
-            self._rmember = torch.empty(2 * N, dtype=torch.int64, device=dev)
-            self._rindex = torch.arange(2 * N, device=dev)
-        if not self.fused_tail:  # the library heads on compact rows, scattered to the joint rows for the draw kernel
-            self._jrow64 = torch.empty(2 * N, dtype=torch.int64, device=dev)
-            self._cscores = torch.zeros((2 * N, self.dense_model.n_actions), dtype=torch.float32, device=dev)
-            self._cvalues = torch.zeros(2 * N, dtype=torch.float32, device=dev)
-
-    @property
     def pair_weights(self):
         """Population play's pair weights (K x K non-negative floats with a positive sum; entry [i][j] weighs member i on
         player 0 next to member j on player 1).  Setting them rewrites the device thresholds the pair draw reads, so run() and
         collect() follow the new weights at the next episode ends without a re-capture."""
-        assert self._pair_play and self._pair_thresholds is not None, "pair_weights: population play with drawn pairs"
-        return [list(r) for r in self._pair_weights]
+        assert self.pair is not None and self._learners._thresholds is not None, "pair_weights: population play with drawn pairs"
+        return self._learners.pair_weights
 
     @pair_weights.setter
     def pair_weights(self, value):
-        assert self._pair_play and self._pair_thresholds is not None, "pair_weights: population play with drawn pairs"
-        K = len(self._members)
-        thr = pair_thresholds(value, K)
-        self._pair_weights = np.asarray(value, dtype=np.float64).tolist()
-        self._pair_thresholds[:K * K - 1].copy_(torch.from_numpy(thr))
-
-    def _assign_pairs(self, done, records):
-        """After K1: the ending episodes' pair into ``records``, then (drawn pairs) a new pair; done None: every environment,
-        no record (construction)."""
-        drawn = self._pair_thresholds is not None
-        self.env.assign_pairs(self.pair, len(self._members), self._pair_thresholds, self._pair_counter if drawn else None,
-                              seed=self.seed ^ PAIR_SALT, done=done, records=records)
-
-    def _policy_pairs(self, actions, vals, logp, scores8, counter):
-        """``_policy`` for population play: ``ovc_group_pairs``, grouped masked K7 into compact rows, K9 (grouped from
-        ``GROUPED_K9_MIN_MEMBERS`` members on, else per member on its compact rows), grouped joint K8 (None returned).  Off
-        K9, each member's library layers run on all compact rows and its rows are selected by the row's member (no host
-        synchronisation); off K8, the heads are scattered to the joint rows of self._scores (returned for the draw kernel)."""
-        env, lib, st, K, rows = self.env, _native.lib(), self.env._stream(), len(self._members), 2 * self.env.n_envs
-        with torch.no_grad():
-            env.group_pairs(self.pair, K, self._plist, self._pfirst, self._pjrow, self._entry_offsets, self._pair_row_offsets)
-            wt, b0 = self._k7_stack
-            _native.check(lib.ovc_encode_linear_grouped_masked(
-                env.tables.data_ptr(), env.n_layouts, env.state.data_ptr(), self._plist.data_ptr(), self._pfirst.data_ptr(),
-                wt.data_ptr(), b0.data_ptr(), self._entry_offsets.data_ptr(), K, self._act0.data_ptr(), rows, env.state_words, self.W,
-                self.H, env.horizon if env.horizon > 0 else 2**31 - 1, wt.shape[2], 0.2, st))
-            flat = self._act0
-            if self.fused_wide and K >= GROUPED_K9_MIN_MEMBERS:
-                _native.check(lib.ovc_wide_layers_grouped(*self._k9_args(flat, self._wide_stack), self._pair_row_offsets.data_ptr(), K,
-                                                          self._z.data_ptr(), st))
-            elif self.fused_wide:
-                for k, f in enumerate(self._members):
-                    _native.check(lib.ovc_wide_layers_range(*f._k9_args(flat), self._pair_row_offsets[k:k + 2].data_ptr(),
-                                                            self._z.data_ptr(), st))
-            else:  # library layers per member on every compact row; bit for bit the member's own rollout only where cuBLAS
-                # computes a row independently of the other rows
-                torch.searchsorted(self._pair_row_offsets[1:], self._rindex, right=True, out=self._rmember)
-                for k, f in enumerate(self._members):
-                    mine = (self._rmember == k).unsqueeze(1)
-                    if self.fused_tail:
-                        torch.where(mine, f.dense_model.trunk(flat, 1), self._z, out=self._z)
-                    else:
-                        logits, value = f.dense_model.forward_from(flat, 1)
-                        torch.where(mine, logits.float(), self._cscores, out=self._cscores)
-                        torch.where(mine[:, 0], value.float(), self._cvalues, out=self._cvalues)
-            if not self.fused_tail:
-                self._jrow64.copy_(self._pjrow)
-                self._scores.index_copy_(0, self._jrow64, self._cscores)
-                vals.index_copy_(0, self._jrow64, self._cvalues)
-                return self._scores
-            _native.check(lib.ovc_policy_tail_grouped_joint(
-                *self._k8_args(self._z, self._tail_stack), counter.data_ptr(), self._pjrow.data_ptr(), self._pair_row_offsets.data_ptr(), K,
-                actions.data_ptr(), vals.data_ptr(), 0 if scores8 is None else scores8.data_ptr(),
-                (self._logp if logp is None else logp).data_ptr(), st))
-        return None
+        assert self.pair is not None and self._learners._thresholds is not None, "pair_weights: population play with drawn pairs"
+        self._learners.pair_weights = value
 
     def sync_weights(self):
         """Re-fold the learner (``_FoldedPolicy.sync_weights``), the partner (a network partner, every population member, or
@@ -1280,8 +1072,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         _FoldedPolicy.sync_weights(self)
         if self._partner is not None:
             self._partner.sync_weights()
-        for f in self._others or []:
-            f.sync_weights()
+        if self._learners is not None:
+            self._learners.sync_weights()
 
     def _agents(self):
         return [self]
@@ -1292,8 +1084,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
             live += [self.h, self.c, self.env.done]  # env.done: the next transition's LSTM reset
         if self.partner is not None:
             live += [self.partner_seat, self._seat_counter] + self._partner.live()
-        if self._pair_play:
-            live += [self.pair, self._pair_counter]
+        if self._learners is not None:
+            live += self._learners.live()
         return live
 
     def _policy(self, actions=None, values=None, logp=None, scores8=None, counter=None, state_out=None, snap=None):
@@ -1307,10 +1099,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         vals = self.values.view(rows) if values is None else values
         scores8 = self._scores8 if scores8 is None else scores8
         counter = self._draw_counter if counter is None else counter
-        if self._pair_play:
-            return self._policy_pairs(actions, vals, logp, scores8, counter)
-        if self._members is not None:
-            return self._policy_members(actions, vals, logp, scores8, counter)
+        if self._learners is not None:
+            return self._learners.act(self, actions, vals, logp, scores8, counter)
         with torch.no_grad():
             if self.fused_first_layer:
                 flat = env.encoded_linear(self._wt0, self._b0, out=self._act0, neg_slope=0.2)  # K7
@@ -1342,7 +1132,7 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
             b.states[t].copy_(env.state)
             actions, values, logp, rewards, dones = b.actions[t], b.values[t], b.logp[t], b.rewards[t], b.dones[t]
             logits = None if b.logits is None else b.logits[t]
-            if self._pair_play:
+            if b.pair is not None:
                 b.pair[t].copy_(self.pair)
         if self.obs is not None:
             env.lossless_state_encoding(out=self.obs)  # K2
@@ -1367,8 +1157,8 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         dense = _env_step(env, actions.view(env.n_envs, 2), self._phi)
         if self.population:  # before the record: both use the slot count[e] the ending episode goes to
             self._pop.assign(env.done, self.episodes if b is None else b.episodes)
-        if self._pair_play:  # before the record, likewise
-            self._assign_pairs(env.done, self.episodes if b is None else b.episodes)
+        if self._learners is not None:  # before the record, likewise
+            self._learners.assign(env.done, self.episodes if b is None else b.episodes)
         # the seat draw below runs after this kernel, so partner_seat is still the ending episode's
         env.record_transition(self._factor, rewards=rewards, dones=dones, ret_sparse=self.ret_sparse, ret_mixed=self.ret_mixed,
                               stats=self.stats, records=self.episodes if b is None else b.episodes,
@@ -1389,7 +1179,7 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         where the learner runs on its own rows only, not written); ``partner_member`` is meaningful where ``partner_seat >=
         0``.  A seat changes hands only at a done, where GAE cuts, so a learner row's advantages never read a partner step."""
         return SampleBatch(self.env, n_steps, keep_logits, partner=self.partner is not None,
-                           seq_len=self.max_seq_len if self.lstm else None, members=self.population, pairs=self._pair_play)
+                           seq_len=self.max_seq_len if self.lstm else None, members=self.population, pairs=self.pair is not None)
 
     def env_only(self, n_steps):
         """The same transitions without the policy: encode + step with the last sampled actions
@@ -1495,9 +1285,10 @@ MAX_MEMBERS = 64  # ovc_group_members / ovc_assign_members
 def member_thresholds(weights):
     """The table ``ovc_assign_members`` draws a member from: int64 [K - 1] with entry k = floor(cdf[k] * 2^32), cdf[k] the
     float64 share of members 0..k in ``weights`` (K non-negative floats with a positive sum).  A member of weight 0 is never
-    drawn: its entry equals the one before (or is 0 for member 0, 2^32 after the last positive weight)."""
+    drawn: its entry equals the one before (or is 0 for member 0, 2^32 after the last positive weight).  K is not bounded
+    here (``pair_thresholds`` passes K^2 pair weights): a population's size is checked where it is built."""
     w = np.asarray(weights, dtype=np.float64)
-    assert w.ndim == 1 and 1 <= w.size <= MAX_MEMBERS, "between 1 and %d member weights" % MAX_MEMBERS
+    assert w.ndim == 1, "member weights: one flat list, one weight per member"
     assert np.all(np.isfinite(w)) and np.all(w >= 0) and w.sum() > 0, "member weights: finite, non-negative, a positive sum"
     c = np.cumsum(w)
     return np.floor(c[:-1] / c[-1] * 2.0**32).astype(np.int64)
@@ -1514,9 +1305,7 @@ def pair_thresholds(weights, n_members):
     w = np.asarray(weights, dtype=np.float64)
     K = int(n_members)
     assert w.shape == (K, K), "pair_weights: a %d x %d array (one weight per ordered pair of members), got shape %s" % (K, K, w.shape)
-    assert np.all(np.isfinite(w)) and np.all(w >= 0) and w.sum() > 0, "pair weights: finite, non-negative, a positive sum"
-    c = np.cumsum(w.ravel())
-    return np.floor(c[:-1] / c[-1] * 2.0**32).astype(np.int64)
+    return member_thresholds(w.ravel())
 
 
 class _Population(object):
@@ -1651,6 +1440,227 @@ class _Population(object):
                     logits, _ = a.dense_model.forward_from(flat, first)
                     a._scores.copy_(logits)
                     env.sample_actions_rows(a._scores, a._counter, 0, self.partner_seat, self.order, rng, seed=a.seed, out=actions)
+
+
+class _Learners(object):
+    """A population of self-play learners in one ``SelfPlayRollout`` (a list ``model``): K members (1..64
+    ``RllibShapedCNN``s of one architecture), every row a learner's, drawn with key ``seed`` on the rollout's one counter.
+    Member 0 is the rollout itself, passed in as ``first`` and never stored: a rollout that held itself would be a reference
+    cycle, freed by the garbage collector at any later point, possibly inside another rollout's graph capture, which its
+    graphs' destruction would then invalidate.  ``others`` are members 1.. folded like it, with the same kernels; their
+    K7 / K9 / K8 tables are views of the stacks the grouped kernels read, so ``sync_weights()`` refreshes the stacks in place.
+    Per transition ``act`` runs K9 on each member's rows as one grouped launch from ``GROUPED_K9_MIN_MEMBERS`` members on,
+    one launch per member below that.  The population takes one of two forms.
+
+    Blocks (fictitious co-play's first stage): member k plays both views of the environments of its block ``[blocks[k],
+    blocks[k + 1])``; blocks (argument): K positive environment counts summing to N, default equal blocks (``blocks[k] = k N
+    // K``).  ``blocks`` is then the offsets (int32 [K + 1]) and ``member`` the member of each environment (int32 [N]).  The
+    fused layers run as one grouped launch each for all members (``ovc_encode_linear_grouped``, K9, ``ovc_policy_tail_grouped``),
+    library layers per member on its block's rows; every row is drawn with the one counter (grouped K8, or, without K8, one
+    ``ovc_sample_actions`` over all rows): block k is bit for bit what ``SelfPlayRollout(env, model[k], seed=seed)`` does on
+    those environments.
+
+    Population play (``pairs`` or ``pair_weights``): member ``pair[e, 0]`` plays player 0 of environment e and member ``pair[e,
+    1]`` player 1.  ``pairs`` (int32 [N, 2] on the environments' device) fixes the pairing (the evaluation form: a cross-play
+    matrix through run()); ``pair_weights`` (K x K non-negative floats with a positive sum) draws the ordered pair (i, j) with
+    probability proportional to ``pair_weights[i][j]`` at construction and at every episode end (the training form: uniform
+    weights are PBT-style population play, a zero diagonal excludes self-play).  ``pair`` (int32 [N, 2]) is the live
+    pairing.  Per transition ``ovc_group_pairs`` groups the entries by member on the device, then
+    ``ovc_encode_linear_grouped_masked`` (the object part once per environment), K9 on each member's compact rows (off K9
+    each member's library layers on all compact rows, its own rows selected on the device) and
+    ``ovc_policy_tail_grouped_joint`` (off K8: the library heads and one ``ovc_sample_actions`` over the joint rows).  Every
+    row is drawn at its joint row ``2 e + v``, so copies of one model draw exactly what ``SelfPlayRollout(env, model)``
+    draws; the pair draw uses key ``seed ^ PAIR_SALT`` and a counter of its own.  collect()'s batches carry ``pair`` and
+    ``episodes.finished()`` reports each episode's ``pair``.  Needs K7 (at most 8 layouts, a grid within its shared memory)
+    and the bf16 policy; not with ``blocks``."""
+
+    def __init__(self, first, models, blocks, pairs, pair_weights, autocast_dtype, fused_first_layer, fused_tail, fused_wide):
+        """Check the arguments (see ``SelfPlayRollout.__init__``), fold member 0 into ``first`` (the rollout, with its
+        ``env`` and ``seed`` set) and the others alike, and stack their tables."""
+        env = self.env = first.env
+        K, N, dev = len(models), env.n_envs, env.device
+        self.K, self.seed = K, first.seed
+        pair_play = pairs is not None or pair_weights is not None
+        if pair_play:
+            assert pairs is None or pair_weights is None, "pairs fixes each environment's pair, pair_weights draws it: pass one of them"
+            assert blocks is None, "population play pairs the members per environment: pass no blocks with pairs / pair_weights"
+            assert autocast_dtype == torch.bfloat16, "population play runs K7 and K8 on the bf16 policy: autocast_dtype=None is not supported"
+        _check_members(models, MAX_MEMBERS, RllibShapedCNN, "a population of learners has 1..%d members" % MAX_MEMBERS,
+                       "a population learner is an RllibShapedCNN (an LSTM member is not supported)")
+        arch = lambda m: (m.dense_slope,) + tuple((n, tuple(p.shape)) for n, p in m.named_parameters())
+        assert len({arch(m) for m in models}) == 1, "the members of a population of learners must share one architecture"
+        if pairs is not None:
+            assert isinstance(pairs, torch.Tensor) and pairs.dtype == torch.int32 and tuple(pairs.shape) == (N, 2) and \
+                pairs.is_contiguous(), "pairs: a contiguous int32 tensor [N, 2] (N = %d environments)" % N
+            assert pairs.device == dev, "pairs: on the environments' device (%s), got %s" % (dev, pairs.device)
+            lo, hi = int(pairs.min()), int(pairs.max())
+            assert 0 <= lo and hi < K, "pairs values must lie in [0, %d): found %d..%d" % (K, lo, hi)
+        elif pair_play:
+            pair_thresholds(pair_weights, K)
+        elif blocks is None:
+            assert N >= K, "equal blocks need at least one environment per member (%d members, %d environments)" % (K, N)
+            counts = [(k + 1) * N // K - k * N // K for k in range(K)]
+        else:
+            counts = [int(b) for b in blocks]
+            assert len(counts) == K, "blocks: one environment count per member (%d)" % K
+            assert all(c > 0 for c in counts) and sum(counts) == N, \
+                "blocks: positive environment counts summing to the %d environments, got %s" % (N, counts)
+        first._fold(env, models[0], autocast_dtype, fused_first_layer, fused_tail, fused_wide)
+        assert not pair_play or first.fused_first_layer, \
+            "population play needs K7: a first layer width a multiple of 64, a grid whose table fits shared memory, and at " \
+            "most %d layouts (this environment has %d layouts on a %dx%d grid)" % (K7_MAX_LAYOUTS, env.n_layouts, first.W, first.H)
+        self.others = []
+        for m in models[1:]:
+            f = _FoldedPolicy()
+            f.env = env
+            f._fold(env, m, autocast_dtype, first.fused_first_layer, first.fused_tail, first.fused_wide)
+            self.others.append(f)
+        members = [first] + self.others
+
+        def stack(attr):  # the grouped kernels' stacked tables; each member's tables become views of them
+            st = tuple(torch.stack(ts) for ts in zip(*(getattr(f, attr) for f in members)))
+            for k, f in enumerate(members):
+                setattr(f, attr, tuple(t[k] for t in st))
+            return st
+        if first.fused_first_layer:
+            self._k7_stack = (torch.stack([f._wt0 for f in members]), torch.stack([f._b0 for f in members]))
+            for k, f in enumerate(members):
+                f._wt0, f._b0 = self._k7_stack[0][k], self._k7_stack[1][k]
+        if first.fused_wide:
+            self._wide_stack = stack("_wide")
+        if first.fused_tail:
+            self._tail_stack = stack("_tail")
+        self.blocks = self.member = self.pair = self._thresholds = None
+        if not pair_play:
+            self._offs = [0] + np.cumsum(counts).tolist()
+            self.blocks = torch.tensor(self._offs, dtype=torch.int32, device=dev)
+            self._row_offsets = 2 * self.blocks  # K9's and K8's offsets are joint rows
+            self.member = torch.repeat_interleave(torch.arange(K, dtype=torch.int32, device=dev),
+                                                  torch.tensor(counts, device=dev)).to(torch.int32)
+            return
+        # population play: the live pairing, its draw, and the compact layout ovc_group_pairs writes
+        i32 = lambda n: torch.zeros(n, dtype=torch.int32, device=dev)
+        self._counter = torch.zeros(2, dtype=torch.int64, device=dev)  # [step, scratch] of the pair draw
+        if pairs is not None:
+            self.pair = pairs
+        else:
+            self.pair = torch.zeros((N, 2), dtype=torch.int32, device=dev)
+            self._thresholds = torch.zeros(max(K * K - 1, 1), dtype=torch.int64, device=dev)  # never NULL: NULL skips the draw
+            self.pair_weights = pair_weights
+        self._plist, self._pfirst, self._pjrow = i32(2 * N), i32(2 * N), i32(2 * N)
+        self._entry_offsets, self._row_offsets = i32(K + 1), i32(K + 1)
+        self._logp = torch.empty(2 * N, dtype=torch.float32, device=dev)  # run()'s logp: the joint K8 always writes it
+        if not first.fused_wide:  # the member of each compact row, for the library layers' selection
+            self._rmember = torch.empty(2 * N, dtype=torch.int64, device=dev)
+            self._rindex = torch.arange(2 * N, device=dev)
+        if not first.fused_tail:  # the library heads on compact rows, scattered to the joint rows for the draw kernel
+            self._jrow64 = torch.empty(2 * N, dtype=torch.int64, device=dev)
+            self._cscores = torch.zeros((2 * N, first.dense_model.n_actions), dtype=torch.float32, device=dev)
+            self._cvalues = torch.zeros(2 * N, dtype=torch.float32, device=dev)
+        if pairs is None:
+            self.assign(None, None)
+
+    @property
+    def pair_weights(self):
+        return [list(r) for r in self._pair_weights]
+
+    @pair_weights.setter
+    def pair_weights(self, value):
+        thr = pair_thresholds(value, self.K)
+        self._pair_weights = np.asarray(value, dtype=np.float64).tolist()
+        self._thresholds[:self.K * self.K - 1].copy_(torch.from_numpy(thr))
+
+    def assign(self, done, records):
+        """After K1, in population play: the ending episodes' pair into ``records``, then (drawn pairs) a new pair; done
+        None: every environment, no record (construction).  Nothing for blocks."""
+        if self.pair is not None:
+            drawn = self._thresholds is not None
+            self.env.assign_pairs(self.pair, self.K, self._thresholds, self._counter if drawn else None, seed=self.seed ^ PAIR_SALT,
+                                  done=done, records=records)
+
+    def live(self):
+        """The tensors a transition advances (restored around graph capture)."""
+        return [] if self.pair is None else [self.pair, self._counter]
+
+    def sync_weights(self):
+        """Re-fold members 1.. in place (the rollout re-folds member 0)."""
+        for f in self.others:
+            f.sync_weights()
+
+    def act(self, first, actions, values, logp, scores8, counter):
+        """``SelfPlayRollout._policy`` for the population, in ``first``'s buffers: grouped K7 (blocks), or ``ovc_group_pairs``
+        then the grouped masked K7 into compact rows; K9 on each member's rows; grouped K8 (blocks) or grouped joint K8 (None
+        returned).  Off K7 (blocks only) the layers start from K2's observation ``first.obs``; off K9 the library layers run
+        per member on its block's rows, or on every compact row with its own rows selected on the device (no host
+        synchronisation); off K8 the logits go to the joint rows of ``first._scores``, returned for the one draw kernel over
+        all rows."""
+        env, lib, st, K, rows = self.env, _native.lib(), self.env._stream(), self.K, 2 * self.env.n_envs
+        members = [first] + self.others
+        block = lambda k: slice(2 * self._offs[k], 2 * self._offs[k + 1])  # member k's rows [2 o_k, 2 o_{k+1}) (blocks)
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        horizon = env.horizon if env.horizon > 0 else 2**31 - 1
+        with torch.no_grad():
+            if self.pair is not None:
+                env.group_pairs(self.pair, K, self._plist, self._pfirst, self._pjrow, self._entry_offsets, self._row_offsets)
+            if first.fused_first_layer:
+                wt, b0 = self._k7_stack
+                if self.pair is None:
+                    _native.check(lib.ovc_encode_linear_grouped(
+                        env.tables.data_ptr(), env.n_layouts, env.state.data_ptr(), wt.data_ptr(), b0.data_ptr(), self.blocks.data_ptr(),
+                        K, first._act0.data_ptr(), env.n_envs, env.state_words, first.W, first.H, horizon, wt.shape[2], 0.2, st))
+                else:
+                    _native.check(lib.ovc_encode_linear_grouped_masked(
+                        env.tables.data_ptr(), env.n_layouts, env.state.data_ptr(), self._plist.data_ptr(), self._pfirst.data_ptr(),
+                        wt.data_ptr(), b0.data_ptr(), self._entry_offsets.data_ptr(), K, first._act0.data_ptr(), rows, env.state_words,
+                        first.W, first.H, horizon, wt.shape[2], 0.2, st))
+                flat, lib_first = first._act0, 1
+            else:
+                flat, lib_first = first.obs.view(rows, first.W * first.H * 26), 0
+            if first.fused_wide and K >= GROUPED_K9_MIN_MEMBERS:
+                _native.check(lib.ovc_wide_layers_grouped(*first._k9_args(flat, self._wide_stack), self._row_offsets.data_ptr(), K,
+                                                          first._z.data_ptr(), st))
+            elif first.fused_wide:  # K9 per member: on its block, or on its range of compact rows
+                for k, f in enumerate(members):
+                    if self.pair is None:
+                        _native.check(lib.ovc_wide_layers(*f._k9_args(flat[block(k)]), first._z[block(k)].data_ptr(), st))
+                    else:
+                        _native.check(lib.ovc_wide_layers_range(*f._k9_args(flat), self._row_offsets[k:k + 2].data_ptr(),
+                                                                first._z.data_ptr(), st))
+            elif self.pair is None:  # library layers per member on its block's rows; bit for bit the member's own rollout only
+                # where cuBLAS computes a row independently of the row count (tested at up to 2 x 300 rows per call)
+                for k, f in enumerate(members):
+                    if first.fused_tail:
+                        f.dense_model.trunk(flat[block(k)], lib_first, out=first._z[block(k)])
+                    else:
+                        logits, value = f.dense_model.forward_from(flat[block(k)], lib_first)
+                        first._scores[block(k)].copy_(logits)
+                        values[block(k)].copy_(value)
+            else:  # library layers per member on every compact row; bit for bit the member's own rollout only where cuBLAS
+                # computes a row independently of the other rows
+                torch.searchsorted(self._row_offsets[1:], self._rindex, right=True, out=self._rmember)
+                for k, f in enumerate(members):
+                    mine = (self._rmember == k).unsqueeze(1)
+                    if first.fused_tail:
+                        torch.where(mine, f.dense_model.trunk(flat, 1), first._z, out=first._z)
+                    else:
+                        logits, value = f.dense_model.forward_from(flat, 1)
+                        torch.where(mine, logits.float(), self._cscores, out=self._cscores)
+                        torch.where(mine[:, 0], value.float(), self._cvalues, out=self._cvalues)
+            if not first.fused_tail:
+                if self.pair is not None:
+                    self._jrow64.copy_(self._pjrow)
+                    first._scores.index_copy_(0, self._jrow64, self._cscores)
+                    values.index_copy_(0, self._jrow64, self._cvalues)
+                return first._scores
+            args = first._k8_args(first._z, self._tail_stack) + (counter.data_ptr(),)
+            if self.pair is None:
+                _native.check(lib.ovc_policy_tail_grouped(*args, self._row_offsets.data_ptr(), K, actions.data_ptr(), values.data_ptr(),
+                                                          ptr(scores8), ptr(logp), st))
+            else:
+                _native.check(lib.ovc_policy_tail_grouped_joint(*args, self._pjrow.data_ptr(), self._row_offsets.data_ptr(), K,
+                                                                actions.data_ptr(), values.data_ptr(), ptr(scores8),
+                                                                (self._logp if logp is None else logp).data_ptr(), st))
+        return None
 
 
 class AgentPairRollout(_Rollout):

@@ -380,7 +380,7 @@ def _own_policy(pop, f, env, states, counter_step):
     return scores, vals, lp, acts
 
 
-@pytest.mark.parametrize("K", [3, 5])
+@pytest.mark.parametrize("K", [2, 3, 4, 5])  # K9 per member at 2 and 3, grouped from 4 on
 def test_distinct_members_act_as_their_own_policy_on_their_rows(K):
     make = CASES["random_starts"][0]
     pop = SelfPlayRollout(make(400), _models(K, seed=K), pair_weights=np.ones((K, K)), seed=31, episode_capacity=4)
@@ -389,7 +389,7 @@ def test_distinct_members_act_as_their_own_policy_on_their_rows(K):
     N = pop.env.n_envs
     rows_member = b.pair.view(T, 2 * N).long()
     for t in range(0, T, 3):
-        for k, f in enumerate(pop._members):
+        for k, f in enumerate([pop] + pop._learners.others):
             mine = rows_member[t] == k
             if not mine.any():
                 continue

@@ -245,11 +245,11 @@ def test_one_member_equals_selfplay_on_every_output(case):
     assert torch.equal(pop.values, single.values) and torch.equal(pop.ret_mixed, single.ret_mixed)
 
 
-@pytest.mark.parametrize("case", ["cramped_room", "grid_5x5"])
+@pytest.mark.parametrize("case", ["cramped_room", "random_starts", "grid_5x5", "pool_9"])
 def test_sync_weights_changes_one_members_block_only(case):
     pop, singles, models = _rollouts(case, 3, [50, 77, 73], True)
     offs = _np(pop.blocks).tolist()
-    before = [b.clone() for b in pop._tail_stack] if pop.fused_tail else None
+    before = [b.clone() for b in pop._learners._tail_stack] if pop.fused_tail else None
     _block_equal(pop, singles, offs, pop.collect(20, GAMMA, LAM), [s.collect(20, GAMMA, LAM) for s in singles])
     with torch.no_grad():  # member 1 after a "learner update"; single 1 shares the module
         for p in models[1].parameters():
@@ -257,7 +257,7 @@ def test_sync_weights_changes_one_members_block_only(case):
     pop.sync_weights()
     singles[1].sync_weights()
     if before is not None:  # the stacked tables changed in member 1's entry only
-        for old, new in zip(before, pop._tail_stack):
+        for old, new in zip(before, pop._learners._tail_stack):
             assert torch.equal(old[0], new[0]) and torch.equal(old[2], new[2]) and not torch.equal(old[1], new[1])
     bp = pop.collect(20, GAMMA, LAM)
     bss = [s.collect(20, GAMMA, LAM) for s in singles]

@@ -80,8 +80,8 @@ counter, pcounter = torch.zeros(2, dtype=torch.int64, device="cuda"), torch.zero
 lst, first, jrow = i32(rows), i32(rows), i32(rows)
 for K in KS:
     sp = SelfPlayRollout(env(max(N // 8, K)), models[:K], use_graph=False)
-    wt, b0 = sp._k7_stack
-    t1, tb1, th, tbh, to, tbo = sp._tail_stack
+    wt, b0 = sp._learners._k7_stack
+    t1, tb1, th, tbh, to, tbo = sp._learners._tail_stack
     pair = torch.randint(0, K, (N, 2), dtype=torch.int32, device="cuda")
     thr = torch.from_numpy(pair_thresholds(np.ones((K, K)), K)).cuda()
     eo, ro = i32(K + 1), i32(K + 1)

@@ -81,9 +81,9 @@ def graph_us(fn, calls=20):
 
 for K in KS:
     sp = SelfPlayRollout(env(max(N // 8, K)), models[:K], use_graph=False)
-    wt, b0 = sp._k7_stack
-    w1, b1, w2, b2 = sp._wide_stack
-    t1, tb1, th, tbh, to, tbo = sp._tail_stack
+    wt, b0 = sp._learners._k7_stack
+    w1, b1, w2, b2 = sp._learners._wide_stack
+    t1, tb1, th, tbh, to, tbo = sp._learners._tail_stack
     eoff = torch.tensor([k * N // K for k in range(K + 1)], dtype=torch.int32, device="cuda")
     roff = 2 * eoff
     ho = eoff.tolist()
