@@ -45,3 +45,15 @@ class Trace(object):
 
 def lut_bytes(layouts):
     return np.stack([l.feature_lut() for l in layouts]).view(np.uint8).reshape(len(layouts), -1)
+
+
+def strip_signature(name):
+    """A demangled kernel name without return type and parameter list: ``void ovc::k<(int)1>(args)`` /
+    ``ovc::k(args)`` -> ``ovc::k<(int)1>`` / ``ovc::k`` (up to the first parenthesis outside the template arguments)."""
+    name = name[5:] if name.startswith("void ") else name
+    depth = 0
+    for i, c in enumerate(name):
+        depth += (c == "<") - (c == ">")
+        if c == "(" and depth == 0:
+            return name[:i]
+    return name

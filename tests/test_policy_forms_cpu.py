@@ -10,6 +10,7 @@ import subprocess
 import pytest
 
 import test_gpu_policy_forms as F
+from helpers import strip_signature
 from overcooked_ai_b200 import _native
 
 TESTS = os.path.dirname(os.path.abspath(__file__))
@@ -23,16 +24,22 @@ def _tool(name):
     return path if os.path.exists(path) else None
 
 
-def _compiled_policy_kernels():
-    """The demangled names of the library's policy-kernel entry points, as ``ovc::<template><(args)>``."""
+def compiled_kernels():
+    """The demangled names of every device entry point of the library, without return type and parameter list."""
     cuobjdump, cufilt = _tool("cuobjdump"), _tool("cu++filt")
     if not cuobjdump or not cufilt:
         pytest.skip("cuobjdump / cu++filt not installed: the compiled kernels cannot be listed")
     syms = subprocess.run([cuobjdump, "-symbols", _native.LIB_PATH], capture_output=True, text=True, check=True).stdout
     mangled = [line.split()[-1] for line in syms.splitlines() if "STO_ENTRY" in line]
     names = subprocess.run([cufilt], input="\n".join(mangled), capture_output=True, text=True, check=True).stdout.splitlines()
-    pattern = re.compile(r"^void (ovc::(%s)<.*>)\(.*\)$" % "|".join(TEMPLATES))
-    return {m.group(1) for m in map(pattern.match, names) if m}
+    assert len(names) == len(mangled) and len(set(names)) == len(names)
+    return {strip_signature(n) for n in names}
+
+
+def _compiled_policy_kernels():
+    """The policy-kernel entry points, as ``ovc::<template><(args)>``."""
+    pattern = re.compile(r"^ovc::(%s)<.*>$" % "|".join(TEMPLATES))
+    return {n for n in compiled_kernels() if pattern.match(n)}
 
 
 def test_every_policy_kernel_instantiation_has_a_float64_test():
@@ -43,7 +50,7 @@ def test_every_policy_kernel_instantiation_has_a_float64_test():
     print("%d policy-kernel instantiations, each with a float64 test" % len(compiled))
 
 
-def _test_functions(module):
+def defined_tests(module):
     with open(os.path.join(TESTS, module)) as f:
         tree = ast.parse(f.read())
     return {n.name for n in tree.body if isinstance(n, ast.FunctionDef) and n.name.startswith("test_")}
@@ -52,10 +59,10 @@ def _test_functions(module):
 def test_every_instantiation_names_a_test_that_exists():
     """An entry is a case of test_gpu_policy_forms.py (one of its test functions takes it) or names an existing test."""
     kinds = {"k8": "test_k8_form_exact", "k7": "test_k7_form_exact", "draw": "test_draw_form_exact", "k9": "test_k9_form_exact"}
-    own = _test_functions("test_gpu_policy_forms.py")
+    own = defined_tests("test_gpu_policy_forms.py")
     for name, entry in F.INSTANTIATIONS.items():
         if isinstance(entry, tuple):
             assert kinds[entry[0]] in own, (name, entry)
         else:
             module, test = entry.split("::")
-            assert test in _test_functions(module), "%s names %s, which does not exist" % (name, entry)
+            assert test in defined_tests(module), "%s names %s, which does not exist" % (name, entry)
