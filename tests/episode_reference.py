@@ -25,7 +25,8 @@ class EpisodeReference(object):
     """The kernel's definition for N environments: ``step`` folds one transition in, ``finished`` lists the records in
     (slot, env) order as ``EpisodeRecords.finished`` does."""
 
-    def __init__(self, deliver_value, layout_id, capacity):
+    def __init__(self, deliver_value, layout_id, capacity, members=False, pairs=False):
+        self.members, self.pairs = bool(members), bool(pairs)
         self.deliver_value = np.asarray(deliver_value, dtype=np.int64).reshape(-1, 16)
         self.layout_id = np.array(layout_id, dtype=np.int32)
         N = len(self.layout_id)
@@ -45,10 +46,31 @@ class EpisodeReference(object):
                         "partner_seat": np.zeros((C, N), np.int32), "sparse_r_by_agent": np.zeros((C, N, 2), np.int64),
                         "shaped_r_by_agent": np.zeros((C, N, 2), np.int64), "game_stats": np.zeros((C, N, 2, N_EVENTS), np.int32),
                         "reward_by_agent": np.zeros((C, N, 2), np.float32)}
+        if self.members:
+            self.records["partner_member"] = np.zeros((C, N), np.int32)
+        if self.pairs:
+            self.records["pair"] = np.zeros((C, N, 2), np.int32)
 
-    def step(self, shaped, done, events, new_layout_id, rewards, partner_seat=None):
+    def save_records(self):
+        """The record set (records, count, dropped, capacity), to be put back by ``load_records``: a rollout keeps run()'s
+        records and each window's apart while the running state is shared."""
+        return self.records, self.count, self.dropped, self.capacity
+
+    def load_records(self, saved):
+        self.records, self.count, self.dropped, self.capacity = saved
+
+    def empty_records(self, capacity):
+        kept = self.save_records()
+        self.capacity = int(capacity)
+        self.clear()
+        fresh = self.save_records()
+        self.load_records(kept)
+        return fresh
+
+    def step(self, shaped, done, events, new_layout_id, rewards, partner_seat=None, member=None, pair=None):
         """shaped [N,2], done [N], events [N,2] of one ovc_step; new_layout_id [N] = word 3 & 0xFF of the records after it;
-        rewards float32 [N,2] (``rewards_f32``); partner_seat [N] or None (-1 in every record)."""
+        rewards float32 [N,2] (``rewards_f32``); partner_seat [N] or None (-1 in every record); member [N] / pair [N, 2]: the
+        ending episodes' member / pair (recorded with ``members`` / ``pairs``)."""
         events = np.asarray(events).astype(np.int64)
         rec = (events >> RECIPE_SHIFT) & 15
         delivered = (events >> SOUP_DELIVERY) & 1
@@ -67,6 +89,10 @@ class EpisodeReference(object):
                 r["partner_seat"][k, e] = -1 if partner_seat is None else partner_seat[e]
                 r["sparse_r_by_agent"][k, e], r["shaped_r_by_agent"][k, e] = self.sparse[e], self.shaped[e]
                 r["game_stats"][k, e], r["reward_by_agent"][k, e] = self.event_counts[e], self.reward[e]
+                if self.members:
+                    r["partner_member"][k, e] = member[e]
+                if self.pairs:
+                    r["pair"][k, e] = pair[e]
                 self.count[e] = k + 1
             else:
                 self.dropped[e] += 1
@@ -78,10 +104,14 @@ class EpisodeReference(object):
     def finished(self):
         k, e = np.nonzero(np.arange(self.capacity)[:, None] < self.count[None, :])
         r = self.records
-        return {"env_index": e, "ep_game_stats": r["game_stats"][k, e], "ep_sparse_r_by_agent": r["sparse_r_by_agent"][k, e],
-                "ep_shaped_r_by_agent": r["shaped_r_by_agent"][k, e], "ep_sparse_r": r["sparse_r_by_agent"][k, e].sum(1),
-                "ep_shaped_r": r["shaped_r_by_agent"][k, e].sum(1), "ep_length": r["length"][k, e],
-                "ep_reward_by_agent": r["reward_by_agent"][k, e], "layout": r["layout"][k, e], "partner_seat": r["partner_seat"][k, e]}
+        out = {"env_index": e, "ep_game_stats": r["game_stats"][k, e], "ep_sparse_r_by_agent": r["sparse_r_by_agent"][k, e],
+               "ep_shaped_r_by_agent": r["shaped_r_by_agent"][k, e], "ep_sparse_r": r["sparse_r_by_agent"][k, e].sum(1),
+               "ep_shaped_r": r["shaped_r_by_agent"][k, e].sum(1), "ep_length": r["length"][k, e],
+               "ep_reward_by_agent": r["reward_by_agent"][k, e], "layout": r["layout"][k, e], "partner_seat": r["partner_seat"][k, e]}
+        for key in ("partner_member", "pair"):
+            if key in r:
+                out[key] = r[key][k, e]
+        return out
 
     def running(self):
         """The running state in the order of ``EpisodeStats.state_tensors``."""

@@ -6,11 +6,13 @@ import pytest
 import torch
 
 import policy_reference as P
+import rollout_reference as R
 from helpers import TRACE_FILES, TRACE_IDS, Trace
 from oracle import cpu
 from overcooked_ai_b200.batched import BatchedOvercookedEnv
 from overcooked_ai_b200.selfplay import PARTNER_DRAW_SALT, PARTNER_SEAT_SALT, BCPolicy, SelfPlayRollout
 from ppo_reference import gae_f32
+from rollout_reference import seats_reference
 
 pytestmark = pytest.mark.gpu
 
@@ -37,18 +39,10 @@ def _tables(ops):
 
 
 def _features(env, states):
-    lut = _np(env.feature_lut())
-    return cpu.featurize(env._tab_host, lut, states, num_pots=2)  # [N, 2, 96]
+    return R.features(env._tab_host, _np(env.feature_lut()), states)  # [N, 2, 96]
 
 
-def _heads(feats, ops):
-    """bf16(features) -> the BC MLP with K8's roundings (ReLU, no input activation); asserts the exactness premise.  K10
-    stages the features in bfloat16 (DESIGN §4, K10 "Exactness"): features above 256 (a cook time remaining) are rounded to
-    nearest even there, and so they are here."""
-    w1, b1, wh, bh, wo, bo = ops
-    s, certs = P.k8_reference(P.bf16(feats), w1, b1, wh, bh, wo, bo, 1.0, 0.0)
-    assert all(c.holds() for c in certs), "premise: the operands are not exact in float32"
-    return s
+_heads = R.bc_heads
 
 
 def _gumbel_rows(heads, rows, seed, step, n_actions):
@@ -202,19 +196,6 @@ def test_k10_refuses_what_it_is_not_built_for():
 
 
 # --------------------------------------------------------------------------------------------------- the seat draw
-def seats_reference(n, seed, step, bc_factor, old, done=None):
-    """numpy restatement of ovc_assign_partners."""
-    e = np.arange(n, dtype=np.uint64)
-    ctr = np.stack([e & np.uint64(0xFFFFFFFF), e >> np.uint64(32), np.full_like(e, step & 0xFFFFFFFF),
-                    np.full_like(e, step >> 32)], 1).astype(np.uint32)
-    w = P.philox4x32_10(seed, ctr)
-    f = float(np.float32(bc_factor))
-    thr = 0xFFFFFFFF if f >= 1 else int(f * 4294967296.0) if f > 0 else 0
-    hit = (w[:, 0].astype(np.int64) < thr) | (thr == 0xFFFFFFFF)
-    new = np.where(hit, (w[:, 1] >> np.uint32(31)).astype(np.int32), -1).astype(np.int32)
-    return new if done is None else np.where(done != 0, new, old).astype(np.int32)
-
-
 @pytest.mark.parametrize("n", [1, 255, 4099])
 def test_assign_partners_matches_the_restatement(n):
     env = BatchedOvercookedEnv("cramped_room", n, horizon=400)

@@ -11,6 +11,7 @@ import policy_reference as P
 from overcooked_ai_b200.batched import BatchedOvercookedEnv, EpisodeRecords, EpisodeStats
 from overcooked_ai_b200.selfplay import (PARTNER_SEAT_SALT, AgentPairRollout, BCPolicy, RllibLSTMShapedCNN, RllibShapedCNN,
                                          SelfPlayRollout)
+from rollout_reference import gae_view_f32
 from test_gpu_agent_pair import _exact_wide
 from test_gpu_bc_partner import POOL_5X4
 
@@ -79,22 +80,6 @@ def test_record_view_equals_two_view_rows(stats):
 # ------------------------------------------------------------------------------------------------ the GAE kernel
 
 
-def _gae_reference(r, v, d, last, gamma, lam):
-    """float32 loop in ovc_gae's documented order."""
-    T, n = r.shape
-    f = np.float32
-    g, gl = f(gamma), f(f(gamma) * f(lam))
-    adv, tgt = np.zeros_like(r), np.zeros_like(r)
-    a, nv = np.zeros(n, np.float32), last.astype(np.float32)
-    for t in range(T - 1, -1, -1):
-        nt = np.where(d[t] != 0, f(0), f(1)).astype(np.float32)
-        delta = ((r[t] + (g * nv).astype(np.float32) * nt).astype(np.float32) - v[t]).astype(np.float32)
-        a = (delta + ((gl * nt).astype(np.float32) * a).astype(np.float32)).astype(np.float32)
-        adv[t], tgt[t] = a, (a + v[t]).astype(np.float32)
-        nv = v[t]
-    return adv, tgt
-
-
 @pytest.mark.parametrize("T", [1, 15, 16, 17, 400])
 def test_gae_view_equals_the_float32_loop_and_the_two_row_kernel(T):
     n = 301
@@ -108,7 +93,7 @@ def test_gae_view_equals_the_float32_loop_and_the_two_row_kernel(T):
     tgt, tgt_full = _guarded(T * n, torch.float32, float("nan"))
     env.gae_view(_dev(r, torch.float32), _dev(v, torch.float32), _dev(d, torch.uint8), _dev(last, torch.float32), GAMMA, LAM,
                  adv.view(T, n), tgt.view(T, n))
-    want_a, want_t = _gae_reference(r, v, d, last, GAMMA, LAM)
+    want_a, want_t = gae_view_f32(r, v, d, last, GAMMA, LAM)
     assert np.array_equal(_np(adv).reshape(T, n).view(np.int32), want_a.view(np.int32))
     assert np.array_equal(_np(tgt).reshape(T, n).view(np.int32), want_t.view(np.int32))
     assert torch.isnan(adv_full[T * n:]).all() and torch.isnan(tgt_full[T * n:]).all()

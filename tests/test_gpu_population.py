@@ -8,11 +8,11 @@ import numpy as np
 import pytest
 import torch
 
-import policy_reference as P
 from overcooked_ai_b200 import _native
 from overcooked_ai_b200.batched import BatchedOvercookedEnv, EpisodeRecords, EpisodeStats
 from overcooked_ai_b200.selfplay import (PARTNER_MEMBER_SALT, AgentPairRollout, BCPolicy, RllibLSTMShapedCNN, RllibShapedCNN,
                                          _NetworkAgent, member_thresholds)
+from rollout_reference import members_reference
 from test_gpu_bc_partner import POOL_5X4
 
 pytestmark = pytest.mark.gpu
@@ -54,16 +54,6 @@ def test_group_members_is_a_stable_counting_sort(k, n, kind):
 
 
 # ------------------------------------------------------------------------------------------------ the population draw
-
-
-def members_reference(n, seed, step, thresholds, old, done=None):
-    """numpy restatement of ovc_assign_members' draw."""
-    e = np.arange(n, dtype=np.uint64)
-    ctr = np.stack([e & np.uint64(0xFFFFFFFF), e >> np.uint64(32), np.full_like(e, step & 0xFFFFFFFF),
-                    np.full_like(e, step >> 32)], 1).astype(np.uint32)
-    w0 = P.philox4x32_10(seed, ctr)[:, 0].astype(np.int64)
-    new = (w0[:, None] >= np.asarray(thresholds, np.int64)[None, :]).sum(1).astype(np.int32)
-    return new if done is None else np.where(done != 0, new, old).astype(np.int32)
 
 
 @pytest.mark.parametrize("n", [1, 255, 4099])

@@ -10,10 +10,10 @@ import pytest
 import torch
 
 import limit_layouts as LL
-import policy_reference as P
 from overcooked_ai_b200 import _native
 from overcooked_ai_b200.batched import BatchedOvercookedEnv, EpisodeRecords
 from overcooked_ai_b200.selfplay import RllibShapedCNN, SelfPlayRollout, pair_thresholds, PAIR_SALT
+from rollout_reference import pairs_reference
 from test_gpu_bc_partner import POOL_5X4
 
 pytestmark = pytest.mark.gpu
@@ -31,17 +31,6 @@ def _dev(a, dt=torch.int32):
 
 
 # ------------------------------------------------------------------------------------------------ ovc_assign_pairs
-
-
-def pairs_reference(n, K, seed, step, thresholds, old, done=None):
-    """numpy restatement of ovc_assign_pairs' draw."""
-    e = np.arange(n, dtype=np.uint64)
-    ctr = np.stack([e & np.uint64(0xFFFFFFFF), e >> np.uint64(32), np.full_like(e, step & 0xFFFFFFFF),
-                    np.full_like(e, step >> 32)], 1).astype(np.uint32)
-    w0 = P.philox4x32_10(seed, ctr)[:, 0].astype(np.int64)
-    p = (w0[:, None] >= np.asarray(thresholds, np.int64)[None, :]).sum(1)
-    new = np.stack([p // K, p % K], 1).astype(np.int32)
-    return new if done is None else np.where(done[:, None] != 0, new, old).astype(np.int32)
 
 
 @pytest.mark.parametrize("K,n", [(1, 33), (3, 255), (8, 4099), (64, 1000)])

@@ -15,9 +15,9 @@ from overcooked_ai_b200 import _native
 from overcooked_ai_b200.batched import BatchedOvercookedEnv
 from overcooked_ai_b200.selfplay import (PARTNER_MEMBER_SALT, PARTNER_SEAT_SALT, AgentPairRollout, BCPolicy, RllibLSTMShapedCNN,
                                          RllibShapedCNN, SelfPlayRollout, _NetworkAgent, member_thresholds)
-from test_gpu_bc_partner import POOL_5X4, seats_reference
+from rollout_reference import learner_rows_reference, members_reference, seats_reference
+from test_gpu_bc_partner import POOL_5X4
 from test_gpu_pair_collect import _check_window
-from test_gpu_population import members_reference
 
 pytestmark = pytest.mark.gpu
 
@@ -36,15 +36,6 @@ def _dev(v, dt):
 
 
 # ------------------------------------------------------------------------------------------------ the kernels
-
-
-def learner_rows_reference(seat):
-    mask = np.where(seat < 0, 3, np.where(seat == 0, 2, 1)).astype(np.int32)
-    cnt = np.where(mask == 3, 2, 1)
-    first = (np.cumsum(cnt) - cnt).astype(np.int32)
-    jrow = [2 * e + v for e in range(len(seat)) for v in (0, 1) if mask[e] >> v & 1]
-    lst = (np.arange(len(seat), dtype=np.int64) << 2 | mask).astype(np.int32)
-    return lst, first, np.asarray(jrow, np.int32), int(cnt.sum())
 
 
 @pytest.mark.parametrize("n", [1, 255, 32771])
