@@ -108,6 +108,7 @@ class BatchedOvercookedEnv(object):
             self._rs = _native.RandomStart(int(seed) & 0xFFFFFFFFFFFFFFFF, thr, int(bool(random_start_pos)),
                                            int(self.random_layout), 0)
         self._lut = None
+        self._greedy = None
         self._segments = None
         self._pot = {}  # gamma -> potential tables; never dropped, so a captured graph's tables stay alive
         with torch.cuda.device(self.device):
@@ -775,6 +776,39 @@ class BatchedOvercookedEnv(object):
         _native.check(self._lib.ovc_assign_partners(0 if done is None else done.data_ptr(), bc_factor.data_ptr(), self.n_envs,
                                                     int(seed) & (2**64 - 1), counter.data_ptr(), partner_seat.data_ptr(), self._stream()))
         return partner_seat
+
+    def greedy_tables(self):
+        """(tables uint8 [n_layouts, 2660], plans uint16): every layout's greedy partner tables on the device
+        (``greedy.build_greedy_tables``), built at the first call and kept, so a captured graph's tables stay alive.
+        Raises ValueError for a layout whose orders are not one 3-onion order."""
+        if self._greedy is None:
+            from . import _greedy_native, greedy
+
+            tab, plans = greedy.build_greedy_tables(self.layouts)
+            assert tab.shape[1] == _greedy_native.lib().ovc_greedy_layout_table_size(), "greedy table size mismatch with the native library"
+            self._greedy = (torch.from_numpy(tab).to(self.device), torch.from_numpy(plans.view(np.int16)).to(self.device))
+        return self._greedy
+
+    def greedy_actions(self, player, prev, counter, seed=0, done=None, out=None):
+        """The greedy partner's actions (ovc_greedy_actions, include/ovc_greedy.h): GreedyHumanModel.action of player
+        ``player[e]`` (int32 [N]; -1: the agent does not play e) on every environment, written to ``out[e, player[e]]``
+        (int32 [N, 2]; default a new zero tensor).  ``prev`` (int32 [N]) holds each environment's previous players' key for
+        the stuck rule and is updated; ``done`` (int32 [N], e.g. ``self.done`` from the previous ``step``) invalidates it;
+        ``counter`` int64 CUDA tensor of 2 zeros that the kernel advances; stuck draws use key ``seed``.  Returns ``out``."""
+        from . import _greedy_native
+
+        tables, plans = self.greedy_tables()
+        for t, n in ((player, self.n_envs), (prev, self.n_envs)) + (() if done is None else ((done, self.n_envs),)):
+            assert t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n, "player / prev / done: int32 CUDA [N]"
+        assert counter.is_cuda and counter.dtype == torch.int64 and counter.numel() == 2 and counter.is_contiguous()
+        if out is None:
+            out = torch.zeros((self.n_envs, 2), dtype=torch.int32, device=self.device)
+        assert out.is_cuda and out.dtype == torch.int32 and out.is_contiguous() and out.numel() == 2 * self.n_envs
+        _greedy_native.check(_greedy_native.lib().ovc_greedy_actions(
+            self.tables.data_ptr(), tables.data_ptr(), plans.data_ptr(), self.n_layouts, self.state.data_ptr(), player.data_ptr(),
+            0 if done is None else done.data_ptr(), prev.data_ptr(), self.n_envs, self.state_words, int(seed) & (2**64 - 1),
+            counter.data_ptr(), out.data_ptr(), self._stream()))
+        return out
 
     def feature_lut(self):
         if self._lut is None:

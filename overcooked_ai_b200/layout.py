@@ -509,7 +509,13 @@ class CompiledLayout(object):
         rec["steady"] = (discount / (1 - discount)) * opt_value
         for k in ("max_delivery_steps", "max_pickup_steps", "pot_onion_steps", "pot_tomato_steps", "onion_value", "tomato_value"):
             rec[k] = _as_int(pp[k], k)
-        # order of list(set().union(one_item_pots, two_item_pots)) for every assignment of pots to classes
+        rec["partial_order"] = self.partial_pot_order()
+        return rec
+
+    def partial_pot_order(self):
+        """uint8 [81, 4]: the order of list(set().union(one_item_pots, two_item_pots)) (get_partially_full_pots,
+        overcooked_mdp.py:1882-1890) for every assignment of pots to classes: row sum_k class_k * 3^k (class 0 other, 1 one
+        item, 2 two items), entries the pots' slots in CPython's set iteration order, NO_SLOT after the last."""
         order = np.full((81, 4), NO_SLOT, np.uint8)
         for code in range(3 ** self.n_pots):
             cls = [(code // 3 ** k) % 3 for k in range(self.n_pots)]
@@ -517,8 +523,7 @@ class CompiledLayout(object):
             twos = [self.pot_locations[k] for k in range(self.n_pots) if cls[k] == 2]
             for j, pos in enumerate(list(set().union(*[ones, twos]))):
                 order[code, j] = self.slot_of[pos]
-        rec["partial_order"] = order
-        return rec
+        return order
 
     def potential_pow_len(self):
         pp = self.potential_params()

@@ -28,6 +28,7 @@ import torch.nn.functional as F
 
 from . import _native
 from .batched import EpisodeRecords, EpisodeStats
+from .greedy import GREEDY_DRAW_SALT, GreedyHumanModel
 
 
 class RllibShapedCNN(nn.Module):
@@ -902,11 +903,15 @@ class _Rollout(object):
         return b
 
     def reset_state(self):
-        """Zero the LSTM policies' live state.  run() and collect() zero it at every auto-reset (through ``env.done``); call
-        this after resetting the environments directly (``env.reset()``), so that the new episodes start from zero state."""
+        """Zero the LSTM policies' live state and forget the greedy agents' previous states.  run() and collect() do both at
+        every auto-reset (through ``env.done``); call this after resetting the environments directly (``env.reset()``), so
+        that the new episodes start from zero state."""
         for a in self._agents():
             if a.lstm:
                 a.h.zero_(), a.c.zero_()
+        for a in self._agents() + [getattr(self, "_partner", None)]:
+            if isinstance(a, _GreedyAgent):  # no previous state for the stuck rule, as Agent.reset()
+                a.prev.zero_()
 
 
 class SelfPlayRollout(_FoldedPolicy, _Rollout):
@@ -935,7 +940,9 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         partner: a ``BCPolicy`` that plays next to the PPO agent (PPO_BC, human_aware_rl's OvercookedMultiAgent): at every
         episode start (and for every environment at construction) an environment gets the partner with probability
         ``bc_factor``, in seat 0 or 1 with equal probability (``env.assign_partners``); per transition K10
-        (``env.partner_actions``) overwrites that seat's action after the PPO policy drew both.
+        (``env.partner_actions``) overwrites that seat's action after the PPO policy drew both.  partner may also be a
+        ``GreedyHumanModel`` (the reference's scripted partner, no weights needed), in the same seats and episodes:
+        ``env.greedy_actions`` then overwrites the seat's action.
         partner may instead be a frozen ``RllibShapedCNN`` or a population: a list of 1..63 members, each an ``RllibShapedCNN``
         or a ``BCPolicy`` (a self-play mixture: each episode is self-play with probability ``1 - bc_factor``, else played
         next to the partner, or next to the population member the environment holds).  The partner, or member k, then
@@ -972,6 +979,7 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         (population play: ``pairs`` or ``pair_weights``).  See ``_Learners`` for both forms; ``self.blocks``, ``self.member``,
         ``self.pair`` and ``self.pair_weights`` describe the population, and ``sync_weights()`` refolds every member.  Not
         with a ``partner`` or an ``RllibLSTMShapedCNN`` member."""
+        assert not isinstance(model, GreedyHumanModel), "a GreedyHumanModel does not learn: pass it as the partner"
         self.env = env
         self.seed = int(seed)
         models = list(model) if isinstance(model, (list, tuple)) else None
@@ -992,7 +1000,7 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         self.partner = partner
         self.bc = float(bc_factor)
         self.population = isinstance(partner, (list, tuple))
-        if partner is not None:
+        if partner is not None and not isinstance(partner, GreedyHumanModel):
             _check_members(partner if self.population else [partner], MAX_MEMBERS - 1, (RllibShapedCNN, BCPolicy),
                            "a mixture's population has 1..%d members (one of ovc_group_members' %d groups holds the self-play "
                            "environments)" % (MAX_MEMBERS - 1, MAX_MEMBERS),
@@ -1009,6 +1017,9 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         if isinstance(partner, BCPolicy):
             self._partner = _BCAgent(env, partner, self.partner_seat, seed)
             self._partner_counter = self._partner._counter  # [step, scratch] of K10's draw
+        elif isinstance(partner, GreedyHumanModel):
+            self._partner = _GreedyAgent(env, self.partner_seat, seed)
+            self._partner_counter = self._partner._counter  # [step, scratch] of the stuck draws
         elif partner is not None:
             members = list(partner) if self.population else [partner]
             if not self.population:  # one network partner: a population of one, its member fixed
@@ -1274,6 +1285,36 @@ class _BCAgent(object):
     def sync_weights(self):
         for dst, src in zip(self._tables, self.policy.tables()):
             dst.copy_(src)
+
+
+class _GreedyAgent(object):
+    """A ``GreedyHumanModel`` agent: ``env.greedy_actions`` (include/ovc_greedy.h) with ``partner_seat`` (int32 [N]: the
+    player it plays in environment e, -1 where it does not play), its previous states for the stuck rule in ``prev``
+    (forgotten where the previous transition ended an episode, through ``env.done``, as ``Agent.reset()``), its stuck draws
+    keyed by ``seed ^ GREEDY_DRAW_SALT`` on a counter of its own.  ``complement_of`` as ``_BCAgent``'s.  The plan tables
+    are built here, never inside a graph capture."""
+
+    lstm = False
+
+    def __init__(self, env, partner_seat, seed, complement_of=None):
+        self.env, self.partner_seat, self.seed, self._complement_of = env, partner_seat, int(seed), complement_of
+        env.greedy_tables()
+        self._counter = torch.zeros(2, dtype=torch.int64, device=env.device)
+        self.prev = torch.zeros(env.n_envs, dtype=torch.int32, device=env.device)
+
+    def live(self):
+        return [self._counter, self.prev, self.env.done] + ([self.partner_seat] if self._complement_of is not None else [])
+
+    def follow_seats(self):
+        if self._complement_of is not None:
+            torch.bitwise_xor(self._complement_of, 1, out=self.partner_seat)
+
+    def act(self, actions):
+        self.env.greedy_actions(self.partner_seat, self.prev, self._counter, seed=self.seed ^ GREEDY_DRAW_SALT, done=self.env.done,
+                                out=actions)
+
+    def sync_weights(self):
+        pass
 
 
 # The population draw's key is seed ^ PARTNER_MEMBER_SALT: its counters (env, step) are the seat draw's, so it needs a key of
@@ -1666,12 +1707,12 @@ class _Learners(object):
 class AgentPairRollout(_Rollout):
     """Two different agents, each evaluated on its own seat's view only: the reference's evaluation of an agent pair
     (rllib.py ``evaluate``: ``AgentEvaluator.evaluate_agent_pair(AgentPair(agent_0_policy, agent_1_policy))``) with N
-    environments on the device — PPO against a held-out BC human proxy, cross-play of two PPO agents, BC against BC — and,
+    environments on the device — PPO against a held-out BC human proxy, cross-play of two PPO agents, BC against BC, PPO against the reference's scripted GreedyHumanModel — and,
     with ``collect()``, PPO training of agent 0 next to a fixed agent 1 (a best response, the second stage of fictitious
     co-play, training against a held-out PPO, LSTM or BC partner).
 
-    agents: (agent0, agent1), each an ``RllibShapedCNN``, an ``RllibLSTMShapedCNN`` or a ``BCPolicy`` (the same object twice
-    is allowed).  agent1 may instead be a population: a list of 1..64 members, each an ``RllibShapedCNN`` or a ``BCPolicy``
+    agents: (agent0, agent1), each an ``RllibShapedCNN``, an ``RllibLSTMShapedCNN``, a ``BCPolicy`` or a ``GreedyHumanModel``
+    (the same object twice is allowed).  agent1 may instead be a population: a list of 1..64 members, each an ``RllibShapedCNN`` or a ``BCPolicy``
     (fictitious co-play's second stage, training against a set of checkpoints, PPO_BC with several BC human proxies).  Agent 0 plays player ``swap[e]`` of environment e, agent 1 the other one.  A network agent runs its own
     policy on N rows (the one-view forms of K7 / K8 / K11 and the draw, with K9 on N rows, where ``fused_kernel_support``
     allows them; K2, the dense model on the agent's rows and the one-view draw elsewhere); a BC agent is K10.
@@ -1682,7 +1723,7 @@ class AgentPairRollout(_Rollout):
     PARTNER_SEAT_SALT``, with a counter of its own, so that ``(learner, bc)`` plays exactly the seats of
     ``SelfPlayRollout(learner, partner=bc, bc_factor=1)``.  Not together with ``swap``.
     seed: the draws' key.  Each agent has its own counter; network agents use ``seed``, BC agents ``seed ^
-    PARTNER_DRAW_SALT`` (K10's key in PPO_BC).  A pair therefore draws what ``SelfPlayRollout`` (both agents one network) or
+    PARTNER_DRAW_SALT`` (K10's key in PPO_BC), greedy agents ``seed ^ GREEDY_DRAW_SALT`` for their stuck steps.  A pair therefore draws what ``SelfPlayRollout`` (both agents one network) or
     PPO_BC (``SelfPlayRollout(partner=..., bc_factor=1)``) draw on the same rows and steps.
     autocast_dtype: as ``SelfPlayRollout``'s, for every network agent (an LSTM agent needs bfloat16).
     episode_capacity: as ``SelfPlayRollout``'s.  Every finished episode's ``partner_seat`` is agent 1's player.
@@ -1717,7 +1758,8 @@ class AgentPairRollout(_Rollout):
         else:
             assert member is None and member_weights is None, "member / member_weights go with a population in agents[1]"
         for a in agents[:1] if self.population else agents:
-            assert isinstance(a, (RllibShapedCNN, BCPolicy)), "an agent is an RllibShapedCNN, an RllibLSTMShapedCNN or a BCPolicy"
+            assert isinstance(a, (RllibShapedCNN, BCPolicy, GreedyHumanModel)), \
+                "an agent is an RllibShapedCNN, an RllibLSTMShapedCNN, a BCPolicy or a GreedyHumanModel"
         if swap is not None:
             assert swap.dtype == torch.int32 and swap.is_cuda and swap.is_contiguous() and swap.numel() == env.n_envs, \
                 "swap: int32 CUDA [N]"
@@ -1738,15 +1780,19 @@ class AgentPairRollout(_Rollout):
             if swap is None:
                 return torch.full((env.n_envs,), seat, dtype=torch.int32, device=env.device)
             return (seat ^ (swap != 0).int()).to(torch.int32).contiguous()
+        def scripted(a, players, complement_of=None):  # a BC or greedy agent on the players ``players``
+            if isinstance(a, GreedyHumanModel):
+                return _GreedyAgent(env, players, seed, complement_of)
+            return _BCAgent(env, a, players, seed, complement_of)
         # with fixed seats partner_seat is made after the agents: a network agent's fold checks its model first
         self.agents = []
         for seat, a in zip(seats, agents[:1] if self.population else agents):
-            if not isinstance(a, BCPolicy):
+            if isinstance(a, RllibShapedCNN):
                 self.agents.append(_NetworkAgent(env, a, seat, swap, seed, autocast_dtype, self.random_seats))
             elif self.random_seats and seat == 0:  # agent 1 plays the drawn seats themselves
-                self.agents.append(_BCAgent(env, a, self.partner_seat, seed))
+                self.agents.append(scripted(a, self.partner_seat))
             else:  # under random_seats, agent 0 plays their complement
-                self.agents.append(_BCAgent(env, a, player(seat), seed, self.partner_seat if self.random_seats else None))
+                self.agents.append(scripted(a, player(seat), self.partner_seat if self.random_seats else None))
         if not self.random_seats:
             self.partner_seat = player(1)  # agent 1's player
         if self.population:
@@ -1821,7 +1867,8 @@ class AgentPairRollout(_Rollout):
         agent 0's action, logp, value, reward and GAE advantages; ``partner_seat`` is agent 1's player), for a PPO update of
         agent 0 next to the fixed agent 1.  After an update, call ``sync_weights()`` (it refolds every population member
         too)."""
-        assert isinstance(self.agents[0], _NetworkAgent), "collect() trains agents[0]: an RllibShapedCNN or RllibLSTMShapedCNN, not a BCPolicy"
+        assert isinstance(self.agents[0], _NetworkAgent), \
+            "collect() trains agents[0]: an RllibShapedCNN or RllibLSTMShapedCNN, not a BCPolicy or a GreedyHumanModel"
         return SampleBatch(self.env, n_steps, keep_logits, seq_len=self.max_seq_len if self.agents[0].lstm else None,
                            one_view=True, members=self.population)
 
