@@ -41,6 +41,8 @@ ap.add_argument("--vf-coef", type=float, default=1e-4)
 ap.add_argument("--entropy-coef", type=float, default=0.1)
 ap.add_argument("--shaping-horizon", type=float, default=2.5e6, help="env-steps over which the shaping factor anneals 1 -> 0")
 ap.add_argument("--seed", type=int, default=0)
+ap.add_argument("--bootstrap-horizon", action="store_true",
+                help="bootstrap the advantages from the value of each episode's last state at the horizon cut")
 ap.add_argument("--use-phi", action="store_true", help="the potential-based dense reward (use_phi) instead of the shaped rewards")
 ap.add_argument("--learner", choices=("conv", "records"), default="conv",
                 help="conv: K2's float32 observation through RllibShapedCNN; records: batch.forward, the folded bf16 network "
@@ -59,7 +61,7 @@ for it in range(args.iters):
     # the reference's linear annealing of the shaping factor (rllib.py:358-368), read by the captured graph
     sp.reward_shaping_factor = max(0.0, 1.0 - env_steps / args.shaping_horizon)
     t0 = time.time()
-    batch = sp.collect(T, args.gamma, args.lam)
+    batch = sp.collect(T, args.gamma, args.lam, bootstrap_horizon=args.bootstrap_horizon)
     torch.cuda.synchronize()
     t_collect = time.time() - t0
     # the episodes that ended in the window (TrainingCallbacks.on_episode_end's metrics, rllib.py:480-483)

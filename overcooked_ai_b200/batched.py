@@ -139,6 +139,15 @@ class BatchedOvercookedEnv(object):
             self.env_layout.data_ptr(), 0 if mask is None else mask.data_ptr(), self.n_envs, self.state_words,
             self._rs_ptr(), self._stream()))
 
+    def reset_ended(self):
+        """Reset every environment whose episode ended with the last ``step(..., auto_reset=False)`` (``self.done``) to
+        exactly the record ``step``'s auto-reset would have written: the start record of the record's own layout, or the
+        next episode's random start (and, with ``random_layout``, its drawn layout).  ``reset(mask)`` takes the layout from
+        the initial assignment ``env_layout``; this reset reads it from the record, as the step kernel does."""
+        _native.check(self._lib.ovc_reset(
+            self.tables.data_ptr(), self.n_layouts, self.start_records.data_ptr(), self.state.data_ptr(), 0, self.done.data_ptr(),
+            self.n_envs, self.state_words, self._rs_ptr(), self._stream()))
+
     def step(self, actions, out=None, auto_reset=None):
         """One joint transition of every environment.
 
@@ -737,6 +746,44 @@ class BatchedOvercookedEnv(object):
         _native.check(self._lib.ovc_gae_view(rewards.data_ptr(), values.data_ptr(), dones.data_ptr(), last_values.data_ptr(), T, N,
                                              float(gamma), float(lam), advantages.data_ptr(), value_targets.data_ptr(), self._stream()))
         return advantages, value_targets
+
+    def gae_horizon(self, rewards, values, dones, terminal_values, last_values, gamma, lam, advantages, value_targets, one_view=False):
+        """``gae`` (``one_view``: ``gae_view``) that bootstraps from ``terminal_values`` (float32, the shape of ``values``) at
+        every episode end instead of counting the state after it terminal (ovc_gae_horizon / ovc_gae_horizon_view,
+        include/ovc_horizon.h gives the recurrence).  Returns (advantages, value_targets)."""
+        from . import _horizon_native
+
+        T, N = rewards.shape[0], self.n_envs
+        R = N if one_view else 2 * N
+        for t, dt, n in ((rewards, torch.float32, T * R), (values, torch.float32, T * R), (dones, torch.uint8, T * N),
+                         (terminal_values, torch.float32, T * R), (last_values, torch.float32, R), (advantages, torch.float32, T * R),
+                         (value_targets, torch.float32, T * R)):
+            assert t.is_cuda and t.dtype == dt and t.is_contiguous() and t.numel() == n, (t.dtype, tuple(t.shape))
+        L = _horizon_native.lib()
+        _horizon_native.check((L.ovc_gae_horizon_view if one_view else L.ovc_gae_horizon)(
+            rewards.data_ptr(), values.data_ptr(), dones.data_ptr(), terminal_values.data_ptr(), last_values.data_ptr(), T, R,
+            float(gamma), float(lam), advantages.data_ptr(), value_targets.data_ptr(), self._stream()))
+        return advantages, value_targets
+
+    def horizon_rows(self, partner_seat, one_view, records, view, jrow, rng, values=None):
+        """The learner rows of the environments whose episode ended with the last ``step`` (``self.done``), compacted on the
+        device (ovc_horizon_rows, include/ovc_horizon.h): both views of a self-play environment (``partner_seat`` None or
+        -1), view ``1 - partner_seat[e]`` of a paired one, and with ``one_view`` that view at row e.  Writes ``records``
+        int32 [rows, S] (the terminal records), ``view`` and ``jrow`` int32 [rows] (each compact row's view and output row)
+        and ``rng`` int32 [2] = (0, the row count), rows = 2N (N with ``one_view``); ``values`` (float32 [rows], optional)
+        is zeroed."""
+        from . import _horizon_native
+
+        R = self.n_envs if one_view else 2 * self.n_envs
+        assert partner_seat is not None or not one_view, "one_view needs partner_seat (agent 1's player)"
+        for t, n in ((partner_seat, self.n_envs), (view, R), (jrow, R), (rng, 2)):
+            assert t is None or (t.is_cuda and t.dtype == torch.int32 and t.is_contiguous() and t.numel() == n)
+        assert records.is_cuda and records.dtype == torch.int32 and records.is_contiguous() and records.shape == (R, self.state_words)
+        assert values is None or (values.is_cuda and values.dtype == torch.float32 and values.is_contiguous() and values.numel() == R)
+        ptr = lambda t: 0 if t is None else t.data_ptr()
+        _horizon_native.check(_horizon_native.lib().ovc_horizon_rows(
+            self.state.data_ptr(), self.state_words, self.done.data_ptr(), ptr(partner_seat), int(bool(one_view)), self.n_envs,
+            records.data_ptr(), view.data_ptr(), jrow.data_ptr(), rng.data_ptr(), ptr(values), self._stream()))
 
     def partner_actions(self, tables, partner_seat, counter, seed=0, n_actions=6, out=None, scores=None):
         """The behaviour-cloned partner's actions (ovc_partner_policy, K10: featurize_state of the partner's view -> the BC

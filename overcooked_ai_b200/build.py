@@ -1,4 +1,4 @@
-"""Build csrc/libovc_b200.so and csrc/libovc_greedy.so for the H100 (sm_90a) with nvcc, in-tree next to the sources.
+"""Build csrc/libovc_b200.so, csrc/libovc_greedy.so and csrc/libovc_horizon.so for the H100 (sm_90a) with nvcc, in-tree next to the sources.
 
     python -m overcooked_ai_b200.build [--force]
 """
@@ -15,6 +15,10 @@ OUT = os.path.join(CSRC, "libovc_b200.so")
 GREEDY_SOURCES = ["ovc_greedy.cu"]
 GREEDY_DEPS = ["ovc_greedy.cu", "ovc_rng.cuh", os.path.join("..", "..", "include", "ovc_b200.h"), os.path.join("..", "..", "include", "ovc_greedy.h")]
 GREEDY_OUT = os.path.join(CSRC, "libovc_greedy.so")
+# the horizon bootstrap's library (include/ovc_horizon.h): its own ABI too
+HORIZON_SOURCES = ["ovc_horizon.cu"]
+HORIZON_DEPS = ["ovc_horizon.cu", os.path.join("..", "..", "include", "ovc_b200.h"), os.path.join("..", "..", "include", "ovc_horizon.h")]
+HORIZON_OUT = os.path.join(CSRC, "libovc_horizon.so")
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
@@ -39,12 +43,13 @@ def _compile(out, sources, deps, force, verbose, defines=()):
 
 
 def build(force=False, verbose=False, variant=None, defines=()):
-    """Both libraries; returns the main one's path.  variant / defines: an experiment build of the main library only
+    """Every library; returns the main one's path.  variant / defines: an experiment build of the main library only
     (csrc/libovc_b200_<variant>.so, compiled with the given -D macros); OVC_B200_LIB=<path> makes _native load it instead
     (tools/k5sweep.py A/B runs)."""
     if variant is not None:
         return _compile(os.path.join(CSRC, "libovc_b200_%s.so" % variant), SOURCES, DEPS, force, verbose, defines)
     _compile(GREEDY_OUT, GREEDY_SOURCES, GREEDY_DEPS, force, verbose)
+    _compile(HORIZON_OUT, HORIZON_SOURCES, HORIZON_DEPS, force, verbose)
     return _compile(OUT, SOURCES, DEPS, force, verbose, defines)
 
 

@@ -477,7 +477,10 @@ class SampleBatch(object):
     rewards       float32 [T, 2N]    sparse + reward_shaping_factor * shaped_i (rllib.py:328-329)
     dones         uint8 [T, N]       the episode ended with transition t (the environment auto-reset)
     last_values   float32 [2N]       value head on the state after the window (bootstrap)
-    advantages, value_targets  float32 [T, 2N]   GAE (ovc_gae)
+    advantages, value_targets  float32 [T, 2N]   GAE (ovc_gae; with ``bootstrap_horizon``, ovc_gae_horizon)
+    terminal_values float32 [T, 2N]  only with collect()'s ``bootstrap_horizon``, else None: the learner's value of the
+                                     terminal state (the record before the reset) where ``dones[t]`` on a learner row, 0
+                                     elsewhere (partner rows included); GAE bootstraps from it at the horizon cut
     logits        float32 [T, 2N, 8] the policy's heads (columns 0..5 the logits), only with ``keep_logits``
     partner_seat  int8 [T, N]        with a partner: its player index at transition t (-1: self-play), else None
                                      (``one_view``: agent 1's player)
@@ -519,6 +522,7 @@ class SampleBatch(object):
         self.dones = z((T, N), torch.uint8)
         self.last_values = z(R, torch.float32)
         self.logits = z((T, R, 8), torch.float32) if keep_logits else None
+        self.terminal_values = None  # set by collect(bootstrap_horizon=True)
         self.partner_seat = z((T, N), torch.int8) if partner or one_view else None
         self.partner_member = z((T, N), torch.int8) if members else None
         self.pair = z((T, N, 2), torch.int8) if pairs else None
@@ -656,6 +660,23 @@ class _FoldedPolicy(object):
             self.h = torch.zeros((rows, cell), dtype=torch.bfloat16, device=dev)
             self.c = torch.zeros((rows, cell), dtype=torch.float32, device=dev)
 
+    def _horizon_values_rows(self, h, partner_seat, one_view, out, counter, actions):
+        """The horizon bootstrap's value pass on K7 -> K9 -> K8: ``ovc_horizon_rows`` compacts the learner rows of the
+        environments that just ended (their terminal records, views and output rows) and zeroes ``out``; K7's rows form
+        on those records, K9 and K8's joint form on the compact range then write each row's value at its output row of
+        ``out``.  With no environment done every launch finds an empty range.  K8's draws go to the scratch ``counter`` and
+        ``actions``.  ``h``: the buffers of ``_Rollout._horizon_buffers``."""
+        env, lib, st = self.env, _native.lib(), self.env._stream()
+        rows = self._act0.shape[0]
+        env.horizon_rows(partner_seat, one_view, h.records, h.view, h.jrow, h.range, out)
+        _native.check(lib.ovc_encode_linear_rows(
+            env.tables.data_ptr(), env.n_layouts, h.records.data_ptr(), h.view.data_ptr(), 0, h.ident.data_ptr(), h.range.data_ptr(),
+            self._wt0.data_ptr(), self._b0.data_ptr(), self._act0.data_ptr(), rows, env.state_words, self.W, self.H,
+            env.horizon if env.horizon > 0 else 2**31 - 1, self._wt0.shape[1], 0.2, st))
+        _native.check(lib.ovc_wide_layers_range(*self._k9_args(self._act0), h.range.data_ptr(), self._z.data_ptr(), st))
+        _native.check(lib.ovc_policy_tail_joint(*self._k8_args(self._z), counter.data_ptr(), h.jrow.data_ptr(), h.range.data_ptr(),
+                                                actions.data_ptr(), out.data_ptr(), 0, h.logp.data_ptr(), st))
+
     def _k9_args(self, x, tables=None):
         """``ovc_wide_layers``' arguments (and its range and grouped forms') up to the slope, on the rows of ``x``
         [rows, k0]: ``tables`` (default this policy's) may be a member stack."""
@@ -740,15 +761,23 @@ class _PhiReward(object):
         self.dense = torch.empty(env.n_envs, dtype=torch.float32, device=env.device)
 
 
-def _env_step(env, actions, phi):
+def _env_step(env, actions, phi, terminal=None):
     """K1 with its auto-reset; with ``phi`` (a ``_PhiReward``), K6 on s, K1 without the reset, then
-    ovc_potential_shaping (phi(s') on the terminal records, the dense reward, the reset).  Returns the dense reward for
-    the record (None without ``phi``)."""
-    if phi is None:
+    ovc_potential_shaping (phi(s') on the terminal records, the dense reward, the reset).  ``terminal`` (a callable, the
+    horizon bootstrap's value pass) runs between K1 without the reset and the reset (``env.reset_ended()``, or inside
+    ovc_potential_shaping with ``phi``), while the ended environments still hold their terminal records.  Returns the
+    dense reward for the record (None without ``phi``)."""
+    if phi is None and terminal is None:
         env.step(actions)  # K1 (auto-reset inside)
         return None
-    env.potential(PHI_GAMMA, out=phi.phi_s)  # K6
+    if phi is not None:
+        env.potential(PHI_GAMMA, out=phi.phi_s)  # K6
     env.step(actions, auto_reset=False)
+    if terminal is not None:
+        terminal()
+    if phi is None:
+        env.reset_ended()
+        return None
     return env.potential_shaping(phi.phi_s, phi.dense)
 
 
@@ -807,8 +836,10 @@ class _Rollout(object):
         self.max_seq_len = int(max_seq_len)
         assert self.max_seq_len >= 1
         self.graph = None          # run()'s CUDA graph of one transition
-        self._collect_graphs = {}  # (n_steps, keep_logits) -> ((gamma, lam), CUDA graph of the window)
-        self._batches = {}         # (n_steps, keep_logits) -> SampleBatch the window writes
+        # (n_steps, keep_logits), and "bootstrap_horizon" after them with the flag -> ((gamma, lam), CUDA graph of the window)
+        self._collect_graphs = {}
+        self._batches = {}         # the same keys -> SampleBatch the window writes
+        self._horizon = None       # the horizon bootstrap's buffers (_horizon_buffers), made at its first collect()
         self._boot_counter = torch.zeros(2, dtype=torch.int64, device=dev)  # the bootstrap's draws leave the learner's counter alone
         self._boot_actions = torch.zeros((N, 2), dtype=torch.int32, device=dev)
         if learner.lstm:  # the bootstrap's (discarded) LSTM state: the next window continues from the live state
@@ -878,20 +909,40 @@ class _Rollout(object):
         for t in range(n_steps):
             self._transition(b, t)
         self._bootstrap(b)
+        if b.terminal_values is not None:
+            self.env.gae_horizon(b.rewards, b.values, b.dones, b.terminal_values, b.last_values, gamma, lam, b.advantages,
+                                 b.value_targets, one_view=b.one_view)
+            return
         gae = self.env.gae_view if b.one_view else self.env.gae
         gae(b.rewards, b.values, b.dones, b.last_values, gamma, lam, b.advantages, b.value_targets)
 
-    def collect(self, n_steps, gamma, lam, keep_logits=False):
+    def collect(self, n_steps, gamma, lam, keep_logits=False, bootstrap_horizon=False):
         """Advance every environment n_steps transitions, as run() does (the same kernels and the same draws from the same
         seed and counters), and return them as a ``SampleBatch`` with GAE(gamma, lam) advantages.  The batch's tensors are
-        reused: the next collect() with the same n_steps / keep_logits overwrites them.  With use_graph the whole window
-        is one CUDA graph (captured once per n_steps / keep_logits; a new gamma or lam re-captures it); no host
-        synchronisation otherwise.  With a population, the batch's ``partner_member`` is each transition's member."""
+        reused: the next collect() with the same n_steps / keep_logits / bootstrap_horizon overwrites them.  With use_graph
+        the whole window is one CUDA graph (captured once per n_steps / keep_logits / bootstrap_horizon; a new gamma or lam
+        re-captures it); no host synchronisation otherwise.  With a population, the batch's ``partner_member`` is each
+        transition's member.
+
+        bootstrap_horizon: every episode ends at the horizon, a time limit, and no state of the MDP is terminal; by default
+        (RLlib's GAE, which the reference trains with) the state after the last step still counts as terminal.  With
+        bootstrap_horizon the learner's value head is evaluated on the terminal record of every environment that ends
+        (between K1, run without its auto-reset, and the reset; only the ended environments' learner rows are evaluated),
+        stored in the batch's ``terminal_values``, and GAE bootstraps from it (``ovc_gae_horizon``): delta = r + gamma *
+        V(s_T) - V(s).  Every other field of the batch, the environments, the counters, the episode records and the
+        statistics are bit for bit those of the same collect() without it.  Not for an LSTM learner, a population of
+        learners or an environment without auto_reset."""
+        if bootstrap_horizon:
+            self._check_bootstrap_horizon()
         assert self.env.auto_reset, "collect() needs an auto_reset environment: a window runs across episode ends"
-        key = (int(n_steps), bool(keep_logits))
+        key = (int(n_steps), bool(keep_logits)) + ("bootstrap_horizon",) * bool(bootstrap_horizon)
         b = self._batches.get(key)
         if b is None:
-            b = self._batches[key] = self._new_batch(n_steps, keep_logits)
+            b = self._new_batch(n_steps, keep_logits)
+            if bootstrap_horizon:
+                b.terminal_values = torch.zeros_like(b.values)
+                self._horizon_buffers()
+            self._batches[key] = b
         if not self.use_graph:
             self._collect_window(b, n_steps, gamma, lam)
             return b
@@ -901,6 +952,34 @@ class _Rollout(object):
                                                                          lambda: self._collect_window(b, n_steps, gamma, lam)))
         g[1].replay()
         return b
+
+    def _check_bootstrap_horizon(self):
+        """The configurations collect(bootstrap_horizon=True) refuses."""
+        assert self.env.auto_reset, "bootstrap_horizon needs an auto_reset environment: the terminal states are evaluated " \
+            "between the step and the reset of the episodes that end"
+        assert getattr(self, "_learners", None) is None, \
+            "bootstrap_horizon is not supported for a population of learners (blocks or population play)"
+        assert not self._agents()[0].lstm, "bootstrap_horizon is not supported for an LSTM learner: the value of the terminal " \
+            "state needs one more ovc_lstm_head step on a scratch copy of the recurrent state"
+
+    def _horizon_buffers(self):
+        """The horizon bootstrap's scratch on the learner's rows (2N, or N for one view): the compaction's records, views,
+        output rows, identity rows map, range and K8's logp where the learner runs K7 -> K9 -> K8, else the full value
+        pass's values."""
+        if self._horizon is not None:
+            return
+        learner, env = self._agents()[0], self.env
+        rows = 2 * env.n_envs if learner is self else env.n_envs
+        i32 = lambda *shape: torch.zeros(shape, dtype=torch.int32, device=env.device)
+        h = SimpleNamespace(fused=learner.fused_first_layer and learner.fused_wide and learner.fused_tail)
+        if h.fused:
+            h.records, h.view, h.jrow, h.range = i32(rows, env.state_words), i32(rows), i32(rows), i32(2)
+            h.ident = torch.arange(rows, dtype=torch.int32, device=env.device)
+            h.logp = torch.zeros(rows, dtype=torch.float32, device=env.device)
+        else:
+            h.values = torch.zeros(rows, dtype=torch.float32, device=env.device)
+            h.zero = torch.zeros((), dtype=torch.float32, device=env.device)
+        self._horizon = h
 
     def reset_state(self):
         """Zero the LSTM policies' live state and forget the greedy agents' previous states.  run() and collect() do both at
@@ -1165,7 +1244,10 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
                 if self.population:
                     b.partner_member[t].copy_(self._pop.member)
             self._partner.act(actions)  # K10, or the network partner / the population
-        dense = _env_step(env, actions.view(env.n_envs, 2), self._phi)
+        terminal = None
+        if b is not None and b.terminal_values is not None:
+            terminal = lambda: self._terminal_values(b.terminal_values[t])
+        dense = _env_step(env, actions.view(env.n_envs, 2), self._phi, terminal)
         if self.population:  # before the record: both use the slot count[e] the ending episode goes to
             self._pop.assign(env.done, self.episodes if b is None else b.episodes)
         if self._learners is not None:  # before the record, likewise
@@ -1183,6 +1265,23 @@ class SelfPlayRollout(_FoldedPolicy, _Rollout):
         # the LSTM's bootstrap step writes its state to scratch: the next window continues from the live state
         self._policy(actions=self._boot_actions, values=b.last_values, counter=self._boot_counter,
                      state_out=(self._h_boot, self._c_boot) if self.lstm else None)
+
+    def _terminal_values(self, out):
+        """The horizon bootstrap's value pass into ``out`` (float32 [2N]): the learner's value on its rows of the ended
+        environments, 0 elsewhere.  On K7 -> K9 -> K8 only those rows are evaluated (``_horizon_values_rows``); otherwise
+        the policy runs on all 2N rows (library layers take their row count from the host) and the rows are selected."""
+        h, env, N = self._horizon, self.env, self.env.n_envs
+        seats = self.partner_seat if self.partner is not None else None
+        if h.fused:
+            self._horizon_values_rows(h, seats, False, out, self._boot_counter, self._boot_actions)
+            return
+        if not self.fused_first_layer:
+            env.lossless_state_encoding(out=self.obs)
+        self._policy(actions=self._boot_actions, values=h.values, counter=self._boot_counter)
+        mine = (env.done != 0).view(N, 1)
+        if seats is not None:
+            mine = mine & (seats.view(N, 1) != torch.arange(2, dtype=torch.int32, device=env.device))
+        torch.where(mine.expand(N, 2).reshape(-1), h.values, h.zero, out=out)
 
     def _new_batch(self, n_steps, keep_logits):
         """collect()'s two-view batch.  With a partner, its ``partner_seat`` / ``learner_mask`` say which rows were the
@@ -1840,7 +1939,10 @@ class AgentPairRollout(_Rollout):
             if self.population:
                 b.partner_member[t].copy_(partner.member)
         partner.act(self.actions)
-        dense = _env_step(env, self.actions, self._phi)
+        terminal = None
+        if b is not None and b.terminal_values is not None:
+            terminal = lambda: self._terminal_values(b.terminal_values[t])
+        dense = _env_step(env, self.actions, self._phi, terminal)
         if self.population:  # before the record: both use the slot count[e] the ending episode goes to
             partner.assign(env.done, self.episodes if b is None else b.episodes)
         if b is None:
@@ -1861,6 +1963,18 @@ class AgentPairRollout(_Rollout):
         learner = self.agents[0]
         learner.act(self._boot_actions, values=b.last_values, counter=self._boot_counter,
                     state_out=(self._h_boot, self._c_boot) if learner.lstm else None)
+
+    def _terminal_values(self, out):
+        """The horizon bootstrap's value pass into ``out`` (float32 [N]): agent 0's value on the terminal record of each
+        ended environment, at the seat it played, 0 elsewhere; as ``SelfPlayRollout._terminal_values``."""
+        h, env, learner = self._horizon, self.env, self.agents[0]
+        if h.fused:
+            learner._horizon_values_rows(h, self.partner_seat, True, out, self._boot_counter, self._boot_actions)
+            return
+        if self.obs is not None:
+            env.lossless_state_encoding(out=self.obs)
+        learner.act(self._boot_actions, values=h.values, counter=self._boot_counter)
+        torch.where(env.done != 0, h.values, h.zero, out=out)
 
     def _new_batch(self, n_steps, keep_logits):
         """collect()'s batch: agent 0's side of the transitions as a one-view ``SampleBatch`` (one row per environment:
