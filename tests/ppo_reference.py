@@ -22,6 +22,22 @@ def gae_f32(rewards, values, dones, last_values, gamma, lam):
     return adv, adv + v
 
 
+def gae_horizon_f32(r, v, d, tv, last, gamma, lam):
+    """include/ovc_horizon.h's recurrence in numpy float32 (every operation rounded on its own): r, v, tv [T, R], d [T, R]
+    or [T, R / 2] (one flag per environment of two rows), last [R]."""
+    T, R = r.shape
+    dd = np.repeat(d, R // d.shape[1], axis=1) != 0
+    g, gl = np.float32(gamma), np.float32(np.float32(gamma) * np.float32(lam))
+    A, nv = np.zeros(R, np.float32), last.astype(np.float32)
+    adv, tgt = np.empty_like(r), np.empty_like(r)
+    for t in reversed(range(T)):
+        nxt = np.where(dd[t], tv[t], nv).astype(np.float32)
+        delta = (r[t] + g * nxt) - v[t]
+        A = delta + (gl * np.where(dd[t], np.float32(0), np.float32(1))) * A
+        adv[t], tgt[t], nv = A, A + v[t], v[t]
+    return adv, tgt
+
+
 def gae_f64(rewards, values, dones, last_values, gamma, lam):
     """The same recurrence in float64."""
     r, v = np.asarray(rewards, np.float64), np.asarray(values, np.float64)

@@ -4,13 +4,14 @@ which agent holds each row, which Philox key and counter each draw uses, when th
 the rewards, the returns, the records and the sample batch.  It uses the C oracle, float64 forwards of the models and numpy
 only: no rollout class, no environment method, no native library.  The per-kernel restatements it is built from are here
 too, so that each is stated once: the seat, member and pair draws, ``ovc_learner_rows``, the BC network on
-``featurize_state`` and GAE on one row per environment.
+``featurize_state`` and GAE on one row per environment; the greedy agent is tests/greedy_reference.py's.
 
 Each agent is evaluated on the rows it holds and nothing else; there is no grouping and no compact row, so the whole grouping
 machinery of the driver is checked by its result.  Draws are Gumbel-max on Philox4x32-10 at the joint row id (``P.gumbel_scores``).
 Wherever the draw is clear the device must have drawn the reference's action; at a near-tie (a top-2 gap within the
 heads' error bound: 1e-4 for the exact networks, the replay tolerance for the LSTM) the device's action must be one of the
-tied actions and the reference continues with it."""
+tied actions and the reference continues with it.  A greedy agent draws nothing but its stuck steps, which are exact: its
+actions must always be the reference's."""
 import copy
 
 import numpy as np
@@ -19,7 +20,9 @@ import torch.nn.functional as F
 
 import policy_reference as P
 from episode_reference import EpisodeReference, rewards_f32
+from greedy_reference import GreedyReference
 from oracle import cpu
+from overcooked_ai_b200.greedy import GreedyHumanModel
 from overcooked_ai_b200.selfplay import (PAIR_SALT, PARTNER_DRAW_SALT, PARTNER_MEMBER_SALT, PARTNER_SEAT_SALT, BCPolicy,
                                          RllibLSTMShapedCNN)
 from ppo_reference import gae_f32, log_softmax_at
@@ -157,17 +160,24 @@ def cnn_certificates(cnn, obs):
 
 # ------------------------------------------------------------------------------------------------ the agents
 class _Agent(object):
-    """One policy as the reference evaluates it: ``kind`` cnn / lstm / bc, its draw key and the name of its counter."""
+    """One policy as the reference evaluates it: ``kind`` cnn / lstm / bc / greedy, its draw key and the name of its
+    counter."""
 
     def __init__(self, model, key, counter, host):
         self.model, self.key, self.counter = model, int(key) & (2**64 - 1), counter
-        self.kind = "bc" if isinstance(model, BCPolicy) else "lstm" if isinstance(model, RllibLSTMShapedCNN) else "cnn"
+        self.kind = "bc" if isinstance(model, BCPolicy) else "lstm" if isinstance(model, RllibLSTMShapedCNN) else \
+            "greedy" if isinstance(model, GreedyHumanModel) else "cnn"
         self.host = host
         self.h = self.c = None  # LSTM: float64 state per joint row [2N, cell]
+        self.greedy = None      # greedy: its GreedyReference (previous states per environment)
         self.sync()
 
     def sync(self):
         """Take the model's current weights (``sync_weights``)."""
+        if self.kind == "greedy":
+            if self.greedy is None:  # salted inside GreedyReference, as the device passes seed ^ GREEDY_DRAW_SALT
+                self.greedy = GreedyReference(self.host.layouts, self.key, self.host.n)
+            return
         if self.kind == "bc":
             self.ops = bc_operands(self.model)
         else:
@@ -175,6 +185,15 @@ class _Agent(object):
         if self.kind == "lstm" and self.h is None:
             cell = self.model.lstm.hidden_size
             self.h, self.c = np.zeros((2 * self.host.n, cell)), np.zeros((2 * self.host.n, cell))
+
+    def greedy_actions(self, state, rows, done, step):
+        """The greedy agent's actions on joint rows ``rows``: ``GreedyReference.act`` on every environment, with the player
+        it holds there (-1 where it holds none, which forgets the previous state), the previous transition's episode ends
+        and its draw counter ``step``."""
+        player = np.full(self.host.n, -1, np.int64)
+        player[rows // 2] = rows % 2
+        self.greedy.step = step
+        return self.greedy.act(state, player, done)[rows // 2]
 
     def heads(self, cache, rows, reset):
         """(scores [len(rows), 8] with the value in column 6, values [len(rows)]) of this agent on joint rows ``rows``; an
@@ -221,11 +240,13 @@ class _StateCache(object):
 class EnvHost(object):
     """What the reference needs of the environments, as host arrays: layout tables and start records, the horizon, the
     random-start parameters (``cpu.random_start`` or None), the grid, the feature LUTs, the 0.99 potential tables (pt, cost
-    LUT, gamma powers), each layout's delivery values, and the environment count."""
+    LUT, gamma powers), each layout's delivery values, the environment count, and the compiled layouts (the greedy
+    agent's planners)."""
 
-    def __init__(self, tables, starts, horizon, rs, W, H, lut, pot, deliver_value, n):
+    def __init__(self, tables, starts, horizon, rs, W, H, lut, pot, deliver_value, n, layouts=None):
         self.tables, self.starts, self.horizon, self.rs = tables, starts, horizon, rs
         self.W, self.H, self.lut, self.pot, self.deliver_value, self.n = W, H, lut, pot, deliver_value, n
+        self.layouts = layouts
 
 
 # ------------------------------------------------------------------------------------------------ the rollout
@@ -236,14 +257,15 @@ class RolloutReference(object):
     learner       self_play: a model or a list of models (a population of learners)
     blocks        environment counts per member (blocks; default equal) when ``learner`` is a list without pairs
     pairs / pair_weights   population play: int32 [N, 2] fixed pairs, or K x K weights drawn per episode
-    partner       self_play: None, a BCPolicy, an RllibShapedCNN, or a list of members (a population)
+    partner       self_play: None, a BCPolicy, a GreedyHumanModel, an RllibShapedCNN, or a list of members (a population)
     member / member_weights   a population of partners (self_play) or agent 1's population (pair): fixed int32 [N] or drawn
     bc_factor     the seat draw's factor (self_play with a partner)
     agents        pair: (agent0, agent1 or a list of members)
     swap          pair: int32 [N] or None;  random_seats: pair, the seats drawn per episode
     seed, factor (reward_shaping_factor), use_phi, capacity (episode_capacity), seq_len (max_seq_len)
 
-    ``state`` is the environments' records at construction."""
+    ``state`` is the environments' records at construction.  A collect() window with ``bootstrap_horizon``
+    (``begin_window``) also returns each transition's ``terminal_values``."""
 
     def __init__(self, host, state, spec):
         self.host, self.spec = host, dict(spec)
@@ -268,6 +290,8 @@ class RolloutReference(object):
         self.bc = float(spec.get("bc_factor", 0.0))
         self.ties = self.draws = 0        # near-ties of the exact networks' draws, and all their draws
         self.lstm_open = self.lstm_draws = 0  # LSTM draws within the heads' error bound (checked only as one of the tied), all
+        self.bootstrap_horizon = False    # the current window's collect(bootstrap_horizon=...)
+        self.terminal_records = []        # the terminal records the window's terminal values were evaluated on
         if self.pair_kind:
             self._init_pair(spec)
         else:
@@ -322,8 +346,9 @@ class RolloutReference(object):
         p = s.get("partner")
         self.partner = None
         if p is not None:
-            if isinstance(p, BCPolicy):
-                self.partner = _Agent(p, self.seed ^ PARTNER_DRAW_SALT, self._count("partner"), self.host)
+            if isinstance(p, (BCPolicy, GreedyHumanModel)):
+                key = self.seed ^ PARTNER_DRAW_SALT if isinstance(p, BCPolicy) else self.seed
+                self.partner = _Agent(p, key, self._count("partner"), self.host)
             else:
                 members = list(p) if isinstance(p, (list, tuple)) else [p]
                 member = np.zeros(n, np.int32) if not isinstance(p, (list, tuple)) else s.get("member")
@@ -458,6 +483,14 @@ class RolloutReference(object):
         for agent, rows in self.holders():
             if agent.counter not in steps:  # learner members share one counter: one advance per transition
                 steps[agent.counter] = self._advance(agent.counter)
+            if agent.kind == "greedy":  # no Gumbel draw and no tie: every known action must be the reference's
+                a = agent.greedy_actions(self.state, rows, self.prev_done, steps[agent.counter])
+                k = known[rows]
+                bad = (k >= 0) & (k != a)
+                assert not bad.any(), "greedy action differs at joint rows %s: device %s, reference %s" % (
+                    rows[bad][:8].tolist(), k[bad][:8].tolist(), a[bad][:8].tolist())
+                actions[rows] = a
+                continue
             s, v = agent.heads(cache, rows, reset)
             scores[rows], values[rows] = s, v
             a, op = self._draw(s, rows, agent.key, steps[agent.counter], known, agent.kind == "lstm")
@@ -472,7 +505,10 @@ class RolloutReference(object):
         if open_rows:
             self._settle(actions, open_rows, next_state, next_reward)
         joint = actions.reshape(n, 2).astype(np.int32)
-        sparse, shaped, done, events, self.state, rewards, dense = self._step(self.state, joint)
+        sparse, shaped, done, events, nxt, rewards, dense, term = self._step(self.state, joint, self.bootstrap_horizon)
+        if self.bootstrap_horizon:
+            out["terminal_values"] = self._terminal_values(term, done != 0, reset)
+        self.state = nxt
         f = np.float32(self.factor)
         if dense is None:
             sh = shaped.astype(np.float32)
@@ -502,22 +538,41 @@ class RolloutReference(object):
                    logp=self._logp(scores, actions))
         return out
 
-    def _step(self, state, joint):
+    def _step(self, state, joint, terminal=False):
         """K1 with its auto-reset from ``state`` (not modified), and the rewards: ``sparse + factor * shaped_i``, or with
         use_phi ``sparse + factor * float32(phi(s') - phi(s))``, s' taken before the reset.  Returns (sparse, shaped, done,
-        events, the next records, rewards [N, 2], the dense reward or None)."""
+        events, the next records, rewards [N, 2], the dense reward or None, the records of K1 without the reset (the
+        ended episodes' terminal records) with use_phi or ``terminal``, else None)."""
         h = self.host
         nxt = state.copy()
         sparse, shaped, done, events = cpu.step(h.tables, h.starts, nxt, joint, horizon=h.horizon, flags=1, rs=h.rs)
         f = np.float32(self.factor)
+        term = None
+        if self.use_phi or terminal:
+            term = state.copy()
+            cpu.step(h.tables, h.starts, term, joint, horizon=h.horizon, flags=0, rs=h.rs)
         if not self.use_phi:
-            return sparse, shaped, done, events, nxt, rewards_f32(sparse, shaped, self.factor), None
-        term = state.copy()
-        cpu.step(h.tables, h.starts, term, joint, horizon=h.horizon, flags=0, rs=h.rs)
+            return sparse, shaped, done, events, nxt, rewards_f32(sparse, shaped, self.factor), None, term
         pt, cl, gpow = h.pot
         dense = (cpu.potential(h.tables, pt, cl, gpow, term) - cpu.potential(h.tables, pt, cl, gpow, state)).astype(np.float32)
         r = (sparse.astype(np.float32) + f * dense).astype(np.float32)
-        return sparse, shaped, done, events, nxt, np.stack([r, r], 1), dense
+        return sparse, shaped, done, events, nxt, np.stack([r, r], 1), dense, term
+
+    def _terminal_values(self, term, d, reset):
+        """float32 [2N]: the horizon bootstrap's value pass, the learner's float64 value on the terminal records ``term``
+        at its rows of the environments that ended (``d``) — both rows in self-play, row 1 - partner_seat when paired, agent
+        0's row of a pair — and 0 on every other row."""
+        n = self.n
+        if self.pair_kind:
+            learner, mine = self.agent0, np.zeros(2 * n, bool)
+            mine[2 * np.arange(n) + (1 - self.partner_seat)] = True
+        else:
+            learner, mine = self.learners[0], learner_mask(self.partner_seat).astype(bool)
+        rows = np.flatnonzero(np.repeat(d, 2) & mine)
+        out = np.zeros(2 * n, np.float32)
+        out[rows] = learner.heads(_StateCache(self.host, term), rows, reset)[1]
+        self.terminal_records.append(term[d])
+        return out
 
     def _settle(self, actions, open_rows, next_state, next_reward):
         """Near-ties on rows whose device action is not known: the tied action whose oracle step gives the device's next
@@ -532,7 +587,7 @@ class RolloutReference(object):
             for a, b in opts:  # the whole batch: a random reset draws from the environment's index
                 joint = np.maximum(actions, 0).reshape(-1, 2).astype(np.int32)
                 joint[e] = a, b
-                _, _, _, _, s, r, _ = self._step(self.state, joint)
+                _, _, _, _, s, r, _, _ = self._step(self.state, joint)
                 if np.array_equal(s[e], next_state[e]) and (next_reward is None or r[e, next_reward[0][e]] == next_reward[1][e]):
                     fit.append((a, b))
             assert fit, "no tied action reaches the device's next state in environment %d" % e
@@ -574,11 +629,14 @@ class RolloutReference(object):
         return a if a.kind == "lstm" else None
 
     # -------------------------------------------------------------------- windows
-    def begin_window(self, n_steps):
-        """collect()'s records: a batch holds ceil(T / horizon) episodes per environment, the most T transitions can end."""
+    def begin_window(self, n_steps, bootstrap_horizon=False):
+        """collect()'s records: a batch holds ceil(T / horizon) episodes per environment, the most T transitions can end;
+        with ``bootstrap_horizon`` each transition also returns the terminal values."""
         self.ep.load_records(self.ep.empty_records(-(-int(n_steps) // self.host.horizon)))
+        self.bootstrap_horizon, self.terminal_records = bool(bootstrap_horizon), []
 
     def end_window(self):
+        self.bootstrap_horizon = False
         return self.ep.save_records()
 
     def begin_run(self):

@@ -9,6 +9,7 @@ from oracle import cpu
 from overcooked_ai_b200.batched import BatchedOvercookedEnv
 from overcooked_ai_b200.greedy import GreedyHumanModel
 from overcooked_ai_b200.selfplay import AgentPairRollout, BCPolicy, RllibShapedCNN, SelfPlayRollout, records_forward
+from ppo_reference import gae_horizon_f32
 from test_gpu_bc_partner import POOL_5X4
 
 pytestmark = pytest.mark.gpu
@@ -30,22 +31,6 @@ def _np(t):
 
 def _dev(v, dt):
     return torch.from_numpy(np.ascontiguousarray(v)).cuda().to(dt)
-
-
-def gae_horizon_f32(r, v, d, tv, last, gamma, lam):
-    """include/ovc_horizon.h's recurrence in numpy float32 (every operation rounded on its own): r, v, tv [T, R], d [T, R]
-    or [T, R / 2] (one flag per environment of two rows), last [R]."""
-    T, R = r.shape
-    dd = np.repeat(d, R // d.shape[1], axis=1) != 0
-    g, gl = np.float32(gamma), np.float32(np.float32(gamma) * np.float32(lam))
-    A, nv = np.zeros(R, np.float32), last.astype(np.float32)
-    adv, tgt = np.empty_like(r), np.empty_like(r)
-    for t in reversed(range(T)):
-        nxt = np.where(dd[t], tv[t], nv).astype(np.float32)
-        delta = (r[t] + g * nxt) - v[t]
-        A = delta + (gl * np.where(dd[t], np.float32(0), np.float32(1))) * A
-        adv[t], tgt[t], nv = A, A + v[t], v[t]
-    return adv, tgt
 
 
 def _done_patterns(T, n, rng):

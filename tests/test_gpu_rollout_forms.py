@@ -4,12 +4,14 @@ float64 networks and the documented draws.
 ``CONFIGURATIONS`` maps a case name to its value on each axis of ``AXES``; ``build`` turns those values into the
 environment, the constructor arguments and the policy path the case claims.  tests/test_rollout_forms_cpu.py fails when a
 value, or a pair of values of two axes, has no case (unless ``REFUSED`` names the test that shows the constructor refuses
-it, or ``NOT_APPLICABLE`` says why it cannot occur), and when a constructor argument belongs to no axis.
+it, or ``NOT_APPLICABLE`` says why it cannot occur), and when a constructor or collect() argument belongs to no axis.
 
-Each case runs with and without CUDA graphs: two collect() windows (keep_logits in the second; between them the case's
-setters change and sync_weights() follows a second set of exact weights), every batch field and the live state after each
-window against the reference, then run() one transition at a time (each joint action checked) and the live state, the
-episode records and the counters again.  The kernels it launched must be the ones its path names.
+Each case runs with and without CUDA graphs: two collect() windows (keep_logits in the second, both with the case's
+bootstrap_horizon; between them the case's setters change and sync_weights() follows a second set of exact weights), every
+batch field and the live state after each window against the reference, then run() one transition at a time (each joint
+action checked) and the live state, the episode records and the counters again.  The kernels it launched must be the ones
+its path names.  A staggered case starts a few environments part-way into their episodes, so that transitions end some
+environments of a warp and not others.
 
 Exactness: the network agents are ``P.exact_cnn`` models (distinct seeds per member; K7 -> library layers -> the draw kernel
 runs on 5x5 grids), the BC agents ``_exact_bc``: every head and value is the float64 network's bit for bit, on the
@@ -25,7 +27,7 @@ import torch
 import policy_reference as P
 import rollout_reference as R
 from oracle import cpu
-from ppo_reference import gae_f32
+from ppo_reference import gae_f32, gae_horizon_f32
 
 GAMMA, LAM = 0.99, 0.95
 
@@ -33,15 +35,17 @@ GAMMA, LAM = 0.99, 0.95
 AXES = {
     "class": ["SelfPlayRollout", "AgentPairRollout"],
     "learner": ["cnn", "lstm", "blocks", "pairs", "pair_weights"],                       # SelfPlayRollout
-    "partner": ["none", "bc", "cnn", "population_fixed", "population_drawn"],            # SelfPlayRollout
+    "partner": ["none", "bc", "cnn", "population_fixed", "population_drawn", "greedy"],  # SelfPlayRollout
     "bc_factor": ["0", "fraction", "1"],                                                 # SelfPlayRollout with a partner
-    "agent0": ["cnn", "lstm", "bc"],                                                     # AgentPairRollout
-    "agent1": ["cnn", "lstm", "bc", "population_fixed", "population_drawn"],             # AgentPairRollout
+    "agent0": ["cnn", "lstm", "bc", "greedy"],                                           # AgentPairRollout
+    "agent1": ["cnn", "lstm", "bc", "population_fixed", "population_drawn", "greedy"],   # AgentPairRollout
     "seats": ["fixed", "swap", "random_seats"],                                          # AgentPairRollout
     "path": ["k7_k9_k8", "k7_library_draw", "k2_library_k8", "k2_library_draw", "float32", "learner_rows"],
     "starts": ["fixed", "random", "pool", "pool_redraw"],
     "use_phi": ["off", "on"],
     "episode_capacity": ["1", "2+"],
+    "bootstrap_horizon": ["off", "on"],                                                  # collect()'s
+    "phase": ["aligned", "staggered"],                                                   # the environments' timesteps
 }
 CLASS_AXES = {"SelfPlayRollout": ("learner", "partner", "bc_factor"), "AgentPairRollout": ("agent0", "agent1", "seats")}
 
@@ -60,8 +64,18 @@ NOT_AN_AXIS = {
     "reward_shaping_factor": "every case sets it, and changes it between its windows",
     "max_seq_len": "every LSTM case cuts its windows into chunks that episodes end inside and at",
 }
+# Every argument of collect() and the axis that covers it, or why no axis varies it.
+COLLECT_PARAMETERS = {"bootstrap_horizon": "bootstrap_horizon"}
+COLLECT_NOT_AN_AXIS = {
+    "n_steps": "every case collects windows of its own length T, longer than its horizon",
+    "gamma": "every case uses the same gamma: GAE's arithmetic is checked bit for bit, not its constants",
+    "lam": "every case uses the same lambda: GAE's arithmetic is checked bit for bit, not its constants",
+    "keep_logits": "every case collects its first window without and its second with keep_logits",
+}
 
-PARTNERS = ("bc", "cnn", "population_fixed", "population_drawn")
+PARTNERS = ("bc", "cnn", "population_fixed", "population_drawn", "greedy")
+HORIZON_REFUSED = "test_horizon_bootstrap_cpu.py::test_refused_configurations"
+SCRIPTED = ("bc", "greedy")  # agents without a network
 
 # (axis, value, axis, value, the existing CPU test that asserts the constructor refuses the pair)
 REFUSED = [
@@ -77,6 +91,8 @@ REFUSED = [
     ("learner", "pair_weights", "path", "k2_library_k8", "test_population_play_cpu.py::test_selfplay_refuses_population_play_beyond_k7"),
     ("learner", "pairs", "path", "k2_library_draw", "test_rollout_forms_cpu.py::test_selfplay_refuses_population_play_on_a_9x5_grid"),
     ("learner", "pair_weights", "path", "k2_library_draw", "test_rollout_forms_cpu.py::test_selfplay_refuses_population_play_on_a_9x5_grid"),
+    ("bootstrap_horizon", "on", "learner", ("lstm", "blocks", "pairs", "pair_weights"), HORIZON_REFUSED),
+    ("bootstrap_horizon", "on", "agent0", "lstm", HORIZON_REFUSED),
 ]
 
 # (axis, value, axis, value, why the pair cannot occur); a value may be "*" (every value) or a tuple of values
@@ -91,13 +107,15 @@ NOT_APPLICABLE = [
     ("partner", "none", "bc_factor", "*", "bc_factor weighs the partner's episodes"),
     ("partner", "none", "path", "learner_rows", "the learner runs on its own rows only next to a network partner"),
     ("partner", "bc", "path", "learner_rows", "the learner runs on its own rows only next to a network partner"),
+    ("partner", "greedy", "path", "learner_rows", "the learner runs on its own rows only next to a network partner"),
     ("learner", "lstm", "path", "learner_rows", "an LSTM learner runs on all 2N rows (K11 has no rows form)"),
     ("learner", "blocks", "path", "learner_rows", "the learner runs on its own rows only next to a partner"),
     ("learner", "pairs", "path", "learner_rows", "the learner runs on its own rows only next to a partner"),
     ("learner", "pair_weights", "path", "learner_rows", "the learner runs on its own rows only next to a partner"),
     ("path", "k2_library_k8", "starts", "fixed", "K2 -> library -> K8 runs on 5x4 pools of more than 8 layouts only"),
     ("path", "k2_library_k8", "starts", "random", "K2 -> library -> K8 runs on 5x4 pools of more than 8 layouts only"),
-    ("agent0", "bc", "agent1", "bc", "BC against BC evaluates no network: there is no policy path to claim"),
+    ("agent0", SCRIPTED, "agent1", SCRIPTED, "a BC or greedy agent against another evaluates no network: no path to claim"),
+    ("bootstrap_horizon", "on", "agent0", SCRIPTED, "a BC or greedy agent 0 has no collect(), so no bootstrap"),
     ("agent0", "*", "path", "learner_rows", "learner rows are a self-play mixture's"),
     ("agent1", "*", "path", "learner_rows", "learner rows are a self-play mixture's"),
     ("seats", "*", "path", "learner_rows", "learner rows are a self-play mixture's"),
@@ -105,71 +123,104 @@ NOT_APPLICABLE = [
 ] + [(a, "*", b, "*", "one axis is SelfPlayRollout's, the other AgentPairRollout's")
      for a in CLASS_AXES["SelfPlayRollout"] for b in CLASS_AXES["AgentPairRollout"]]
 
-# the cases: each value of every axis of its class and of the shared axes; sizes N, T, horizon and the LSTM's chunk
+# the cases: each value of every axis of its class and of the shared axes; sizes N, T, horizon and the LSTM's chunk.  The
+# sizes are free, with one constraint: pair_cnn_lstm_random_seats_k7_k9_k8_pool_phi1_cap2_bh1 runs at horizon 12, because
+# at 13 environment 0's LSTM agent 1 meets a near-tie at its episode's last step between picking up a dish and an action
+# that leaves the same reset record and reward; the reference cannot tell them apart (_settle), and the dish pickup shows
+# only in the episode's game statistics.
 CONFIGURATIONS = {
-    "sp_lstm_cnn_bcf_k2_library_draw_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "cnn", "bc_factor": "fraction", "path": "k2_library_draw", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "n": 97, "T": 17, "horizon": 7},
-    "pair_lstm_cnn_random_seats_k7_library_draw_pool_phi1_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "cnn", "seats": "random_seats", "path": "k7_library_draw", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "n": 101, "T": 18, "horizon": 8},
-    "sp_cnn_population_drawn_bc0_float32_fixed_phi1_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_drawn", "bc_factor": "0", "path": "float32", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "n": 103, "T": 19, "horizon": 9},
-    "pair_cnn_lstm_swap_k7_k9_k8_fixed_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "lstm", "seats": "swap", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "n": 107, "T": 17, "horizon": 10},
-    "pair_bc_population_fixed_fixed_k2_library_k8_pool_redraw_phi1_cap2": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "population_fixed", "seats": "fixed", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "on", "episode_capacity": "2+", "n": 109, "T": 18, "horizon": 11},
-    "sp_cnn_population_fixed_bc1_learner_rows_random_phi0_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_fixed", "bc_factor": "1", "path": "learner_rows", "starts": "random", "use_phi": "off", "episode_capacity": "2+", "n": 113, "T": 19, "horizon": 12},
-    "pair_bc_population_drawn_random_seats_float32_random_phi0_cap1": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "population_drawn", "seats": "random_seats", "path": "float32", "starts": "random", "use_phi": "off", "episode_capacity": "1", "n": 115, "T": 17, "horizon": 13},
-    "sp_lstm_bc_bc1_k2_library_k8_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "bc", "bc_factor": "1", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "n": 117, "T": 18, "horizon": 7},
-    "pair_cnn_bc_swap_k2_library_draw_random_phi1_cap2": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "bc", "seats": "swap", "path": "k2_library_draw", "starts": "random", "use_phi": "on", "episode_capacity": "2+", "n": 119, "T": 19, "horizon": 8},
-    "pair_lstm_bc_fixed_k7_library_draw_fixed_phi0_cap1": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "bc", "seats": "fixed", "path": "k7_library_draw", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "n": 121, "T": 17, "horizon": 9},
-    "sp_lstm_population_fixed_bcf_k7_k9_k8_pool_phi1_cap2": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_fixed", "bc_factor": "fraction", "path": "k7_k9_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "n": 123, "T": 18, "horizon": 10},
-    "sp_lstm_population_drawn_bc0_k7_library_draw_random_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_drawn", "bc_factor": "0", "path": "k7_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "1", "n": 125, "T": 19, "horizon": 11},
-    "sp_blocks_none_k2_library_draw_pool_phi0_cap1": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "k2_library_draw", "starts": "pool", "use_phi": "off", "episode_capacity": "1", "n": 127, "T": 17, "horizon": 12},
-    "sp_cnn_cnn_bc0_learner_rows_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "0", "path": "learner_rows", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "n": 97, "T": 18, "horizon": 13},
-    "sp_pairs_none_k7_k9_k8_random_phi1_cap2": {"class": "SelfPlayRollout", "learner": "pairs", "partner": "none", "path": "k7_k9_k8", "starts": "random", "use_phi": "on", "episode_capacity": "2+", "n": 101, "T": 19, "horizon": 7},
-    "pair_cnn_cnn_random_seats_k2_library_k8_pool_redraw_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "cnn", "seats": "random_seats", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "n": 103, "T": 17, "horizon": 8},
-    "pair_lstm_population_drawn_swap_k7_library_draw_pool_redraw_phi1_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "population_drawn", "seats": "swap", "path": "k7_library_draw", "starts": "pool_redraw", "use_phi": "on", "episode_capacity": "2+", "n": 107, "T": 18, "horizon": 9},
-    "sp_cnn_bc_bc0_k7_k9_k8_pool_redraw_phi0_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "bc", "bc_factor": "0", "path": "k7_k9_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "2+", "n": 109, "T": 19, "horizon": 10},
-    "pair_cnn_population_fixed_swap_float32_pool_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "population_fixed", "seats": "swap", "path": "float32", "starts": "pool", "use_phi": "off", "episode_capacity": "1", "n": 113, "T": 17, "horizon": 11},
-    "pair_lstm_lstm_fixed_k2_library_draw_random_phi1_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "lstm", "seats": "fixed", "path": "k2_library_draw", "starts": "random", "use_phi": "on", "episode_capacity": "2+", "n": 115, "T": 18, "horizon": 12},
-    "sp_pair_weights_none_k7_library_draw_fixed_phi1_cap2": {"class": "SelfPlayRollout", "learner": "pair_weights", "partner": "none", "path": "k7_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "n": 117, "T": 19, "horizon": 13},
-    "pair_bc_cnn_swap_k2_library_draw_fixed_phi1_cap1": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "cnn", "seats": "swap", "path": "k2_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "n": 119, "T": 17, "horizon": 7},
-    "pair_bc_population_drawn_fixed_k7_k9_k8_pool_phi0_cap2": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "population_drawn", "seats": "fixed", "path": "k7_k9_k8", "starts": "pool", "use_phi": "off", "episode_capacity": "2+", "n": 121, "T": 18, "horizon": 8},
-    "sp_cnn_cnn_bcf_k7_library_draw_random_phi0_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "fraction", "path": "k7_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "2+", "n": 123, "T": 19, "horizon": 9},
-    "sp_blocks_none_float32_pool_redraw_phi1_cap2": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "float32", "starts": "pool_redraw", "use_phi": "on", "episode_capacity": "2+", "n": 125, "T": 17, "horizon": 10},
-    "pair_lstm_population_fixed_random_seats_k7_k9_k8_fixed_phi0_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "population_fixed", "seats": "random_seats", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "2+", "n": 127, "T": 18, "horizon": 11},
-    "sp_cnn_population_fixed_bc0_k2_library_draw_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_fixed", "bc_factor": "0", "path": "k2_library_draw", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "n": 97, "T": 19, "horizon": 12},
-    "sp_lstm_cnn_bc1_k7_k9_k8_fixed_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "cnn", "bc_factor": "1", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "n": 101, "T": 17, "horizon": 13},
-    "pair_bc_lstm_random_seats_k7_library_draw_pool_phi0_cap2": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "lstm", "seats": "random_seats", "path": "k7_library_draw", "starts": "pool", "use_phi": "off", "episode_capacity": "2+", "n": 103, "T": 18, "horizon": 7},
-    "sp_cnn_population_drawn_bcf_k2_library_k8_pool_phi1_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_drawn", "bc_factor": "fraction", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "n": 107, "T": 19, "horizon": 8},
-    "pair_cnn_cnn_fixed_float32_random_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "cnn", "seats": "fixed", "path": "float32", "starts": "random", "use_phi": "off", "episode_capacity": "1", "n": 109, "T": 17, "horizon": 9},
-    "sp_cnn_bc_bcf_float32_fixed_phi0_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "bc", "bc_factor": "fraction", "path": "float32", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "n": 113, "T": 18, "horizon": 10},
-    "sp_lstm_population_drawn_bc1_k2_library_draw_pool_redraw_phi1_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_drawn", "bc_factor": "1", "path": "k2_library_draw", "starts": "pool_redraw", "use_phi": "on", "episode_capacity": "1", "n": 115, "T": 19, "horizon": 11},
-    "pair_lstm_bc_swap_k2_library_k8_pool_redraw_phi0_cap1": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "bc", "seats": "swap", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "n": 117, "T": 17, "horizon": 12},
-    "sp_pair_weights_none_k7_k9_k8_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "pair_weights", "partner": "none", "path": "k7_k9_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "n": 119, "T": 18, "horizon": 13},
-    "sp_pairs_none_k7_library_draw_pool_phi0_cap1": {"class": "SelfPlayRollout", "learner": "pairs", "partner": "none", "path": "k7_library_draw", "starts": "pool", "use_phi": "off", "episode_capacity": "1", "n": 121, "T": 19, "horizon": 7},
-    "pair_cnn_population_drawn_random_seats_k2_library_draw_fixed_phi1_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "population_drawn", "seats": "random_seats", "path": "k2_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "n": 123, "T": 17, "horizon": 8},
-    "sp_lstm_bc_bc1_k7_library_draw_random_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "bc", "bc_factor": "1", "path": "k7_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "1", "n": 125, "T": 18, "horizon": 9},
-    "sp_cnn_population_fixed_bc1_float32_fixed_phi1_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_fixed", "bc_factor": "1", "path": "float32", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "n": 127, "T": 19, "horizon": 10},
-    "sp_cnn_population_drawn_bcf_learner_rows_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_drawn", "bc_factor": "fraction", "path": "learner_rows", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "n": 97, "T": 17, "horizon": 11},
-    "pair_cnn_population_fixed_swap_k7_library_draw_random_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "population_fixed", "seats": "swap", "path": "k7_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "1", "n": 101, "T": 18, "horizon": 12},
-    "pair_cnn_bc_random_seats_float32_pool_phi1_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "bc", "seats": "random_seats", "path": "float32", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "n": 103, "T": 19, "horizon": 13},
-    "sp_blocks_none_k7_library_draw_fixed_phi1_cap2": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "k7_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "n": 107, "T": 17, "horizon": 7},
-    "sp_cnn_population_fixed_bc0_k2_library_k8_pool_phi0_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_fixed", "bc_factor": "0", "path": "k2_library_k8", "starts": "pool", "use_phi": "off", "episode_capacity": "2+", "n": 109, "T": 18, "horizon": 8},
-    "pair_lstm_lstm_fixed_k2_library_k8_pool_redraw_phi0_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "lstm", "seats": "fixed", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "2+", "n": 113, "T": 19, "horizon": 9},
-    "sp_blocks_none_k2_library_k8_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "n": 115, "T": 17, "horizon": 10},
-    "sp_blocks_none_k7_k9_k8_random_phi1_cap2": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "k7_k9_k8", "starts": "random", "use_phi": "on", "episode_capacity": "2+", "n": 117, "T": 18, "horizon": 11},
-    "sp_lstm_bc_bcf_k2_library_draw_pool_phi1_cap2": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "bc", "bc_factor": "fraction", "path": "k2_library_draw", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "n": 119, "T": 19, "horizon": 12},
-    "sp_cnn_cnn_bc1_float32_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "1", "path": "float32", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "n": 121, "T": 17, "horizon": 13},
-    "sp_pairs_none_k7_k9_k8_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "pairs", "partner": "none", "path": "k7_k9_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "n": 123, "T": 18, "horizon": 7},
-    "pair_lstm_population_drawn_fixed_k2_library_k8_pool_phi1_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "population_drawn", "seats": "fixed", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "n": 125, "T": 19, "horizon": 8},
-    "sp_lstm_population_fixed_bc0_k7_library_draw_pool_phi0_cap2": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_fixed", "bc_factor": "0", "path": "k7_library_draw", "starts": "pool", "use_phi": "off", "episode_capacity": "2+", "n": 127, "T": 17, "horizon": 9},
-    "pair_bc_cnn_random_seats_k7_k9_k8_pool_phi1_cap1": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "cnn", "seats": "random_seats", "path": "k7_k9_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "n": 97, "T": 18, "horizon": 10},
-    "pair_bc_population_fixed_random_seats_k2_library_draw_random_phi0_cap2": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "population_fixed", "seats": "random_seats", "path": "k2_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "2+", "n": 101, "T": 19, "horizon": 11},
-    "sp_lstm_none_k2_library_k8_pool_phi1_cap2": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "none", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "n": 103, "T": 17, "horizon": 12},
-    "pair_lstm_bc_random_seats_k7_k9_k8_fixed_phi0_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "bc", "seats": "random_seats", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "2+", "n": 107, "T": 18, "horizon": 13},
-    "sp_cnn_cnn_bc1_k2_library_k8_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "1", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "n": 109, "T": 19, "horizon": 7},
-    "sp_cnn_none_k2_library_draw_fixed_phi1_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "none", "path": "k2_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "n": 113, "T": 17, "horizon": 8},
-    "sp_cnn_cnn_bc1_learner_rows_fixed_phi1_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "1", "path": "learner_rows", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "n": 115, "T": 18, "horizon": 9},
-    "sp_lstm_population_drawn_bcf_k7_k9_k8_fixed_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_drawn", "bc_factor": "fraction", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "n": 117, "T": 19, "horizon": 10},
-    "sp_pairs_none_k7_library_draw_fixed_phi1_cap1": {"class": "SelfPlayRollout", "learner": "pairs", "partner": "none", "path": "k7_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "n": 119, "T": 17, "horizon": 11},
-    "sp_pair_weights_none_k7_library_draw_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "pair_weights", "partner": "none", "path": "k7_library_draw", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "n": 121, "T": 18, "horizon": 12},
-    "sp_pair_weights_none_k7_library_draw_random_phi1_cap1": {"class": "SelfPlayRollout", "learner": "pair_weights", "partner": "none", "path": "k7_library_draw", "starts": "random", "use_phi": "on", "episode_capacity": "1", "n": 123, "T": 19, "horizon": 13},
+    "sp_lstm_cnn_bcf_k2_library_draw_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "cnn", "bc_factor": "fraction", "path": "k2_library_draw", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 97, "T": 17, "horizon": 7},
+    "pair_lstm_cnn_random_seats_k7_library_draw_pool_phi1_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "cnn", "seats": "random_seats", "path": "k7_library_draw", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 101, "T": 18, "horizon": 8},
+    "sp_cnn_population_drawn_bc0_float32_fixed_phi1_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_drawn", "bc_factor": "0", "path": "float32", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 103, "T": 19, "horizon": 9},
+    "pair_cnn_lstm_swap_k7_k9_k8_fixed_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "lstm", "seats": "swap", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 107, "T": 17, "horizon": 10},
+    "pair_bc_population_fixed_fixed_k2_library_k8_pool_redraw_phi1_cap2": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "population_fixed", "seats": "fixed", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 109, "T": 18, "horizon": 11},
+    "sp_cnn_population_fixed_bc1_learner_rows_random_phi0_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_fixed", "bc_factor": "1", "path": "learner_rows", "starts": "random", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 113, "T": 19, "horizon": 12},
+    "pair_bc_population_drawn_random_seats_float32_random_phi0_cap1": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "population_drawn", "seats": "random_seats", "path": "float32", "starts": "random", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 115, "T": 17, "horizon": 13},
+    "sp_lstm_bc_bc1_k2_library_k8_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "bc", "bc_factor": "1", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 117, "T": 18, "horizon": 7},
+    "pair_cnn_bc_swap_k2_library_draw_random_phi1_cap2": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "bc", "seats": "swap", "path": "k2_library_draw", "starts": "random", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 119, "T": 19, "horizon": 8},
+    "pair_lstm_bc_fixed_k7_library_draw_fixed_phi0_cap1": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "bc", "seats": "fixed", "path": "k7_library_draw", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 121, "T": 17, "horizon": 9},
+    "sp_lstm_population_fixed_bcf_k7_k9_k8_pool_phi1_cap2": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_fixed", "bc_factor": "fraction", "path": "k7_k9_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 123, "T": 18, "horizon": 10},
+    "sp_lstm_population_drawn_bc0_k7_library_draw_random_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_drawn", "bc_factor": "0", "path": "k7_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 125, "T": 19, "horizon": 11},
+    "sp_blocks_none_k2_library_draw_pool_phi0_cap1": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "k2_library_draw", "starts": "pool", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 127, "T": 17, "horizon": 12},
+    "sp_cnn_cnn_bc0_learner_rows_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "0", "path": "learner_rows", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 97, "T": 18, "horizon": 13},
+    "sp_pairs_none_k7_k9_k8_random_phi1_cap2": {"class": "SelfPlayRollout", "learner": "pairs", "partner": "none", "path": "k7_k9_k8", "starts": "random", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 101, "T": 19, "horizon": 7},
+    "pair_cnn_cnn_random_seats_k2_library_k8_pool_redraw_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "cnn", "seats": "random_seats", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 103, "T": 17, "horizon": 8},
+    "pair_lstm_population_drawn_swap_k7_library_draw_pool_redraw_phi1_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "population_drawn", "seats": "swap", "path": "k7_library_draw", "starts": "pool_redraw", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 107, "T": 18, "horizon": 9},
+    "sp_cnn_bc_bc0_k7_k9_k8_pool_redraw_phi0_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "bc", "bc_factor": "0", "path": "k7_k9_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 109, "T": 19, "horizon": 10},
+    "pair_cnn_population_fixed_swap_float32_pool_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "population_fixed", "seats": "swap", "path": "float32", "starts": "pool", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 113, "T": 17, "horizon": 11},
+    "pair_lstm_lstm_fixed_k2_library_draw_random_phi1_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "lstm", "seats": "fixed", "path": "k2_library_draw", "starts": "random", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 115, "T": 18, "horizon": 12},
+    "sp_pair_weights_none_k7_library_draw_fixed_phi1_cap2": {"class": "SelfPlayRollout", "learner": "pair_weights", "partner": "none", "path": "k7_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 117, "T": 19, "horizon": 13},
+    "pair_bc_cnn_swap_k2_library_draw_fixed_phi1_cap1": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "cnn", "seats": "swap", "path": "k2_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 119, "T": 17, "horizon": 7},
+    "pair_bc_population_drawn_fixed_k7_k9_k8_pool_phi0_cap2": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "population_drawn", "seats": "fixed", "path": "k7_k9_k8", "starts": "pool", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 121, "T": 18, "horizon": 8},
+    "sp_cnn_cnn_bcf_k7_library_draw_random_phi0_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "fraction", "path": "k7_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 123, "T": 19, "horizon": 9},
+    "sp_blocks_none_float32_pool_redraw_phi1_cap2": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "float32", "starts": "pool_redraw", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 125, "T": 17, "horizon": 10},
+    "pair_lstm_population_fixed_random_seats_k7_k9_k8_fixed_phi0_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "population_fixed", "seats": "random_seats", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 127, "T": 18, "horizon": 11},
+    "sp_cnn_population_fixed_bc0_k2_library_draw_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_fixed", "bc_factor": "0", "path": "k2_library_draw", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 97, "T": 19, "horizon": 12},
+    "sp_lstm_cnn_bc1_k7_k9_k8_fixed_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "cnn", "bc_factor": "1", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 101, "T": 17, "horizon": 13},
+    "pair_bc_lstm_random_seats_k7_library_draw_pool_phi0_cap2": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "lstm", "seats": "random_seats", "path": "k7_library_draw", "starts": "pool", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 103, "T": 18, "horizon": 7},
+    "sp_cnn_population_drawn_bcf_k2_library_k8_pool_phi1_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_drawn", "bc_factor": "fraction", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 107, "T": 19, "horizon": 8},
+    "pair_cnn_cnn_fixed_float32_random_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "cnn", "seats": "fixed", "path": "float32", "starts": "random", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 109, "T": 17, "horizon": 9},
+    "sp_cnn_bc_bcf_float32_fixed_phi0_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "bc", "bc_factor": "fraction", "path": "float32", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 113, "T": 18, "horizon": 10},
+    "sp_lstm_population_drawn_bc1_k2_library_draw_pool_redraw_phi1_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_drawn", "bc_factor": "1", "path": "k2_library_draw", "starts": "pool_redraw", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 115, "T": 19, "horizon": 11},
+    "pair_lstm_bc_swap_k2_library_k8_pool_redraw_phi0_cap1": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "bc", "seats": "swap", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 117, "T": 17, "horizon": 12},
+    "sp_pair_weights_none_k7_k9_k8_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "pair_weights", "partner": "none", "path": "k7_k9_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 119, "T": 18, "horizon": 13},
+    "sp_pairs_none_k7_library_draw_pool_phi0_cap1": {"class": "SelfPlayRollout", "learner": "pairs", "partner": "none", "path": "k7_library_draw", "starts": "pool", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 121, "T": 19, "horizon": 7},
+    "pair_cnn_population_drawn_random_seats_k2_library_draw_fixed_phi1_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "population_drawn", "seats": "random_seats", "path": "k2_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 123, "T": 17, "horizon": 8},
+    "sp_lstm_bc_bc1_k7_library_draw_random_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "bc", "bc_factor": "1", "path": "k7_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 125, "T": 18, "horizon": 9},
+    "sp_cnn_population_fixed_bc1_float32_fixed_phi1_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_fixed", "bc_factor": "1", "path": "float32", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 127, "T": 19, "horizon": 10},
+    "sp_cnn_population_drawn_bcf_learner_rows_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_drawn", "bc_factor": "fraction", "path": "learner_rows", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 97, "T": 17, "horizon": 11},
+    "pair_cnn_population_fixed_swap_k7_library_draw_random_phi0_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "population_fixed", "seats": "swap", "path": "k7_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 101, "T": 18, "horizon": 12},
+    "pair_cnn_bc_random_seats_float32_pool_phi1_cap1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "bc", "seats": "random_seats", "path": "float32", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 103, "T": 19, "horizon": 13},
+    "sp_blocks_none_k7_library_draw_fixed_phi1_cap2": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "k7_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 107, "T": 17, "horizon": 7},
+    "sp_cnn_population_fixed_bc0_k2_library_k8_pool_phi0_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_fixed", "bc_factor": "0", "path": "k2_library_k8", "starts": "pool", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 109, "T": 18, "horizon": 8},
+    "pair_lstm_lstm_fixed_k2_library_k8_pool_redraw_phi0_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "lstm", "seats": "fixed", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 113, "T": 19, "horizon": 9},
+    "sp_blocks_none_k2_library_k8_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 115, "T": 17, "horizon": 10},
+    "sp_blocks_none_k7_k9_k8_random_phi1_cap2": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "k7_k9_k8", "starts": "random", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 117, "T": 18, "horizon": 11},
+    "sp_lstm_bc_bcf_k2_library_draw_pool_phi1_cap2": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "bc", "bc_factor": "fraction", "path": "k2_library_draw", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 119, "T": 19, "horizon": 12},
+    "sp_cnn_cnn_bc1_float32_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "1", "path": "float32", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 121, "T": 17, "horizon": 13},
+    "sp_pairs_none_k7_k9_k8_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "pairs", "partner": "none", "path": "k7_k9_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 123, "T": 18, "horizon": 7},
+    "pair_lstm_population_drawn_fixed_k2_library_k8_pool_phi1_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "population_drawn", "seats": "fixed", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 125, "T": 19, "horizon": 8},
+    "sp_lstm_population_fixed_bc0_k7_library_draw_pool_phi0_cap2": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_fixed", "bc_factor": "0", "path": "k7_library_draw", "starts": "pool", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 127, "T": 17, "horizon": 9},
+    "pair_bc_cnn_random_seats_k7_k9_k8_pool_phi1_cap1": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "cnn", "seats": "random_seats", "path": "k7_k9_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 97, "T": 18, "horizon": 10},
+    "pair_bc_population_fixed_random_seats_k2_library_draw_random_phi0_cap2": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "population_fixed", "seats": "random_seats", "path": "k2_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 101, "T": 19, "horizon": 11},
+    "sp_lstm_none_k2_library_k8_pool_phi1_cap2": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "none", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 103, "T": 17, "horizon": 12},
+    "pair_lstm_bc_random_seats_k7_k9_k8_fixed_phi0_cap2": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "bc", "seats": "random_seats", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 107, "T": 18, "horizon": 13},
+    "sp_cnn_cnn_bc1_k2_library_k8_pool_redraw_phi0_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "1", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 109, "T": 19, "horizon": 7},
+    "sp_cnn_none_k2_library_draw_fixed_phi1_cap2": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "none", "path": "k2_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "aligned", "n": 113, "T": 17, "horizon": 8},
+    "sp_cnn_cnn_bc1_learner_rows_fixed_phi1_cap1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "1", "path": "learner_rows", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 115, "T": 18, "horizon": 9},
+    "sp_lstm_population_drawn_bcf_k7_k9_k8_fixed_phi0_cap1": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "population_drawn", "bc_factor": "fraction", "path": "k7_k9_k8", "starts": "fixed", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 117, "T": 19, "horizon": 10},
+    "sp_pairs_none_k7_library_draw_fixed_phi1_cap1": {"class": "SelfPlayRollout", "learner": "pairs", "partner": "none", "path": "k7_library_draw", "starts": "fixed", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 119, "T": 17, "horizon": 11},
+    "sp_pair_weights_none_k7_library_draw_pool_phi1_cap1": {"class": "SelfPlayRollout", "learner": "pair_weights", "partner": "none", "path": "k7_library_draw", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 121, "T": 18, "horizon": 12},
+    "sp_pair_weights_none_k7_library_draw_random_phi1_cap1": {"class": "SelfPlayRollout", "learner": "pair_weights", "partner": "none", "path": "k7_library_draw", "starts": "random", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 123, "T": 19, "horizon": 13},
+    "sp_cnn_greedy_bcf_k7_library_draw_pool_redraw_phi0_cap2_bh1_stag": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "greedy", "bc_factor": "fraction", "path": "k7_library_draw", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "on", "phase": "staggered", "n": 125, "T": 17, "horizon": 7},
+    "pair_cnn_greedy_fixed_k7_k9_k8_pool_phi1_cap1_bh1_stag": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "greedy", "seats": "fixed", "path": "k7_k9_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "on", "phase": "staggered", "n": 127, "T": 18, "horizon": 8},
+    "pair_greedy_cnn_swap_float32_fixed_phi1_cap2_stag": {"class": "AgentPairRollout", "agent0": "greedy", "agent1": "cnn", "seats": "swap", "path": "float32", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "staggered", "n": 97, "T": 19, "horizon": 9},
+    "pair_greedy_population_drawn_random_seats_k7_k9_k8_random_phi0_cap1_stag": {"class": "AgentPairRollout", "agent0": "greedy", "agent1": "population_drawn", "seats": "random_seats", "path": "k7_k9_k8", "starts": "random", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "staggered", "n": 101, "T": 17, "horizon": 10},
+    "pair_cnn_greedy_random_seats_k7_library_draw_pool_redraw_phi0_cap2_bh1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "greedy", "seats": "random_seats", "path": "k7_library_draw", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "on", "phase": "aligned", "n": 103, "T": 18, "horizon": 11},
+    "sp_lstm_greedy_bc1_k2_library_k8_pool_phi1_cap1_stag": {"class": "SelfPlayRollout", "learner": "lstm", "partner": "greedy", "bc_factor": "1", "path": "k2_library_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "staggered", "n": 107, "T": 19, "horizon": 12},
+    "sp_cnn_greedy_bc0_k2_library_draw_random_phi1_cap1_bh1_stag": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "greedy", "bc_factor": "0", "path": "k2_library_draw", "starts": "random", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "on", "phase": "staggered", "n": 109, "T": 17, "horizon": 13},
+    "pair_greedy_lstm_fixed_k2_library_k8_pool_redraw_phi0_cap2_stag": {"class": "AgentPairRollout", "agent0": "greedy", "agent1": "lstm", "seats": "fixed", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "staggered", "n": 113, "T": 18, "horizon": 7},
+    "pair_greedy_population_fixed_swap_k2_library_draw_random_phi0_cap1_stag": {"class": "AgentPairRollout", "agent0": "greedy", "agent1": "population_fixed", "seats": "swap", "path": "k2_library_draw", "starts": "random", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "staggered", "n": 115, "T": 19, "horizon": 8},
+    "sp_cnn_greedy_bc1_float32_fixed_phi1_cap2_bh1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "greedy", "bc_factor": "1", "path": "float32", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "on", "phase": "aligned", "n": 117, "T": 17, "horizon": 9},
+    "sp_cnn_greedy_bcf_k7_k9_k8_pool_redraw_phi0_cap1_bh1_stag": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "greedy", "bc_factor": "fraction", "path": "k7_k9_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "on", "phase": "staggered", "n": 119, "T": 18, "horizon": 10},
+    "pair_cnn_greedy_swap_float32_random_phi0_cap1_bh1_stag": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "greedy", "seats": "swap", "path": "float32", "starts": "random", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "on", "phase": "staggered", "n": 121, "T": 19, "horizon": 11},
+    "pair_lstm_greedy_random_seats_k2_library_k8_pool_redraw_phi0_cap1_stag": {"class": "AgentPairRollout", "agent0": "lstm", "agent1": "greedy", "seats": "random_seats", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "staggered", "n": 123, "T": 17, "horizon": 12},
+    "pair_greedy_population_drawn_random_seats_k7_library_draw_pool_phi1_cap1": {"class": "AgentPairRollout", "agent0": "greedy", "agent1": "population_drawn", "seats": "random_seats", "path": "k7_library_draw", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "aligned", "n": 125, "T": 18, "horizon": 13},
+    "pair_cnn_greedy_fixed_k2_library_draw_fixed_phi0_cap2_bh1_stag": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "greedy", "seats": "fixed", "path": "k2_library_draw", "starts": "fixed", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "on", "phase": "staggered", "n": 127, "T": 19, "horizon": 7},
+    "sp_cnn_cnn_bc1_learner_rows_pool_phi0_cap2_bh1_stag": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "cnn", "bc_factor": "1", "path": "learner_rows", "starts": "pool", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "on", "phase": "staggered", "n": 97, "T": 17, "horizon": 8},
+    "sp_cnn_population_fixed_bcf_k2_library_k8_pool_redraw_phi0_cap1_bh1_stag": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_fixed", "bc_factor": "fraction", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "on", "phase": "staggered", "n": 101, "T": 18, "horizon": 9},
+    "sp_pairs_none_k7_k9_k8_random_phi1_cap2_stag": {"class": "SelfPlayRollout", "learner": "pairs", "partner": "none", "path": "k7_k9_k8", "starts": "random", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "staggered", "n": 103, "T": 19, "horizon": 10},
+    "sp_cnn_bc_bcf_k7_k9_k8_pool_redraw_phi1_cap1_bh1_stag": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "bc", "bc_factor": "fraction", "path": "k7_k9_k8", "starts": "pool_redraw", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "on", "phase": "staggered", "n": 107, "T": 17, "horizon": 11},
+    "pair_cnn_bc_random_seats_float32_pool_phi1_cap2_bh1_stag": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "bc", "seats": "random_seats", "path": "float32", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "on", "phase": "staggered", "n": 109, "T": 18, "horizon": 12},
+    "sp_cnn_population_drawn_bcf_k7_library_draw_pool_redraw_phi0_cap1_bh1_stag": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "population_drawn", "bc_factor": "fraction", "path": "k7_library_draw", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "on", "phase": "staggered", "n": 113, "T": 19, "horizon": 13},
+    "sp_blocks_none_k2_library_k8_pool_redraw_phi0_cap1_stag": {"class": "SelfPlayRollout", "learner": "blocks", "partner": "none", "path": "k2_library_k8", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "staggered", "n": 115, "T": 17, "horizon": 7},
+    "pair_bc_cnn_swap_float32_pool_phi1_cap2_stag": {"class": "AgentPairRollout", "agent0": "bc", "agent1": "cnn", "seats": "swap", "path": "float32", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "off", "phase": "staggered", "n": 117, "T": 18, "horizon": 8},
+    "pair_cnn_cnn_fixed_k7_k9_k8_random_phi0_cap1_bh1_stag": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "cnn", "seats": "fixed", "path": "k7_k9_k8", "starts": "random", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "on", "phase": "staggered", "n": 119, "T": 19, "horizon": 9},
+    "sp_cnn_none_float32_fixed_phi1_cap2_bh1": {"class": "SelfPlayRollout", "learner": "cnn", "partner": "none", "path": "float32", "starts": "fixed", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "on", "phase": "aligned", "n": 121, "T": 17, "horizon": 10},
+    "pair_cnn_population_fixed_random_seats_float32_fixed_phi0_cap2_bh1_stag": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "population_fixed", "seats": "random_seats", "path": "float32", "starts": "fixed", "use_phi": "off", "episode_capacity": "2+", "bootstrap_horizon": "on", "phase": "staggered", "n": 123, "T": 18, "horizon": 11},
+    "pair_cnn_population_drawn_swap_float32_pool_redraw_phi0_cap1_bh1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "population_drawn", "seats": "swap", "path": "float32", "starts": "pool_redraw", "use_phi": "off", "episode_capacity": "1", "bootstrap_horizon": "on", "phase": "aligned", "n": 125, "T": 19, "horizon": 12},
+    "pair_cnn_lstm_random_seats_k7_k9_k8_pool_phi1_cap2_bh1": {"class": "AgentPairRollout", "agent0": "cnn", "agent1": "lstm", "seats": "random_seats", "path": "k7_k9_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "2+", "bootstrap_horizon": "on", "phase": "aligned", "n": 127, "T": 17, "horizon": 12},
+    "sp_pair_weights_none_k7_k9_k8_pool_phi1_cap1_stag": {"class": "SelfPlayRollout", "learner": "pair_weights", "partner": "none", "path": "k7_k9_k8", "starts": "pool", "use_phi": "on", "episode_capacity": "1", "bootstrap_horizon": "off", "phase": "staggered", "n": 97, "T": 18, "horizon": 7},
 }
 
 
@@ -187,6 +238,17 @@ GRIDS = {  # path -> (the single layout, the pool); K2 -> library -> K8 needs mo
     "k2_library_k8": (None, None),
     "k2_library_draw": ("asymmetric_advantages", ["asymmetric_advantages", "counter_circuit", "cramped_corridor"]),
 }
+# A case with a greedy agent plays layouts of one 3-onion order only (GreedyHumanModel's ml_action asserts it): mdp_test,
+# bonus_order_test, counter_circuit and cramped_corridor do not qualify.  Nine 5x4 layouts (duplicates allowed) turn K7 off
+# for K2 -> library -> K8; on the 9x5 grid only asymmetric_advantages qualifies, so no pool there.
+GREEDY_POOL_5X4 = ["cramped_room", "m_shaped_s", "simple_o"]
+GREEDY_GRIDS = {
+    "k7_k9_k8": ("cramped_room", GREEDY_POOL_5X4),
+    "float32": ("cramped_room", GREEDY_POOL_5X4),
+    "k7_library_draw": GRIDS["k7_library_draw"],
+    "k2_library_k8": (None, GREEDY_POOL_5X4 * 3),
+    "k2_library_draw": ("asymmetric_advantages", None),
+}
 BC_FACTOR = {"0": 0.0, "fraction": 0.6, "1": 1.0}
 BC_FACTOR_LATER = {"0": 0.5, "fraction": 0.25, "1": 0.8}
 WEIGHTS, WEIGHTS_LATER = [1.0, 2.0, 0.5], [0.5, 0.0, 2.0]
@@ -197,6 +259,21 @@ SEQ_LEN = 4
 # its arguments, not only their defaults (AgentPairRollout takes no such arguments: its agents follow the defaults)
 FUSED = {"k7_k9_k8": (True, True, True), "learner_rows": (True, True, True), "k7_library_draw": (True, False, False),
          "k2_library_k8": (False, True, False), "k2_library_draw": (False, False, False), "float32": (False, False, False)}
+
+
+def is_greedy(case):
+    return "greedy" in (case.get("partner"), case.get("agent0"), case.get("agent1"))
+
+
+def staggered_timesteps(n, horizon):
+    """The staggered phase's starting timesteps: 0 but for one environment in each warp of 32 from the second on, at
+    horizon - 1 in odd warps (its episode ends alone at the first transition, where the start it resets to is the one it
+    played from) and at horizon // 2 in even ones.  The first warp, and every warp at its common horizon, ends every
+    environment at once; the others end one environment alone, or all but one."""
+    t = np.zeros(n, np.int32)
+    for w in range(1, -(-n // 32)):
+        t[32 * w + (7 * w) % min(32, n - 32 * w)] = horizon - 1 if w % 2 else horizon // 2
+    return t
 
 
 def passed_arguments(case):
@@ -219,12 +296,12 @@ def passed_arguments(case):
 
 
 def _env(case, seed):
-    """(env, cpu.random_start or None) of the case's starts on the grid its path runs on."""
+    """(env, cpu.random_start or None) of the case's starts on the grid its path runs on, at the case's phase."""
     from overcooked_ai_b200.batched import BatchedOvercookedEnv
 
-    single, pool = GRIDS[case["path"]]
-    if single is None:
-        single, pool = None, _pool_5x4()
+    single, pool = (GREEDY_GRIDS if is_greedy(case) else GRIDS)[case["path"]]
+    if pool is None and not is_greedy(case):
+        pool = _pool_5x4()
     n, st = case["n"], case["starts"]
     kw = dict(horizon=case["horizon"], auto_reset=True)
     rs = None
@@ -241,7 +318,10 @@ def _env(case, seed):
         layouts = pool
         kw.update(random_layout=True, seed=seed)
         rs = cpu.random_start(seed, 0.0, False, True)
-    return BatchedOvercookedEnv(layouts, n, **kw), rs
+    env = BatchedOvercookedEnv(layouts, n, **kw)
+    if case["phase"] == "staggered":  # word 0 of a record is its timestep (DESIGN §3)
+        env.state[:, 0] = torch.from_numpy(staggered_timesteps(n, case["horizon"])).to(env.device)
+    return env, rs
 
 
 def _host(env, rs, use_phi):
@@ -250,7 +330,7 @@ def _host(env, rs, use_phi):
     lut = np.stack([l.feature_lut() for l in env.layouts]).view(np.uint8).reshape(env.n_layouts, -1)
     pot = L.build_potential_tables(env.layouts, R.PHI_GAMMA) if use_phi else None
     return R.EnvHost(env._tab_host, env._starts_host, env.horizon, rs, env.layouts[0].width, env.layouts[0].height, lut, pot,
-                     np.stack([l.deliver_value for l in env.layouts]), env.n_envs)
+                     np.stack([l.deliver_value for l in env.layouts]), env.n_envs, env.layouts)
 
 
 class _Models(object):
@@ -263,8 +343,11 @@ class _Models(object):
 
     def _weights(self, kind, seed, head_scale=30.0):
         from test_gpu_bc_partner import _exact_bc
+        from overcooked_ai_b200.greedy import GreedyHumanModel
         from overcooked_ai_b200.selfplay import RllibLSTMShapedCNN
 
+        if kind == "greedy":
+            return GreedyHumanModel()
         if kind == "cnn":
             return P.exact_cnn(self.W, self.H, seed, cook_time=self.cook)
         if kind == "bc":
@@ -286,6 +369,8 @@ class _Models(object):
 
     def second(self):
         for m, kind, seed, scale in self.made:
+            if kind == "greedy":  # no weights
+                continue
             m.load_state_dict(self._weights(kind, seed + 1000, scale).state_dict())
 
 
@@ -322,7 +407,7 @@ def build(case, use_graph, seed=7):
         elif learner == "pair_weights":
             kw["pair_weights"] = spec["pair_weights"] = PAIR_WEIGHTS
         partner = case["partner"]
-        p = None if partner == "none" else models.make(partner, 11) if partner in ("bc", "cnn") else _population(models)
+        p = None if partner == "none" else models.make(partner, 11) if partner in ("bc", "cnn", "greedy") else _population(models)
         if p is not None:
             kw["partner"] = p
             kw["bc_factor"] = spec["bc_factor"] = BC_FACTOR[case["bc_factor"]]
@@ -340,7 +425,7 @@ def build(case, use_graph, seed=7):
     else:
         a0 = models.make(case["agent0"], 1)
         a1 = case["agent1"]
-        a1 = models.make(a1, 11, head_scale=1.0) if a1 in ("cnn", "bc", "lstm") else _population(models)
+        a1 = models.make(a1, 11, head_scale=1.0) if a1 in ("cnn", "bc", "lstm", "greedy") else _population(models)
         if case["agent1"] == "population_fixed":
             member = rng.randint(0, 3, size=n)
             kw["member"], spec["member"] = dev(member), member
@@ -355,6 +440,8 @@ def build(case, use_graph, seed=7):
         assert set(kw) | {"env", "agents"} == passed_arguments(case), sorted(set(kw) ^ passed_arguments(case))
         ro = AgentPairRollout(env, (a0, a1), **kw)
         spec.update(kind="pair", agents=(a0, a1), factor=1.0)
+    if case["phase"] == "staggered":  # construction kept the timesteps
+        assert np.array_equal(_np(env.state[:, 0]), staggered_timesteps(n, case["horizon"])), "phase"
     return ro, spec, models, env, rs
 
 
@@ -425,12 +512,13 @@ def _close(got, want, tol=R.REPLAY_TOL):
     return np.abs(np.asarray(got, np.float64) - want) <= tol * (1 + np.abs(want))
 
 
-def _check_window(ro, ref, b, T, keep_logits, where, live_h=None):
+def _check_window(ro, ref, b, T, keep_logits, where, live_h=None, bootstrap=False):
     n, pair = ro.env.n_envs, ref.pair_kind
     e = np.arange(n)
     st, ac, dn = _np(b.states), _np(b.actions), _np(b.dones)
     lstm = ref.lstm_agent() is not None
-    ref.begin_window(T)
+    assert (b.terminal_values is None) == (not bootstrap), where
+    ref.begin_window(T, bootstrap)
     outs = []
     for t in range(T):
         p0 = 1 - ref.partner_seat if pair else None
@@ -499,7 +587,13 @@ def _check_window(ro, ref, b, T, keep_logits, where, live_h=None):
     # GAE on the reference's rewards and dones, and its values (the device's own for the LSTM, whose values are not exact)
     v = np.where(mask, gv if lstm else values, 0).astype(np.float32)
     lv = _np(b.last_values) if lstm else last
-    adv, tgt = (R.gae_view_f32 if pair else gae_f32)(want_r, v, dn, lv, GAMMA, LAM)
+    if bootstrap:  # the terminal values on every row, the zeros included; GAE bootstraps from them at each episode end
+        tv = pick("terminal_values")
+        got = _np(b.terminal_values)
+        assert np.array_equal(got.view(np.int32), tv.view(np.int32)), (where, np.argwhere(got != tv)[:8].tolist())
+        adv, tgt = gae_horizon_f32(want_r, v, dn, tv, np.asarray(lv, np.float32), GAMMA, LAM)
+    else:
+        adv, tgt = (R.gae_view_f32 if pair else gae_f32)(want_r, v, dn, lv, GAMMA, LAM)
     assert np.array_equal(_np(b.advantages)[mask], adv[mask]), where
     assert np.array_equal(_np(b.value_targets)[mask], tgt[mask]), where
     _check_records(b.episodes, ref.ep.finished(), where)
@@ -508,11 +602,15 @@ def _check_window(ro, ref, b, T, keep_logits, where, live_h=None):
     return outs
 
 
-def _certify(ref, case):
+def _certify(ref, case, states=None):
     """The exactness premise on this path: every accumulation of every exact network, with its current weights, is
-    certified on the reference's current states, with operands of at most 8 significant bits (bf16; TF32 keeps 11,
-    float32 24).  ``P.exact_cnn`` bounds every unit over all encodings; this checks that claim where it is relied on."""
-    obs = cpu.encode_lossless(ref.host.tables, ref.state, ref.host.W, ref.host.H, ref.host.horizon)
+    certified on the reference's current states (or ``states``: the window's terminal records), with operands of at most
+    8 significant bits (bf16; TF32 keeps 11, float32 24).  ``P.exact_cnn`` bounds every unit over all encodings; this
+    checks that claim where it is relied on."""
+    states = ref.state if states is None else states
+    if len(states) == 0:
+        return
+    obs = cpu.encode_lossless(ref.host.tables, states, ref.host.W, ref.host.H, ref.host.horizon)
     tf32 = torch.backends.cuda.matmul.allow_tf32
     for a in ref.agents():
         if a.kind != "cnn":
@@ -568,6 +666,26 @@ def _check_path(case, models, names):
     if path == "learner_rows":
         assert has("ovc::learner_rows_kernel") and has("ovc::encode_linear_masked"), (case, sorted(names))
     assert has("ovc::partner_policy") == ("bc" in kinds), (case, sorted(names))
+    assert has("ovc::greedy_actions_kernel") == ("greedy" in kinds), (case, sorted(names))
+
+
+def _check_window_path(case, names):
+    """The kernels of the first eager collect() window: with bootstrap_horizon, the compaction (ovc_horizon_rows) and K7's
+    rows form exactly where the learner runs K7 -> K9 -> K8 (a network partner's members run the rows form too), and the
+    horizon GAE in the batch's form (two views, or agent 0's one) in place of the plain GAE kernel."""
+    has = lambda prefix: any(k.startswith(prefix) for k in names)
+    on = case["bootstrap_horizon"] == "on"
+    fused = case["path"] in ("k7_k9_k8", "learner_rows")
+    rows_form = any(re.fullmatch(r"ovc::encode_linear_kernel<\d+,1,1>", k) for k in names)
+    assert has("ovc::horizon_rows_kernel") == (on and fused), (case, sorted(names))
+    if case.get("partner", case.get("agent1")) in ("cnn", "population_fixed", "population_drawn"):
+        assert rows_form or not (on and fused), (case, sorted(names))
+    else:
+        assert rows_form == (on and fused), (case, sorted(names))
+    form = "float" if case["class"] == "AgentPairRollout" else "float2"
+    horizon_gae = {k for k in names if k.startswith("ovc::gae_horizon_kernel")}
+    assert horizon_gae == ({"ovc::gae_horizon_kernel<%s>" % form} if on else set()), (case, sorted(names))
+    assert has("ovc::gae_kernel<") == (not on), (case, sorted(names))
 
 
 # ---------------------------------------------------------------------------------------------------------- the test
@@ -587,7 +705,8 @@ def test_rollout_form_vs_reference(name, use_graph):
     certify()
     _check_live(ro, ref, "construction")
     T = case["T"]
-    collect_agent0 = case.get("agent0") != "bc"
+    bootstrap = case["bootstrap_horizon"] == "on"
+    collect_agent0 = case.get("agent0") not in SCRIPTED
     if collect_agent0:
         for w in range(2):
             if w == 1:
@@ -598,10 +717,18 @@ def test_rollout_form_vs_reference(name, use_graph):
                 certify()  # the second weights, on the states the first window reached
             lstm = ref.lstm_agent()
             live_h = None if lstm is None else _np((ro.h if not ref.pair_kind else ro.agents[0].h).float()).copy()
-            b = ro.collect(T, GAMMA, LAM, keep_logits=w == 1)
-            _check_window(ro, ref, b, T, w == 1, (name, "window", w), live_h)
+            collect = lambda: ro.collect(T, GAMMA, LAM, keep_logits=w == 1, bootstrap_horizon=bootstrap)
+            if w == 0 and not use_graph:  # the kernels of the first eager window
+                got = []
+                _check_window_path(case, _launched(lambda: got.append(collect())))
+                b = got[0]
+            else:
+                b = collect()
+            _check_window(ro, ref, b, T, w == 1, (name, "window", w), live_h, bootstrap)
+            if bootstrap and not use_graph:  # the terminal values are exact only where the premise holds on their records
+                _certify(ref, name, np.concatenate(ref.terminal_records))
             _check_live(ro, ref, (name, "after window", w))
-    else:  # a BC agent 0 has no learner: run() only
+    else:  # a BC or greedy agent 0 has no learner: run() only
         _setters(ro, ref, case)
     certify()
     ref.begin_run()

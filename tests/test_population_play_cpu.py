@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from overcooked_ai_b200 import _native
+from overcooked_ai_b200.greedy import GreedyHumanModel
 from overcooked_ai_b200.selfplay import (BCPolicy, RllibLSTMShapedCNN, RllibShapedCNN, SelfPlayRollout, member_thresholds,
                                          pair_thresholds)
 
@@ -168,6 +169,8 @@ def test_selfplay_refuses_population_play_with_what_it_excludes():
         SelfPlayRollout(env, two, pair_weights=uniform, blocks=[4, 4])
     with pytest.raises(AssertionError, match="no partner"):
         SelfPlayRollout(env, two, pairs=pairs, partner=BCPolicy(), bc_factor=0.5)
+    with pytest.raises(AssertionError, match="no partner"):
+        SelfPlayRollout(env, two, pair_weights=uniform, partner=GreedyHumanModel(), bc_factor=0.5)
     with pytest.raises(AssertionError, match="LSTM member"):
         SelfPlayRollout(env, [RllibShapedCNN(5, 4), RllibLSTMShapedCNN(5, 4)], pair_weights=uniform)
     with pytest.raises(AssertionError, match="autocast_dtype=None"):

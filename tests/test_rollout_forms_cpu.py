@@ -1,6 +1,7 @@
 """The rollout driver's configuration table (tests/test_gpu_rollout_forms.py) covers every axis value, every pair of values of
-two axes (unless the pair is refused by the constructor, with the test that shows it, or cannot occur), and every
-constructor argument of SelfPlayRollout and AgentPairRollout; and the refusals it names exist."""
+two axes (unless the pair is refused by the constructor, with the test that shows it, or cannot occur), every
+constructor argument of SelfPlayRollout and AgentPairRollout and every argument of their collect(); and the refusals it
+names exist."""
 import inspect
 import itertools
 from types import SimpleNamespace
@@ -85,6 +86,43 @@ def test_every_constructor_argument_belongs_to_an_axis_and_some_case_passes_it()
         assert axis in G.AXES, (p, axis)
     passed = set().union(*(G.passed_arguments(c) for c in G.CONFIGURATIONS.values()))
     assert params <= passed, "constructor arguments no case passes: %s" % sorted(params - passed)
+
+
+def test_every_collect_argument_belongs_to_an_axis_or_has_a_reason():
+    """A new collect() argument fails here until it is given an axis (or listed with the reason no axis varies it); the
+    flag of the horizon bootstrap is passed by some case that collects."""
+    params = set()
+    for cls in (SelfPlayRollout, AgentPairRollout):
+        params |= set(inspect.signature(cls.collect).parameters) - {"self"}
+    assert not set(G.COLLECT_PARAMETERS) & set(G.COLLECT_NOT_AN_AXIS)
+    listed = set(G.COLLECT_PARAMETERS) | set(G.COLLECT_NOT_AN_AXIS)
+    assert params == listed, ("collect() arguments not listed: %s; listed but gone: %s"
+                              % (sorted(params - listed), sorted(listed - params)))
+    for p, axis in G.COLLECT_PARAMETERS.items():
+        assert axis in G.AXES, (p, axis)
+    assert any(c["bootstrap_horizon"] == "on" and c.get("agent0") not in G.SCRIPTED for c in G.CONFIGURATIONS.values())
+
+
+def test_greedy_cases_play_qualifying_layouts():
+    """GreedyHumanModel plays layouts of one 3-onion order only; the 9x5 grid has one such layout, so no pool there."""
+    from overcooked_ai_b200 import greedy, layout
+
+    for name, case in G.CONFIGURATIONS.items():
+        if not G.is_greedy(case):
+            continue
+        single, pool = G.GREEDY_GRIDS[case["path"]]
+        assert case["starts"] in (("fixed", "random") if pool is None else ("pool", "pool_redraw") if single is None else
+                                  ("fixed", "random", "pool", "pool_redraw")), name
+        for l in ([single] if single else []) + (pool or []):
+            greedy.check_layout(layout.compile_layout(l))
+
+
+def test_staggered_timesteps_end_some_warps_partly():
+    for n, horizon in ((97, 7), (127, 13), (113, 10)):
+        t = G.staggered_timesteps(n, horizon)
+        assert ((0 <= t) & (t < horizon)).all() and (t == 0).sum() > 0.9 * n
+        warps = [t[k:k + 32] for k in range(0, n, 32)]
+        assert (warps[0] == 0).all() and all((w != 0).sum() == 1 for w in warps[1:]) and (t == horizon - 1).any()
 
 
 def test_every_refusal_names_a_test_that_exists():

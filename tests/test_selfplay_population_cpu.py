@@ -9,6 +9,7 @@ import pytest
 import torch
 
 from overcooked_ai_b200 import _native
+from overcooked_ai_b200.greedy import GreedyHumanModel
 from overcooked_ai_b200.selfplay import BCPolicy, RllibLSTMShapedCNN, RllibShapedCNN, SelfPlayRollout
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -74,6 +75,8 @@ def test_selfplay_refuses_a_malformed_population_of_learners():
         SelfPlayRollout(env, [RllibShapedCNN(5, 4), RllibShapedCNN(5, 4, num_filters=16)])
     with pytest.raises(AssertionError, match="no partner"):
         SelfPlayRollout(env, [RllibShapedCNN(5, 4)] * 2, partner=BCPolicy(), bc_factor=0.5)
+    with pytest.raises(AssertionError, match="no partner"):
+        SelfPlayRollout(env, [RllibShapedCNN(5, 4)] * 2, partner=GreedyHumanModel(), bc_factor=0.5)
     with pytest.raises(AssertionError, match="blocks go with"):
         SelfPlayRollout(env, RllibShapedCNN(5, 4), blocks=[4, 4])
 
