@@ -864,18 +864,20 @@ class BatchedOvercookedEnv(object):
             self._lut = torch.from_numpy(lut).to(self.device)
         return self._lut
 
-    def featurize_state(self, num_pots=2, out=None, view_swap=None):
+    def featurize_state(self, num_pots=2, out=None, view_swap=None, states=None):
         """featurize_state (overcooked_mdp.py:2579-2898; default NO_COUNTERS_PARAMS planner):
-        float32 [N, 2, 2*(10*num_pots+28)]."""
+        float32 [N, 2, 2*(10*num_pots+28)].  ``states``: featurize these records (int32 CUDA tensor [M, S], e.g. stored
+        games) instead of ``self.state``; N is then M."""
         F = 2 * (10 * num_pots + 28)
+        recs, n = self._records(states)
         if view_swap is not None:
-            assert view_swap.dtype == torch.int32 and view_swap.is_cuda and view_swap.is_contiguous() and view_swap.numel() == self.n_envs
+            assert view_swap.dtype == torch.int32 and view_swap.is_cuda and view_swap.is_contiguous() and view_swap.numel() == n
         if out is None:
-            out = torch.empty((self.n_envs, 2, F), dtype=torch.float32, device=self.device)
-        assert out.dtype == torch.float32 and out.is_cuda and out.is_contiguous() and out.numel() == self.n_envs * 2 * F
+            out = torch.empty((n, 2, F), dtype=torch.float32, device=self.device)
+        assert out.dtype == torch.float32 and out.is_cuda and out.is_contiguous() and out.numel() == n * 2 * F
         _native.check(self._lib.ovc_featurize(
-            self.tables.data_ptr(), self.n_layouts, self.feature_lut().data_ptr(), self.state.data_ptr(),
-            0 if view_swap is None else view_swap.data_ptr(), out.data_ptr(), self.n_envs, self.state_words, num_pots,
+            self.tables.data_ptr(), self.n_layouts, self.feature_lut().data_ptr(), recs.data_ptr(),
+            0 if view_swap is None else view_swap.data_ptr(), out.data_ptr(), n, self.state_words, num_pots,
             self._stream()))
         return out
 

@@ -1,4 +1,4 @@
-"""Build csrc/libovc_b200.so, csrc/libovc_greedy.so and csrc/libovc_horizon.so for the H100 (sm_90a) with nvcc, in-tree next to the sources.
+"""Build csrc/libovc_b200.so, csrc/libovc_greedy.so, csrc/libovc_horizon.so and csrc/libovc_bc.so for the H100 (sm_90a) with nvcc, in-tree next to the sources.
 
     python -m overcooked_ai_b200.build [--force]
 """
@@ -19,6 +19,10 @@ GREEDY_OUT = os.path.join(CSRC, "libovc_greedy.so")
 HORIZON_SOURCES = ["ovc_horizon.cu"]
 HORIZON_DEPS = ["ovc_horizon.cu", os.path.join("..", "..", "include", "ovc_b200.h"), os.path.join("..", "..", "include", "ovc_horizon.h")]
 HORIZON_OUT = os.path.join(CSRC, "libovc_horizon.so")
+# behaviour-cloning training (include/ovc_bc.h): its own ABI too
+BC_SOURCES = ["ovc_bc.cu"]
+BC_DEPS = ["ovc_bc.cu", os.path.join("..", "..", "include", "ovc_b200.h"), os.path.join("..", "..", "include", "ovc_bc.h")]
+BC_OUT = os.path.join(CSRC, "libovc_bc.so")
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
@@ -50,6 +54,7 @@ def build(force=False, verbose=False, variant=None, defines=()):
         return _compile(os.path.join(CSRC, "libovc_b200_%s.so" % variant), SOURCES, DEPS, force, verbose, defines)
     _compile(GREEDY_OUT, GREEDY_SOURCES, GREEDY_DEPS, force, verbose)
     _compile(HORIZON_OUT, HORIZON_SOURCES, HORIZON_DEPS, force, verbose)
+    _compile(BC_OUT, BC_SOURCES, BC_DEPS, force, verbose)
     return _compile(OUT, SOURCES, DEPS, force, verbose, defines)
 
 
